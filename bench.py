@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py — Lloyd-iteration samples/sec of the B200 KMeans engine (BASELINE.json metric).
+"""bench.py — Lloyd-iteration samples/sec of the H100 KMeans engine (BASELINE.json metric).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 Headline workload (BASELINE.json configs[1], "C2"): synthetic blobs 10M x 64 float32, k = 256, one chunk per GPU,
@@ -17,7 +17,7 @@ Numbers reported:
   e2e           same metric through ``lloyd_iteration_host`` with X in pinned HOST memory: every step copies X
                 host->device (double-buffered row blocks) and reads the new centres back
   roofline      the fused chunk kernel against the tensor (dense 16-bit) and HBM roofs, algorithmic work 2*d*k flops and
-                d*4+4 bytes per sample (SURVEY.md §8d)
+                d*4+4 bytes per sample
   parity_check  labels of the LAST timed iteration on a >= 1M-row slice against the float64 arg-min evaluated on the
                 device (mismatches must be float64 near-ties; worst relative margin reported) + deferred-row fraction
   configs       the other BASELINE shapes as sub-records, same loop, same parity check: C3 (4.9M x 41, k=100; with N>1
@@ -27,6 +27,9 @@ Numbers reported:
   cpu_baseline  the dask-ml path restated without dask (oracle/: scikit-learn float64 E-step + the reference's numba
                 scatter-add, thread pool over row blocks) on a bounded row sample of C2
 ``--impl reference`` times that CPU path alone on the FULL 10M-row C2 chunk and prints the same line shape.
+``--dump-outputs DIR`` writes what the headline's last timed iteration computed (rank 0) as DIR/<name>.npy: the new
+centres, the reduced sums and counts, the shift and every LABEL_STRIDE-th label.  The inputs are generated from fixed
+seeds, so two builds run with the same arguments can be compared output for output.
 """
 import argparse
 import json
@@ -71,8 +74,9 @@ def _peaks():
             m = json.load(f)
         src = "measured"
     else:
-        m = {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}
-        src = "fallback"
+        # NVIDIA H100 SXM data sheet (700 W card): HBM3 bandwidth and dense BF16/FP16 tensor rate
+        m = {"hbm_gbs": 3350.0, "bf16_tflops": 989.0}
+        src = "data sheet (H100 SXM)"
     return m, src
 
 
@@ -94,7 +98,7 @@ def synth_blobs_device(n, d, k_true, seed, device, dtype):
 
 
 def synth_config_device(name, n, seed, device):
-    """SURVEY.md §8(d) generators.  C3: 38 blob columns + 3 low-cardinality integer-coded columns (values 0..69) like the
+    """Generators of the BASELINE shapes.  C3: 38 blob columns + 3 low-cardinality integer-coded columns (values 0..69) like the
     coded categoricals of the KDD table; C4: 20 true centres, heterogeneous column scales 1 ... 1e3."""
     import torch
 
@@ -149,6 +153,7 @@ class ClockSampler(threading.Thread):
         self.samples = []
         self.reasons = set()
         self.max_mhz = None
+        self.power_limit_w = None
         self._stop_evt = threading.Event()
 
     def run(self):
@@ -158,6 +163,7 @@ class ClockSampler(threading.Thread):
             pynvml.nvmlInit()
             h = pynvml.nvmlDeviceGetHandleByIndex(self.index)
             self.max_mhz = pynvml.nvmlDeviceGetMaxClockInfo(h, pynvml.NVML_CLOCK_SM)
+            self.power_limit_w = pynvml.nvmlDeviceGetPowerManagementLimit(h) / 1000.0
             names = {
                 pynvml.nvmlClocksThrottleReasonHwSlowdown: "hw_slowdown",
                 pynvml.nvmlClocksThrottleReasonSwThermalSlowdown: "sw_thermal_slowdown",
@@ -179,7 +185,8 @@ class ClockSampler(threading.Thread):
         self._stop_evt.set()
         self.join(timeout=2)
         med = float(np.median(self.samples)) if self.samples else None
-        return {"sm_mhz": med, "sm_max_mhz": self.max_mhz, "reasons": sorted(self.reasons)}
+        return {"sm_mhz": med, "sm_max_mhz": self.max_mhz, "power_limit_w": self.power_limit_w,
+                "reasons": sorted(self.reasons)}
 
 
 # ------------------------------------------------------------------------------------------
@@ -346,15 +353,18 @@ def time_lloyd(st, steps, warmup, barrier, world, dev):
     return float(t[0]) / steps, float(t[1]), int(launches)
 
 
-def _static_traffic(name):
-    """DRAM bytes per launch of the config's dominant kernel from the committed ncu --set full capture
-    (profiles/ncu_traffic.json; not measured in this run), or None."""
-    tp = os.path.join(ROOT, "profiles", "ncu_traffic.json")
-    try:
-        with open(tp) as f:
-            return json.load(f).get("configs", {}).get(name, {}).get("dram_bytes_per_launch")
-    except (OSError, ValueError):
-        return None
+LABEL_STRIDE = 4          # every 4th label: 10M rows -> 10 MB of float32
+
+
+def dump_outputs(path, st):
+    """What the last timed iteration computed: new centres, reduced [k*d sums | k counts], shift, sampled labels."""
+    os.makedirs(path, exist_ok=True)
+    k, d = st.k, st.d
+    red = st.red.double().cpu().numpy()
+    outs = {"centers": st.C.double().cpu().numpy(), "sums": red[:k * d].reshape(k, d), "counts": red[k * d:k * d + k],
+            "shift": st.shift.double().cpu().numpy(), "labels": st.labels[0][::LABEL_STRIDE].float().cpu().numpy()}
+    for name, a in outs.items():
+        np.save(os.path.join(path, name + ".npy"), a)
 
 
 def run_config(name, args, be, comm, dev, rank, world, barrier, peaks):
@@ -393,7 +403,7 @@ def run_config(name, args, be, comm, dev, rank, world, barrier, peaks):
     data = DeviceData(Xs, be, comm)
     init = data.global_rows(list(range(k))).astype(np.float64)
     st = LloydState(data, init)
-    steps = max(5, args.steps)
+    steps = args.steps
     ms, kern_ms, _ = time_lloyd(st, steps, args.warmup, barrier, world, dev)
     C_used = st.C_new.clone()                 # after accept(): the centres the last E-step ran against
     par = parity_check(X, st.labels[0], C_used, be, k)
@@ -417,7 +427,6 @@ def run_config(name, args, be, comm, dev, rank, world, barrier, peaks):
                      "unit": "GB/s" if bound == "hbm" else "TFLOP/s",
                      "frac": (gbs / float(peaks["hbm_gbs"])) if bound == "hbm" else tf / peak_tf,
                      "hbm_gbs": gbs, "tflops": tf,
-                     "traffic": _static_traffic(name),
                      "algorithmic": {"bytes_per_sample": d * esz + 4, "flops_per_sample": 2 * d * k}},
         "parity_check": par, "final_shift": float(st.shift.item()),
     }
@@ -438,7 +447,10 @@ def main():
     ap.add_argument("--no-e2e", action="store_true", help="skip the host-buffer e2e leg")
     ap.add_argument("--no-configs", action="store_true", help="skip the C3/C4/C5 sub-records")
     ap.add_argument("--configs", default="C3,C4,C5", help="comma-separated sub-records to run")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed iteration's outputs as DIR/<name>.npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     args.warmup = max(3, args.warmup)
 
     rank = int(os.environ.get("RANK", "0"))
@@ -453,7 +465,7 @@ def main():
     import torch.distributed as dist
 
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py needs a GPU (the hot path is sm_100a CUDA; there is no CPU fallback)")
+        raise SystemExit("bench.py needs a GPU (the hot path is sm_90a CUDA; there is no CPU fallback)")
     torch.cuda.set_device(local_rank)
     dev = torch.device("cuda", local_rank)
     if world > 1:
@@ -484,6 +496,9 @@ def main():
     sampler.start()
     ms_per_step, kern_ms, launches = time_lloyd(st, args.steps, args.warmup, barrier, world, dev)
     clocks = sampler.stop()
+    clocks["gpu"] = torch.cuda.get_device_name(dev)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, st)
     value = n * world / (ms_per_step * 1e-3)
     shift = float(st.shift.item())
     C_used = st.C_new.clone()
@@ -600,26 +615,17 @@ def main():
     bytes_alg = (N_FEAT * 4 + 4) * n
     ach_tf = flops / (kern_ms * 1e-3) / 1e12
     ach_gbs = bytes_alg / (kern_ms * 1e-3) / 1e9
-    # The product runs on the kind::f16 tensor pipe (split-fp16, 3 products + the ||c||^2 step = 3.25x the
-    # algorithmic flops), so the roof is the measured dense 16-bit peak: the sustained figure, because the
-    # kernel is timed inside a long step.
+    # The product runs on the fp16 tensor pipe (split-fp16, 3 products = 3x the algorithmic flops), so the roof is the
+    # dense 16-bit peak.
     peak_tf = float(peaks.get("bf16_tflops_sustained", peaks["bf16_tflops"]))
-    peak_note = "%s dense bf16/fp16 tensor peak, sustained (MEASURED_PEAKS.json)" % peak_src
-    issued_ratio = 3.25
-    traffic = None
-    tp = os.path.join(ROOT, "profiles", "ncu_traffic.json")
-    if os.path.exists(tp):
-        with open(tp) as f:
-            traffic = json.load(f).get("dram_bytes_per_launch")
+    peak_note = "%s dense bf16/fp16 tensor peak" % peak_src
+    issued_ratio = 3.0
     roofline = {
         "bound": "tensor", "achieved": ach_tf, "peak": peak_tf, "unit": "TFLOP/s", "frac": ach_tf / peak_tf,
-        "traffic": traffic, "traffic_source": "static: ncu --set full capture committed under profiles/ (not measured in this run)",
         "peak_source": peak_note, "kernel_ms": kern_ms,
-        "kernel": "tc_chunk_kernel<true,false> (tcgen05 split-fp16 fused E+M) + tc_recheck + reduce_partials",
-        "limiter": "three 128-column TMEM accumulator buffers x (epilogue ~3.0-3.6k cycles at ~6.8 B/clk of TMEM reads per warp "
-                   "+ MMA refill ~1.0-1.5k) per 2-unit tile; tensor pipe 43 %, issue slots 71 % (DESIGN.md (d), profiles/r02_ncu_tc_chunk_C2.md)",
+        "kernel": "tc_chunk_kernel<256,true,false,false> (wgmma split-fp16 fused E+M) + tc_recheck + reduce_partials",
         "issued": {"tflops": ach_tf * issued_ratio, "frac": ach_tf * issued_ratio / peak_tf,
-                   "note": "tensor-pipe work actually issued: 3 fp16 products + ||c||^2 step per algorithmic product"},
+                   "note": "tensor-pipe work actually issued: 3 fp16 products per algorithmic product"},
         "hbm": {"achieved": ach_gbs, "peak": float(peaks["hbm_gbs"]), "unit": "GB/s",
                 "frac": ach_gbs / float(peaks["hbm_gbs"]), "peak_source": peak_src},
         "algorithmic": {"flops_per_sample": 2 * N_FEAT * N_CLUST, "bytes_per_sample": N_FEAT * 4 + 4,
@@ -635,8 +641,8 @@ def main():
         "warmup": args.warmup, "ms_per_step": ms_per_step, "higher_is_better": True, "scaling": "weak",
         "vs_baseline": None, "dtype": "f32", "data": "synthetic",
         "config": cfg,
-        "detail": {"arithmetic": "split-fp16 (hi,lo) x3 product on tcgen05 kind::f16, fp32 accumulate, float64 re-check of near-ties + float64 centre update",
-                   "l2": "inputs (%.2f GB per GPU) are larger than L2 (126 MB); no explicit flush" % (n * N_FEAT * 4 / 1e9),
+        "detail": {"arithmetic": "split-fp16 (hi,lo) x3 product on wgmma (f16, fp32 accumulate), float64 re-check of near-ties + float64 centre update",
+                   "l2": "inputs (%.2f GB per GPU) are larger than L2 (50 MB); no explicit flush" % (n * N_FEAT * 4 / 1e9),
                    "step": "lloyd_loop() as KMeans.fit runs it: fused E+M kernel + reduce + re-check (+ all-reduce) + finalize_step (centre update, shift, device-side stop test, next pack); one host read of the loop state per 8 iterations",
                    "kernel_family": fam_c2, "final_shift": shift},
         "clocks": clocks, "e2e": e2e, "gpu_launches": int(launches), "roofline": roofline, "parity_check": par,

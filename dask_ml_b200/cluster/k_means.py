@@ -1,11 +1,11 @@
-"""KMeans with the dask_ml.cluster.KMeans API, executed by the B200 engine.
+"""KMeans with the dask_ml.cluster.KMeans API, executed by the H100 engine.
 
 Mirrors dask_ml/cluster/k_means.py (reference @ 0310a90):
   KMeans                      :26-233     k_means            :236-275
   k_init                      :291-369    init_pp            :372-384
   init_random                 :387-393    init_scalable      :396-463
   evaluate_cost/_sample_points :466-491   _kmeans_single_lloyd :499-569
-The host loop keeps the reference's control flow (including its quirks Q1-Q6, SURVEY.md §8a);
+The host loop keeps the reference's control flow (including its quirks Q1-Q6, DESIGN.md (a));
 all arithmetic over X runs in the CUDA kernels behind include/bkm_b200.h.
 """
 import logging
@@ -359,7 +359,7 @@ def init_scalable(X, n_clusters, random_state=None, max_iter=None, oversampling_
     Bernoulli draw kernel (``bkm_sample_chunk``).  The reference draws U with dask's per-chunk RandomState
     (k_means.py:487); here U comes from a counter-based Philox stream keyed by a per-round seed and the global row
     index, so a run is reproducible for a given ``random_state`` independent of chunking and of the number of GPUs
-    (k-means|| sampling parity with the reference is therefore distributional, not bit-exact: SURVEY.md §8c).
+    (k-means|| sampling parity with the reference is therefore distributional, not bit-exact: DESIGN.md (c)).
 
     The final reduce of the candidates to ``n_clusters`` centres (k_means.py:457-463: an in-memory scikit-learn KMeans,
     unweighted) runs on the GPU through this engine (``_reduce_candidates``).  ``weighted=True`` gives every candidate
@@ -691,15 +691,15 @@ class LloydState(object):
 
 
 def _check_engine(be, value, what):
-    """A tcgen05 pipeline wait that timed out poisons the step with NaN (bkm_tc.cu): turn that into an error."""
+    """A poisoned step (NaN shift / cost, see bkm_debug_abort_code) becomes an error."""
     if value == value and abs(value) != float("inf"):
         return
     code = be.abort_code() if hasattr(be, "abort_code") else 0
     if code:
         be.reset_abort()
-        raise RuntimeError("B200 KMeans engine: a pipeline wait inside the tensor kernel timed out (abort code 0x%08x) "
+        raise RuntimeError("KMeans engine: a pipeline wait inside the tensor kernel timed out (abort code 0x%08x) "
                            "while computing %s; the results of this call are invalid" % (code, what))
-    raise RuntimeError("B200 KMeans engine: non-finite %s (%r) — X or the centres hold values outside the range of "
+    raise RuntimeError("KMeans engine: non-finite %s (%r) — X or the centres hold values outside the range of "
                        "their dtype" % (what, value))
 
 

@@ -53,13 +53,13 @@ static float tau_for(int d, int dtype, int flags, int family) {
   // so |sum x_i r_i| <= 2^-19 (||x||^2 + ||c||^2), doubled by the -2 factor and again for the difference of two
   // distances: 2^-17.  To that the fp32 accumulation of 2 products per 16-element K-step (same model as family 1).
   if (family == 3) return 1.0f / 131072.0f + (8.0f * sqrtf(2.0f * (float)((d + 7) / 8)) + 16.0f) * eps;
-  // tcgen05 path (split-fp16 triple, scaled by a power of two): error sources relative to ||x||^2+||c||^2 are the
+  // tensor path (split-fp16 triple, scaled by a power of two): error sources relative to ||x||^2+||c||^2 are the
   // fp16 (hi, lo) representation of both operands (2^-22 each; 2^-25 absolute in scaled units when lo falls into
   // fp16's subnormals, negligible because the scale puts max|c| at 2^9..2^10), the dropped lo*lo term (2^-24),
-  // the 3*ceil(d/16)+1 accumulations into the fp32 TMEM accumulator, and the accumulator's own rounding.
-  // Measured with the re-check switched off (tests/tau_probe.py, 14M rows of blobs / uniform / badly scaled data):
-  // worst margin of a label that differs from float64 = 4.8e-7; the bound below (3.3e-6 at d=64) leaves ~7x
-  // headroom, and the parity tests assert that every remaining difference is a float64 near-tie (<= 1e-9).
+  // the 3*ceil(d/16) accumulations into the fp32 accumulator, the fp32 addition of ||s c||^2, and the accumulator's own
+  // rounding.  tests/test_gpu_tau.py measures, with the re-check switched off, the worst margin of a label that differs
+  // from float64 and asserts at least 4x headroom to this bound (3.3e-6 at d=64); the parity tests assert that every
+  // remaining difference is a float64 near-tie (<= 1e-9).
   if (family == 1) return (8.0f * sqrtf(3.0f * (float)((d + 7) / 8)) + 16.0f) * eps;
   // CUDA-core kernels (generic and streaming): fp32 FMA chains of length d plus the rounding of ||c||^2
   return 8.0f * (sqrtf((float)d) + 2.0f) * eps;
@@ -210,7 +210,7 @@ int bkm_workspace_bytes(int64_t n, int d, int k, int x_dtype, size_t* out) {
   if (k <= 0 || d <= 0 || n < 0 || !out) return BKM_EINVAL;
   if (!dtype_ok(x_dtype)) return BKM_EDTYPE;
   int sm = 0;
-  if (sm_count_of_current(&sm)) sm = kDefaultSMs;       // no device (CPU-side sizing): the B200 figure
+  if (sm_count_of_current(&sm)) sm = kDefaultSMs;       // no device (CPU-side sizing): the H100 SXM figure
   *out = ws_layout(n, d, k, x_dtype, sm).total;
   return 0;
 }
@@ -252,7 +252,7 @@ int bkm_transform_chunk(const void* X, int64_t n, int d, int64_t ldx, int x_dtyp
   int sm = 0;
   int rc = sm_count_of_current(&sm);
   if (rc) return rc;
-  // fp32, d <= 64, k <= 256: the tcgen05 pipeline with the transform epilogue (callers cut wider Y into column blocks)
+  // fp32, d <= 64, k <= 256: the tensor-core kernel with the transform epilogue (callers cut wider Y into column blocks)
   if (x_dtype == BKM_F32 && tc_supported(d, k, x_dtype) && !(flags & BKM_FLAG_FORCE_SIMT)) {
     ChunkArgs a = {};
     a.X = X; a.n = n; a.d = d; a.ldx = ldx;

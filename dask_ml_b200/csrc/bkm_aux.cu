@@ -35,7 +35,7 @@ __global__ void pack_centers_kernel(const double* __restrict__ C, unsigned char*
       int r = i / L.d4, c = i - r * L.d4;
       cT[i] = c < d ? (float)C[(size_t)r * d + c] : 0.f;
     }
-    // tcgen05 operands: B = -2 s C as an fp16 pair (hi + lo carries 22 significant bits); rows/columns
+    // tensor-core operands: B = -2 s C as an fp16 pair (hi + lo carries 22 significant bits); rows/columns
     // beyond (k, d) are zero.  Only shapes the tensor path takes (d <= 64) have room in the pack.
     if (d <= L.dh) {
       const double sc = (double)reinterpret_cast<const PackHeader*>(pack)->scale;
@@ -425,7 +425,7 @@ int launch_pack(const double* C, int k, int d, int dtype, void* pack, cudaStream
   int nb = (L.kp * L.dk + 255) / 256; if (nb > 296) nb = 296; if (nb < 1) nb = 1;
   pack_scale_kernel<<<1, 1024, 0, s>>>(C, (unsigned char*)pack, L);
   pack_centers_kernel<<<nb, 256, 0, s>>>(C, (unsigned char*)pack, L);
-  int nb2 = (L.kp + 7) / 8; if (nb2 > 148) nb2 = 148;
+  int nb2 = (L.kp + 7) / 8; if (nb2 > 132) nb2 = 132;
   pack_norms_kernel<<<nb2, 256, 0, s>>>(C, (unsigned char*)pack, L);
   pack_header_kernel<<<1, 256, 0, s>>>((unsigned char*)pack, L);
   note_launch(4);
@@ -640,7 +640,7 @@ __global__ void sample_kernel(const T* __restrict__ d2, long long n, double ell_
 int launch_sample(const void* d2, long long n, int dtype, double eop, uint64_t seed, uint64_t off,
                   long long* picked, long long cap, int* n_picked, cudaStream_t s) {
   if (n == 0) return 0;
-  long long nb = (n + 255) / 256; if (nb > 148 * 8) nb = 148 * 8;
+  long long nb = (n + 255) / 256; if (nb > 132 * 8) nb = 132 * 8;
   if (dtype == BKM_F32)
     sample_kernel<float><<<(int)nb, 256, 0, s>>>((const float*)d2, n, eop, seed, off, picked, cap, n_picked);
   else

@@ -1,4 +1,4 @@
-// bkm_common.cuh — shared definitions for the B200 KMeans hot-path kernels.
+// bkm_common.cuh — shared definitions for the KMeans hot-path kernels (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -54,7 +54,7 @@ static inline bool tc2_shape(int d, int k, int dtype) {
 struct PackLayout {
   int k, d, dtype;
   int d4;      // d rounded up to a multiple of 4 (SIMT row pitch, zero padded)
-  int kp;      // k rounded up to a multiple of 16 (UMMA N granularity)
+  int kp;      // k rounded up to a multiple of 16 (MMA N granularity)
   int dk;      // d rounded up to a multiple of 32 (one 128-byte swizzle atom of fp32 per K-block)
   int dh;      // row length of the fp16 MMA operand tiles: 64 halves = one 128-byte swizzle atom (d <= 64)
   size_t esz;  // sizeof(T)
@@ -77,7 +77,7 @@ static inline PackLayout pack_layout(int k, int d, int dtype) {
   L.off_cnT = o;  o = align_up(o + (size_t)k * L.esz, 256);
   L.off_c64 = o;  o = align_up(o + (size_t)k * d * 8, 256);
   L.off_cn64 = o; o = align_up(o + (size_t)k * 8, 256);
-  L.off_bhi = o;  o = align_up(o + (size_t)L.kp * L.dh * 2, 256);   // fp16 tiles (tcgen05 path, d <= 64)
+  L.off_bhi = o;  o = align_up(o + (size_t)L.kp * L.dh * 2, 256);   // fp16 tiles (tensor path, d <= 64)
   L.off_blo = o;  o = align_up(o + (size_t)L.kp * L.dh * 2, 256);
   L.off_cn32 = o; o = align_up(o + (size_t)L.kp * 4, 256);
   L.off_bcn = o;  o = align_up(o + (size_t)L.kp * 32, 256);   // ||c||^2 as an MMA operand tile (see bkm_tc.cu)
@@ -99,7 +99,7 @@ static inline PackLayout pack_layout(int k, int d, int dtype) {
 struct PackHeader {
   int k, d, dtype, pad;
   double cn_max;   // max_j ||c_j||^2 (float64) — used by the near-tie margin bound
-  float scale;     // power of two s with s * max|c_ji| in [2^9, 2^10): the tcgen05 path multiplies X and C by s
+  float scale;     // power of two s with s * max|c_ji| in [2^9, 2^10): the tensor path multiplies X and C by s
   float pad2;      // before the fp16 split, so that both fit fp16's range (exact: only exponents change)
 };
 
@@ -109,7 +109,7 @@ struct PackHeader {
 // Per-CTA partial sums: one [k*d] slot per CTA of the largest grid a CUDA-core kernel launches (8 CTAs per SM),
 // fewer when a slot is large (a kernel whose per-CTA sums occupy most of the shared memory runs 1-2 CTAs per SM), and a
 // single slot when k*d cannot be CTA-resident at all (generic kernel's GLOBAL mode: atomics into slot 0).
-static const int kDefaultSMs = 148;
+static const int kDefaultSMs = 132;     // H100 SXM: sizing when no device is visible
 
 struct WsLayout {
   size_t off_bal, off_psum, off_pcnt, off_pin, off_flag, off_defer, off_rec, off_lab, off_bin, off_binoff, total;
@@ -178,7 +178,7 @@ struct ChunkArgs {
   double* pin;        // [grid] partial sum of min distances
   float tau;          // near-tie margin coefficient (0 disables the f64 re-check)
   int want_sum;       // caller wants the summed min distance (inertia / cost)
-  int* defer_cnt;     // tcgen05 path: number of rows deferred to the float64 re-check kernel
+  int* defer_cnt;     // tensor paths: number of rows deferred to the float64 re-check kernel
   int* defer_idx;     // [n] their row indices
   int psum_slots;     // capacity of psum in [k*d] slots (grid clamp of the kernels that keep per-CTA sums)
   int part_slots;     // capacity of pcnt / pin

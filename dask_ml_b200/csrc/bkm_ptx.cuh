@@ -1,5 +1,4 @@
-// bkm_ptx.cuh — inline-PTX wrappers shared by the sm_100a kernels written in round 2 (bkm_stream.cu, bkm_tc2.cu,
-// bkm_xform.cu).  bkm_tc.cu keeps its own copies (its waits report into its abort word).
+// bkm_ptx.cuh — inline-PTX wrappers shared by the CUDA-core kernels (bkm_stream.cu, bkm_rowpass.cu, bkm_p2p.cu).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -57,7 +56,8 @@ __device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t
 }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
-// packed fp32 pairs (FFMA2 on sm_100: two fused multiply-adds per issued instruction)
+// packed fp32 pairs: two fused multiply-adds on the halves of a 64-bit register pair (sm_90 has no paired FFMA, so this
+// is two FFMA; keeping the pair form lets the callers load / store operands as 64-bit pairs)
 __device__ __forceinline__ unsigned long long pack2(float lo, float hi) {
   unsigned long long r;
   asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
@@ -67,88 +67,17 @@ __device__ __forceinline__ void unpack2(unsigned long long v, float& lo, float& 
   asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v));
 }
 __device__ __forceinline__ unsigned long long ffma2(unsigned long long a, unsigned long long b, unsigned long long c) {
-  unsigned long long d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-  return d;
+  float a0, a1, b0, b1, c0, c1;
+  unpack2(a, a0, a1); unpack2(b, b0, b1); unpack2(c, c0, c1);
+  return pack2(fmaf(a0, b0, c0), fmaf(a1, b1, c1));
 }
-__device__ __forceinline__ float fmin3(float a, float b, float c) {
-  float d;
-  asm("min.f32 %0, %1, %2, %3;" : "=f"(d) : "f"(a), "f"(b), "f"(c));
-  return d;
-}
+__device__ __forceinline__ float fmin3(float a, float b, float c) { return fminf(fminf(a, b), c); }
 // 1.0f if a <= b else 0.0f (FSET: no predicate / select pair)
 __device__ __forceinline__ float fset_le(float a, float b) {
   float r;
   asm("set.le.f32.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b));
   return r;
 }
-
-// ------------------------------------------------------------------ TMA (tensor maps) and tcgen05 / TMEM
-__device__ __forceinline__ void tma_load_2d(uint32_t dst, const void* tmap, uint32_t bar, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(dst), "l"(tmap), "r"(bar), "r"(c0), "r"(c1) : "memory");
-}
-__device__ __forceinline__ void tma_prefetch_2d(const void* tmap, int c0, int c1) {
-  asm volatile("cp.async.bulk.prefetch.tensor.2d.L2.global.tile [%0, {%1, %2}];" ::"l"(tmap), "r"(c0), "r"(c1) : "memory");
-}
-__device__ __forceinline__ void tmap_prefetch(const void* tmap) { asm volatile("prefetch.tensormap [%0];" ::"l"(tmap)); }
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred;
-  asm volatile("{\n.reg .pred P;\nelect.sync _|P, 0xffffffff;\nselp.u32 %0, 1, 0, P;\n}" : "=r"(pred));
-  return pred != 0;
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tc_alloc(uint32_t smem_dst, uint32_t cols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_dst), "r"(cols));
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-}
-__device__ __forceinline__ void tc_dealloc(uint32_t tmem, uint32_t cols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(cols));
-}
-// D[tmem] (+)= A[smem] . B[smem]^T, both operands through shared-memory matrix descriptors
-__device__ __forceinline__ void mma_f16_ss(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t acc) {
-  asm volatile(
-      "{\n.reg .pred p;\nsetp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n}"
-      ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(acc) : "memory");
-}
-__device__ __forceinline__ void mma_tf32_ss(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t acc) {
-  asm volatile(
-      "{\n.reg .pred p;\nsetp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n}"
-      ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(acc) : "memory");
-}
-#define BKM_TC_LD16(taddr, r)                                                                          \
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 "                                               \
-               "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"                       \
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),   \
-                 "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]),            \
-                 "=r"(r[13]), "=r"(r[14]), "=r"(r[15])                                                 \
-               : "r"(taddr) : "memory")
-__device__ __forceinline__ void tc_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// K-major SWIZZLE_128B shared-memory matrix descriptor (sm_100, version 1): 8-row x 128-byte swizzle atoms,
-// SBO = 1024 B between atoms along M/N; a K-step of 32 bytes inside the atom advances the start address by 2 (>> 4).
-__device__ __forceinline__ uint64_t desc_sw128(uint32_t saddr) {
-  return (uint64_t)((saddr >> 4) & 0x3FFF) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) | ((uint64_t)1 << 46) |
-         ((uint64_t)2 << 61);
-}
-// K-major, no swizzle, 32-byte rows: core matrices of 8 rows x 16 B; second K chunk 128 B further (LBO), next 8-row
-// group 256 B further (SBO)
-__device__ __forceinline__ uint64_t desc_noswz32(uint32_t saddr) {
-  return (uint64_t)((saddr >> 4) & 0x3FFF) | ((uint64_t)(128 >> 4) << 16) | ((uint64_t)(256 >> 4) << 32) | ((uint64_t)1 << 46);
-}
-// instruction descriptor: fp32 accumulate, K-major A and B, M = 128; formats: 0 = fp16, 1 = bf16, 2 = tf32
-__device__ __forceinline__ uint32_t idesc_m128(int n, int afmt, int bfmt) {
-  return (1u << 4) | ((uint32_t)afmt << 7) | ((uint32_t)bfmt << 10) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-}
-// byte offset of 16-byte chunk q (0..7) of row r inside one SWIZZLE_128B K-block ([rows][128 B])
-__device__ __forceinline__ uint32_t sw128_chunk(int r, int q) { return (uint32_t)(r * 128 + ((q ^ (r & 7)) << 4)); }
 
 }  // namespace ptx
 }  // namespace bkm

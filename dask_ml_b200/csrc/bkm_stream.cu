@@ -6,8 +6,8 @@
 //     (cp.async.bulk global -> shared, completion on a per-stage mbarrier, issued by lane 0): no CTA-wide barrier in
 //     the main loop, HBM requests stay in flight while the warp computes;
 //   * E-step (sklearn pairwise_distances_argmin_min per chunk, dask_ml/metrics/pairwise.py:35-38): thread = row, the row
-//     in registers, centres in shared memory as PAIRS {-2 c_2p, -2 c_2p+1} per feature so that one FFMA2 (packed fp32x2
-//     fma, sm_100) advances two distances; all k distances stay in registers, the arg-min and the near-tie test are
+//     in registers, centres in shared memory as PAIRS {-2 c_2p, -2 c_2p+1} per feature so that one 64-bit load feeds
+//     two distances (ptx::ffma2: two FFMA on sm_90); all k distances stay in registers, the arg-min and the near-tie test are
 //     decoded from one FSET+FFMA per distance (same scheme as the tensor-path epilogue);
 //   * rows whose best/second margin is inside the fp32 rounding bound are re-decided by the SAME thread in float64
 //     against the float64 centres (rare: the warp diverges for them only);
@@ -51,7 +51,7 @@ static inline StreamSmem stream_smem(int k, int d, long long ldx, int kpt, int d
 }
 
 // DH >= ceil(d / 2) feature pairs; KPT = number of centre pairs rounded up to an even number (k <= 4, 8, ..., 32).
-// Both are compile-time so that the distance loop is branch-free straight-line FFMA2 code.
+// Both are compile-time so that the distance loop is branch-free straight-line FFMA code.
 template <int DH, int KPT, bool MSTEP>
 __global__ void __launch_bounds__(SW * 32, 2)
 stream_chunk_kernel(ChunkArgs a, StreamSmem S) {
@@ -165,14 +165,14 @@ stream_chunk_kernel(ChunkArgs a, StreamSmem S) {
 #pragma unroll
     for (int i = 0; i < DP; ++i) xn = fmaf(x[i], x[i], xn);
 
-    // ---- E-step: all k distances (GEMM form ||c||^2 - 2 x.c), two per FFMA2 ----
+    // ---- E-step: all k distances (GEMM form ||c||^2 - 2 x.c), two per ffma2 ----
     unsigned long long dp[KPT];
 #pragma unroll
     for (int g = 0; g + 4 <= KPT; g += 4) {
       unsigned long long a0 = cn2[g], a1 = cn2[g + 1], a2 = cn2[g + 2], a3 = cn2[g + 3];
 #pragma unroll
       for (int i = 0; i < DP; i += 2) {
-        // {x_i, x_i}: FFMA2 takes the scalar as a broadcast operand, no second register is spent on it
+        // {x_i, x_i}: the scalar as both halves of the pair
         const unsigned long long x0 = pack2(x[i], x[i]), x1 = pack2(x[i + 1], x[i + 1]);
         const ulonglong2 c0 = *reinterpret_cast<const ulonglong2*>(cp + (g + 0) * DP + i);
         const ulonglong2 c1 = *reinterpret_cast<const ulonglong2*>(cp + (g + 1) * DP + i);
@@ -332,12 +332,10 @@ stream_chunk_kernel(ChunkArgs a, StreamSmem S) {
 }
 
 // ==========================================================================================================
-// Two rows per thread (k <= 24): the FFMA2 pair is {row l, row l + 32} of a 64-row warp tile against ONE centre value
+// Two rows per thread (k <= 24): the ffma2 pair is {row l, row l + 32} of a 64-row warp tile against ONE centre value
 // (broadcast operand), so every centre load (LDS.128 of four features) feeds two rows, the per-tile overheads (ring
 // refill, label masks, M-step loop) are paid once per 64 rows and the lane-owns-cluster M-step sees twice the rows per
-// cluster and pass (better lane utilisation: its trip count is the LARGEST list of the tile).  ncu of the one-row
-// kernel on C4 (profiles/r02_stream_kernel.md): 780 warp instructions and 235 shared-memory wavefronts per 32 rows, both
-// pipes near saturation; this layout needs ~430 / ~140.
+// cluster and pass (better lane utilisation: its trip count is the LARGEST list of the tile).
 // ==========================================================================================================
 static const int S2_NSTG = 3;       // ring stages per warp (64 rows each)
 

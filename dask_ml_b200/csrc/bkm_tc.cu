@@ -1,988 +1,329 @@
-// bkm_tc.cu — fused E+M chunk kernel on the 5th-gen tensor cores (tcgen05 / TMEM / TMA), sm_100a.
+// bkm_tc.cu — fused E+M chunk kernel on the Hopper tensor cores (wgmma, sm_90a).
 //
 // Shapes: fp32 X with d <= 64 and a 16-byte aligned row pitch, k <= 256 (BASELINE config C2: 10M x 64, k = 256).
 //
-// Per 128-row tile of X the kernel computes  acc = s^2 ||c||^2 + (s X) . (-2 s C)^T  with the product as a
-// split-fp16 triple on the kind::f16 tensor pipe (twice the TF32 rate):
+// Per 64-row tile of X a warpgroup computes  acc = (s X) . (-2 s C)^T  with the product as a split-fp16 triple
+// (twice the TF32 rate):
 //     Xhi.Bhi + Xhi.Blo + Xlo.Bhi        (hi = rn_fp16(v), lo = rn_fp16(v - hi): 22 significant bits)
-// s is a power of two chosen from the centres (PackHeader::scale) so that both operands sit in fp16's range;
-// scaling by s is exact, so the result is the fp32-GEMM-class distance (~2^-22 relative error per product)
-// and labels agree with the reference's float64 E-step (sklearn pairwise_distances_argmin_min,
-// dask_ml/metrics/pairwise.py:35-38) except on near-ties, which are re-decided in float64 (as are rows whose
-// scaled entries leave fp16's range).  ||c||^2 enters through one extra tf32 K-step (rows [hi,mid,lo,0..]
-// against a constant [1,1,1,0..] tile).  The M-step (_centers_dense, dask_ml/cluster/k_means.py:572-582) is
-// fused: rows are added into REGISTER-resident per-CTA sums, X is read from HBM once.
+// and adds s^2 ||c||^2 per column in fp32 in the epilogue.  s is a power of two chosen from the centres
+// (PackHeader::scale) so that both operands sit in fp16's range; scaling by s is exact, so the result is the
+// fp32-GEMM-class distance (~2^-22 relative error per product) and labels agree with the reference's float64 E-step
+// (sklearn pairwise_distances_argmin_min, dask_ml/metrics/pairwise.py:35-38) except on near-ties, which are
+// re-decided in float64 (as are rows whose scaled entries leave fp16's range).  The M-step (_centers_dense,
+// dask_ml/cluster/k_means.py:572-582) is fused: rows are added into shared-memory per-CTA sums, X is read from HBM once.
 //
-// Warp roles (768 threads; roles are assigned per aligned warpgroup, setmaxnreg moves registers between them):
-//   0       TMA producer: polls the A ring (2-4 x 128-row fp32 X tiles, SWIZZLE_128B, L2 prefetch ahead) and the
-//           M ring (the same tiles re-fetched from L2 for the M-step / distance warps); allocates TMEM
-//   1, 2    MMA issuers on alternate accumulator units (warp-converged, uniform-register operands, one elected lane
-//           issues tcgen05.mma / commit); 3 spare
-//   4-7     converter: s X -> fp16 (hi, lo) pairs -> TMEM operand slot, ||s x||^2 -> shared memory; runs ahead
-//   8-11, 12-15   two epilogue sets on alternate tiles (thread == row == TMEM lane), single pass over the accumulator
-//   16-23   M-step / distance warps, lane-owns-cluster flavour: lane j of warp w walks the row lists of cluster
-//           32w+j that the epilogue linked, keeping the cluster's sums (Lloyd step) or centre (distances) in
-//           registers.  The <MSTEP, WANT_DIST> = <true, true> variant keeps the older flavour instead (16 warps,
-//           warp w owns clusters c % 16 == w, lane l holds features l, l+32, fp32 centres in shared memory).
-// TMEM (512 columns): 3 x 128 accumulator buffers + 2 x (32 Xhi + 32 Xlo) operand columns.
-// Pipelines (mbarriers): A ring full/empty, M ring full/empty, operands ready (8 deep) / operand slot free,
-// accumulator full per (epilogue set, buffer) / empty per (set, buffer, issuer), labels full/empty.
-// Every barrier has one kind of waiter that sees consecutive phases: a parity wait asked before the previous
-// phase or after the next one has completed would succeed spuriously / never return.  DESIGN.md has the rest.
+// CTA = 2 warpgroups (1 CTA per SM).  Each warpgroup owns alternate 64-row tiles of the CTA and runs, per tile:
+//   cp.async of the NEXT tile into its second stage (fp32 rows, zero-filled beyond n and d);
+//   the fp16 (hi, lo) A fragments of s X built in registers (and ||s x||^2);
+//   3 ceil(d/16) wgmma.m64nNk16 with B (= -2 s C as fp16 hi / lo, SWIZZLE_128B K-major) resident in shared memory;
+//   the arg-min epilogue from the register accumulators (best, second best, near-tie test);
+//   the winning distance in direct form (x - c)^2 in fp32, and the M-step.
+// The M-step adds the tile's rows in row order into the CTA's sums; the two warpgroups take turns (named barriers),
+// so every cluster's sum is formed in one fixed order and the sums are bit-reproducible.  One warpgroup's MMAs
+// overlap the other's epilogue / M-step.
 #include "bkm_common.cuh"
-#include <cuda.h>
+#include "bkm_wgmma.cuh"
 #include <cuda_fp16.h>
 #include <math_constants.h>
 
 namespace bkm {
 
-static const int BM = 128;           // rows per tile
-// Roles are assigned per aligned group of 4 warps (setmaxnreg moves registers between whole warpgroups):
-// warps 0-3: TMA producer (0), MMA issuer (1), 2 spare; 4-7 converter; 8-11 / 12-15 epilogue sets; 16+ M-step
-static const int MW0 = 16;
-static const int NMW = 16;               // sums AND distances in one pass: 16 distance + M-step warps (warp owns the clusters c % 16)
-static const int NMW_LANE = 8;           // every other variant: 8 warps, LANE j of warp w owns cluster 32 w + j (its sums or its centre)
-static const int LIST_BYTES = 256 * 4 + BM * 4;   // per label buffer: head[256] + next[128] (row lists per cluster)
-__host__ __device__ constexpr int tc_mwarps(bool mstep, bool want_dist) { return (mstep && want_dist) ? NMW : NMW_LANE; }
-// register cap: registers are allocated per warp in units of 512 (16 per thread)
-// (each of the 4 SM sub-partitions holds 16384 registers and ceil(warps / 4) of the CTA's warps)
-__host__ __device__ constexpr int tc_maxreg(bool mstep, bool want_dist) { return 16384 / ((MW0 + tc_mwarps(mstep, want_dist) + 3) / 4) / 512 * 16; }
-__host__ __device__ constexpr int tc_threads(bool mstep, bool want_dist) { return (MW0 + tc_mwarps(mstep, want_dist)) * 32; }
-static const int KBLK_BYTES = BM * 128;   // one K-block (32 fp32 columns) of a 128-row tile
-static const int MH = 32;                 // rows per M-ring stage (a quarter tile)
-static const int MKBLK_BYTES = MH * 128;
+static const int TBM = 64;           // rows per warpgroup tile (wgmma M)
+static const int XP = 72;            // fp32 row pitch of a staged X tile (16-byte multiple; rows 8 banks apart)
+static const int TC_THREADS = 256;   // two warpgroups
 
 struct TcCfg {
-  int KB;        // 32-float K-blocks per row of the fp32 X tiles (1 or 2)
   int KS;        // MMA K-steps of 16 (ceil(d/16))
   int NP;        // padded centre count (multiple of 16, <= 256)
-  int NU0, NU1;  // columns of unit 0 / unit 1 (NU1 == 0 -> one unit per tile)
-  int U;
-  int NST;       // X stages
-  int direct;    // 1: the (warp-owns-clusters) M-step warps read the A ring
-  int mring;     // 1: separate M ring (quarter-tile or whole-tile slots)
-  int SSH;       // lane-owns flavour: every cluster has 2^SSH row lists (rows r with the same r mod 2^SSH), one lane each,
-                 // so that k < 256 still uses all 256 lanes: 2^SSH = 256 / next_pow2(k)
-  int MR;        // rows per M-ring slot (32: quarter tiles, 128: whole tiles)
-  uint32_t off_bhi, off_blo, off_bcn, off_ones, off_c32, off_x, off_m, off_lab, off_xn, off_red, off_bar, off_tptr, total;
+  uint32_t off_bhi, off_blo, off_x, off_sum, off_cn, off_cnt, off_lab, off_dp, off_red, total;
 };
 
-static const int NBUF = 3;               // 128-column TMEM accumulator buffers (3*128 acc + 2*(32 Xhi + 32 Xlo) = 512)
-static const int NSTMAX = 6;             // A ring stages (barrier slots)
-static const int NLAB = 4;               // label buffers between the epilogue sets and the M-step warps
-static const uint32_t TM_XHI = 384, TM_XLO = 448;   // TMEM columns of the fp16 X operands (+ (tile & 1) * 32)
-
-enum {
-  BAR_B_FULL = 0,
-  BAR_X_FULL = 1,                          // [NSTMAX]
-  BAR_X_EMPTY = BAR_X_FULL + NSTMAX,       // [NSTMAX]
-  BAR_ACC_FULL = BAR_X_EMPTY + NSTMAX,     // [set 2][buf 3]  one barrier per (epilogue warp set, accumulator buffer): every
-  BAR_ACC_EMPTY = BAR_ACC_FULL + 6,        // [set 2][buf 3][issuer 2]  waiter then observes consecutive phases (a parity wait
-                                           //   that is asked before the PREVIOUS phase has completed succeeds spuriously)
-  BAR_XOP_FULL = BAR_ACC_EMPTY + 12,       // [8]   X operands (and ||x||^2) of tile it are ready; indexed it & 7: the converter can
-                                           //       run up to 6 tiles ahead of a late epilogue set (one-unit tiles), and a wait that
-                                           //       is asked after the NEXT phase has completed as well would never return
-  BAR_XOP_EMPTY = BAR_XOP_FULL + 8,        // [2]   ... and the MMAs that read them have completed
-  BAR_LAB_FULL = BAR_XOP_EMPTY + 2,        // [NLAB]
-  BAR_LAB_EMPTY = BAR_LAB_FULL + NLAB,     // [NLAB]
-  BAR_M_FULL = BAR_LAB_EMPTY + NLAB,       // [2]  M ring (ring mode): 32-row quarter tiles re-fetched (L2 hits)
-  BAR_M_EMPTY = BAR_M_FULL + 2,            // [2]
-  BAR_COUNT = BAR_M_EMPTY + 2
-};
-
-// ------------------------------------------------------------------------------------ PTX
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-// Accumulator unit g (g = tile*U + u) uses TMEM buffer g % NBUF and is consumed by epilogue set (g/U) & 1.
-// Parity of the phase of barrier [set][buf] that belongs to unit g = number of earlier units with the same
-// (set, buffer), mod 2.  The pattern repeats every lcm(2U, 3) units: U=1 -> each pair once per 6 units,
-// U=2 -> twice per 12 units (second occurrences: g % 12 in {4,6,8,9,10,11}).
-__device__ __forceinline__ uint32_t acc_parity(long long g, int U) {
-  if (NBUF == 2) return (uint32_t)((U == 1 ? (g >> 1) : (g >> 2)) & 1);     // each (set, buffer) pair: every 2U-th unit
-  if (U == 1) return (uint32_t)((g / 6) & 1);
-  return (uint32_t)((0xF50u >> (int)(g % 12)) & 1u);
-}
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
-}
-__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-// A pipeline bug must fail, not hang the GPU: a wait that times out records (barrier offset, parity,
-// warp) in g_tc_abort and returns; every later wait returns at once, the kernel drains with garbage and
-// the host reports the code (bkm_debug_abort_code).
+// The deferred-row re-check reports a failed fused kernel through this word (see tc_recheck_kernel); the wgmma kernel
+// has no waits that can time out, so it stays 0 unless a debugging build sets it.
 __device__ unsigned int g_tc_abort = 0;
-#ifndef BKM_TC_PSLEEP
-#define BKM_TC_PSLEEP 0
-#endif
-#ifndef BKM_EXP_1P
-#define BKM_EXP_1P 0
-#endif
-#ifndef BKM_TRACE
-#define BKM_TRACE 0
-#endif
-// Pipeline timeline of CTA 0 (debug builds, `make TRACE=1`): SM clock of event `slot` for its first 128 tiles.
-#if BKM_TRACE
-__device__ long long g_tc_trace[16 * 128];
-#define TRACE(slot, it) do { if (blockIdx.x == 0 && (it) < 128) g_tc_trace[(slot) * 128 + (int)(it)] = clock64(); } while (0)
-#else
-#define TRACE(slot, it) do { } while (0)
-#endif
-__device__ unsigned int g_tc_dbg[64];     // per-warp abort code of the first CTA that aborts (debug)
-__device__ __forceinline__ unsigned long long tc_now_ns() {
-  unsigned long long t;
-  asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t));
-  return t;
-}
-// Wait limits are WALL-CLOCK (2 s): spin counts shrink under ncu replay, compute-sanitizer or time-slicing.
-static const unsigned long long TC_WAIT_LIMIT_NS = 2000000000ull;
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-  uint32_t done = 0;
-  unsigned long long t0 = 0;
-  for (uint32_t spin = 0; !done; ++spin) {
-    asm volatile(
-        "{\n.reg .pred p;\n"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2, %3;\n"   // suspend-time hint: the hardware
-        "selp.u32 %0, 1, 0, p;\n}"                                        // parks the warp instead of polling
-        : "=r"(done) : "r"(bar), "r"(parity), "r"(2000u) : "memory");
-    if (!done && (spin & 15) == 15) {
-      const unsigned long long now = tc_now_ns();
-      if (t0 == 0) t0 = now;
-      if (now - t0 > TC_WAIT_LIMIT_NS || *(volatile unsigned int*)&g_tc_abort) {
-        atomicCAS(&g_tc_abort, 0u, 0x80000000u | ((bar & 0xfff) << 12) | (parity << 8) | (threadIdx.x >> 5));
-        if ((threadIdx.x & 31) == 0) g_tc_dbg[threadIdx.x >> 5] = 0x80000000u | ((bar & 0xfff) << 12) | (parity << 8) | blockIdx.x;
-        return;
-      }
-    }
-  }
-}
-__device__ __forceinline__ bool mbar_test(uint32_t bar, uint32_t parity) {
-  uint32_t done;
-  asm volatile(
-      "{\n.reg .pred p;\n"
-      "mbarrier.test_wait.parity.shared::cta.b64 p, [%1], %2;\n"
-      "selp.u32 %0, 1, 0, p;\n}"
-      : "=r"(done) : "r"(bar), "r"(parity) : "memory");
-  return done != 0;
-}
-// Long waits (a whole pipeline stage away): poll with back-off so that the poller does not steal
-// issue slots from the warps doing the work on the same SM sub-partition.
-__device__ __forceinline__ void mbar_wait_sleep(uint32_t bar, uint32_t parity) {
-  uint32_t done = 0;
-  unsigned long long t0 = 0;
-  for (uint32_t spin = 0; !done; ++spin) {
-    asm volatile(
-        "{\n.reg .pred p;\n"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n"
-        "selp.u32 %0, 1, 0, p;\n}"
-        : "=r"(done) : "r"(bar), "r"(parity) : "memory");
-    if (!done) __nanosleep(256);
-    if (!done && (spin & 15) == 15) {
-      const unsigned long long now = tc_now_ns();
-      if (t0 == 0) t0 = now;
-      if (now - t0 > TC_WAIT_LIMIT_NS || *(volatile unsigned int*)&g_tc_abort) {
-        atomicCAS(&g_tc_abort, 0u, 0x80000000u | ((bar & 0xfff) << 12) | (parity << 8) | (threadIdx.x >> 5));
-        return;
-      }
-    }
-  }
-}
-__device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
-  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
-}
-__device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* tm, uint32_t bar, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(dst), "l"(tm), "r"(bar), "r"(c0), "r"(c1) : "memory");
-}
-__device__ __forceinline__ void tma_prefetch_2d(const CUtensorMap* tm, int c0, int c1) {
-  asm volatile("cp.async.bulk.prefetch.tensor.2d.L2.global.tile [%0, {%1, %2}];" ::"l"(tm), "r"(c0), "r"(c1) : "memory");
-}
-__device__ __forceinline__ float fmin3(float a, float b, float c) {
-  float d;
-  asm("min.f32 %0, %1, %2, %3;" : "=f"(d) : "f"(a), "f"(b), "f"(c));     // FMNMX3 on sm_100
-  return d;
-}
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred;
-  asm volatile("{\n.reg .pred P;\nelect.sync _|P, 0xffffffff;\nselp.u32 %0, 1, 0, P;\n}" : "=r"(pred));
-  return pred != 0;
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void mma_tf32_ss(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t acc) {
-  asm volatile(
-      "{\n.reg .pred p;\nsetp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n}"
-      ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(acc) : "memory");
-}
-// A (128 rows x 16 fp16 = 8 TMEM columns, two K elements per 32-bit column) from TMEM, B from shared memory
-__device__ __forceinline__ void mma_f16_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t bdesc, uint32_t idesc, uint32_t acc) {
-  asm volatile(
-      "{\n.reg .pred p;\nsetp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n}"
-      ::"r"(d_tmem), "r"(a_tmem), "l"(bdesc), "r"(idesc), "r"(acc) : "memory");
-}
-#define TC_LD16(taddr, r)                                                                              \
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 "                                               \
-               "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"                       \
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),   \
-                 "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]),            \
-                 "=r"(r[13]), "=r"(r[14]), "=r"(r[15])                                                 \
-               : "r"(taddr) : "memory")
-// 16 columns from r[o], r[o+2], ..., r[o+30]
-#define TC_ST16S(taddr, r, o)                                                                          \
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "                                         \
-               "{%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16};"                             \
-               ::"r"(taddr), "r"(r[o + 0]), "r"(r[o + 2]), "r"(r[o + 4]), "r"(r[o + 6]), "r"(r[o + 8]), \
-                 "r"(r[o + 10]), "r"(r[o + 12]), "r"(r[o + 14]), "r"(r[o + 16]), "r"(r[o + 18]),       \
-                 "r"(r[o + 20]), "r"(r[o + 22]), "r"(r[o + 24]), "r"(r[o + 26]), "r"(r[o + 28]),       \
-                 "r"(r[o + 30]) : "memory")
+__device__ unsigned int g_tc_dbg[64];
 
-// K-major, SWIZZLE_128B shared-memory matrix descriptor (sm_100 format, version 1):
-// 8-row x 128-byte swizzle atoms, SBO = 1024 B between atoms along M/N, LBO unused (1).
-__device__ __forceinline__ uint64_t make_desc(uint32_t saddr) {
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr >> 4) & 0x3FFF);
-  d |= (uint64_t)1 << 16;                 // leading byte offset (>>4), ignored for swizzled K-major
-  d |= (uint64_t)(1024 >> 4) << 32;       // stride byte offset (>>4)
-  d |= (uint64_t)1 << 46;                 // descriptor version (Blackwell)
-  d |= (uint64_t)2 << 61;                 // SWIZZLE_128B
-  return d;
+__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
+__device__ __forceinline__ void bar_sync(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
+__device__ __forceinline__ void bar_arrive(int id, int n) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(n) : "memory"); }
+__device__ __forceinline__ uint32_t pack_half2(float lo, float hi) {
+  const __half2 h = __floats2half2_rn(lo, hi);          // low half = lower column
+  return *reinterpret_cast<const uint32_t*>(&h);
 }
-// instruction descriptors: fp32 accumulate, A and B K-major, M = 128, N = n; operand format 2 = tf32, 0 = fp16
-__device__ __forceinline__ uint32_t make_idesc_tf32(int n) {
-  return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
-}
-__device__ __forceinline__ uint32_t make_idesc_f16(int n) {
-  return (1u << 4) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
-}
-// byte offset of 16-byte chunk q (0..7) of row r inside one swizzled K-block
-__device__ __forceinline__ uint32_t sw_chunk(int r, int q) { return (uint32_t)(r * 128 + ((q ^ (r & 7)) << 4)); }
-
-#define ACC32_CASE(j) case j: acc[j][0] += x0; acc[j][1] += x1; break;
 
 // XFORM: the epilogue writes the whole (rows x k) block of distances / kernel values instead of the arg-min
-// (euclidean_distances, dask_ml/metrics/pairwise.py:69-97; rbf_kernel :131-139) — same pipeline, no M-step warps' work.
-template <bool MSTEP, bool WANT_DIST, bool XFORM = false>
-__global__ void __launch_bounds__(tc_threads(MSTEP, WANT_DIST), 1)
-tc_chunk_kernel(ChunkArgs a, TcCfg cfg, const __grid_constant__ CUtensorMap tm_x,
-                const __grid_constant__ CUtensorMap tm_bhi, const __grid_constant__ CUtensorMap tm_blo,
-                const __grid_constant__ CUtensorMap tm_xm) {
+// (euclidean_distances, dask_ml/metrics/pairwise.py:69-97; rbf_kernel :131-139) — same MMAs, no M-step.
+template <int N, bool MSTEP, bool WANT_DIST, bool XFORM>
+__global__ void __launch_bounds__(TC_THREADS, 1)
+tc_chunk_kernel(ChunkArgs a, TcCfg cfg) {
   if (a.skip && *a.skip) return;                            // converged loop: no-op iteration
 
   extern __shared__ __align__(1024) unsigned char smem[];
-  constexpr bool LANE_OWNS = !(MSTEP && WANT_DIST);   // M-step flavour (see the two M-step blocks below)
-  constexpr bool HAS_M = MSTEP || WANT_DIST;          // labels-only assignment has no M-step / distance stage at all
-  constexpr int NMWK = tc_mwarps(MSTEP, WANT_DIST);
-  constexpr int NTHREADS = tc_threads(MSTEP, WANT_DIST);
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  constexpr bool HAS_M = MSTEP || WANT_DIST;
+  const int tid = threadIdx.x, lane = tid & 31, wgi = tid >> 7, t = tid & 127, wq = t >> 5;
   const uint32_t sbase = smem_u32(smem);
-  if (tid == 0 && (sbase & 1023)) __trap();
-  const uint32_t s_bhi = sbase + cfg.off_bhi, s_blo = sbase + cfg.off_blo, s_x = sbase + cfg.off_x;
-  int* lab_s = reinterpret_cast<int*>(smem + cfg.off_lab);          // [NLAB][BM]
-  double* red_s = reinterpret_cast<double*>(smem + cfg.off_red);    // [NMW + 1]
-  const uint32_t bars = sbase + cfg.off_bar;
-  uint32_t* tptr_s = reinterpret_cast<uint32_t*>(smem + cfg.off_tptr);
-#define BAR(i) (bars + 8u * (uint32_t)(i))
+  if (tid == 0 && (sbase & 1023)) __trap();                 // the swizzle pattern assumes 1024-byte aligned tiles
+  const int KS = cfg.KS, d = a.d, k = a.k;
+  float* cn_s = reinterpret_cast<float*>(smem + cfg.off_cn);          // [N] s^2 ||c||^2 (padded columns: 3e38)
+  int* cnt_s = reinterpret_cast<int*>(smem + cfg.off_cnt);            // [N]
+  float* sum_s = reinterpret_cast<float*>(smem + cfg.off_sum);        // [N][64]
+  int* lab_s = reinterpret_cast<int*>(smem + cfg.off_lab) + wgi * TBM;        // label of each row of the tile, -1: none
+  float* dp_s = reinterpret_cast<float*>(smem + cfg.off_dp) + wgi * 2 * TBM;  // [2][TBM] halves of the direct distances
+  double* red_s = reinterpret_cast<double*>(smem + cfg.off_red);
+  const PackHeader* hdr = reinterpret_cast<const PackHeader*>(a.pack);
+  const float sc = hdr->scale;
 
-  const int NST = cfg.NST, KB = cfg.KB, KS = cfg.KS, NP = cfg.NP, U = cfg.U;
-  const bool direct = cfg.direct != 0;
-  const uint32_t stage_bytes = (uint32_t)KB * KBLK_BYTES;
-  const long long ntiles = (a.n + BM - 1) / BM;
-  const long long my_tiles = blockIdx.x < ntiles ? (ntiles - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;
-
-  // ---------------- setup ----------------
-  if (warp == 0 && lane == 0) {
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tm_x));
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tm_bhi));
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tm_blo));
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tm_xm));
-    mbar_init(BAR(BAR_B_FULL), 1);
-    for (int s = 0; s < NSTMAX; ++s) {
-      mbar_init(BAR(BAR_X_FULL + s), 1);
-      // a stage is released by the 128 converter threads of a set and, in direct mode, the M-step warps
-      mbar_init(BAR(BAR_X_EMPTY + s), direct ? 128 + NMWK : 128);
-    }
-    for (int b = 0; b < 2 * NBUF; ++b) {
-      mbar_init(BAR(BAR_ACC_FULL + b), 1);
-      mbar_init(BAR(BAR_ACC_EMPTY + 2 * b), 128);
-      mbar_init(BAR(BAR_ACC_EMPTY + 2 * b + 1), 128);
-    }
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(BAR(BAR_M_FULL + b), 1);
-      mbar_init(BAR(BAR_M_EMPTY + b), NMWK);
-      for (int q = 0; q < 4; ++q) mbar_init(BAR(BAR_XOP_FULL + 4 * b + q), 128);
-      mbar_init(BAR(BAR_XOP_EMPTY + b), (uint32_t)U);
-    }
-    for (int b = 0; b < NLAB; ++b) {
-      mbar_init(BAR(BAR_LAB_FULL + b), 128);
-      mbar_init(BAR(BAR_LAB_EMPTY + b), NMWK);
-    }
-    red_s[NMWK] = 0.0;
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tptr_s)), "r"(512));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
+  // ---------------- setup: B tiles, column offsets, sums ----------------
   {
-    // s^2 ||c||^2 enters the accumulator through one extra tf32 MMA K-step: B rows [hi,mid,lo,0,...] (exact
-    // 3-way tf32 split, built by pack_norms_kernel) against a constant A tile of rows [1,1,1,0,...]; both
-    // tiles use the canonical no-swizzle K-major layout (8-row groups of 256 B).  Plain stores + proxy fence.
-    const float4* g = reinterpret_cast<const float4*>(a.pack + a.L.off_bcn);
-    float4* sdst = reinterpret_cast<float4*>(smem + cfg.off_bcn);
-    for (int i = tid; i < NP * 2; i += NTHREADS) sdst[i] = g[i];
-    float4* odst = reinterpret_cast<float4*>(smem + cfg.off_ones);
-    for (int i = tid; i < BM * 2; i += NTHREADS)
-      odst[i] = ((i >> 3) & 1) ? make_float4(0.f, 0.f, 0.f, 0.f) : make_float4(1.f, 1.f, 1.f, 0.f);
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    if (LANE_OWNS && HAS_M) {
-      // row lists: every head starts empty
-      int* hd = reinterpret_cast<int*>(smem + cfg.off_lab);
-      for (int i = tid; i < NLAB * (LIST_BYTES / 4); i += NTHREADS) hd[i] = -1;
+    // pack rows are 64 halves = 8 chunks of 16 bytes: chunk q of row r goes to its SWIZZLE_128B position
+    const uint4* ghi = reinterpret_cast<const uint4*>(a.pack + a.L.off_bhi);
+    const uint4* glo = reinterpret_cast<const uint4*>(a.pack + a.L.off_blo);
+    for (int i = tid; i < N * 8; i += TC_THREADS) {
+      const int r = i >> 3, q = i & 7;
+      uint4 h = make_uint4(0u, 0u, 0u, 0u), l = h;
+      if (r < a.L.kp) { h = ghi[i]; l = glo[i]; }
+      *reinterpret_cast<uint4*>(smem + cfg.off_bhi + wg::sw128_chunk(r, q)) = h;
+      *reinterpret_cast<uint4*>(smem + cfg.off_blo + wg::sw128_chunk(r, q)) = l;
     }
-    if (WANT_DIST && !LANE_OWNS) {
-      // fp32 centres [NP][KB*32] for the exact direct-form winning distance (rows >= k / columns >= d: zero)
-      const float* gc = reinterpret_cast<const float*>(a.pack + a.L.off_cT);      // [k][d4]
-      float* cdst = reinterpret_cast<float*>(smem + cfg.off_c32);
-      const int pitch = KB * 32;
-      for (int i = tid; i < NP * pitch; i += NTHREADS) {
-        const int j = i / pitch, c = i - j * pitch;
-        cdst[i] = (j < a.k && c < a.d) ? gc[(size_t)j * a.L.d4 + c] : 0.f;
-      }
+    // s^2 ||c_j||^2 from the pack's exact 3-way split [hi, mid, lo] (hi + mid + lo == the fp32 value)
+    const float* bcn = reinterpret_cast<const float*>(a.pack + a.L.off_bcn);
+    for (int j = tid; j < N; j += TC_THREADS) {
+      float v = 3.0e38f;
+      if (j < a.L.kp) { const float* p = bcn + (j >> 3) * 64 + (j & 7) * 4; v = (p[0] + p[1]) + p[2]; }
+      cn_s[j] = v;
+      cnt_s[j] = 0;
     }
+    if (MSTEP)
+      for (int i = tid; i < N * 64; i += TC_THREADS) sum_s[i] = 0.f;
+    wg::fence_proxy_async();                                 // generic-proxy stores -> visible to wgmma
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tptr_s;
 
-  // Register re-allocation between warpgroups (pure Lloyd variant, launched with 80 registers per thread): the
-  // producer / MMA group and the converter give registers up, the M-step warps (64 running sums per lane plus
-  // several 16-byte loads in flight) take them.  Per SM sub-partition: 40+72+80+80+104+104 = 6*80.  The
-  // instruction sits at the top of every role's branch so that the compiler sees one budget per branch.
-#define REG_DEC(n) do { if (LANE_OWNS) asm volatile("setmaxnreg.dec.sync.aligned.u32 " #n ";"); } while (0)
-#define REG_INC(n) do { if (LANE_OWNS) asm volatile("setmaxnreg.inc.sync.aligned.u32 " #n ";"); } while (0)
+  const long long ntiles = (a.n + TBM - 1) / TBM;
+  const long long my_tiles = blockIdx.x < ntiles ? (ntiles - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;
+  const long long npairs = (my_tiles + 1) / 2;               // warpgroup w takes the CTA's tiles 2p + w
+  const float* X = reinterpret_cast<const float*>(a.X);
+  const uint32_t stage_bytes = TBM * XP * 4;
+  const uint32_t xs_u32 = sbase + cfg.off_x + (uint32_t)wgi * 2u * stage_bytes;
+  const float* xs_f = reinterpret_cast<const float*>(smem + cfg.off_x) + wgi * 2 * TBM * XP;
+  const int nq = KS * 4;                                     // 16-byte chunks per staged row
+  auto load_tile = [&](long long p, int stage) {
+    const long long lt = 2 * p + wgi;
+    if (lt < my_tiles) {
+      const long long row0 = (blockIdx.x + lt * gridDim.x) * TBM;
+      for (int i = t; i < TBM * nq; i += 128) {
+        const int r = i / nq, col = (i - r * nq) * 4;
+        const long long row = row0 + r;
+        const int bytes = (row < a.n && col < d) ? min(16, (d - col) * 4) : 0;
+        wg::cp16(xs_u32 + (uint32_t)stage * stage_bytes + (uint32_t)(r * XP + col) * 4u, bytes ? X + row * a.ldx + col : X, bytes);
+      }
+    }
+    wg::cp_commit();
+  };
 
-  if (warp == 0 || warp == 3) {
-    REG_DEC(40);
-    // =========================== TMA producer (warp 0; warp 3 is spare) ===========================
-    // One thread feeds both rings from a polling loop (neither ring may block the other).  A ring: 128-row X
-    // tiles, with an L2 prefetch PF tiles ahead.  M ring (ring mode only): every tile is re-fetched as four
-    // 32-row quarters for the M-step / distance warps; the same rows were loaded for the converter a few
-    // microseconds earlier, so these are L2 hits and HBM traffic stays at one read of X per iteration.
-    if (warp == 0 && lane == 0) {
-      mbar_expect_tx(BAR(BAR_B_FULL), 2u * (uint32_t)NP * 128u);
-      tma_load_2d(s_bhi, &tm_bhi, BAR(BAR_B_FULL), 0, 0);
-      tma_load_2d(s_blo, &tm_blo, BAR(BAR_B_FULL), 0, 0);
-      const int PF = 6;        // L2 prefetch distance (tiles) ahead of the shared-memory ring
-      for (long long it = 0; it < PF && it < my_tiles; ++it)
-        for (int kb = 0; kb < KB; ++kb) tma_prefetch_2d(&tm_x, kb * 32, (int)((blockIdx.x + it * gridDim.x) * BM));
-      const uint32_t s_m = sbase + cfg.off_m;
-      const int MR = cfg.MR;                              // rows per M-ring slot: 32 (quarter tiles) or 128
-      const int qpt = BM / MR;                            // slots per tile
-      const uint32_t mkblk = (uint32_t)MR * 128u;
-      const uint32_t mbytes = (uint32_t)KB * mkblk;
-      const long long m_total = cfg.mring ? qpt * my_tiles : 0;
-      // Ring positions are carried as counters (stage / slot, phase bit, tile, quarter): the poll below runs every
-      // ~100 cycles.  With `ait % NST`, `ait / NST`, `mi / qpt` (64-bit divisions by run-time values, a few hundred
-      // cycles each in software) one poll took ~2000 cycles, and that reaction time sat in BOTH ring periods:
-      // (reaction + TMA latency + consumer) / 2 slots.
-      long long ait = 0, mi = 0;
-      int a_stage = 0;                      // ait % NST
-      uint32_t a_par = 1;                   // ((ait / NST) & 1) ^ 1
-      long long a_tile = blockIdx.x;        // blockIdx.x + ait * gridDim.x
-      int m_slot = 0;                       // mi & 1
-      uint32_t m_par = 1;                   // ((mi >> 1) & 1) ^ 1
-      long long m_tile_i = 0;               // mi / qpt
-      int m_q = 0;                          // mi % qpt
-      long long m_tile = blockIdx.x;        // blockIdx.x + m_tile_i * gridDim.x
-      uint32_t idle = 0;
-      unsigned long long idle_t0 = 0;
+  const int g = lane >> 2, c2 = (lane & 3) * 2;
+  const int rA = wq * 16 + g;                                // this thread's accumulator rows: rA, rA + 8
+  const uint64_t dbh = wg::desc_sw128(sbase + cfg.off_bhi), dbl = wg::desc_sw128(sbase + cfg.off_blo);
+  const float cnmax = (float)(hdr->cn_max * (double)sc * (double)sc);
+  double dsum = 0.0;
+
+  load_tile(0, 0);
 #pragma unroll 1
-      while (ait < my_tiles || mi < m_total) {
-        bool progressed = false;
-        if (ait < my_tiles) {
-          if (mbar_test(BAR(BAR_X_EMPTY + a_stage), a_par)) {
-            TRACE(0, ait);
-            if (ait + PF < my_tiles)
-              for (int kb = 0; kb < KB; ++kb) tma_prefetch_2d(&tm_x, kb * 32, (int)((a_tile + (long long)PF * gridDim.x) * BM));
-            mbar_expect_tx(BAR(BAR_X_FULL + a_stage), stage_bytes);
-            for (int kb = 0; kb < KB; ++kb)
-              tma_load_2d(s_x + a_stage * stage_bytes + (uint32_t)kb * KBLK_BYTES, &tm_x, BAR(BAR_X_FULL + a_stage),
-                          kb * 32, (int)(a_tile * BM));
-            ++ait;
-            a_tile += gridDim.x;
-            if (++a_stage == NST) { a_stage = 0; a_par ^= 1u; }
-            progressed = true;
-          }
-        }
-        if (mi < m_total && m_tile_i < ait) {
-          if (mbar_test(BAR(BAR_M_EMPTY + m_slot), m_par)) {
-            mbar_expect_tx(BAR(BAR_M_FULL + m_slot), mbytes);
-            for (int kb = 0; kb < KB; ++kb)
-              tma_load_2d(s_m + m_slot * mbytes + (uint32_t)kb * mkblk, &tm_xm, BAR(BAR_M_FULL + m_slot), kb * 32,
-                          (int)(m_tile * BM + m_q * MR));
-            ++mi;
-            if (++m_q == qpt) { m_q = 0; ++m_tile_i; m_tile += gridDim.x; }
-            if ((m_slot ^= 1) == 0) m_par ^= 1u;
-            progressed = true;
-          }
-        }
-        if (progressed) { idle = 0; idle_t0 = 0; continue; }
-        if (BKM_TC_PSLEEP > 0) __nanosleep(BKM_TC_PSLEEP);
-        if ((++idle & 255) == 255) {
-          const unsigned long long now = tc_now_ns();
-          if (idle_t0 == 0) idle_t0 = now;
-          if (now - idle_t0 > TC_WAIT_LIMIT_NS || *(volatile unsigned int*)&g_tc_abort) {
-            atomicCAS(&g_tc_abort, 0u, 0x80000000u | (0xfffu << 12));
-            break;
+  for (long long p = 0; p < npairs; ++p) {
+    const int stage = (int)(p & 1);
+    load_tile(p + 1, stage ^ 1);
+    wg::cp_wait1();
+    wg::wg_sync(1 + wgi);                                    // tile p is in shared memory (every thread's copies)
+    const long long lt = 2 * p + wgi;
+    const bool has = lt < my_tiles;
+    const long long row0 = (blockIdx.x + lt * gridDim.x) * TBM;
+    const float* xs = xs_f + stage * TBM * XP;
+    if (has) {
+      // ---- s X -> fp16 (hi, lo) A fragments, ||s x||^2 of rows rA / rA + 8 ----
+      uint32_t ahi[4][4], alo[4][4];
+      float xn0 = 0.f, xn1 = 0.f;
+#pragma unroll
+      for (int s = 0; s < 4; ++s) {
+#pragma unroll
+        for (int h = 0; h < 4; ++h) {
+          ahi[s][h] = 0u; alo[s][h] = 0u;
+          if (s < KS) {
+            const float2 v = *reinterpret_cast<const float2*>(xs + (rA + (h & 1) * 8) * XP + s * 16 + c2 + (h >> 1) * 8);
+            const float e0 = v.x * sc, e1 = v.y * sc;
+            const __half2 hh = __floats2half2_rn(e0, e1);
+            const float2 hf = __half22float2(hh);
+            ahi[s][h] = *reinterpret_cast<const uint32_t*>(&hh);
+            alo[s][h] = pack_half2(e0 - hf.x, e1 - hf.y);      // the subtraction is exact
+            if (h & 1) xn1 = fmaf(e1, e1, fmaf(e0, e0, xn1));
+            else xn0 = fmaf(e1, e1, fmaf(e0, e0, xn0));
           }
         }
       }
-    }
-  } else if (warp == 1 || warp == 2) {
-    REG_DEC(40);
-    // =========================== MMA issuers ===========================
-    // Two dedicated warps take alternate accumulator units (unit g = tile * U + u goes to warp 1 + (g & 1)):
-    // the thread that issues tcgen05.mma stalls on its next instructions until the tensor core has accepted
-    // the queued MMAs, so a single issuer leaves the tensor pipe idle between units.  Each warp runs its loop
-    // converged (all addresses / descriptors are warp-uniform and live in uniform registers); only the
-    // tcgen05 instructions themselves are issued by one elected lane.
-    const bool leader = elect_one();      // one lane issues every tcgen05.mma / commit (same thread: ordered)
-    mbar_wait(BAR(BAR_B_FULL), 0);
-    tc_fence_after();
-    const uint64_t dflags = ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) | ((uint64_t)1 << 46) | ((uint64_t)2 << 61);
-    // no-swizzle K-major operands of the ||c||^2 K-step: LBO = 128 B (second 16-byte K chunk), SBO = 256 B
-    const uint64_t dns = ((uint64_t)(128 >> 4) << 16) | ((uint64_t)(256 >> 4) << 32) | ((uint64_t)1 << 46);
-    const uint64_t dcn = dns | (uint64_t)(((sbase + cfg.off_bcn) >> 4) & 0x3FFF);
-    const uint64_t dones = dns | (uint64_t)(((sbase + cfg.off_ones) >> 4) & 0x3FFF);
-    const long long g_total = my_tiles * U;
-    uint32_t empty_ph = 0;      // phase bit of each accumulator-empty barrier this issuer waits on
-#pragma unroll 1
-    for (long long g = warp - 1; g < g_total; g += 2) {
-      const long long it = U == 2 ? (g >> 1) : g;
-      const int u = U == 2 ? (int)(g & 1) : 0;
-      // Both X operands live in TMEM (fp16 pairs written by the converter): only the 4 KB B slice of each
-      // K-step is fetched from shared memory.
-      const uint32_t xhi_t = tmem + TM_XHI + (uint32_t)(it & 1) * 32u;
-      const uint32_t xlo_t = tmem + TM_XLO + (uint32_t)(it & 1) * 32u;
-      const int buf = (int)(g % NBUF);
-      if (g >= NBUF) {
-        // the buffer was last used by unit g-NBUF, drained by epilogue set ((g-NBUF)/U) & 1, which signals the
-        // barrier of (its set, the buffer, the issuer of the buffer's next unit = this warp)
-        const long long gp = g - NBUF;
-        const int eb = (int)((U == 2 ? (gp >> 1) : gp) & 1) * NBUF + buf;
-        mbar_wait(BAR(BAR_ACC_EMPTY + 2 * eb + (warp - 1)), (empty_ph >> eb) & 1u);
-        empty_ph ^= 1u << eb;
-      }
-      mbar_wait(BAR(BAR_XOP_FULL + (it & 7)), (uint32_t)((it >> 3) & 1));
-      tc_fence_after();
-      if (leader) TRACE(3 + 2 * u, it);
-      const int ncols = u == 0 ? cfg.NU0 : cfg.NU1;
-      const uint32_t rowoff = u == 0 ? 0u : (uint32_t)cfg.NU0 * 128u;
-      const uint32_t idesc = make_idesc_f16(ncols);
-      const uint32_t d_t = tmem + (uint32_t)buf * 128u;
-      const uint64_t dbh = dflags | (uint64_t)(((s_bhi + rowoff) >> 4) & 0x3FFF);
-      const uint64_t dbl = dflags | (uint64_t)(((s_blo + rowoff) >> 4) & 0x3FFF);
-      if (leader) {
-        // Xhi . Bhi   (K-step s: 16 halves = 32 bytes inside the 128-byte swizzle atom, 8 TMEM columns)
+      xn0 += __shfl_xor_sync(0xffffffffu, xn0, 1); xn0 += __shfl_xor_sync(0xffffffffu, xn0, 2);
+      xn1 += __shfl_xor_sync(0xffffffffu, xn1, 1); xn1 += __shfl_xor_sync(0xffffffffu, xn1, 2);
+
+      // ---- acc = Xhi.Bhi + Xhi.Blo + Xlo.Bhi ----
+      float acc[N / 2];
 #pragma unroll
-        for (int s = 0; s < 4; ++s)
-          if (s < KS) mma_f16_ts(d_t, xhi_t + (uint32_t)s * 8u, dbh + (uint64_t)(s * 2), idesc, s > 0 ? 1u : 0u);
-#if !BKM_EXP_1P      // (measurement knob BKM_EXP_1P=1: hi x hi product only — how fast would a one-product first pass be?)
-        // Xhi . Blo
+      for (int i = 0; i < N / 2; ++i) acc[i] = 0.f;
+      wg::fence();
 #pragma unroll
-        for (int s = 0; s < 4; ++s)
-          if (s < KS) mma_f16_ts(d_t, xhi_t + (uint32_t)s * 8u, dbl + (uint64_t)(s * 2), idesc, 1u);
-        // Xlo . Bhi
+      for (int s = 0; s < 4; ++s)
+        if (s < KS) wg::Mma<N>::rs_f16(acc, ahi[s], dbh + (uint64_t)(2 * s), s > 0);
 #pragma unroll
-        for (int s = 0; s < 4; ++s)
-          if (s < KS) mma_f16_ts(d_t, xlo_t + (uint32_t)s * 8u, dbh + (uint64_t)(s * 2), idesc, 1u);
-#endif
-        mma_tf32_ss(d_t, dones, dcn + (uint64_t)(rowoff >> 6), make_idesc_tf32(ncols), 1u);     // + s^2 ||c_j||^2
-        tc_commit(BAR(BAR_ACC_FULL + (int)(it & 1) * NBUF + buf));
-        tc_commit(BAR(BAR_XOP_EMPTY + (it & 1)));      // one arrival per unit: the tile's X operands are free after U of them
-        TRACE(4 + 2 * u, it);
-      }
-      __syncwarp();
-    }
-  } else if (warp >= 4 && warp < 8) {
-    REG_DEC(72);
-    // =========================== X converter ===========================
-    // Thread == row == TMEM lane (warp & 3 selects the lane quarter).  Runs ahead of the MMA: tile it + 2 is
-    // converted as soon as the MMAs of tile it have released the TMEM operand slot.
-    const int q4 = warp & 3;
-    const int r = q4 * 32 + lane;
-    const uint32_t lane_addr = (uint32_t)(q4 * 32) << 16;
-    const float sc = reinterpret_cast<const PackHeader*>(a.pack)->scale;
-    float* xn_s = reinterpret_cast<float*>(smem + cfg.off_xn);       // [8][BM]
-    uint32_t xoff[8];                              // swizzled 16-byte chunk offsets of this thread's row
+      for (int s = 0; s < 4; ++s)
+        if (s < KS) wg::Mma<N>::rs_f16(acc, ahi[s], dbl + (uint64_t)(2 * s), 1);
 #pragma unroll
-    for (int q = 0; q < 8; ++q) xoff[q] = sw_chunk(r, q);
-#pragma unroll 1
-    for (long long it = 0; it < my_tiles; ++it) {
-      // (32-bit arithmetic: a 64-bit division by a run-time value costs a few hundred cycles)
-      const int stage = (int)((unsigned)it % (unsigned)NST);
-      // ---- s X -> fp16 (hi, lo) pairs in TMEM, and ||s x||^2 ----
-      mbar_wait(BAR(BAR_X_FULL + stage), (uint32_t)(((unsigned)it / (unsigned)NST) & 1u));
-      mbar_wait(BAR(BAR_XOP_EMPTY + (it & 1)), (uint32_t)(((it >> 1) & 1) ^ 1));
-      tc_fence_after();
-      if (r == 0) TRACE(1, it);
-      const unsigned char* xs = smem + cfg.off_x + stage * stage_bytes;
-      float xn4[4] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll 1
-      for (int kb = 0; kb < KB; ++kb) {
-        uint32_t v[32];
-#pragma unroll
-        for (int q = 0; q < 8; ++q) {
-          const float4 t = *reinterpret_cast<const float4*>(xs + kb * KBLK_BYTES + xoff[q]);
-          v[q * 4 + 0] = __float_as_uint(t.x); v[q * 4 + 1] = __float_as_uint(t.y);
-          v[q * 4 + 2] = __float_as_uint(t.z); v[q * 4 + 3] = __float_as_uint(t.w);
-        }
-#pragma unroll
-        for (int j = 0; j < 16; ++j) {
-          const float e0 = __uint_as_float(v[2 * j]) * sc, e1 = __uint_as_float(v[2 * j + 1]) * sc;
-          xn4[j & 3] = fmaf(e0, e0, xn4[j & 3]);
-          xn4[(j + 2) & 3] = fmaf(e1, e1, xn4[(j + 2) & 3]);
-          const __half2 h = __floats2half2_rn(e0, e1);          // low half = K element 2j
-          const float2 hf = __half22float2(h);
-          const __half2 l = __floats2half2_rn(e0 - hf.x, e1 - hf.y);      // the subtraction is exact
-          v[2 * j] = *reinterpret_cast<const uint32_t*>(&h);
-          v[2 * j + 1] = *reinterpret_cast<const uint32_t*>(&l);
-        }
-        TC_ST16S(tmem + lane_addr + TM_XHI + (uint32_t)(it & 1) * 32u + (uint32_t)kb * 16u, v, 0);
-        TC_ST16S(tmem + lane_addr + TM_XLO + (uint32_t)(it & 1) * 32u + (uint32_t)kb * 16u, v, 1);
-      }
-      xn_s[(it & 7) * BM + r] = (xn4[0] + xn4[1]) + (xn4[2] + xn4[3]);
-      mbar_arrive(BAR(BAR_X_EMPTY + stage));        // the converter is done with the smem stage
-      asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-      tc_fence_before();
-      mbar_arrive(BAR(BAR_XOP_FULL + (it & 7)));      // release: also publishes xn_s
-      if (r == 0) TRACE(2, it);
-    }
-  } else if (warp >= 8 && warp < MW0) {
-    // =========================== epilogue ===========================
-    // Two warp sets (warps 8-11 and 12-15) take alternate tiles, so each SM sub-partition has two epilogue
-    // warps whose TMEM loads and instruction streams interleave.  Thread == row == TMEM lane.
-    const int set = (warp - 8) >> 2;
-    const int q4 = warp & 3;
-    const int r = q4 * 32 + lane;
-    const uint32_t lane_addr = (uint32_t)(q4 * 32) << 16;
-    const PackHeader* hdr = reinterpret_cast<const PackHeader*>(a.pack);
-    const float cnmax = (float)(hdr->cn_max * (double)hdr->scale * (double)hdr->scale);
-    const float* xn_s = reinterpret_cast<const float*>(smem + cfg.off_xn);
-    const float one = __uint_as_float(0x3f800000u + ((uint32_t)a.k >> 30));       // 1.0f, -0.0f: not known to the compiler
-    const float nzero = __uint_as_float(0x80000000u + ((uint32_t)a.k >> 30));
-#pragma unroll 1
-    for (long long it = set; it < my_tiles; it += 2) {
-      const long long tile = blockIdx.x + it * gridDim.x;
-      // the converter published ||s x||^2 before it released the operands (completed long ago: acquire only)
-      mbar_wait(BAR(BAR_XOP_FULL + (it & 7)), (uint32_t)((it >> 3) & 1));
-      const float xn = xn_s[(it & 7) * BM + r];
-      const float bound = a.tau * (xn + cnmax);
-      // an entry beyond fp16's range (|s x| >= 65504 => xn >= 4.29e9) or a non-finite one: float64 path
-      const bool out_of_range = !(xn < 4.29e9f);
-      // ---- single-pass epilogue ----
-      // TMEM reads (64 B/cycle/SM) are the scarcest resource of this kernel, so every accumulator is read
-      // exactly once, in 16-column chunks.  Running state per row: m1 = smallest chunk minimum so far,
-      // sv[] = a copy of that chunk, m2 = smallest value seen outside it (chunk minima only: enough to
-      // decide whether anything outside the best chunk is within `bound` of m1).  After the last chunk the
-      // saved chunk is scanned once: every element within `bound` of m1 adds (1 + i/1024) to an accumulator:
-      //   exactly one hit  -> 1 + i/1024 : the arg-min, decoded exactly
-      //   two or more hits (or m2 within the bound) -> near-tie, the row is deferred to float64
+      for (int s = 0; s < 4; ++s)
+        if (s < KS) wg::Mma<N>::rs_f16(acc, alo[s], dbh + (uint64_t)(2 * s), 1);
+      wg::commit();
+      wg::wait_all();
+      wg::pin(acc);
+
       if (XFORM) {
-        // d^2 = (acc + ||s x||^2) / s^2, clamped at 0; mode 0: sqrt, 1: squared, 2: exp(-gamma d^2).  Thread = row: every
-        // 16-column chunk is 64 contiguous bytes of the output row (four 16-byte stores when the row is 16-byte aligned).
-        const float sc = hdr->scale;
+        // d^2 = (acc + s^2 ||c||^2 + ||s x||^2) / s^2, clamped at 0; mode 0: sqrt, 1: squared, 2: exp(-gamma d^2)
         const float inv_s2 = 1.0f / (sc * sc);
-        const long long row = tile * BM + r;
-        const bool valid = row < a.n;
-        float* orow = a.xf_out + (valid ? row : 0) * a.xf_ld;
-        const bool vec_ok = ((reinterpret_cast<uintptr_t>(a.xf_out) & 15) == 0) && ((a.xf_ld & 3) == 0);
-#pragma unroll 1
-        for (int u = 0; u < U; ++u) {
-          const long long g = it * U + u;
-          const int buf = (int)(g % NBUF);
-          const int nch = (u == 0 ? cfg.NU0 : cfg.NU1) >> 4;
-          const int col0 = u == 0 ? 0 : cfg.NU0;
-          mbar_wait(BAR(BAR_ACC_FULL + set * NBUF + buf), acc_parity(g, U));
-          tc_fence_after();
-          const uint32_t tbase = tmem + lane_addr + (uint32_t)buf * 128u;
-#pragma unroll 1
-          for (int c = 0; c < nch; ++c) {
-            uint32_t v[16];
-            TC_LD16(tbase + (uint32_t)c * 16u, v);
-            asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-            float o[16];
+        const bool vec_ok = ((reinterpret_cast<uintptr_t>(a.xf_out) & 7) == 0) && ((a.xf_ld & 1) == 0);
 #pragma unroll
-            for (int i = 0; i < 16; ++i) {
-              float d2 = fmaxf((__uint_as_float(v[i]) + xn) * inv_s2, 0.f);
-              o[i] = a.xf_mode == 0 ? sqrtf(d2) : (a.xf_mode == 1 ? d2 : __expf(-a.xf_gamma * d2));
+        for (int h = 0; h < 2; ++h) {
+          const long long row = row0 + rA + 8 * h;
+          if (row >= a.n) continue;
+          const float xn = h ? xn1 : xn0;
+          float* orow = a.xf_out + row * a.xf_ld;
+#pragma unroll
+          for (int i = 0; i < N / 8; ++i) {
+            const int col = 8 * i + c2;
+            float o[2];
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const float d2 = fmaxf(((acc[4 * i + 2 * h + e] + cn_s[col + e]) + xn) * inv_s2, 0.f);
+              o[e] = a.xf_mode == 0 ? sqrtf(d2) : (a.xf_mode == 1 ? d2 : __expf(-a.xf_gamma * d2));
             }
-            const int cb = col0 + c * 16;
-            if (valid) {
-              if (vec_ok && cb + 16 <= a.k) {
-#pragma unroll
-                for (int q = 0; q < 4; ++q)
-                  __stcs(reinterpret_cast<float4*>(orow + cb) + q, make_float4(o[4 * q], o[4 * q + 1], o[4 * q + 2], o[4 * q + 3]));
-              } else {
-#pragma unroll
-                for (int i = 0; i < 16; ++i)
-                  if (cb + i < a.k) orow[cb + i] = o[i];
-              }
+            if (vec_ok && col + 1 < k) __stcs(reinterpret_cast<float2*>(orow + col), make_float2(o[0], o[1]));
+            else {
+              if (col < k) orow[col] = o[0];
+              if (col + 1 < k) orow[col + 1] = o[1];
             }
           }
-          tc_fence_before();
-          mbar_arrive(BAR(BAR_ACC_EMPTY + 2 * (set * NBUF + buf) + (int)((g + NBUF) & 1)));
         }
-        continue;
-      }
-      float m1 = CUDART_INF_F, m2 = CUDART_INF_F, sbase = 0.f;
-      float sv[16];
+      } else {
+        // ---- arg-min, near-tie test (bound = tau (||s x||^2 + max ||s c||^2)) ----
+        wg::Best2 b0, b1;
+        wg::tile_best2<N>(acc, cn_s, lane, b0, b1);
+        if ((lane & 3) == 0) {
 #pragma unroll
-      for (int i = 0; i < 16; ++i) sv[i] = CUDART_INF_F;
-// sv[o..o+7] = V[o..o+7] where `better`.  Selects run on the half-rate ALU pipe, which the min tree already
-// loads; a predicated v * 1 + (-0) is exact and runs on the otherwise idle FMA pipe (`one` / `nzero` are
-// opaque run-time registers so that the assembler keeps the FFMA).
-#define PMOV8(S, V, o, B)                                                                              \
-  asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %16, 0;\n"                                            \
-               "@p fma.rn.f32 %0, %8, %17, %18;\n@p fma.rn.f32 %1, %9, %17, %18;\n"                     \
-               "@p fma.rn.f32 %2, %10, %17, %18;\n@p fma.rn.f32 %3, %11, %17, %18;\n"                   \
-               "@p fma.rn.f32 %4, %12, %17, %18;\n@p fma.rn.f32 %5, %13, %17, %18;\n"                   \
-               "@p fma.rn.f32 %6, %14, %17, %18;\n@p fma.rn.f32 %7, %15, %17, %18;\n}"                  \
-               : "+f"(S[o + 0]), "+f"(S[o + 1]), "+f"(S[o + 2]), "+f"(S[o + 3]), "+f"(S[o + 4]),       \
-                 "+f"(S[o + 5]), "+f"(S[o + 6]), "+f"(S[o + 7])                                        \
-               : "f"(__uint_as_float(V[o + 0])), "f"(__uint_as_float(V[o + 1])),                       \
-                 "f"(__uint_as_float(V[o + 2])), "f"(__uint_as_float(V[o + 3])),                       \
-                 "f"(__uint_as_float(V[o + 4])), "f"(__uint_as_float(V[o + 5])),                       \
-                 "f"(__uint_as_float(V[o + 6])), "f"(__uint_as_float(V[o + 7])), "r"((int)(B)),        \
-                 "f"(one), "f"(nzero));
-#define EPI_CHUNK(V, COLBASE)                                                            \
-  {                                                                                      \
-    const float t0 = fmin3(__uint_as_float(V[0]), __uint_as_float(V[1]), __uint_as_float(V[2]));    \
-    const float t1 = fmin3(__uint_as_float(V[3]), __uint_as_float(V[4]), __uint_as_float(V[5]));    \
-    const float t2 = fmin3(__uint_as_float(V[6]), __uint_as_float(V[7]), __uint_as_float(V[8]));    \
-    const float t3 = fmin3(__uint_as_float(V[9]), __uint_as_float(V[10]), __uint_as_float(V[11]));  \
-    const float t4 = fmin3(__uint_as_float(V[12]), __uint_as_float(V[13]), __uint_as_float(V[14])); \
-    const float cm = fminf(fmin3(t0, t1, t2), fmin3(t3, t4, __uint_as_float(V[15])));    \
-    const bool better = cm < m1;                                                         \
-    m2 = fminf(m2, fmaxf(m1, cm));                                                       \
-    m1 = fminf(m1, cm);                                                                  \
-    PMOV8(sv, V, 0, better) PMOV8(sv, V, 8, better)                                      \
-    sbase = better ? (float)(COLBASE) : sbase;                                           \
-  }
-#pragma unroll 1
-      for (int u = 0; u < U; ++u) {
-        const long long g = it * U + u;
-        const int buf = (int)(g % NBUF);
-        const int nch = (u == 0 ? cfg.NU0 : cfg.NU1) >> 4;
-        const int col0 = u == 0 ? 0 : cfg.NU0;
-        mbar_wait(BAR(BAR_ACC_FULL + set * NBUF + buf), acc_parity(g, U));
-        tc_fence_after();
-        if (r == 0) TRACE(7 + 2 * u, it);
-        const uint32_t tbase = tmem + lane_addr + (uint32_t)buf * 128u;
-        uint32_t v0[16], v1[16];
-        // the next chunk's load is in flight while the current one is reduced.  (Measured r02: two chunks per
-        // tcgen05.wait::ld do NOT help — a warp's TMEM loads are served one after the other, ~2 KB per 300 cycles, and 8
-        // epilogue warps together already draw ~54 of the 64 B/clk the SM's TMEM read path delivers.)
-        TC_LD16(tbase, v0);
-#pragma unroll 1
-        for (int c = 0; c < nch; c += 2) {
-          asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-          if (c + 1 < nch) TC_LD16(tbase + (uint32_t)(c + 1) * 16u, v1);
-          EPI_CHUNK(v0, col0 + c * 16)
-          if (c + 1 < nch) {
-            asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-            if (c + 2 < nch) TC_LD16(tbase + (uint32_t)(c + 2) * 16u, v0);
-            EPI_CHUNK(v1, col0 + (c + 1) * 16)
+          for (int h = 0; h < 2; ++h) {
+            const wg::Best2 b = h ? b1 : b0;
+            const float xn = h ? xn1 : xn0;
+            const int r = rA + 8 * h;
+            const long long row = row0 + r;
+            // an entry beyond fp16's range (|s x| >= 65504 => xn >= 4.29e9) or a non-finite one: float64 path
+            const bool out_of_range = !(xn < 4.29e9f);
+            const bool tie = !(b.m2 > b.m1 + a.tau * (xn + cnmax)) || out_of_range;
+            const bool valid = row < a.n;
+            const bool flagged = valid && tie && k > 1;
+            const int bj = (tie || b.j >= k) ? 0 : b.j;
+            if (valid && !flagged && a.labels) a.labels[row] = bj;
+            if (flagged) {
+              // deferred: tc_recheck_kernel decides this row in float64 and adds its M-step contribution
+              const int slot = atomicAdd(a.defer_cnt, 1);
+              a.defer_idx[slot] = (int)row;
+            }
+            if (HAS_M) lab_s[r] = (valid && !flagged) ? bj : -1;
+            if (MSTEP && valid && !flagged) atomicAdd(&cnt_s[bj], 1);
           }
         }
-        tc_fence_before();
-        mbar_arrive(BAR(BAR_ACC_EMPTY + 2 * (set * NBUF + buf) + (int)((g + NBUF) & 1)));    // -> issuer of unit g + NBUF
-        if (r == 0) TRACE(8 + 2 * u, it);
-      }
-#undef EPI_CHUNK
-      const float thr = m1 + bound;
-      float p0 = 0.f, p1 = 0.f;
-#pragma unroll
-      for (int i = 0; i < 16; i += 2) {
-        p0 = fmaf(sv[i] <= thr ? 1.f : 0.f, 1.f + (float)i * 0.0009765625f, p0);
-        p1 = fmaf(sv[i + 1] <= thr ? 1.f : 0.f, 1.f + (float)(i + 1) * 0.0009765625f, p1);
-      }
-      const float hits = p0 + p1;
-      // hits < 2: one hit, (hits - 1) * 1024 = its index inside the saved chunk
-      const bool tie = !(hits >= 1.f && hits < 2.f) || !(m2 > thr) || out_of_range;
-      const int bj = tie ? 0 : (int)(sbase + (hits - 1.f) * 1024.f + 0.5f);
-      const long long row = tile * BM + r;
-      const bool valid = row < a.n;
-      const bool flagged = valid && tie && a.k > 1;
-      if (valid && !flagged && a.labels) a.labels[row] = bj;
-      if (flagged) {
-        // deferred: tc_recheck_kernel decides this row in float64 and adds its M-step contribution
-        const int slot = atomicAdd(a.defer_cnt, 1);
-        a.defer_idx[slot] = (int)row;
-      }
-      if (HAS_M) {
-        const int lb = (int)(it % NLAB);
-        mbar_wait(BAR(BAR_LAB_EMPTY + lb), (uint32_t)(((it / NLAB) & 1) ^ 1));
-        if (LANE_OWNS) {
-          // push the row onto its cluster's list (the owner lane of the M-step warps walks it)
-          int* head = reinterpret_cast<int*>(smem + cfg.off_lab + lb * LIST_BYTES);
-          if (valid && !flagged) head[256 + r] = atomicExch(&head[(bj << cfg.SSH) | (r & ((1 << cfg.SSH) - 1))], r);
-        } else {
-          lab_s[lb * BM + r] = (valid && !flagged) ? bj : -1;
-        }
-        mbar_arrive(BAR(BAR_LAB_FULL + lb));       // release semantics order the smem stores
-        if (r == 0) TRACE(11, it);
       }
     }
-  } else if (warp >= MW0 && LANE_OWNS) {
-    REG_INC(104);
-    // =========================== M-step warps, lane-owns-cluster flavour ===========================
-    // Lane j of warp w owns cluster c = 32 w + j and keeps its d partial sums (or, when only distances are
-    // wanted, its centre) in registers.  The rows come
-    // from the M ring (two full-tile slots, re-fetched from L2 while the tile's epilogue runs), so the A ring
-    // only has to cover load -> convert and two stages are enough.  The epilogue
-    // threads have linked the tile's rows into one list per cluster (head[c] -> next[row] -> ...); every lane
-    // walks its own list and adds whole rows (float4 reads of the swizzled tile: lanes with different
-    // row & 7 hit different banks).  No cross-lane traffic, no selection of an accumulator at run time,
-    // and 64 independent adds per row instead of a dependent chain per row.
-    const int wm = warp - MW0;
-    const int v = wm * 32 + lane;            // list index: (cluster << SSH) | (row mod 2^SSH)
-    const int c = v >> cfg.SSH;              // this lane's cluster
-    double dsum = 0.0;
     if (HAS_M) {
-      // MSTEP: the running sums of cluster c.  Distance variant: the fp32 centre c itself, so that the winning
-      // distance of every row of the list is evaluated in direct form sum (x - c)^2 without leaving the lane.
-      float acc[64];
-      if (MSTEP) {
-#pragma unroll
-        for (int i = 0; i < 64; ++i) acc[i] = 0.f;
-      } else {
-        const float* gc = reinterpret_cast<const float*>(a.pack + a.L.off_cT) + (size_t)(c < a.k ? c : 0) * a.L.d4;
-#pragma unroll
-        for (int i = 0; i < 64; ++i) acc[i] = (c < a.k && i < a.d) ? gc[i] : 0.f;
+      wg::wg_sync(1 + wgi);                                  // lab_s of the tile is complete
+      if (WANT_DIST && has) {
+        // winning distance in direct form sum (x - c)^2 (fp32 centres of the pack): thread (row r, feature half hh),
+        // features visited in a per-row rotated order so that the 32 rows of a warp hit 32 different banks
+        const int r = t & 63, hh = t >> 6;
+        const int lab = lab_s[r];
+        float s0 = 0.f, s1 = 0.f;
+        if (lab >= 0) {
+          const float* cr = reinterpret_cast<const float*>(a.pack + a.L.off_cT) + (size_t)lab * a.L.d4;
+#pragma unroll 8
+          for (int i = 0; i < 32; i += 2) {
+            const int f0 = hh * 32 + ((i + r) & 31), f1 = hh * 32 + ((i + 1 + r) & 31);
+            if (f0 < d) { const float e = xs[r * XP + f0] - cr[f0]; s0 = fmaf(e, e, s0); }
+            if (f1 < d) { const float e = xs[r * XP + f1] - cr[f1]; s1 = fmaf(e, e, s1); }
+          }
+        }
+        dp_s[hh * TBM + r] = s0 + s1;
+        wg::wg_sync(1 + wgi);
+        if (t < TBM && lab >= 0) {
+          const float d2 = dp_s[t] + dp_s[TBM + t];
+          const float outv = a.squared ? d2 : sqrtf(d2);
+          dsum += (double)outv;
+          if (a.min_out) reinterpret_cast<float*>(a.min_out)[row0 + t] = outv;
+        }
       }
-      int cnt = 0;
-      const bool two = KB > 1;
-      const int nq2 = (a.d - 32 + 3) >> 2;          // chunks of the second K-block in use
+      if (MSTEP) {
+        // turn order of the CTA's M-steps: warpgroup 0 tile p, warpgroup 1 tile p, warpgroup 0 tile p + 1, ...
+        if (wgi == 1) bar_sync(3, 256);
+        else if (p > 0) bar_sync(4, 256);
+        if (has) {
+          // thread (feature f, half h): half 0 adds rows 0-31, then half 1 rows 32-63, 8 rows at a time; when the 8
+          // labels are distinct their read-modify-writes are independent, otherwise they run one after the other
+          const int f = t & 63, h = t >> 6;
 #pragma unroll 1
-      for (long long it = 0; it < my_tiles; ++it) {
-        const long long tile = blockIdx.x + it * gridDim.x;
-        const int lb = (int)(it % NLAB);
-        const int slot = (int)(it & 1);
-        mbar_wait_sleep(BAR(BAR_LAB_FULL + lb), (uint32_t)((it / NLAB) & 1));
-        mbar_wait(BAR(BAR_M_FULL + slot), (uint32_t)((it >> 1) & 1));
-        if (wm == 0 && lane == 0) TRACE(12, it);
-        int* head = reinterpret_cast<int*>(smem + cfg.off_lab + lb * LIST_BYTES);
-        const unsigned char* xs = smem + cfg.off_m + slot * stage_bytes;      // full-tile slot: same layout as an A stage
-        int rr = head[v];
-        head[v] = -1;
-        int guard = BM;                                 // a list holds at most the tile's rows (a corrupted list must not spin)
+          for (int ph = 0; ph < 2; ++ph) {
+            if (h == ph) {
 #pragma unroll 1
-        while (__any_sync(0xffffffffu, rr >= 0) && guard-- > 0) {
-          if (rr >= 0) {
-            const unsigned char* xr = xs + rr * 128;
-            const int sw = rr & 7;
-            if (MSTEP) {
+              for (int r0 = 32 * ph; r0 < 32 * ph + 32; r0 += 8) {
+                const int lr = lane < 8 ? lab_s[r0 + lane] : -2 - lane;
+                const unsigned peers = __match_any_sync(0xffffffffu, lr);
+                const bool conflict = __any_sync(0xffffffffu, lr >= 0 && __popc(peers) > 1);
+                int l[8];
 #pragma unroll
-              for (int q = 0; q < 8; ++q) {
-                const float4 t = *reinterpret_cast<const float4*>(xr + ((q ^ sw) << 4));
-                acc[q * 4 + 0] += t.x; acc[q * 4 + 1] += t.y; acc[q * 4 + 2] += t.z; acc[q * 4 + 3] += t.w;
-              }
-              if (two) {
-                // second K-block: only the 16-byte chunks that hold features (d = 41: 3 of 8)
+                for (int q = 0; q < 8; ++q) l[q] = __shfl_sync(0xffffffffu, lr, q);
+                if (f < d) {
+                  if (!conflict) {
+                    float v[8];
 #pragma unroll
-                for (int q = 0; q < 8; ++q) {
-                  if (q < nq2) {
-                    const float4 t = *reinterpret_cast<const float4*>(xr + KBLK_BYTES + ((q ^ sw) << 4));
-                    acc[32 + q * 4 + 0] += t.x; acc[32 + q * 4 + 1] += t.y; acc[32 + q * 4 + 2] += t.z; acc[32 + q * 4 + 3] += t.w;
+                    for (int q = 0; q < 8; ++q) v[q] = l[q] >= 0 ? sum_s[l[q] * 64 + f] : 0.f;
+#pragma unroll
+                    for (int q = 0; q < 8; ++q)
+                      if (l[q] >= 0) sum_s[l[q] * 64 + f] = v[q] + xs[(r0 + q) * XP + f];
+                  } else {
+#pragma unroll
+                    for (int q = 0; q < 8; ++q)
+                      if (l[q] >= 0) sum_s[l[q] * 64 + f] += xs[(r0 + q) * XP + f];
                   }
                 }
               }
-              ++cnt;
-            } else {
-              float s0 = 0.f, s1 = 0.f, s2 = 0.f, s3 = 0.f;
-#pragma unroll
-              for (int q = 0; q < 8; ++q) {
-                const float4 t = *reinterpret_cast<const float4*>(xr + ((q ^ sw) << 4));
-                const float e0 = t.x - acc[q * 4 + 0], e1 = t.y - acc[q * 4 + 1];
-                const float e2 = t.z - acc[q * 4 + 2], e3 = t.w - acc[q * 4 + 3];
-                s0 = fmaf(e0, e0, s0); s1 = fmaf(e1, e1, s1); s2 = fmaf(e2, e2, s2); s3 = fmaf(e3, e3, s3);
-              }
-              if (two) {
-#pragma unroll
-                for (int q = 0; q < 8; ++q) {
-                  const float4 t = *reinterpret_cast<const float4*>(xr + KBLK_BYTES + ((q ^ sw) << 4));
-                  const float e0 = t.x - acc[32 + q * 4 + 0], e1 = t.y - acc[32 + q * 4 + 1];
-                  const float e2 = t.z - acc[32 + q * 4 + 2], e3 = t.w - acc[32 + q * 4 + 3];
-                  s0 = fmaf(e0, e0, s0); s1 = fmaf(e1, e1, s1); s2 = fmaf(e2, e2, s2); s3 = fmaf(e3, e3, s3);
-                }
-              }
-              const float d2 = (s0 + s1) + (s2 + s3);
-              const float outv = a.squared ? d2 : sqrtf(d2);
-              dsum += (double)outv;
-              if (a.min_out) reinterpret_cast<float*>(a.min_out)[tile * BM + rr] = outv;
             }
-            rr = head[256 + rr];
+            if (ph == 0) wg::wg_sync(1 + wgi);
           }
         }
-        __syncwarp();
-        if (wm == 0 && lane == 0) TRACE(13, it);
-        if (lane == 0) {
-          mbar_arrive(BAR(BAR_M_EMPTY + slot));
-          mbar_arrive(BAR(BAR_LAB_EMPTY + lb));
-        }
-      }
-      if (MSTEP) {
-        // the 2^SSH lanes of a cluster are adjacent: fold them (fixed shuffle tree), the first one writes
-        for (int o = (1 << cfg.SSH) >> 1; o > 0; o >>= 1) {
-#pragma unroll
-          for (int i = 0; i < 64; ++i) acc[i] += __shfl_xor_sync(0xffffffffu, acc[i], o);
-          cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
-        }
-        if (c < a.k && (v & ((1 << cfg.SSH) - 1)) == 0) {
-          float* g = reinterpret_cast<float*>(a.psum) + (size_t)blockIdx.x * a.k * a.d + (size_t)c * a.d;
-#pragma unroll
-          for (int i = 0; i < 64; ++i) if (i < a.d) g[i] = acc[i];
-          a.pcnt[(size_t)blockIdx.x * a.k + c] = cnt;
-        }
+        __threadfence_block();
+        if (wgi == 0) bar_arrive(3, 256);
+        else if (p + 1 < npairs) bar_arrive(4, 256);
       }
     }
-    // per-CTA sum of the distances: fixed shuffle tree per warp, warps added in order at the end
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) dsum += __shfl_xor_sync(0xffffffffu, dsum, o);
-    if (lane == 0) red_s[wm] = dsum;
-  } else if (warp >= MW0 && !LANE_OWNS) {
-    // =========================== distance + M-step warps ===========================
-    // Warp wm owns the rows whose label c satisfies c % NMW == wm.  Lane l holds features l and l+32 of
-    // the row (conflict-free reads of the swizzled tile): (a) [WANT_DIST] the winning distance is
-    // re-evaluated exactly in fp32 direct form sum (x-c)^2 against the fp32 centres in shared memory,
-    // (b) [MSTEP] the row is added to the register-resident sums of cluster c.
-    const int wm = warp - MW0;
-    float acc[256 / NMW][2];
-#pragma unroll
-    for (int j = 0; j < 256 / NMW; ++j) { acc[j][0] = 0.f; acc[j][1] = 0.f; }
-    int cnt = 0;
-    double inertia_acc = 0.0;
-    const bool two = KB > 1;
-    const float* c32 = reinterpret_cast<const float*>(smem + cfg.off_c32);
-    const int cpitch = KB * 32;
-    const uint32_t kstride = direct ? (uint32_t)KBLK_BYTES : (uint32_t)MKBLK_BYTES;   // bytes between K-blocks
-#define MSTEP_ROW(XA, XB, CC, ROWG)                                                               \
-  {                                                                                               \
-    const int c = (CC);                                                                           \
-    const float x0 = (XA), x1 = (XB);                                                             \
-    if (WANT_DIST) {                                                                              \
-      float t = x0 - c32[c * cpitch + lane];                                                      \
-      float s2 = t * t;                                                                           \
-      if (two) {                                                                                  \
-        t = x1 - c32[c * cpitch + 32 + lane];                                                     \
-        s2 = fmaf(t, t, s2);                                                                      \
-      }                                                                                           \
-      _Pragma("unroll") for (int o = 16; o > 0; o >>= 1) s2 += __shfl_xor_sync(0xffffffffu, s2, o); \
-      if (lane == 0) {                                                                            \
-        const float outv = a.squared ? s2 : sqrtf(s2);                                            \
-        inertia_acc += (double)outv;                                                              \
-        if (a.min_out) reinterpret_cast<float*>(a.min_out)[(ROWG)] = outv;                        \
-      }                                                                                           \
-    }                                                                                             \
-    if (MSTEP) {                                                                                  \
-      const int cl = c / NMW;                                                                     \
-      switch (cl) {                                                                               \
-        ACC32_CASE(0) ACC32_CASE(1) ACC32_CASE(2) ACC32_CASE(3) ACC32_CASE(4) ACC32_CASE(5)       \
-        ACC32_CASE(6) ACC32_CASE(7) ACC32_CASE(8) ACC32_CASE(9) ACC32_CASE(10) ACC32_CASE(11)     \
-        ACC32_CASE(12) ACC32_CASE(13) ACC32_CASE(14) ACC32_CASE(15)                               \
-        default: break;                                                                           \
-      }                                                                                           \
-      cnt += (lane == cl) ? 1 : 0;                                                                \
-    }                                                                                             \
-  }
-#pragma unroll 1
-    for (long long it = 0; it < my_tiles; ++it) {
-      const long long tile = blockIdx.x + it * gridDim.x;
-      const int lb = (int)(it % NLAB);
-      const int stage = (int)((unsigned)it % (unsigned)NST);
-      // every warp polls on its own: a barrier across the 16 warps would make each step as slow as its
-      // most loaded warp
-      mbar_wait_sleep(BAR(BAR_LAB_FULL + lb), (uint32_t)((it / NLAB) & 1));
-      if (direct) mbar_wait(BAR(BAR_X_FULL + stage), (uint32_t)(((unsigned)it / (unsigned)NST) & 1u));   // completed long ago: acquire only
-      if (wm == 0 && lane == 0) TRACE(12, it);
-#pragma unroll 1
-      for (int h = 0; h < 4; ++h) {
-        const long long mi = it * 4 + h;
-        const int slot = (int)(mi & 1);
-        const unsigned char* xs;
-        if (direct) {
-          xs = smem + cfg.off_x + stage * stage_bytes + h * MKBLK_BYTES;
-        } else {
-          mbar_wait(BAR(BAR_M_FULL + slot), (uint32_t)((mi >> 1) & 1));
-          xs = smem + cfg.off_m + slot * (KB * MKBLK_BYTES);
-        }
-        const int ml = lab_s[lb * BM + h * MH + lane];
-        unsigned m = __ballot_sync(0xffffffffu, ml >= 0 && (ml & (NMW - 1)) == wm);
-#pragma unroll 1
-        while (m) {
-          const int b = __ffs(m) - 1;
-          m &= m - 1;
-          const int cq = __shfl_sync(0xffffffffu, ml, b) & 255;
-          const uint32_t ro = (uint32_t)(b * 128 + (((lane >> 2) ^ (b & 7)) << 4) + ((lane & 3) << 2));
-          const float xa = *reinterpret_cast<const float*>(xs + ro);
-          const float xb = two ? *reinterpret_cast<const float*>(xs + kstride + ro) : 0.f;
-          MSTEP_ROW(xa, xb, cq, tile * BM + h * MH + b)
-        }
-        if (!direct) {
-          __syncwarp();
-          if (lane == 0) mbar_arrive(BAR(BAR_M_EMPTY + slot));
-        }
-      }
-      __syncwarp();
-      if (wm == 0 && lane == 0) TRACE(13, it);
-      if (lane == 0) {
-        if (direct) mbar_arrive(BAR(BAR_X_EMPTY + stage));
-        mbar_arrive(BAR(BAR_LAB_EMPTY + lb));
-      }
-    }
-#undef MSTEP_ROW
-    if (lane == 0) red_s[wm] = inertia_acc;
-    if (MSTEP) {
-      // flush the register-resident sums: cluster c = wm + NMW j, features lane and lane + 32
-      float* g = reinterpret_cast<float*>(a.psum) + (size_t)blockIdx.x * a.k * a.d;
-#pragma unroll
-      for (int j = 0; j < 256 / NMW; ++j) {
-        const int c = wm + NMW * j;
-        if (c < a.k) {
-          if (lane < a.d) g[(size_t)c * a.d + lane] = acc[j][0];
-          if (lane + 32 < a.d) g[(size_t)c * a.d + lane + 32] = acc[j][1];
-        }
-      }
-      const int cc = wm + NMW * lane;
-      if (lane < 256 / NMW && cc < a.k) a.pcnt[(size_t)blockIdx.x * a.k + cc] = cnt;
-    }
+    wg::wg_sync(1 + wgi);                                    // the stage and lab_s may be refilled
   }
 
-  // ---------------- teardown ----------------
-  tc_fence_before();
+  // ---------------- teardown: per-CTA partials ----------------
   __syncthreads();
-  tc_fence_after();
+  if (MSTEP) {
+    float* gs = reinterpret_cast<float*>(a.psum) + (size_t)blockIdx.x * k * d;
+    for (int i = tid; i < k * d; i += TC_THREADS) {
+      const int c = i / d;
+      gs[i] = sum_s[c * 64 + (i - c * d)];
+    }
+    for (int c = tid; c < k; c += TC_THREADS) a.pcnt[(size_t)blockIdx.x * k + c] = cnt_s[c];
+  }
+  red_s[tid] = dsum;
+  __syncthreads();
   if (tid == 0) {
-    double t = red_s[NMWK];
-    for (int w = 0; w < NMWK; ++w) t += red_s[w];
-    if (a.pin) a.pin[blockIdx.x] = t;             // (the transform variant has no per-CTA partials)
+    double tt = 0.0;
+    for (int i = 0; i < TC_THREADS; ++i) tt += red_s[i];
+    if (a.pin) a.pin[blockIdx.x] = tt;             // (the transform variant has no per-CTA partials)
   }
-  if (warp == 0) {
-    __syncwarp();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(512));
-  }
-#undef BAR
 }
 
 // ------------------------------------------------------------------------------------------
@@ -1096,54 +437,14 @@ int launch_tc_recheck(const ChunkArgs& a, bool mstep, int sm_count, cudaStream_t
 }
 
 // ------------------------------------------------------------------------------------ host
-int launch_tc_transform(const ChunkArgs& a, int sm_count, cudaStream_t s);
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-static EncodeTiledFn get_encode() {
-  static EncodeTiledFn fn = nullptr;
-  if (!fn) {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess &&
-        q == cudaDriverEntryPointSuccess)
-      fn = (EncodeTiledFn)p;
-  }
-  return fn;
-}
-
-// 2-D tensor [rows][cols] (fp32, or fp16 when half16) with row pitch `pitch_elems`; box = one 128-byte
-// swizzle atom of columns (32 fp32 / 64 fp16) x box_rows
-static int make_map(CUtensorMap* tm, const void* base, long long rows, int cols, long long pitch_elems, int box_rows,
-                    bool half16 = false) {
-  EncodeTiledFn enc = get_encode();
-  if (!enc) return BKM_EUNSUPPORTED;
-  cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
-  cuuint64_t strides[1] = {(cuuint64_t)pitch_elems * (half16 ? 2 : 4)};
-  cuuint32_t box[2] = {half16 ? 64u : 32u, (cuuint32_t)box_rows};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult r = enc(tm, half16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2,
-                   const_cast<void*>(base), dims, strides, box, estr,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  return r == CUDA_SUCCESS ? 0 : BKM_EUNSUPPORTED;
-}
-
 unsigned int tc_abort_code() {
   unsigned int v = 0;
   cudaMemcpyFromSymbol(&v, g_tc_abort, sizeof(v));
   return v;
 }
 int tc_trace(long long* out, int n) {
-#if BKM_TRACE
-  if (n > 16 * 128) n = 16 * 128;
-  cudaMemcpyFromSymbol(out, g_tc_trace, (size_t)n * sizeof(long long));
-  return n;
-#else
   (void)out; (void)n;
   return 0;
-#endif
 }
 void tc_abort_detail(unsigned int* out64) { cudaMemcpyFromSymbol(out64, g_tc_dbg, 64 * sizeof(unsigned int)); }
 // Clear the sticky abort word (after the host has reported it): later launches run normally again.
@@ -1155,88 +456,66 @@ void tc_abort_reset() {
 }
 
 bool tc_supported(int d, int k, int dtype) {
-  // any d <= 64: columns beyond d are zero-filled by TMA; what TMA does need is a 16-byte row pitch and base
-  // (launch_tc returns BKM_EALIGN otherwise and the caller falls back to the CUDA-core kernel), which the host
-  // side provides by uploading row chunks with a padded pitch (engine.CudaBackend.to_device)
+  // any d <= 64: columns beyond d are zero-filled when a tile is staged; what the staging copies do need is a
+  // 16-byte row pitch and base (launch_tc returns BKM_EALIGN otherwise and the caller falls back to the CUDA-core
+  // kernel), which the host side provides by uploading row chunks with a padded pitch (engine.CudaBackend.to_device)
   return dtype == BKM_F32 && d >= 1 && d <= 64 && k >= 1 && k <= 256;
 }
 
-static bool make_cfg(int d, int k, bool mstep, bool want_dist, TcCfg* c) {
-  const bool lane_owns = !(mstep && want_dist);
-  const bool has_m = mstep || want_dist;
-  c->KB = (d + 31) / 32;
+static bool make_cfg(int d, int k, bool mstep, TcCfg* c) {
   c->KS = (d + 15) / 16;
   c->NP = (k + 15) / 16 * 16;
-  if (c->NP <= 128) { c->NU0 = c->NP; c->NU1 = 0; c->U = 1; }
-  else { c->NU0 = (c->NP / 2 + 15) / 16 * 16; c->NU1 = c->NP - c->NU0; c->U = c->NU1 > 0 ? 2 : 1; }
-  const uint32_t bbytes = (uint32_t)c->NP * 128u;               // one fp16 B tile: NP rows x 64 halves
-  // Shared-memory plans, tried in order:
-  //  lane-owns-cluster variants: 2 A stages (load -> convert) + 2 whole-tile M slots; labels only: A ring alone
-  //  sums + distances in one pass: direct mode (the M-step warps read the A ring) when >= 4 stages fit, which
-  //  covers load -> convert -> MMA -> epilogue -> M-step; otherwise 2-3 stages plus a quarter-tile M ring.
-  struct Plan { int direct, mring, mr, nst_hi, nst_lo; };
-  Plan plans[2];
-  int nplans = 0;
-  if (lane_owns) plans[nplans++] = has_m ? Plan{0, 1, BM, 2, 2} : Plan{0, 0, BM, 4, 2};
-  else { plans[nplans++] = Plan{1, 0, MH, NSTMAX, 4}; plans[nplans++] = Plan{0, 1, MH, 3, 2}; }
-  for (int pi = 0; pi < nplans; ++pi) {
-    const Plan& P = plans[pi];
-    for (int nst = P.nst_hi; nst >= P.nst_lo; --nst) {
-      uint32_t o = 0;
-      c->off_bhi = o; o += bbytes;
-      c->off_blo = o; o += bbytes;
-      c->off_bcn = o; o += (uint32_t)c->NP * 32u;                  // ||c||^2 operand tile
-      c->off_ones = o; o += BM * 32u;                              // constant [1,1,1,0..] A tile
-      c->off_c32 = o; if (!lane_owns) o += (uint32_t)c->NP * c->KB * 128u;   // fp32 centres (sums + distances variant)
-      o = (uint32_t)align_up(o, 1024);
-      c->off_x = o; o += (uint32_t)nst * c->KB * KBLK_BYTES;       // A ring
-      c->off_m = o; if (P.mring) o += 2u * c->KB * P.mr * 128u;    // M ring
-      c->off_lab = o; o += NLAB * (lane_owns ? LIST_BYTES : BM * 4);   // per-cluster row lists / label buffers
-      c->off_xn = o; o += 8 * BM * 4;                              // ||s x||^2 of the last 8 tiles (converter -> epilogue)
-      c->off_red = o; o += (NMW + 1) * 8;
-      c->off_bar = o; o += BAR_COUNT * 8;
-      c->off_tptr = o; o += 16;
-      c->total = o;
-      c->NST = nst;
-      c->direct = P.direct;
-      c->mring = P.mring;
-      c->MR = P.mr;
-      c->SSH = 0;
-      if (lane_owns) { int p2 = 1; while (p2 < k) p2 <<= 1; while ((p2 << c->SSH) < 256 && c->SSH < 5) ++c->SSH; }   // <= one warp per cluster
-      if (o <= 227 * 1024) return true;
-    }
+  const uint32_t N = (uint32_t)wg::mma_n(c->NP);
+  uint32_t o = 0;
+  c->off_bhi = o; o += N * 128u;                    // fp16 B tiles: N rows x 64 halves (one 128-byte swizzle atom)
+  c->off_blo = o; o += N * 128u;
+  c->off_x = o; o += 2u * 2u * TBM * XP * 4u;       // 2 warpgroups x 2 stages of fp32 X tiles
+  c->off_sum = o; if (mstep) o += N * 64u * 4u;     // per-CTA sums [N][64]
+  c->off_cn = o; o += N * 4u;
+  c->off_cnt = o; o += N * 4u;
+  c->off_lab = o; o += 2u * TBM * 4u;
+  c->off_dp = o; o += 2u * 2u * TBM * 4u;
+  c->off_red = o; o += TC_THREADS * 8u;
+  c->total = o;
+  return o <= 227u * 1024u;
+}
+
+template <int N, bool M, bool W, bool XF>
+static int launch_variant(const ChunkArgs& a, const TcCfg& cfg, int grid, cudaStream_t s) {
+  auto kern = tc_chunk_kernel<N, M, W, XF>;
+  BKM_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cfg.total));
+  kern<<<grid, TC_THREADS, cfg.total, s>>>(a, cfg);
+  return 0;
+}
+template <bool M, bool W, bool XF>
+static int launch_n(const ChunkArgs& a, const TcCfg& cfg, int grid, cudaStream_t s) {
+  switch (wg::mma_n(cfg.NP)) {
+    case 16: return launch_variant<16, M, W, XF>(a, cfg, grid, s);
+    case 32: return launch_variant<32, M, W, XF>(a, cfg, grid, s);
+    case 64: return launch_variant<64, M, W, XF>(a, cfg, grid, s);
+    case 128: return launch_variant<128, M, W, XF>(a, cfg, grid, s);
+    default: return launch_variant<256, M, W, XF>(a, cfg, grid, s);
   }
-  return false;
+}
+
+static int tc_grid(long long n, int sm_count) {
+  const long long ntiles = (n + TBM - 1) / TBM;
+  int grid = (int)(ntiles < sm_count ? ntiles : sm_count);
+  return grid < 1 ? 1 : grid;
 }
 
 int launch_tc(const ChunkArgs& a, bool mstep, int sm_count, int* grid_out, cudaStream_t s) {
   if ((reinterpret_cast<uintptr_t>(a.X) & 15) || (a.ldx % 4)) return BKM_EALIGN;
   const bool want_dist = a.min_out != nullptr || a.want_sum;
   TcCfg cfg;
-  if (!make_cfg(a.d, a.k, mstep, want_dist, &cfg)) return BKM_EUNSUPPORTED;
-  CUtensorMap tm_x, tm_bhi, tm_blo, tm_xm;
-  int rc = make_map(&tm_x, a.X, a.n, a.d, a.ldx, BM);
-  if (rc) return rc;
-  rc = make_map(&tm_xm, a.X, a.n, a.d, a.ldx, cfg.MR);
-  if (rc) return rc;
-  rc = make_map(&tm_bhi, a.pack + a.L.off_bhi, a.L.kp, a.L.dh, a.L.dh, cfg.NP, true);
-  if (rc) return rc;
-  rc = make_map(&tm_blo, a.pack + a.L.off_blo, a.L.kp, a.L.dh, a.L.dh, cfg.NP, true);
-  if (rc) return rc;
-  long long ntiles = (a.n + BM - 1) / BM;
-  int grid = (int)(ntiles < sm_count ? ntiles : sm_count);
-  if (grid < 1) grid = 1;
+  if (!make_cfg(a.d, a.k, mstep, &cfg)) return BKM_EUNSUPPORTED;
+  const int grid = tc_grid(a.n, sm_count);
   *grid_out = grid;
   BKM_CUDA_TRY(cudaMemsetAsync(a.defer_cnt, 0, sizeof(int), s));
-#define TC_LAUNCH(M, W)                                                                                       \
-  {                                                                                                           \
-    BKM_CUDA_TRY(cudaFuncSetAttribute(tc_chunk_kernel<M, W>, cudaFuncAttributeMaxDynamicSharedMemorySize,     \
-                                      (int)cfg.total));                                                       \
-    tc_chunk_kernel<M, W><<<grid, tc_threads(M, W), cfg.total, s>>>(a, cfg, tm_x, tm_bhi, tm_blo, tm_xm);                  \
-  }
-  if (mstep) { if (want_dist) TC_LAUNCH(true, true) else TC_LAUNCH(true, false) }
-  else { if (want_dist) TC_LAUNCH(false, true) else TC_LAUNCH(false, false) }
-#undef TC_LAUNCH
+  int rc;
+  if (mstep) rc = want_dist ? launch_n<true, true, false>(a, cfg, grid, s) : launch_n<true, false, false>(a, cfg, grid, s);
+  else rc = want_dist ? launch_n<false, true, false>(a, cfg, grid, s) : launch_n<false, false, false>(a, cfg, grid, s);
+  if (rc) return rc;
   note_launch(2);
   BKM_CUDA_TRY(cudaGetLastError());
   return 0;
@@ -1246,22 +525,9 @@ int launch_tc(const ChunkArgs& a, bool mstep, int sm_count, int* grid_out, cudaS
 int launch_tc_transform(const ChunkArgs& a, int sm_count, cudaStream_t s) {
   if ((reinterpret_cast<uintptr_t>(a.X) & 15) || (a.ldx % 4)) return BKM_EALIGN;
   TcCfg cfg;
-  if (!make_cfg(a.d, a.k, false, false, &cfg)) return BKM_EUNSUPPORTED;
-  CUtensorMap tm_x, tm_bhi, tm_blo, tm_xm;
-  int rc = make_map(&tm_x, a.X, a.n, a.d, a.ldx, BM);
+  if (!make_cfg(a.d, a.k, false, &cfg)) return BKM_EUNSUPPORTED;
+  const int rc = launch_n<false, false, true>(a, cfg, tc_grid(a.n, sm_count), s);
   if (rc) return rc;
-  rc = make_map(&tm_xm, a.X, a.n, a.d, a.ldx, cfg.MR);
-  if (rc) return rc;
-  rc = make_map(&tm_bhi, a.pack + a.L.off_bhi, a.L.kp, a.L.dh, a.L.dh, cfg.NP, true);
-  if (rc) return rc;
-  rc = make_map(&tm_blo, a.pack + a.L.off_blo, a.L.kp, a.L.dh, a.L.dh, cfg.NP, true);
-  if (rc) return rc;
-  long long ntiles = (a.n + BM - 1) / BM;
-  int grid = (int)(ntiles < sm_count ? ntiles : sm_count);
-  if (grid < 1) grid = 1;
-  auto kern = tc_chunk_kernel<false, false, true>;
-  BKM_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cfg.total));
-  kern<<<grid, tc_threads(false, false), cfg.total, s>>>(a, cfg, tm_x, tm_bhi, tm_blo, tm_xm);
   note_launch();
   BKM_CUDA_TRY(cudaGetLastError());
   return 0;

@@ -1,312 +1,185 @@
-// bkm_tc2.cu — E-step on the 5th-gen tensor cores for LARGE shapes: bf16 rows, any k, d <= 128
-// (BASELINE config C5: 1B x 128 bf16, k = 1024 — the tensor-bound configuration).
+// bkm_tc2.cu — E-step on the Hopper tensor cores (wgmma, sm_90a) for LARGE shapes: bf16 rows, any k, d <= 128
+// (BASELINE config C5: bf16 rows, d = 128, k = 1024 — the tensor-bound configuration).
 //
 // Reference operator: sklearn pairwise_distances_argmin_min(x, centers) per chunk (dask_ml/metrics/pairwise.py:35-38).
 //
 // Layout of the work ("B-stationary"): the k centres are cut into S = ceil(k / 256) slices of NS <= 256 centres.
 // CTA b serves slice b % S for the row tiles of group b / S (G = SMs / S groups): its slice of -2 C, as a bf16
 // (hi, lo) pair per 64-feature K-block, is loaded ONCE and stays resident in shared memory (128 KB at NS = 256,
-// d = 128); the kernel then streams 128-row bf16 tiles of X through a TMA ring and issues, per tile,
-//     acc[128 x NS] = ||c||^2  +  X . (-2 C)_hi^T  +  X . (-2 C)_lo^T          (fp32, in TMEM)
-// X is multiplied as it lies in HBM (bf16 operands straight from TMA, no converter, no scaling: bf16 has fp32's
-// range); the centres carry 16 significant bits through the bf16 pair (representation error <= 2^-18 |c|), which the
-// near-tie bound accounts for (tau_for, bkm_api.cu).  Measured on the box (tests/probes/mma_mix_probe.cu):
-// kind::f16 does NOT accept different 16-bit formats for A and B (bf16 x fp16 raises an illegal-instruction fault although
-// the instruction descriptor has separate a_format / b_format fields), so the centre splits are bf16 like the rows.
-// Each centre slice is read from L2 once per CTA, X tiles are read by the S CTAs of a group at about the same time
-// (one HBM read, S - 1 L2 hits): no operand is re-streamed per tile, which is what bounds a C-streaming design
-// (SURVEY.md Appendix A: 2 KB of L2 traffic per row).
+// d = 128); the kernel then streams 64-row bf16 tiles of X (cp.async, double-buffered per warpgroup) and computes, per
+// tile,
+//     acc[64 x NS] = X . (-2 C)_hi^T  +  X . (-2 C)_lo^T          (fp32 accumulators in registers)
+// plus ||c||^2 per column in the epilogue.  X is multiplied as it lies in HBM (bf16 operands, no scaling: bf16 has
+// fp32's range); the centres carry 16 significant bits through the bf16 pair (representation error <= 2^-18 |c|),
+// which the near-tie bound accounts for (tau_for, bkm_api.cu).  wgmma needs A and B in the same 16-bit format, so the
+// centre splits are bf16 like the rows.  Each centre slice is read from L2 once per CTA, X tiles are read by the S
+// CTAs of a group at about the same time (one HBM read, S - 1 L2 hits).
 //
-// Warp roles (512 threads, 1 CTA per SM):
-//   0        TMA producer (B slice once, X ring) + TMEM allocation
-//   1        MMA issuer (one elected lane): ceil(d/16) K-steps x 2 products + the ||c||^2 K-step per tile, N = NS
-//   4-7      row norms ||x||^2 from the staged tile (thread = row) -> shared memory, 8 tiles deep
-//   8-11, 12-15   two epilogue sets on alternate tiles (set = accumulator buffer): single pass over the NS columns,
-//            running (m1, copy of the best 16-column chunk, m2) per row exactly as in bkm_tc.cu
-// TMEM: 2 accumulator buffers x 256 columns.
+// CTA = 2 warpgroups, 1 CTA per SM; each warpgroup owns alternate tiles: row norms ||x||^2 from the staged tile,
+// 2 ceil(d/16) wgmma.m64nNk16 (A and B from SWIZZLE_128B shared memory), the arg-min epilogue from registers.
 // S == 1: the epilogue decides the row (label, or deferred to the float64 re-check).  S > 1: it writes a partial
 // record {m1, label-or-tie, ||x||^2} per (slice, row); tc2_combine_kernel folds the S records of a row.
 // The M-step and the winning distances for these shapes are label-indexed row passes (bkm_rowpass.cu): k * d partial
-// sums (512 KB at C5) do not fit a CTA, so the sums are accumulated by feature slice in a second sweep.
+// sums (512 KB at C5) do not fit a CTA, so the sums are accumulated by cluster slice in a second sweep.
 #include "bkm_common.cuh"
-#include "bkm_ptx.cuh"
-#include <cuda.h>
+#include "bkm_wgmma.cuh"
 #include <cuda_bf16.h>
 #include <math_constants.h>
 
 namespace bkm {
 
-using namespace ptx;
-
-static const int T2_BM = 128;
-static const int T2_THREADS = 512;
-static const int T2_NSTMAX = 4;
+static const int T2_BM = 64;          // rows per warpgroup tile (wgmma M)
+static const int T2_THREADS = 256;    // two warpgroups
 
 struct Tc2Cfg {
   int S, NS, KB, KS;        // slices, slice width, 64-element K-blocks, 16-element K-steps (ceil(d/16))
-  int NST;                  // X ring stages
   int G;                    // row-tile groups (grid = G * S)
-  uint32_t off_b, off_bcn, off_ones, off_x, off_xn, off_bar, off_tptr, total;
+  uint32_t off_b, off_x, off_cn, off_xn, total;
 };
 
-enum {
-  T2_B_FULL = 0,
-  T2_X_FULL = 1,                           // [NSTMAX]
-  T2_X_EMPTY = T2_X_FULL + T2_NSTMAX,      // [NSTMAX]  MMA commit + 128 norm threads
-  T2_ACC_FULL = T2_X_EMPTY + T2_NSTMAX,    // [2]
-  T2_ACC_EMPTY = T2_ACC_FULL + 2,          // [2]  128 epilogue threads
-  T2_XN_FULL = T2_ACC_EMPTY + 2,           // [8]
-  T2_BAR_COUNT = T2_XN_FULL + 8
-};
-
-// every wait can time out (wall clock): the abort word makes all roles drain instead of hanging the GPU
-#define T2_WAIT(bar, par)                                                              \
-  do {                                                                                 \
-    if (!mbar_wait_timed((bar), (par), abort_w)) {                                     \
-      atomicCAS(const_cast<unsigned int*>(abort_w), 0u, 0x80000000u | (((bar) & 0xfff) << 12) | ((par) << 8) | (threadIdx.x >> 5)); \
-    }                                                                                  \
-  } while (0)
-
+template <int N>
 __global__ void __launch_bounds__(T2_THREADS, 1)
-tc2_assign_kernel(ChunkArgs a, Tc2Cfg cfg, const __grid_constant__ CUtensorMap tm_x,
-                  const __grid_constant__ CUtensorMap tm_bhi, const __grid_constant__ CUtensorMap tm_blo) {
+tc2_assign_kernel(ChunkArgs a, Tc2Cfg cfg) {
   if (a.skip && *a.skip) return;                            // converged loop: no-op iteration
 
   extern __shared__ __align__(1024) unsigned char smem[];
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const uint32_t sbase = smem_u32(smem);
-  if (tid == 0 && (sbase & 1023)) __trap();
-  const uint32_t bars = sbase + cfg.off_bar;
-  uint32_t* tptr_s = reinterpret_cast<uint32_t*>(smem + cfg.off_tptr);
-#define BAR(i) (bars + 8u * (uint32_t)(i))
-  volatile unsigned int* abort_w = reinterpret_cast<volatile unsigned int*>(a.defer_cnt + 1);
-
-  const int S = cfg.S, NS = cfg.NS, KB = cfg.KB, NST = cfg.NST;
+  const int tid = threadIdx.x, lane = tid & 31, wgi = tid >> 7, t = tid & 127, wq = t >> 5;
+  const uint32_t sbase = (uint32_t)__cvta_generic_to_shared(smem);
+  if (tid == 0 && (sbase & 1023)) __trap();                 // the swizzle pattern assumes 1024-byte aligned tiles
+  const int S = cfg.S, NS = cfg.NS, KB = cfg.KB, d = a.d;
   const int slice = blockIdx.x % S, group = blockIdx.x / S;
+  const uint32_t btile = (uint32_t)N * 128u;                // one (variant, K-block) tile of the slice
+  const uint32_t xkblk = T2_BM * 128u;                      // one K-block of a staged X tile
+  const uint32_t stage_bytes = (uint32_t)KB * xkblk;
+  float* cn_s = reinterpret_cast<float*>(smem + cfg.off_cn);            // [N] ||c||^2 of the slice (padded: 3e38)
+  float* xn_s = reinterpret_cast<float*>(smem + cfg.off_xn) + wgi * 2 * T2_BM;   // [2][T2_BM] halves of ||x||^2
+
+  // ---------------- setup: the slice's B tiles and ||c||^2 ----------------
+  {
+    const int rq = KB * 8;                                  // 16-byte chunks per pack row ([kp2][KB * 64] bf16)
+    const uint4* ghi = reinterpret_cast<const uint4*>(a.pack + a.L.off_b2hi);
+    const uint4* glo = reinterpret_cast<const uint4*>(a.pack + a.L.off_b2lo);
+    for (int i = tid; i < 2 * KB * N * 8; i += T2_THREADS) {
+      const int v = i / (KB * N * 8), rem = i - v * (KB * N * 8);
+      const int kb = rem / (N * 8), r = (rem - kb * N * 8) >> 3, q = rem & 7;
+      uint4 val = make_uint4(0u, 0u, 0u, 0u);
+      if (r < NS) val = (v ? glo : ghi)[(size_t)(slice * NS + r) * rq + kb * 8 + q];
+      *reinterpret_cast<uint4*>(smem + cfg.off_b + (uint32_t)(v * KB + kb) * btile + wg::sw128_chunk(r, q)) = val;
+    }
+    // ||c_j||^2 from the pack's exact 3-way split [hi, mid, lo] (hi + mid + lo == the fp32 value)
+    const float* bcn = reinterpret_cast<const float*>(a.pack + a.L.off_bcn2);
+    for (int j = tid; j < N; j += T2_THREADS) {
+      float v = 3.0e38f;
+      if (j < NS) { const int jg = slice * NS + j; const float* p = bcn + (jg >> 3) * 64 + (jg & 7) * 4; v = (p[0] + p[1]) + p[2]; }
+      cn_s[j] = v;
+    }
+    wg::fence_proxy_async();                                 // generic-proxy stores -> visible to wgmma
+  }
+  __syncthreads();
+
   const long long ntiles = (a.n + T2_BM - 1) / T2_BM;
   const long long my_tiles = group < ntiles ? (ntiles - group + cfg.G - 1) / cfg.G : 0;
-  const uint32_t stage_bytes = (uint32_t)KB * T2_BM * 128u;
-  const uint32_t btile = (uint32_t)NS * 128u;            // one (variant, K-block) tile of the slice
-
-  // ---------------- setup ----------------
-  if (warp == 0 && lane == 0) {
-    tmap_prefetch(&tm_x); tmap_prefetch(&tm_bhi); tmap_prefetch(&tm_blo);
-    mbar_init(BAR(T2_B_FULL), 1);
-    for (int s = 0; s < T2_NSTMAX; ++s) { mbar_init(BAR(T2_X_FULL + s), 1); mbar_init(BAR(T2_X_EMPTY + s), 1 + 128); }
-    for (int b = 0; b < 2; ++b) { mbar_init(BAR(T2_ACC_FULL + b), 1); mbar_init(BAR(T2_ACC_EMPTY + b), 128); }
-    for (int q = 0; q < 8; ++q) mbar_init(BAR(T2_XN_FULL + q), 128);
-    mbar_fence_init();
-  }
-  if (warp == 0) tc_alloc(smem_u32(tptr_s), 512);
-  {
-    // ||c||^2 of this slice as a tf32 operand tile (rows [hi, mid, lo, 0..], no-swizzle K-major) and the constant
-    // [1,1,1,0..] A tile it is multiplied with: plain stores + proxy fence
-    const float4* g = reinterpret_cast<const float4*>(a.pack + a.L.off_bcn2) + (size_t)slice * NS * 2;
-    float4* sdst = reinterpret_cast<float4*>(smem + cfg.off_bcn);
-    for (int i = tid; i < NS * 2; i += T2_THREADS) sdst[i] = g[i];
-    float4* odst = reinterpret_cast<float4*>(smem + cfg.off_ones);
-    for (int i = tid; i < T2_BM * 2; i += T2_THREADS)
-      odst[i] = ((i >> 3) & 1) ? make_float4(0.f, 0.f, 0.f, 0.f) : make_float4(1.f, 1.f, 1.f, 0.f);
-    fence_proxy_async();
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tptr_s;
-
-  if (warp == 0) {
-    // =========================== TMA producer ===========================
-    if (lane == 0) {
-      mbar_expect_tx(BAR(T2_B_FULL), 2u * (uint32_t)KB * btile);
-      for (int kb = 0; kb < KB; ++kb) {
-        tma_load_2d(sbase + cfg.off_b + (uint32_t)(0 * KB + kb) * btile, &tm_bhi, BAR(T2_B_FULL), kb * 64, slice * NS);
-        tma_load_2d(sbase + cfg.off_b + (uint32_t)(1 * KB + kb) * btile, &tm_blo, BAR(T2_B_FULL), kb * 64, slice * NS);
-      }
-#pragma unroll 1
-      for (long long it = 0; it < my_tiles; ++it) {
-        const int stage = (int)(it % NST);
-        const long long tile = group + it * cfg.G;
-        T2_WAIT(BAR(T2_X_EMPTY + stage), (uint32_t)(((it / NST) & 1) ^ 1));
-        if (*abort_w) break;
-        mbar_expect_tx(BAR(T2_X_FULL + stage), stage_bytes);
-        for (int kb = 0; kb < KB; ++kb)
-          tma_load_2d(sbase + cfg.off_x + (uint32_t)stage * stage_bytes + (uint32_t)kb * (T2_BM * 128u), &tm_x,
-                      BAR(T2_X_FULL + stage), kb * 64, (int)(tile * T2_BM));
+  const long long npairs = (my_tiles + 1) / 2;              // warpgroup w takes the group's tiles 2p + w
+  const __nv_bfloat16* X = reinterpret_cast<const __nv_bfloat16*>(a.X);
+  const uint32_t xs_u32 = sbase + cfg.off_x + (uint32_t)wgi * 2u * stage_bytes;
+  const int nq = KB * 8;
+  auto load_tile = [&](long long p, int stage) {
+    const long long lt = 2 * p + wgi;
+    if (lt < my_tiles) {
+      const long long row0 = (group + lt * cfg.G) * T2_BM;
+      for (int i = t; i < T2_BM * nq; i += 128) {
+        const int r = i / nq, rem = i - r * nq, kb = rem >> 3, q = rem & 7;
+        const int col = kb * 64 + q * 8;
+        const long long row = row0 + r;
+        const int bytes = (row < a.n && col < d) ? min(16, (d - col) * 2) : 0;
+        wg::cp16(xs_u32 + (uint32_t)stage * stage_bytes + (uint32_t)kb * xkblk + wg::sw128_chunk(r, q),
+                 bytes ? X + row * a.ldx + col : X, bytes);
       }
     }
-  } else if (warp == 1) {
-    // =========================== MMA issuer ===========================
-    const bool leader = elect_one();
-    T2_WAIT(BAR(T2_B_FULL), 0u);
-    tc_fence_after();
-    const uint32_t idesc = idesc_m128(NS, /*A: bf16*/ 1, /*B: bf16*/ 1);
-    const uint32_t idesc_n = idesc_m128(NS, 2, 2);                       // tf32 x tf32: the ||c||^2 K-step
-    const uint64_t dcn = desc_noswz32(sbase + cfg.off_bcn);
-    const uint64_t dones = desc_noswz32(sbase + cfg.off_ones);
-    const uint64_t dbh0 = desc_sw128(sbase + cfg.off_b);
-    const uint64_t dbl0 = desc_sw128(sbase + cfg.off_b + (uint32_t)KB * btile);
+    wg::cp_commit();
+  };
+
+  const int rA = wq * 16 + (lane >> 2);                      // this thread's accumulator rows: rA, rA + 8
+  const uint64_t db0 = wg::desc_sw128(sbase + cfg.off_b);
+  const float cnmax = (float)reinterpret_cast<const PackHeader*>(a.pack)->cn_max;
+
+  load_tile(0, 0);
 #pragma unroll 1
-    for (long long it = 0; it < my_tiles; ++it) {
-      const int stage = (int)(it % NST), buf = (int)(it & 1);
-      T2_WAIT(BAR(T2_X_FULL + stage), (uint32_t)((it / NST) & 1));
-      T2_WAIT(BAR(T2_ACC_EMPTY + buf), (uint32_t)(((it >> 1) & 1) ^ 1));
-      tc_fence_after();
-      if (leader) {
-        const uint32_t d_t = tmem + (uint32_t)buf * 256u;
-        const uint64_t da0 = desc_sw128(sbase + cfg.off_x + (uint32_t)stage * stage_bytes);
-        uint32_t acc = 0u;
-#pragma unroll 1
-        for (int ks = 0; ks < cfg.KS; ++ks) {
-          const int kb = ks >> 2, kq = ks & 3;
-          // K-block kb: A tile 16 KB further, B tile `btile` further; K-step kq: 32 bytes inside the swizzle atom
-          const uint64_t da = da0 + (uint64_t)((kb * (T2_BM * 128) + kq * 32) >> 4);
-          const uint64_t boff = (uint64_t)(((uint32_t)kb * btile + (uint32_t)kq * 32u) >> 4);
-          mma_f16_ss(d_t, da, dbh0 + boff, idesc, acc);
-          acc = 1u;
-          mma_f16_ss(d_t, da, dbl0 + boff, idesc, 1u);
-        }
-        mma_tf32_ss(d_t, dones, dcn, idesc_n, 1u);                        // + ||c_j||^2
-        tc_commit(BAR(T2_ACC_FULL + buf));
-        tc_commit(BAR(T2_X_EMPTY + stage));
-      }
-      __syncwarp();
-    }
-  } else if (warp >= 4 && warp < 8) {
-    // =========================== row norms ===========================
-    const int r = (warp & 3) * 32 + lane;
-    float* xn_s = reinterpret_cast<float*>(smem + cfg.off_xn);         // [8][128]
-#pragma unroll 1
-    for (long long it = 0; it < my_tiles; ++it) {
-      const int stage = (int)(it % NST);
-      T2_WAIT(BAR(T2_X_FULL + stage), (uint32_t)((it / NST) & 1));
-      const unsigned char* xs = smem + cfg.off_x + (size_t)stage * stage_bytes;
-      float sq[4] = {0.f, 0.f, 0.f, 0.f};                  // four independent chains
-#pragma unroll 1
-      for (int kb = 0; kb < KB; ++kb) {
+  for (long long p = 0; p < npairs; ++p) {
+    const int stage = (int)(p & 1);
+    load_tile(p + 1, stage ^ 1);
+    wg::cp_wait1();
+    wg::wg_sync(1 + wgi);                                    // tile p is in shared memory (every thread's copies)
+    const long long lt = 2 * p + wgi;
+    if (lt < my_tiles) {
+      const long long row0 = (group + lt * cfg.G) * T2_BM;
+      const uint32_t xs = xs_u32 + (uint32_t)stage * stage_bytes;
+      // ---- acc = X . Bhi^T + X . Blo^T ----
+      float acc[N / 2];
 #pragma unroll
-        for (int q = 0; q < 8; ++q) {
-          const uint4 t = *reinterpret_cast<const uint4*>(xs + kb * (T2_BM * 128) + sw128_chunk(r, q));
-          const uint32_t w[4] = {t.x, t.y, t.z, t.w};
+      for (int i = 0; i < N / 2; ++i) acc[i] = 0.f;
+      wg::fence();
+#pragma unroll 1
+      for (int ks = 0; ks < cfg.KS; ++ks) {
+        // K-block kb: A tile 8 KB further, B tile `btile` further; K-step kq: 32 bytes inside the swizzle atom
+        const int kb = ks >> 2, kq = ks & 3;
+        const uint64_t da = wg::desc_sw128(xs + (uint32_t)kb * xkblk) + (uint64_t)(2 * kq);
+        const uint64_t boff = (uint64_t)(((uint32_t)kb * btile) >> 4) + (uint64_t)(2 * kq);
+        wg::Mma<N>::ss_bf16(acc, da, db0 + boff, ks > 0);
+        wg::Mma<N>::ss_bf16(acc, da, db0 + (uint64_t)(((uint32_t)KB * btile) >> 4) + boff, 1);
+      }
+      wg::commit();
+      // ---- row norms ||x||^2 while the MMAs run: thread (row r, half of the 16-byte chunks) ----
+      {
+        const int r = t & 63, part = t >> 6;
+        float s0 = 0.f, s1 = 0.f;
+        for (int j = part; j < nq; j += 2) {
+          const uint4 v = *reinterpret_cast<const uint4*>(smem + (xs - sbase) + (uint32_t)(j >> 3) * xkblk + wg::sw128_chunk(r, j & 7));
+          const uint32_t w[4] = {v.x, v.y, v.z, v.w};
 #pragma unroll
           for (int e = 0; e < 4; ++e) {
-            // two bf16 per word: the low half is element 2e, the high half element 2e + 1
+            // two bf16 per word: the low half is the lower element
             const float lo = __uint_as_float(w[e] << 16), hi = __uint_as_float(w[e] & 0xffff0000u);
-            sq[(q & 1) * 2] = fmaf(lo, lo, sq[(q & 1) * 2]);
-            sq[(q & 1) * 2 + 1] = fmaf(hi, hi, sq[(q & 1) * 2 + 1]);
+            s0 = fmaf(lo, lo, s0);
+            s1 = fmaf(hi, hi, s1);
           }
         }
+        xn_s[part * T2_BM + r] = s0 + s1;
       }
-      xn_s[(it & 7) * T2_BM + r] = (sq[0] + sq[1]) + (sq[2] + sq[3]);
-      mbar_arrive(BAR(T2_X_EMPTY + stage));
-      mbar_arrive(BAR(T2_XN_FULL + (it & 7)));             // release: publishes xn_s
-    }
-  } else if (warp >= 8) {
-    // =========================== epilogue ===========================
-    const int set = (warp - 8) >> 2;
-    const int q4 = warp & 3;
-    const int r = q4 * 32 + lane;
-    const uint32_t lane_addr = (uint32_t)(q4 * 32) << 16;
-    const PackHeader* hdr = reinterpret_cast<const PackHeader*>(a.pack);
-    const float cnmax = (float)hdr->cn_max;
-    const float* xn_s = reinterpret_cast<const float*>(smem + cfg.off_xn);
-    const float one = __uint_as_float(0x3f800000u + ((uint32_t)a.k >> 30));       // 1.0f / -0.0f, opaque to the compiler
-    const float nzero = __uint_as_float(0x80000000u + ((uint32_t)a.k >> 30));
-    const int nch = NS >> 4;
-#pragma unroll 1
-    for (long long it = set; it < my_tiles; it += 2) {
-      const long long tile = group + it * cfg.G;
-      T2_WAIT(BAR(T2_XN_FULL + (it & 7)), (uint32_t)((it >> 3) & 1));
-      const float xn = xn_s[(it & 7) * T2_BM + r];
-      const float bound = a.tau * (xn + cnmax);                // the accumulator holds ||c||^2 - 2 x.c
-      const bool out_of_range = !(xn < 3.0e38f);
-      float m1 = CUDART_INF_F, m2 = CUDART_INF_F, sb = 0.f;
-      float sv[16];
-#pragma unroll
-      for (int i = 0; i < 16; ++i) sv[i] = CUDART_INF_F;
-#define T2_PMOV8(SV, V, o, B)                                                                          \
-  asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %16, 0;\n"                                            \
-               "@p fma.rn.f32 %0, %8, %17, %18;\n@p fma.rn.f32 %1, %9, %17, %18;\n"                     \
-               "@p fma.rn.f32 %2, %10, %17, %18;\n@p fma.rn.f32 %3, %11, %17, %18;\n"                   \
-               "@p fma.rn.f32 %4, %12, %17, %18;\n@p fma.rn.f32 %5, %13, %17, %18;\n"                   \
-               "@p fma.rn.f32 %6, %14, %17, %18;\n@p fma.rn.f32 %7, %15, %17, %18;\n}"                  \
-               : "+f"(SV[o + 0]), "+f"(SV[o + 1]), "+f"(SV[o + 2]), "+f"(SV[o + 3]), "+f"(SV[o + 4]),  \
-                 "+f"(SV[o + 5]), "+f"(SV[o + 6]), "+f"(SV[o + 7])                                     \
-               : "f"(__uint_as_float(V[o + 0])), "f"(__uint_as_float(V[o + 1])),                       \
-                 "f"(__uint_as_float(V[o + 2])), "f"(__uint_as_float(V[o + 3])),                       \
-                 "f"(__uint_as_float(V[o + 4])), "f"(__uint_as_float(V[o + 5])),                       \
-                 "f"(__uint_as_float(V[o + 6])), "f"(__uint_as_float(V[o + 7])), "r"((int)(B)),        \
-                 "f"(one), "f"(nzero));
-#define T2_EPI_CHUNK(V, COLBASE)                                                         \
-  {                                                                                      \
-    const float t0 = fmin3(__uint_as_float(V[0]), __uint_as_float(V[1]), __uint_as_float(V[2]));    \
-    const float t1 = fmin3(__uint_as_float(V[3]), __uint_as_float(V[4]), __uint_as_float(V[5]));    \
-    const float t2 = fmin3(__uint_as_float(V[6]), __uint_as_float(V[7]), __uint_as_float(V[8]));    \
-    const float t3 = fmin3(__uint_as_float(V[9]), __uint_as_float(V[10]), __uint_as_float(V[11]));  \
-    const float t4 = fmin3(__uint_as_float(V[12]), __uint_as_float(V[13]), __uint_as_float(V[14])); \
-    const float cm = fminf(fmin3(t0, t1, t2), fmin3(t3, t4, __uint_as_float(V[15])));    \
-    const bool better = cm < m1;                                                         \
-    m2 = fminf(m2, fmaxf(m1, cm));                                                       \
-    m1 = fminf(m1, cm);                                                                  \
-    T2_PMOV8(sv, V, 0, better) T2_PMOV8(sv, V, 8, better)                                \
-    sb = better ? (float)(COLBASE) : sb;                                                 \
-  }
-      const int buf = set;
-      T2_WAIT(BAR(T2_ACC_FULL + buf), (uint32_t)((it >> 1) & 1));
-      tc_fence_after();
-      const uint32_t tbase = tmem + lane_addr + (uint32_t)buf * 256u;
-      uint32_t v0[16], v1[16];
-      BKM_TC_LD16(tbase, v0);
-#pragma unroll 1
-      for (int c = 0; c < nch; c += 2) {
-        tc_wait_ld();
-        if (c + 1 < nch) BKM_TC_LD16(tbase + (uint32_t)(c + 1) * 16u, v1);
-        T2_EPI_CHUNK(v0, c * 16)
-        if (c + 1 < nch) {
-          tc_wait_ld();
-          if (c + 2 < nch) BKM_TC_LD16(tbase + (uint32_t)(c + 2) * 16u, v0);
-          T2_EPI_CHUNK(v1, (c + 1) * 16)
-        }
-      }
-      tc_fence_before();
-      mbar_arrive(BAR(T2_ACC_EMPTY + buf));
-#undef T2_EPI_CHUNK
-      const float thr = m1 + bound;
-      float p0 = 0.f, p1 = 0.f;
-#pragma unroll
-      for (int i = 0; i < 16; i += 2) {
-        p0 = fmaf(sv[i] <= thr ? 1.f : 0.f, 1.f + (float)i * 0.0009765625f, p0);
-        p1 = fmaf(sv[i + 1] <= thr ? 1.f : 0.f, 1.f + (float)(i + 1) * 0.0009765625f, p1);
-      }
-      const float hits = p0 + p1;
-      const bool tie = !(hits >= 1.f && hits < 2.f) || !(m2 > thr) || out_of_range;
-      const int bj = slice * NS + (tie ? 0 : (int)(sb + (hits - 1.f) * 1024.f + 0.5f));
-      const long long row = tile * T2_BM + r;
-      if (row < a.n) {
-        if (S == 1) {
-          const bool flagged = tie && a.k > 1;
-          if (!flagged) {
-            if (a.labels) a.labels[row] = bj;
-          } else {
-            const int slot = atomicAdd(a.defer_cnt, 1);
-            a.defer_idx[slot] = (int)row;
-          }
-        } else {
-          // partial record of this (slice, row): slice minimum, label or -1 (near-tie inside the slice), ||x||^2
-          a.rec[(size_t)slice * a.n + row] = make_float4(m1, m2, __int_as_float(tie ? -1 : bj), xn);
-        }
-      }
-    }
-  }
+      wg::wait_all();
+      wg::pin(acc);
+      wg::wg_sync(1 + wgi);                                  // xn_s complete
 
-  // ---------------- teardown ----------------
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  if (warp == 0) {
-    __syncwarp();
-    tc_dealloc(tmem, 512);
+      // ---- arg-min, near-tie test (bound = tau (||x||^2 + max ||c||^2): the accumulator holds ||c||^2 - 2 x.c) ----
+      wg::Best2 b0, b1;
+      wg::tile_best2<N>(acc, cn_s, lane, b0, b1);
+      if ((lane & 3) == 0) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const wg::Best2 b = h ? b1 : b0;
+          const int r = rA + 8 * h;
+          const long long row = row0 + r;
+          if (row >= a.n) continue;
+          const float xn = xn_s[r] + xn_s[T2_BM + r];
+          const bool out_of_range = !(xn < 3.0e38f);
+          const bool tie = !(b.m2 > b.m1 + a.tau * (xn + cnmax)) || out_of_range;
+          const int bj = slice * NS + ((tie || b.j >= NS) ? 0 : b.j);
+          if (S == 1) {
+            if (!(tie && a.k > 1)) {
+              if (a.labels) a.labels[row] = bj;
+            } else {
+              const int slot = atomicAdd(a.defer_cnt, 1);
+              a.defer_idx[slot] = (int)row;
+            }
+          } else {
+            // partial record of this (slice, row): slice minimum, label or -1 (near-tie inside the slice), ||x||^2
+            a.rec[(size_t)slice * a.n + row] = make_float4(b.m1, b.m2, __int_as_float(tie ? -1 : bj), xn);
+          }
+        }
+      }
+    }
+    wg::wg_sync(1 + wgi);                                    // the stage and xn_s may be refilled
   }
-#undef BAR
 }
 
 // ------------------------------------------------------------------------------------------
@@ -430,60 +303,28 @@ tc2_recheck_kernel(ChunkArgs a, int kp2) {
   }
 }
 
-// ------------------------------------------------------------------------------------ host
-typedef CUresult (*EncodeTiledFn2)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                   const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                   CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-static EncodeTiledFn2 get_encode2() {
-  static std::atomic<EncodeTiledFn2> fn{nullptr};
-  EncodeTiledFn2 f = fn.load();
-  if (!f) {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess &&
-        q == cudaDriverEntryPointSuccess) {
-      f = (EncodeTiledFn2)p;
-      fn.store(f);
-    }
-  }
-  return f;
-}
-// [rows][cols] 16-bit tensor, row pitch in elements; box = 64 columns (one 128-byte swizzle atom) x box_rows
-static int make_map16(CUtensorMap* tm, const void* base, long long rows, int cols, long long pitch_elems, int box_rows,
-                      bool bf16) {
-  EncodeTiledFn2 enc = get_encode2();
-  if (!enc) return BKM_EUNSUPPORTED;
-  cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
-  cuuint64_t strides[1] = {(cuuint64_t)pitch_elems * 2};
-  cuuint32_t box[2] = {64u, (cuuint32_t)box_rows};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult r = enc(tm, bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2,
-                   const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  return r == CUDA_SUCCESS ? 0 : BKM_EUNSUPPORTED;
-}
 
+// ------------------------------------------------------------------------------------ host
 static bool make_cfg2(int d, int k, int sm_count, Tc2Cfg* c) {
   const Tc2Geom g = tc2_geom(k, d);
   c->S = g.S; c->NS = g.NS; c->KB = g.KB; c->KS = (d + 15) / 16;
   if (g.S > sm_count) return false;
   c->G = sm_count / g.S;
-  const uint32_t bbytes = 2u * (uint32_t)g.KB * (uint32_t)g.NS * 128u;
-  for (int nst = T2_NSTMAX; nst >= 2; --nst) {
-    uint32_t o = 0;
-    c->off_b = o; o += bbytes;
-    c->off_bcn = o; o += (uint32_t)g.NS * 32u;
-    c->off_ones = o; o += T2_BM * 32u;
-    o = (uint32_t)align_up(o, 1024);
-    c->off_x = o; o += (uint32_t)nst * g.KB * T2_BM * 128u;
-    c->off_xn = o; o += 8 * T2_BM * 4;
-    c->off_bar = o; o += T2_BAR_COUNT * 8;
-    c->off_tptr = o; o += 16;
-    c->total = o;
-    c->NST = nst;
-    if (o <= 227 * 1024) return true;
-  }
-  return false;
+  const uint32_t N = (uint32_t)wg::mma_n(g.NS);
+  uint32_t o = 0;
+  c->off_b = o; o += 2u * (uint32_t)g.KB * N * 128u;                 // (hi, lo) x K-blocks of the slice
+  c->off_x = o; o += 2u * 2u * (uint32_t)g.KB * T2_BM * 128u;        // 2 warpgroups x 2 stages
+  c->off_cn = o; o += N * 4u;
+  c->off_xn = o; o += 2u * 2u * T2_BM * 4u;
+  c->total = o;
+  return o <= 227u * 1024u;
+}
+
+template <int N>
+static int launch_assign(const ChunkArgs& a, const Tc2Cfg& cfg, cudaStream_t s) {
+  BKM_CUDA_TRY(cudaFuncSetAttribute(tc2_assign_kernel<N>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cfg.total));
+  tc2_assign_kernel<N><<<cfg.G * cfg.S, T2_THREADS, cfg.total, s>>>(a, cfg);
+  return 0;
 }
 
 // E-step of one chunk on the large-shape tensor path; the M-step / distances follow as row passes (bkm_rowpass.cu).
@@ -491,25 +332,23 @@ static bool make_cfg2(int d, int k, int sm_count, Tc2Cfg* c) {
 int launch_tc2(const ChunkArgs& a0, bool mstep, int sm_count, int* grid_out, cudaStream_t s) {
   ChunkArgs a = a0;
   if (!tc2_shape(a.d, a.k, BKM_BF16)) return BKM_EUNSUPPORTED;
-  if ((reinterpret_cast<uintptr_t>(a.X) & 15) || (a.ldx % 8)) return BKM_EALIGN;     // TMA: 16-byte rows
+  if ((reinterpret_cast<uintptr_t>(a.X) & 15) || (a.ldx % 8)) return BKM_EALIGN;     // 16-byte staging copies
   Tc2Cfg cfg;
   if (!make_cfg2(a.d, a.k, sm_count, &cfg)) return BKM_EUNSUPPORTED;
   const Tc2Geom g = tc2_geom(a.k, a.d);
-  CUtensorMap tm_x, tm_bhi, tm_blo;
-  int rc = make_map16(&tm_x, a.X, a.n, a.d, a.ldx, T2_BM, true);
-  if (rc) return rc;
-  rc = make_map16(&tm_bhi, a.pack + a.L.off_b2hi, g.kp2, g.dk2, g.dk2, g.NS, true);
-  if (rc) return rc;
-  rc = make_map16(&tm_blo, a.pack + a.L.off_b2lo, g.kp2, g.dk2, g.dk2, g.NS, true);
-  if (rc) return rc;
   const long long ntiles = (a.n + T2_BM - 1) / T2_BM;
-  int G = cfg.G;
-  if (ntiles < G) G = (int)ntiles;
-  if (G < 1) G = 1;
-  cfg.G = G;
+  if (ntiles < cfg.G) cfg.G = (int)ntiles;
+  if (cfg.G < 1) cfg.G = 1;
   BKM_CUDA_TRY(cudaMemsetAsync(a.defer_cnt, 0, 2 * sizeof(int), s));          // [0] deferred rows, [1] abort word
-  BKM_CUDA_TRY(cudaFuncSetAttribute(tc2_assign_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cfg.total));
-  tc2_assign_kernel<<<G * cfg.S, T2_THREADS, cfg.total, s>>>(a, cfg, tm_x, tm_bhi, tm_blo);
+  int rc;
+  switch (wg::mma_n(cfg.NS)) {
+    case 16: rc = launch_assign<16>(a, cfg, s); break;
+    case 32: rc = launch_assign<32>(a, cfg, s); break;
+    case 64: rc = launch_assign<64>(a, cfg, s); break;
+    case 128: rc = launch_assign<128>(a, cfg, s); break;
+    default: rc = launch_assign<256>(a, cfg, s); break;
+  }
+  if (rc) return rc;
   note_launch(2);
   BKM_CUDA_TRY(cudaGetLastError());
   if (cfg.S > 1) {

@@ -167,7 +167,7 @@ def _p2p_state(comm):
 
 
 class CudaBackend(object):
-    """Calls the sm_100a kernels through the C ABI.  Fails loudly without a GPU/library."""
+    """Calls the sm_90a kernels through the C ABI.  Fails loudly without a GPU/library."""
 
     name = "b200"
     supports_bf16 = True          # bfloat16 rows: large-shape tensor path (bkm_tc2.cu), d <= 128
@@ -175,7 +175,7 @@ class CudaBackend(object):
     def __init__(self, device=None, flags=0):
         if not torch.cuda.is_available():
             raise RuntimeError(
-                "dask_ml_b200 needs a CUDA device: the KMeans hot path is sm_100a CUDA only "
+                "dask_ml_b200 needs a CUDA device: the KMeans hot path is sm_90a CUDA only "
                 "and has no CPU fallback."
             )
         self.lib = _lib.load()
@@ -227,7 +227,7 @@ class CudaBackend(object):
             if first:
                 import warnings
                 warnings.warn("dask_ml_b200: a chunk with shape %s, row pitch %d elements, base address %% 16 = %d is not "
-                              "16-byte aligned; the generic CUDA-core kernel is used instead of the tcgen05 / streaming "
+                              "16-byte aligned; the generic CUDA-core kernel is used instead of the tensor-core / streaming "
                               "kernel (pass the data through CudaBackend.to_device, which pads the row pitch)"
                               % (tuple(x.shape), x.stride(0), x.data_ptr() % 16), RuntimeWarning, stacklevel=3)
 

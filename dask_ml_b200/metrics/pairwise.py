@@ -32,7 +32,7 @@ def pairwise_distances_argmin_min(X, Y, axis=1, metric="euclidean", batch_size=N
     if type(Y).__module__.startswith("dask"):
         raise TypeError("`Y` must be a numpy array")
     if metric not in ("euclidean", "sqeuclidean", "l2"):
-        raise NotImplementedError("only the euclidean metric is on the B200 KMeans path, got %r" % (metric,))
+        raise NotImplementedError("only the euclidean metric is on the GPU KMeans path, got %r" % (metric,))
     if axis != 1:
         raise NotImplementedError("axis must be 1")
     squared = bool((metric_kwargs or {}).get("squared", False)) or metric == "sqeuclidean"
@@ -54,7 +54,7 @@ def pairwise_distances(X, Y, metric="euclidean", n_jobs=None, **kwargs):
     if type(Y).__module__.startswith("dask"):
         raise TypeError("`Y` must be a numpy array")
     if metric != "euclidean":
-        raise NotImplementedError("only the euclidean metric is on the B200 KMeans path, got %r" % (metric,))
+        raise NotImplementedError("only the euclidean metric is on the GPU KMeans path, got %r" % (metric,))
     return euclidean_distances(X, Y)
 
 
@@ -194,5 +194,5 @@ def pairwise_kernels(X, Y=None, metric="linear", filter_params=False, n_jobs=1, 
             kwds = dict((k, kwds[k]) for k in kwds if k in ("gamma",))
         return rbf_kernel(X, Y, **kwds)
     if metric in ("linear", "polynomial", "sigmoid"):
-        raise NotImplementedError("kernel %r is outside the KMeans hot path of the B200 engine" % metric)
+        raise NotImplementedError("kernel %r is outside the KMeans hot path of the GPU engine" % metric)
     raise ValueError("Unknown kernel %r" % metric)

@@ -1,5 +1,5 @@
 /*
- * bkm_b200.h — C ABI of the B200-native KMeans hot path (libbkm_b200.so).
+ * bkm_b200.h — C ABI of the GPU-native KMeans hot path (libbkm_b200.so; built for H100, sm_90a).
  *
  * This is the drop-in boundary for the per-chunk operators that the reference
  * (mrocklin/dask-ml) invokes from its task graph.  dask-ml has no FFI layer of its
@@ -56,7 +56,7 @@ extern "C" {
 #define BKM_EALIGN       -5   /* pointer alignment requirement violated */
 
 /* flags */
-#define BKM_FLAG_FORCE_SIMT   1   /* never use the tcgen05 path (exact-fp32 CUDA-core kernel) */
+#define BKM_FLAG_FORCE_SIMT   1   /* never use the tensor-core path (exact-fp32 CUDA-core kernel) */
 #define BKM_FLAG_FORCE_TC     2   /* fail with BKM_EUNSUPPORTED instead of falling back to SIMT */
 #define BKM_FLAG_NO_RECHECK   4   /* skip the float64 re-check of near-tie rows */
 #define BKM_FLAG_FIRST_CHUNK  8   /* bkm_lloyd_chunk: OVERWRITE sums / counts / inertia (first chunk of an iteration)
@@ -71,7 +71,7 @@ const char* bkm_error_string(int code);
 int bkm_device_info(int device, int* sm_count, int* cc_major, int* cc_minor);
 
 /* Which kernel family a (d, k, dtype, flags) problem dispatches to:
- * 0 = generic CUDA-core kernel (any d/k, fp32/fp64), 1 = tcgen05 tensor-core path (split-fp16 x3 product, fp32
+ * 0 = generic CUDA-core kernel (any d/k, fp32/fp64), 1 = wgmma tensor-core path (split-fp16 x3 product, fp32
  * accumulate; d <= 64, k <= 256), 2 = streaming CUDA-core kernel for tiny k*d (HBM-bound shapes: d <= 16, k <= 32).
  * <0 = error. */
 int bkm_kernel_family(int d, int k, int x_dtype, int flags);
@@ -80,7 +80,7 @@ int bkm_kernel_family(int d, int k, int x_dtype, int flags);
  * Kernels read the centres from an opaque "pack" built on the device from the float64
  * centres (the reference keeps centres in float64 from iteration 2 on: k_means.py:551-552).
  * The pack holds the layouts each kernel family wants (padded fp32/fp64 rows and ||c||^2 for
- * the CUDA-core kernels; -2c split into tf32 hi/lo operand tiles for tcgen05) plus the
+ * the CUDA-core kernels; -2sc split into fp16 hi/lo operand tiles for the tensor cores) plus the
  * float64 originals used by the near-tie re-check. */
 int bkm_centers_pack_bytes(int k, int d, int x_dtype, size_t* out);
 int bkm_pack_centers(const double* centers64, int k, int d, int x_dtype,
@@ -139,7 +139,7 @@ int bkm_min_fold_chunk(void* run_min, const void* new_min, int64_t n, int x_dtyp
  *                     metrics.rbf_kernel(X, Y, gamma) = exp(-gamma * d^2)  pairwise.py:131-139
  *   out [n][ld_out] x-dtype, row-major, ld_out >= k (so that callers can fill column blocks of a wider matrix):
  *   mode 0: sqrt(max(||x||^2 - 2 x.c + ||c||^2, 0))   mode 1: the squared distance   mode 2: exp(-gamma * d^2)
- * fp32 with d <= 64, k <= 256 runs on the tcgen05 pipeline (transform epilogue); other shapes on the CUDA cores. */
+ * fp32 with d <= 64, k <= 256 runs on the tensor-core kernel (transform epilogue); other shapes on the CUDA cores. */
 int bkm_transform_chunk(const void* X, int64_t n, int d, int64_t ldx, int x_dtype,
                         const void* pack, int k, void* out, int64_t ld_out, int mode, double gamma, int flags,
                         void* stream);
@@ -201,22 +201,22 @@ int bkm_allreduce_p2p(double* buf, int64_t n, void* const* mailboxes_dev, int ra
 
 /* Number of kernel launches this library has enqueued since load (for bench accounting). */
 int64_t bkm_launch_count(void);
-/* Number of chunk calls whose shape belongs to the tcgen05 / streaming family but whose rows were not 16-byte aligned
+/* Number of chunk calls whose shape belongs to the tensor-core / streaming family but whose rows were not 16-byte aligned
  * (base or pitch), so that the generic CUDA-core kernel ran instead: correct, several times slower.  The Python host
  * warns once when this moves. */
 int64_t bkm_debug_fallback_count(void);
 
-/* Debug: nonzero once a pipeline wait inside the tcgen05 kernel has timed out (the kernel then drains
+/* Debug: nonzero once a pipeline wait inside a tensor-core kernel has timed out (the kernel then drains
  * instead of hanging); encodes barrier / parity / warp.  Synchronises the device. */
 unsigned int bkm_debug_abort_code(void);
 void bkm_debug_abort_detail(unsigned int* out64_host);   /* per-warp wait that timed out (64 words) */
 /* Clears the abort word once the host has reported it (the host side raises RuntimeError on a non-finite shift /
  * cost and calls this, so that one timed-out wait does not poison the process).  Synchronises the device. */
 void bkm_debug_reset(void);
-/* Number of rows the LAST tcgen05 chunk call that used `workspace` (same n, d, k, dtype) deferred to the float64
+/* Number of rows the LAST tensor-core chunk call that used `workspace` (same n, d, k, dtype) deferred to the float64
  * re-check (near-ties and out-of-range rows).  Synchronises the device; used by bench.py's parity record. */
 int bkm_debug_deferred_rows(const void* workspace, int64_t n, int d, int k, int x_dtype, int* count_host);
-/* `make TRACE=1` builds only: SM-clock timeline of CTA 0 (16 events x 128 tiles); returns words written, 0 otherwise */
+/* Pipeline timeline of the tensor-core kernel: not recorded by the sm_90a kernels; returns 0 (kept for ABI stability) */
 int bkm_debug_trace(long long* out_host, int n);
 
 #ifdef __cplusplus

@@ -1,21 +1,20 @@
 """TEST INFRASTRUCTURE — run the UNMODIFIED reference source files without dask.
 
-    python tests/golden/ref_shim.py          # regenerates tests/golden/ref_*.npz  (needs /root/reference)
+    BKM_REFERENCE=<dask-ml checkout> python tests/golden/ref_shim.py   # regenerates tests/golden/ref_*.npz
 
-The reference (mrocklin/dask-ml @ 0310a90) cannot be imported in this image: dask / distributed / toolz are
+The reference (mrocklin/dask-ml @ 0310a90) cannot be imported on a current Python stack: dask / distributed / toolz are
 absent and the 2018 code targets Python <= 3.9 / scikit-learn 0.19.  Its KMeans path, however, only uses a
 small slice of dask: row-chunked arrays that are mapped block-wise and reduced on the client.  This module
 installs an EAGER stand-in for exactly that slice (``dask``, ``dask.array``, ``dask.dataframe``) into
 ``sys.modules``, stubs the two removed scikit-learn names the reference imports, and then loads the reference's
-own files from ``/root/reference`` with importlib — ``dask_ml/utils.py``, ``dask_ml/metrics/pairwise.py``,
+own files from the checkout named by ``BKM_REFERENCE`` with importlib — ``dask_ml/utils.py``, ``dask_ml/metrics/pairwise.py``,
 ``dask_ml/cluster/k_means.py`` — byte for byte, nothing copied into this repository.  The per-chunk arithmetic
 therefore runs through the reference's own code: its graph construction (``pairwise_distances_argmin_min``,
 ``da.atop(_centers_dense, ...)``, the sequential ``sum`` of block partials, ``da.bincount``), its numba kernel
 ``_centers_dense`` and its Lloyd control flow.
 
 The outputs are written as golden fixtures (inputs + reference outputs) that tests/test_oracle.py replays
-against the oracle and tests/test_gpu_kmeans.py against the CUDA engine on the GPU box, where /root/reference
-does not exist.
+against the oracle and tests/test_gpu_kmeans.py against the CUDA engine; neither needs the reference checkout.
 """
 import collections
 import collections.abc
@@ -26,7 +25,7 @@ import types
 
 import numpy as np
 
-REF = os.environ.get("BKM_REFERENCE", "/root/reference")
+REF = os.environ.get("BKM_REFERENCE", "")
 HERE = os.path.dirname(os.path.abspath(__file__))
 
 

@@ -1,7 +1,7 @@
 """Manual probe (not collected by pytest): how wrong can the tensor path be WITHOUT the float64 re-check?
-Runs the tcgen05 kernel with BKM_FLAG_NO_RECHECK and reports, over the rows whose label differs from the float64
+Runs the tensor-core kernel with BKM_FLAG_NO_RECHECK and reports, over the rows whose label differs from the float64
 arg-min, the largest float64 margin relative to ||x||^2 + max||c||^2 — the quantity the near-tie bound tau
-(bkm_api.cu: tau_for) must dominate.  Run on the GPU box:  python tests/tau_probe.py"""
+(bkm_api.cu: tau_for) must dominate.  Run on a GPU:  python tests/tau_probe.py"""
 import sys, os
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch

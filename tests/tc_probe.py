@@ -1,5 +1,5 @@
-"""Manual probe of the tcgen05 path (not collected by pytest): accuracy of the split-fp16 product and parity
-with the oracle on a few shapes.  Run on the GPU box:  python tests/tc_probe.py"""
+"""Manual probe of the tensor-core path (not collected by pytest): accuracy of the split-fp16 product and parity
+with the oracle on a few shapes.  Run on a GPU:  python tests/tc_probe.py"""
 import sys, os
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np

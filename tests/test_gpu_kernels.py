@@ -45,7 +45,7 @@ SHAPES = [
 
 
 @pytest.mark.parametrize("n,d,k,dtype", SHAPES)
-@pytest.mark.parametrize("flags", [1, 0])      # 1 = FORCE_SIMT, 0 = auto (tcgen05 where supported)
+@pytest.mark.parametrize("flags", [1, 0])      # 1 = FORCE_SIMT, 0 = auto (tensor cores where supported)
 def test_lloyd_chunk_matches_oracle(be, oracle, n, d, k, dtype, flags):
     import torch
 
@@ -201,7 +201,7 @@ def _exact_labels_f64(x, C):
     return out, second
 
 
-# Pipeline stress of the tcgen05 kernels: row counts that leave every kind of tail (fewer tiles than SMs, one
+# Pipeline stress of the tensor-core kernels: row counts that leave every kind of tail (fewer tiles than SMs, one
 # tile more on some SMs, a partial last tile), both kernel variants (pure Lloyd = lane-owns-cluster M-step with
 # the whole-tile M ring; with distances = quarter-tile ring), one and two accumulator units.
 @pytest.mark.parametrize("n", [1, 127, 128, 129, 148 * 128 - 1, 148 * 128 * 3 + 77, 200_000, 1_000_003])

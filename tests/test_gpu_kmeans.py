@@ -193,7 +193,7 @@ def test_dtypes():
 
 def test_kmeans_parallel_init_quality(oracle):
     """k-means|| (init_scalable): with enough rounds the candidate set covers every blob, so the fit
-    reaches the same inertia as scikit-learn's (smoke-level pin, see SURVEY §8c)."""
+    reaches the same inertia as scikit-learn's (smoke-level pin: the reference's own dask draws cannot be reproduced)."""
     from dask_ml_b200 import ChunkedArray
     from dask_ml_b200.cluster import KMeans
 

@@ -66,7 +66,7 @@ def test_rbf_kernel_and_pairwise_kernels():
 @pytest.mark.parametrize("n,d,k", [(20000, 64, 256), (5001, 41, 100), (3000, 64, 300), (777, 13, 20), (100, 8, 600)])
 @pytest.mark.parametrize("mode", [0, 1, 2])
 def test_transform_tensor_path(n, d, k, mode):
-    """fp32 blocks of distances / squared distances / rbf values from the tcgen05 transform epilogue (column blocks of
+    """fp32 blocks of distances / squared distances / rbf values from the tensor-core transform epilogue (column blocks of
     256 for wider Y) against float64 on the device; error relative to ||x||^2 + ||y||^2 like the reference's own
     float32 formula (pairwise.py:93-97 cancels at that scale)."""
     import torch

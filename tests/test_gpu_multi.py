@@ -1,4 +1,4 @@
-"""N-GPU result == 1-GPU result == oracle (SURVEY Appendix B.9).  Needs >= 2 GPUs; run with -m gpu."""
+"""N-GPU result == 1-GPU result == oracle.  Needs >= 2 GPUs; run with -m gpu."""
 import os
 import subprocess
 import sys

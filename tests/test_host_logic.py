@@ -39,8 +39,8 @@ def test_library_exports_every_declared_symbol():
     assert lib.bkm_centers_pack_bytes(256, 64, 0, ctypes.byref(out)) == 0 and out.value > 256 * 64 * 4
     assert lib.bkm_workspace_bytes(1000, 64, 256, 0, ctypes.byref(out)) == 0 and out.value > 0
     assert lib.bkm_workspace_bytes(1000, 64, 256, 7, ctypes.byref(out)) == -2          # BKM_EDTYPE
-    assert lib.bkm_kernel_family(64, 256, 0, 0) == 1      # tcgen05 path
-    assert lib.bkm_kernel_family(41, 100, 0, 0) == 1      # tcgen05 too (given a 16-byte row pitch; else the launch falls back)
+    assert lib.bkm_kernel_family(64, 256, 0, 0) == 1      # tensor-core path
+    assert lib.bkm_kernel_family(41, 100, 0, 0) == 1      # tensor-core path too (given a 16-byte row pitch; else the launch falls back)
     assert lib.bkm_kernel_family(100, 100, 0, 0) == 0     # CUDA-core path: d > 64
     assert lib.bkm_kernel_family(13, 20, 0, 0) == 2       # streaming CUDA-core kernel: tiny k*d is HBM-bound
     assert lib.bkm_kernel_family(13, 20, 0, 1) == 0       # FORCE_SIMT -> the generic CUDA-core kernel

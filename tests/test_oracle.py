@@ -1,5 +1,5 @@
 """The CPU oracle pinned against the reference's own test expectations (which are run-time comparisons
-with scikit-learn — the reference holds no golden vectors, SURVEY.md §8c) and against the committed
+with scikit-learn — the reference holds no golden vectors) and against the committed
 fixtures in tests/golden/.  Runs without a GPU."""
 import json
 import os
@@ -28,7 +28,7 @@ def test_fit_given_init_equals_sklearn(oracle):
     sk = SKKMeans(3, init=init, random_state=0, n_init=1).fit(X)
     np.testing.assert_allclose(inertia, sk.inertia_, rtol=1e-12)
     np.testing.assert_array_equal(np.concatenate(lab), sk.labels_)
-    # the number SURVEY.md §7 records for this restatement
+    # the inertia this restatement reproduces on the reference's test data
     np.testing.assert_allclose(inertia, 3966.9294065453428, rtol=1e-13)
 
 
