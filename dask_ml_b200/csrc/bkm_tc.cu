@@ -15,12 +15,15 @@
 // CTA = 2 warpgroups (1 CTA per SM).  Each warpgroup owns alternate 64-row tiles of the CTA and runs, per tile:
 //   cp.async of the NEXT tile into its second stage (fp32 rows, zero-filled beyond n and d);
 //   the fp16 (hi, lo) A fragments of s X built in registers (and ||s x||^2);
-//   3 ceil(d/16) wgmma.m64nNk16 with B (= -2 s C as fp16 hi / lo, SWIZZLE_128B K-major) resident in shared memory;
-//   the arg-min epilogue from the register accumulators (best, second best, near-tie test);
+//   3 KS wgmma.m64nNk16 (KS = ceil(d/16), a template parameter so that they issue back to back) with B
+//   (= -2 s C as fp16 hi / lo, SWIZZLE_128B K-major) resident in shared memory; N = 256 runs as two column halves in
+//   two commit groups;
+//   the arg-min epilogue from the register accumulators (best, second best, near-tie test), over the first column
+//   half while the tensor cores compute the second;
 //   the winning distance in direct form (x - c)^2 in fp32, and the M-step.
 // The M-step adds the tile's rows in row order into the CTA's sums; the two warpgroups take turns (named barriers),
-// so every cluster's sum is formed in one fixed order and the sums are bit-reproducible.  One warpgroup's MMAs
-// overlap the other's epilogue / M-step.
+// so every cluster's sum is formed in one fixed order and the sums are bit-reproducible.  Inside a turn each sums
+// element has one owning thread.  One warpgroup's MMAs overlap the other's epilogue / M-step.
 #include "bkm_common.cuh"
 #include "bkm_wgmma.cuh"
 #include <cuda_fp16.h>
@@ -53,17 +56,19 @@ __device__ __forceinline__ uint32_t pack_half2(float lo, float hi) {
 
 // XFORM: the epilogue writes the whole (rows x k) block of distances / kernel values instead of the arg-min
 // (euclidean_distances, dask_ml/metrics/pairwise.py:69-97; rbf_kernel :131-139) — same MMAs, no M-step.
-template <int N, bool MSTEP, bool WANT_DIST, bool XFORM>
+template <int N, int KS, bool MSTEP, bool WANT_DIST, bool XFORM>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 tc_chunk_kernel(ChunkArgs a, TcCfg cfg) {
   if (a.skip && *a.skip) return;                            // converged loop: no-op iteration
 
   extern __shared__ __align__(1024) unsigned char smem[];
   constexpr bool HAS_M = MSTEP || WANT_DIST;
+  // N = 256: two MMA column halves of 128 (the second half's B rows start 128 x 128 bytes = 16 whole swizzle atoms on)
+  constexpr int NH = N == 256 ? 2 : 1, NC = N / NH;
   const int tid = threadIdx.x, lane = tid & 31, wgi = tid >> 7, t = tid & 127, wq = t >> 5;
   const uint32_t sbase = smem_u32(smem);
   if (tid == 0 && (sbase & 1023)) __trap();                 // the swizzle pattern assumes 1024-byte aligned tiles
-  const int KS = cfg.KS, d = a.d, k = a.k;
+  const int d = a.d, k = a.k;
   float* cn_s = reinterpret_cast<float*>(smem + cfg.off_cn);          // [N] s^2 ||c||^2 (padded columns: 3e38)
   int* cnt_s = reinterpret_cast<int*>(smem + cfg.off_cnt);            // [N]
   float* sum_s = reinterpret_cast<float*>(smem + cfg.off_sum);        // [N][64]
@@ -106,7 +111,7 @@ tc_chunk_kernel(ChunkArgs a, TcCfg cfg) {
   const uint32_t stage_bytes = TBM * XP * 4;
   const uint32_t xs_u32 = sbase + cfg.off_x + (uint32_t)wgi * 2u * stage_bytes;
   const float* xs_f = reinterpret_cast<const float*>(smem + cfg.off_x) + wgi * 2 * TBM * XP;
-  const int nq = KS * 4;                                     // 16-byte chunks per staged row
+  constexpr int nq = KS * 4;                                 // 16-byte chunks per staged row
   auto load_tile = [&](long long p, int stage) {
     const long long lt = 2 * p + wgi;
     if (lt < my_tiles) {
@@ -162,25 +167,28 @@ tc_chunk_kernel(ChunkArgs a, TcCfg cfg) {
       xn0 += __shfl_xor_sync(0xffffffffu, xn0, 1); xn0 += __shfl_xor_sync(0xffffffffu, xn0, 2);
       xn1 += __shfl_xor_sync(0xffffffffu, xn1, 1); xn1 += __shfl_xor_sync(0xffffffffu, xn1, 2);
 
-      // ---- acc = Xhi.Bhi + Xhi.Blo + Xlo.Bhi ----
+      // ---- acc = Xhi.Bhi + Xhi.Blo + Xlo.Bhi, column half by column half (NH commit groups of NC columns; the
+      //      accumulator fragment of columns [h NC, (h + 1) NC) is acc[h NC / 2 ...]) ----
       float acc[N / 2];
 #pragma unroll
       for (int i = 0; i < N / 2; ++i) acc[i] = 0.f;
       wg::fence();
 #pragma unroll
-      for (int s = 0; s < 4; ++s)
-        if (s < KS) wg::Mma<N>::rs_f16(acc, ahi[s], dbh + (uint64_t)(2 * s), s > 0);
+      for (int hf = 0; hf < NH; ++hf) {
+        float(&ah)[NC / 2] = *reinterpret_cast<float(*)[NC / 2]>(acc + hf * (NC / 2));
+        const uint64_t bh = dbh + (uint64_t)(hf * NC * 128 / 16), bl = dbl + (uint64_t)(hf * NC * 128 / 16);
 #pragma unroll
-      for (int s = 0; s < 4; ++s)
-        if (s < KS) wg::Mma<N>::rs_f16(acc, ahi[s], dbl + (uint64_t)(2 * s), 1);
+        for (int s = 0; s < KS; ++s) wg::Mma<NC>::rs_f16(ah, ahi[s], bh + (uint64_t)(2 * s), s > 0);
 #pragma unroll
-      for (int s = 0; s < 4; ++s)
-        if (s < KS) wg::Mma<N>::rs_f16(acc, alo[s], dbh + (uint64_t)(2 * s), 1);
-      wg::commit();
-      wg::wait_all();
-      wg::pin(acc);
+        for (int s = 0; s < KS; ++s) wg::Mma<NC>::rs_f16(ah, ahi[s], bl + (uint64_t)(2 * s), 1);
+#pragma unroll
+        for (int s = 0; s < KS; ++s) wg::Mma<NC>::rs_f16(ah, alo[s], bh + (uint64_t)(2 * s), 1);
+        wg::commit();
+      }
 
       if (XFORM) {
+        wg::wait_all();
+        wg::pin(acc);
         // d^2 = (acc + s^2 ||c||^2 + ||s x||^2) / s^2, clamped at 0; mode 0: sqrt, 1: squared, 2: exp(-gamma d^2)
         const float inv_s2 = 1.0f / (sc * sc);
         const bool vec_ok = ((reinterpret_cast<uintptr_t>(a.xf_out) & 7) == 0) && ((a.xf_ld & 1) == 0);
@@ -208,8 +216,23 @@ tc_chunk_kernel(ChunkArgs a, TcCfg cfg) {
         }
       } else {
         // ---- arg-min, near-tie test (bound = tau (||s x||^2 + max ||s c||^2)) ----
-        wg::Best2 b0, b1;
-        wg::tile_best2<N>(acc, cn_s, lane, b0, b1);
+        // columns still reach each thread in increasing order: the lowest column wins exact ties as before
+        wg::Best2 b0 = wg::best2_init(), b1 = b0;
+        if constexpr (NH == 2) {
+          float(&a0)[NC / 2] = *reinterpret_cast<float(*)[NC / 2]>(acc);
+          float(&a1)[NC / 2] = *reinterpret_cast<float(*)[NC / 2]>(acc + NC / 2);
+          wg::wait_1();                                      // first column half done, second still running
+          wg::pin(a0);
+          wg::best2_cols<NC>(a0, cn_s, 0, lane, b0, b1);
+          wg::wait_all();
+          wg::pin(a1);
+          wg::best2_cols<NC>(a1, cn_s, NC, lane, b0, b1);
+        } else {
+          wg::wait_all();
+          wg::pin(acc);
+          wg::best2_cols<N>(acc, cn_s, 0, lane, b0, b1);
+        }
+        wg::best2_quad_merge(b0, b1);
         if ((lane & 3) == 0) {
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
@@ -265,41 +288,37 @@ tc_chunk_kernel(ChunkArgs a, TcCfg cfg) {
         // turn order of the CTA's M-steps: warpgroup 0 tile p, warpgroup 1 tile p, warpgroup 0 tile p + 1, ...
         if (wgi == 1) bar_sync(3, 256);
         else if (p > 0) bar_sync(4, 256);
-        if (has) {
-          // thread (feature f, half h): half 0 adds rows 0-31, then half 1 rows 32-63, 8 rows at a time; when the 8
-          // labels are distinct their read-modify-writes are independent, otherwise they run one after the other
-          const int f = t & 63, h = t >> 6;
+        // thread (feature f, parity q) owns sums[c][f] of the clusters c with c % 2 == q (q is warp-uniform) and adds
+        // the tile's rows with those labels in row order, 8 rows at a time: the batch's sums are read before any is
+        // written, and a row whose label repeats an earlier one of the batch continues from that row's running sum,
+        // so every element receives its rows in tile order, then row order, one rounded addition each
+        const int f = t & 63, q = t >> 6;
+        if (has && f < d) {
 #pragma unroll 1
-          for (int ph = 0; ph < 2; ++ph) {
-            if (h == ph) {
-#pragma unroll 1
-              for (int r0 = 32 * ph; r0 < 32 * ph + 32; r0 += 8) {
-                const int lr = lane < 8 ? lab_s[r0 + lane] : -2 - lane;
-                const unsigned peers = __match_any_sync(0xffffffffu, lr);
-                const bool conflict = __any_sync(0xffffffffu, lr >= 0 && __popc(peers) > 1);
-                int l[8];
+          for (int r0 = 0; r0 < TBM; r0 += 8) {
+            const int4 la = *reinterpret_cast<const int4*>(lab_s + r0), lb = *reinterpret_cast<const int4*>(lab_s + r0 + 4);
+            const int l[8] = {la.x, la.y, la.z, la.w, lb.x, lb.y, lb.z, lb.w};
+            bool own[8];
+            float v[8];
 #pragma unroll
-                for (int q = 0; q < 8; ++q) l[q] = __shfl_sync(0xffffffffu, lr, q);
-                if (f < d) {
-                  if (!conflict) {
-                    float v[8];
-#pragma unroll
-                    for (int q = 0; q < 8; ++q) v[q] = l[q] >= 0 ? sum_s[l[q] * 64 + f] : 0.f;
-#pragma unroll
-                    for (int q = 0; q < 8; ++q)
-                      if (l[q] >= 0) sum_s[l[q] * 64 + f] = v[q] + xs[(r0 + q) * XP + f];
-                  } else {
-#pragma unroll
-                    for (int q = 0; q < 8; ++q)
-                      if (l[q] >= 0) sum_s[l[q] * 64 + f] += xs[(r0 + q) * XP + f];
-                  }
-                }
-              }
+            for (int j = 0; j < 8; ++j) {
+              own[j] = l[j] >= 0 && (l[j] & 1) == q;
+              v[j] = own[j] ? sum_s[l[j] * 64 + f] : 0.f;
             }
-            if (ph == 0) wg::wg_sync(1 + wgi);
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+#pragma unroll
+              for (int i = 0; i < j; ++i)
+                if (l[i] == l[j]) v[j] = v[i];
+              v[j] += xs[(r0 + j) * XP + f];
+            }
+#pragma unroll
+            for (int j = 0; j < 8; ++j)
+              if (own[j]) sum_s[l[j] * 64 + f] = v[j];       // a repeated label: the last store is the full sum
           }
         }
-        __threadfence_block();
+        // bar.arrive -> bar.sync orders these shared-memory writes before the next turn's accesses (PTX memory model:
+        // the arrive synchronizes with the sync on the same barrier)
         if (wgi == 0) bar_arrive(3, 256);
         else if (p + 1 < npairs) bar_arrive(4, 256);
       }
@@ -480,21 +499,30 @@ static bool make_cfg(int d, int k, bool mstep, TcCfg* c) {
   return o <= 227u * 1024u;
 }
 
-template <int N, bool M, bool W, bool XF>
+template <int N, int KS, bool M, bool W, bool XF>
 static int launch_variant(const ChunkArgs& a, const TcCfg& cfg, int grid, cudaStream_t s) {
-  auto kern = tc_chunk_kernel<N, M, W, XF>;
+  auto kern = tc_chunk_kernel<N, KS, M, W, XF>;
   BKM_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cfg.total));
   kern<<<grid, TC_THREADS, cfg.total, s>>>(a, cfg);
   return 0;
 }
+template <int N, bool M, bool W, bool XF>
+static int launch_ks(const ChunkArgs& a, const TcCfg& cfg, int grid, cudaStream_t s) {
+  switch (cfg.KS) {
+    case 1: return launch_variant<N, 1, M, W, XF>(a, cfg, grid, s);
+    case 2: return launch_variant<N, 2, M, W, XF>(a, cfg, grid, s);
+    case 3: return launch_variant<N, 3, M, W, XF>(a, cfg, grid, s);
+    default: return launch_variant<N, 4, M, W, XF>(a, cfg, grid, s);
+  }
+}
 template <bool M, bool W, bool XF>
 static int launch_n(const ChunkArgs& a, const TcCfg& cfg, int grid, cudaStream_t s) {
   switch (wg::mma_n(cfg.NP)) {
-    case 16: return launch_variant<16, M, W, XF>(a, cfg, grid, s);
-    case 32: return launch_variant<32, M, W, XF>(a, cfg, grid, s);
-    case 64: return launch_variant<64, M, W, XF>(a, cfg, grid, s);
-    case 128: return launch_variant<128, M, W, XF>(a, cfg, grid, s);
-    default: return launch_variant<256, M, W, XF>(a, cfg, grid, s);
+    case 16: return launch_ks<16, M, W, XF>(a, cfg, grid, s);
+    case 32: return launch_ks<32, M, W, XF>(a, cfg, grid, s);
+    case 64: return launch_ks<64, M, W, XF>(a, cfg, grid, s);
+    case 128: return launch_ks<128, M, W, XF>(a, cfg, grid, s);
+    default: return launch_ks<256, M, W, XF>(a, cfg, grid, s);
   }
 }
 

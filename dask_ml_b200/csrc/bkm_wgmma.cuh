@@ -17,6 +17,8 @@ namespace wg {
 __device__ __forceinline__ void fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// all but the most recently committed group have completed
+__device__ __forceinline__ void wait_1() { asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory"); }
 // keeps the compiler from moving accumulator reads / writes across the asynchronous MMAs
 template <int R>
 __device__ __forceinline__ void pin(float (&d)[R]) {
@@ -133,14 +135,12 @@ __device__ __forceinline__ void best2_merge(Best2& b, int mask) {
   if (om1 < b.m1 || (om1 == b.m1 && oj < b.j)) { b.m2 = fminf(b.m1, om2); b.m1 = om1; b.j = oj; }
   else b.m2 = fminf(b.m2, om1);
 }
-// Arg-min epilogue of a 64 x N accumulator tile: value of column j = d[..] + cn[j] (cn: shared memory, padded columns
-// hold a huge value).  Returns the (best, column, second best) of the thread's two rows (g and g + 8), complete over
-// all N columns (merged across the four lanes of the quad).
+__device__ __forceinline__ Best2 best2_init() { return Best2{CUDART_INF_F, CUDART_INF_F, 0x7fffffff}; }
+// Adds columns j0 .. j0 + N - 1 of the thread's two rows (g and g + 8) to (r0, r1): d is the 64 x N accumulator tile of
+// those columns, value of column j = d[..] + cn[j] (cn: shared memory, padded columns hold a huge value).
 template <int N>
-__device__ __forceinline__ void tile_best2(const float (&d)[N / 2], const float* cn, int lane, Best2& r0, Best2& r1) {
-  const int c2 = (lane & 3) * 2;
-  r0 = Best2{CUDART_INF_F, CUDART_INF_F, 0x7fffffff};
-  r1 = r0;
+__device__ __forceinline__ void best2_cols(const float (&d)[N / 2], const float* cn, int j0, int lane, Best2& r0, Best2& r1) {
+  const int c2 = j0 + (lane & 3) * 2;
 #pragma unroll
   for (int i = 0; i < N / 8; ++i) {
     const float2 cv = *reinterpret_cast<const float2*>(cn + 8 * i + c2);
@@ -149,8 +149,20 @@ __device__ __forceinline__ void tile_best2(const float (&d)[N / 2], const float*
     best2_add(r1, d[4 * i + 2] + cv.x, 8 * i + c2);
     best2_add(r1, d[4 * i + 3] + cv.y, 8 * i + c2 + 1);
   }
+}
+// merge over the four lanes of the quad: every lane ends with its rows' result over all the columns
+__device__ __forceinline__ void best2_quad_merge(Best2& r0, Best2& r1) {
   best2_merge(r0, 1); best2_merge(r0, 2);
   best2_merge(r1, 1); best2_merge(r1, 2);
+}
+// Arg-min epilogue of a 64 x N accumulator tile.  Returns the (best, column, second best) of the thread's two rows,
+// complete over all N columns.
+template <int N>
+__device__ __forceinline__ void tile_best2(const float (&d)[N / 2], const float* cn, int lane, Best2& r0, Best2& r1) {
+  r0 = best2_init();
+  r1 = r0;
+  best2_cols<N>(d, cn, 0, lane, r0, r1);
+  best2_quad_merge(r0, r1);
 }
 
 // named barrier of one warpgroup (ids 1.. : id 0 is __syncthreads)
