@@ -22,8 +22,11 @@
 //   half while the tensor cores compute the second;
 //   the winning distance in direct form (x - c)^2 in fp32, and the M-step.
 // The M-step adds the tile's rows in row order into the CTA's sums; the two warpgroups take turns (named barriers),
-// so every cluster's sum is formed in one fixed order and the sums are bit-reproducible.  Inside a turn each sums
-// element has one owning thread.  One warpgroup's MMAs overlap the other's epilogue / M-step.
+// so every cluster's sum is formed in one fixed order and the sums are bit-reproducible.  Each sums element has one
+// owning thread (feature f, label parity q); before its turn a warp lists the tile's rows of its parity, so that the
+// turn touches only owned rows, and marks the batches of 8 rows in which a label repeats (only those forward running
+// sums).  The turn order is kept per warp pair: warp w of each warpgroup owns the same elements.  One warpgroup's MMAs
+// overlap the other's epilogue / M-step.
 #include "bkm_common.cuh"
 #include "bkm_wgmma.cuh"
 #include <cuda_fp16.h>
@@ -38,7 +41,7 @@ static const int TC_THREADS = 256;   // two warpgroups
 struct TcCfg {
   int KS;        // MMA K-steps of 16 (ceil(d/16))
   int NP;        // padded centre count (multiple of 16, <= 256)
-  uint32_t off_bhi, off_blo, off_x, off_sum, off_cn, off_cnt, off_lab, off_dp, off_red, total;
+  uint32_t off_bhi, off_blo, off_x, off_sum, off_cn, off_cnt, off_lab, off_dp, off_red, off_cls, total;
 };
 
 // The deferred-row re-check reports a failed fused kernel through this word (see tc_recheck_kernel); the wgmma kernel
@@ -49,6 +52,12 @@ __device__ unsigned int g_tc_dbg[64];
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void bar_sync(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
 __device__ __forceinline__ void bar_arrive(int id, int n) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(n) : "memory"); }
+// M-step class-list entry of row `row` of a tile with label `c`: the byte offset of sums row c (bits 0-16) and of the
+// staged X row (bits 17-31).  Rows of the sums are 64 floats, so a thread adds 4 f to the first.
+static const int CLS_ROW_SHIFT = 17;
+static const uint32_t CLS_SUM_MASK = (1u << CLS_ROW_SHIFT) - 1u;
+static_assert((256 + 1) * 64 * 4 <= (int)CLS_SUM_MASK && (TBM - 1) * XP * 4 < (1 << (32 - CLS_ROW_SHIFT)), "class-list entry fields");
+__device__ __forceinline__ uint32_t cls_entry(int c, int row) { return ((uint32_t)(row * XP * 4) << CLS_ROW_SHIFT) | (uint32_t)(c * 64 * 4); }
 __device__ __forceinline__ uint32_t pack_half2(float lo, float hi) {
   const __half2 h = __floats2half2_rn(lo, hi);          // low half = lower column
   return *reinterpret_cast<const uint32_t*>(&h);
@@ -71,7 +80,7 @@ tc_chunk_kernel(ChunkArgs a, TcCfg cfg) {
   const int d = a.d, k = a.k;
   float* cn_s = reinterpret_cast<float*>(smem + cfg.off_cn);          // [N] s^2 ||c||^2 (padded columns: 3e38)
   int* cnt_s = reinterpret_cast<int*>(smem + cfg.off_cnt);            // [N]
-  float* sum_s = reinterpret_cast<float*>(smem + cfg.off_sum);        // [N][64]
+  float* sum_s = reinterpret_cast<float*>(smem + cfg.off_sum);        // [N + 2][64] (rows N, N + 1: M-step list padding)
   int* lab_s = reinterpret_cast<int*>(smem + cfg.off_lab) + wgi * TBM;        // label of each row of the tile, -1: none
   float* dp_s = reinterpret_cast<float*>(smem + cfg.off_dp) + wgi * 2 * TBM;  // [2][TBM] halves of the direct distances
   double* red_s = reinterpret_cast<double*>(smem + cfg.off_red);
@@ -99,7 +108,7 @@ tc_chunk_kernel(ChunkArgs a, TcCfg cfg) {
       cnt_s[j] = 0;
     }
     if (MSTEP)
-      for (int i = tid; i < N * 64; i += TC_THREADS) sum_s[i] = 0.f;
+      for (int i = tid; i < (N + 2) * 64; i += TC_THREADS) sum_s[i] = 0.f;
     wg::fence_proxy_async();                                 // generic-proxy stores -> visible to wgmma
   }
   __syncthreads();
@@ -285,42 +294,81 @@ tc_chunk_kernel(ChunkArgs a, TcCfg cfg) {
         }
       }
       if (MSTEP) {
-        // turn order of the CTA's M-steps: warpgroup 0 tile p, warpgroup 1 tile p, warpgroup 0 tile p + 1, ...
-        if (wgi == 1) bar_sync(3, 256);
-        else if (p > 0) bar_sync(4, 256);
-        // thread (feature f, parity q) owns sums[c][f] of the clusters c with c % 2 == q (q is warp-uniform) and adds
-        // the tile's rows with those labels in row order, 8 rows at a time: the batch's sums are read before any is
-        // written, and a row whose label repeats an earlier one of the batch continues from that row's running sum,
-        // so every element receives its rows in tile order, then row order, one rounded addition each
+        // thread (feature f, parity q) owns sums[c][f] of the clusters c with c % 2 == q (q is warp-uniform).  Before
+        // its turn each warp lists the tile's rows of its class in row order, as byte offsets (cls_entry), and pads the
+        // list to a multiple of 8 with the warp's spare sums row N + q (never read back); deferred rows are left out.
+        // Then it marks the list positions whose label repeats an earlier one of the same batch of 8
         const int f = t & 63, q = t >> 6;
-        if (has && f < d) {
+        uint32_t* cls = reinterpret_cast<uint32_t*>(smem + cfg.off_cls) + (tid >> 5) * TBM;
+        int ncls = 0;
+        uint64_t rep = 0;                                    // bit i: list position i repeats a label of its batch
+        if (has) {
+          const int la = lab_s[lane], lb = lab_s[32 + lane];
+          const unsigned ma = __ballot_sync(0xffffffffu, la >= 0 && (la & 1) == q);
+          const unsigned mb = __ballot_sync(0xffffffffu, lb >= 0 && (lb & 1) == q);
+          const unsigned lt = (1u << lane) - 1u;
+          if ((ma >> lane) & 1u) cls[__popc(ma & lt)] = cls_entry(la, lane);
+          if ((mb >> lane) & 1u) cls[__popc(ma) + __popc(mb & lt)] = cls_entry(lb, 32 + lane);
+          ncls = __popc(ma) + __popc(mb);
+          if (lane < ((-ncls) & 7)) cls[ncls + lane] = cls_entry(N + q, 0);
+          __syncwarp();
+          for (int h = 0; h < 2 && 32 * h < ncls; ++h) {
+            const int pos = 32 * h + lane;
+            const uint32_t c = cls[pos] & CLS_SUM_MASK;
+            bool r = false;
+#pragma unroll
+            for (int s = 1; s < 8; ++s) {
+              const uint32_t o = __shfl_up_sync(0xffffffffu, c, s);   // position pos - s
+              r |= (lane & 7) >= s && o == c;
+            }
+            rep |= (uint64_t)__ballot_sync(0xffffffffu, r && pos < ncls) << (32 * h);
+          }
+        }
+        // turn order of the CTA's M-steps: warpgroup 0 tile p, warpgroup 1 tile p, warpgroup 0 tile p + 1, ...; only
+        // warp w of the other warpgroup owns the same sums elements, so the order is kept per warp pair (named barriers
+        // 3 + 2w: warpgroup 0 -> 1, 4 + 2w: warpgroup 1 -> 0)
+        if (wgi == 1) bar_sync(3 + 2 * wq, 64);
+        else if (p > 0) bar_sync(4 + 2 * wq, 64);
+        // the rows of the list go in 8 at a time: the batch's sums are read before any is written; in a batch with a
+        // repeated label, a row continues from the running sum of that label's earlier row.  So every element receives
+        // its rows in tile order, then row order, one rounded addition each
+        if (f < d) {
+          const uint32_t fo = (uint32_t)f * 4u;
+          unsigned char* sum_b = reinterpret_cast<unsigned char*>(sum_s);
+          const unsigned char* xs_b = reinterpret_cast<const unsigned char*>(xs) + fo;
+          const uint4* cl4 = reinterpret_cast<const uint4*>(cls);
+          uint4 ea = cl4[0], eb = cl4[1];
 #pragma unroll 1
-          for (int r0 = 0; r0 < TBM; r0 += 8) {
-            const int4 la = *reinterpret_cast<const int4*>(lab_s + r0), lb = *reinterpret_cast<const int4*>(lab_s + r0 + 4);
-            const int l[8] = {la.x, la.y, la.z, la.w, lb.x, lb.y, lb.z, lb.w};
-            bool own[8];
-            float v[8];
+          for (int b = 0; 8 * b < ncls; ++b) {
+            const uint32_t e[8] = {ea.x, ea.y, ea.z, ea.w, eb.x, eb.y, eb.z, eb.w};
+            float v[8], x[8];
 #pragma unroll
             for (int j = 0; j < 8; ++j) {
-              own[j] = l[j] >= 0 && (l[j] & 1) == q;
-              v[j] = own[j] ? sum_s[l[j] * 64 + f] : 0.f;
+              v[j] = *reinterpret_cast<const float*>(sum_b + ((e[j] & CLS_SUM_MASK) | fo));
+              x[j] = *reinterpret_cast<const float*>(xs_b + (e[j] >> CLS_ROW_SHIFT));
             }
+            if (8 * (b + 1) < ncls) { ea = cl4[2 * b + 2]; eb = cl4[2 * b + 3]; }
+            if ((rep >> (8 * b)) & 0xffu) {
 #pragma unroll
-            for (int j = 0; j < 8; ++j) {
+              for (int j = 0; j < 8; ++j) {
 #pragma unroll
-              for (int i = 0; i < j; ++i)
-                if (l[i] == l[j]) v[j] = v[i];
-              v[j] += xs[(r0 + j) * XP + f];
+                for (int i = 0; i < j; ++i)
+                  if (((e[i] ^ e[j]) & CLS_SUM_MASK) == 0u) v[j] = v[i];
+                v[j] += x[j];
+              }
+            } else {
+#pragma unroll
+              for (int j = 0; j < 8; ++j) v[j] += x[j];
             }
+            // a repeated label: the last store is the full sum
 #pragma unroll
-            for (int j = 0; j < 8; ++j)
-              if (own[j]) sum_s[l[j] * 64 + f] = v[j];       // a repeated label: the last store is the full sum
+            for (int j = 0; j < 8; ++j) *reinterpret_cast<float*>(sum_b + ((e[j] & CLS_SUM_MASK) | fo)) = v[j];
           }
         }
         // bar.arrive -> bar.sync orders these shared-memory writes before the next turn's accesses (PTX memory model:
         // the arrive synchronizes with the sync on the same barrier)
-        if (wgi == 0) bar_arrive(3, 256);
-        else if (p + 1 < npairs) bar_arrive(4, 256);
+        if (wgi == 0) bar_arrive(3 + 2 * wq, 64);
+        else if (p + 1 < npairs) bar_arrive(4 + 2 * wq, 64);
       }
     }
     wg::wg_sync(1 + wgi);                                    // the stage and lab_s may be refilled
@@ -489,12 +537,13 @@ static bool make_cfg(int d, int k, bool mstep, TcCfg* c) {
   c->off_bhi = o; o += N * 128u;                    // fp16 B tiles: N rows x 64 halves (one 128-byte swizzle atom)
   c->off_blo = o; o += N * 128u;
   c->off_x = o; o += 2u * 2u * TBM * XP * 4u;       // 2 warpgroups x 2 stages of fp32 X tiles
-  c->off_sum = o; if (mstep) o += N * 64u * 4u;     // per-CTA sums [N][64]
+  c->off_sum = o; if (mstep) o += (N + 2u) * 64u * 4u;   // per-CTA sums [N][64] + 2 spare rows
   c->off_cn = o; o += N * 4u;
   c->off_cnt = o; o += N * 4u;
   c->off_lab = o; o += 2u * TBM * 4u;
   c->off_dp = o; o += 2u * 2u * TBM * 4u;
   c->off_red = o; o += TC_THREADS * 8u;
+  c->off_cls = o; if (mstep) o += TC_THREADS / 32u * TBM * 4u;   // per-warp class lists of the M-step
   c->total = o;
   return o <= 227u * 1024u;
 }

@@ -128,27 +128,37 @@ __device__ __forceinline__ void best2_add(Best2& b, float v, int j) {     // col
   if (v < b.m1) { b.m2 = b.m1; b.m1 = v; b.j = j; }
   else b.m2 = fminf(b.m2, v);
 }
+// (best, column, second best) over the columns of b and o together, lowest column on exact ties
+__device__ __forceinline__ void best2_join(Best2& b, const Best2& o) {
+  if (o.m1 < b.m1 || (o.m1 == b.m1 && o.j < b.j)) { b.m2 = fminf(b.m1, o.m2); b.m1 = o.m1; b.j = o.j; }
+  else b.m2 = fminf(b.m2, o.m1);
+}
 // merge with the lane `mask` away; both lanes end with the same result, lowest column on exact ties
 __device__ __forceinline__ void best2_merge(Best2& b, int mask) {
-  const float om1 = __shfl_xor_sync(0xffffffffu, b.m1, mask), om2 = __shfl_xor_sync(0xffffffffu, b.m2, mask);
-  const int oj = __shfl_xor_sync(0xffffffffu, b.j, mask);
-  if (om1 < b.m1 || (om1 == b.m1 && oj < b.j)) { b.m2 = fminf(b.m1, om2); b.m1 = om1; b.j = oj; }
-  else b.m2 = fminf(b.m2, om1);
+  Best2 o;
+  o.m1 = __shfl_xor_sync(0xffffffffu, b.m1, mask);
+  o.m2 = __shfl_xor_sync(0xffffffffu, b.m2, mask);
+  o.j = __shfl_xor_sync(0xffffffffu, b.j, mask);
+  best2_join(b, o);
 }
 __device__ __forceinline__ Best2 best2_init() { return Best2{CUDART_INF_F, CUDART_INF_F, 0x7fffffff}; }
 // Adds columns j0 .. j0 + N - 1 of the thread's two rows (g and g + 8) to (r0, r1): d is the 64 x N accumulator tile of
 // those columns, value of column j = d[..] + cn[j] (cn: shared memory, padded columns hold a huge value).
 template <int N>
 __device__ __forceinline__ void best2_cols(const float (&d)[N / 2], const float* cn, int j0, int lane, Best2& r0, Best2& r1) {
+  // two independent chains per row (the thread's even and its odd columns), joined at the end
   const int c2 = j0 + (lane & 3) * 2;
+  Best2 o0 = best2_init(), o1 = o0;
 #pragma unroll
   for (int i = 0; i < N / 8; ++i) {
     const float2 cv = *reinterpret_cast<const float2*>(cn + 8 * i + c2);
     best2_add(r0, d[4 * i + 0] + cv.x, 8 * i + c2);
-    best2_add(r0, d[4 * i + 1] + cv.y, 8 * i + c2 + 1);
+    best2_add(o0, d[4 * i + 1] + cv.y, 8 * i + c2 + 1);
     best2_add(r1, d[4 * i + 2] + cv.x, 8 * i + c2);
-    best2_add(r1, d[4 * i + 3] + cv.y, 8 * i + c2 + 1);
+    best2_add(o1, d[4 * i + 3] + cv.y, 8 * i + c2 + 1);
   }
+  best2_join(r0, o0);
+  best2_join(r1, o1);
 }
 // merge over the four lanes of the quad: every lane ends with its rows' result over all the columns
 __device__ __forceinline__ void best2_quad_merge(Best2& r0, Best2& r1) {
