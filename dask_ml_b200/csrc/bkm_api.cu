@@ -136,9 +136,9 @@ static int chunk_common(const void* X, long long n, int d, long long ldx, int x_
   }
   if (family == 0) rc = launch_simt(a, mstep, x_dtype, sm, &grid, s);
   if (rc) return rc;
-  // grid < 0: the generic kernel ran in GLOBAL mode (sums accumulated by atomics into slot 0)
+  // grid < 0: the generic kernel ran in GLOBAL mode (sums accumulated by float64 atomics into slot 0)
   const int g = grid < 0 ? -grid : grid;
-  rc = launch_reduce_partials(a, grid < 0 ? 1 : g, g, g, mstep, x_dtype, sums, counts, dist_sum, s);
+  rc = launch_reduce_partials(a, grid < 0 ? 1 : g, g, g, mstep, grid < 0 ? BKM_F64 : x_dtype, sums, counts, dist_sum, s);
   if (rc) return rc;
   if (family == 1) rc = launch_tc_recheck(a, mstep, sm, s);     // float64 decisions of the deferred rows, added on top
   return rc;

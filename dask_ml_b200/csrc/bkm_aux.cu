@@ -529,12 +529,13 @@ __global__ void reduce_partials_kernel(const PS* __restrict__ psum, const int* _
 
 // sum_parts / cnt_parts / pin_parts: how many partial slots the chunk kernel(s) wrote of the sums, the counts and the
 // distance sums (one per CTA for the fused kernels; 1 sums slot in the generic kernel's GLOBAL mode; row blocks and
-// distance-pass CTAs for the large-shape path)
-int launch_reduce_partials(const ChunkArgs& a, int sum_parts, int cnt_parts, int pin_parts, bool mstep, int dtype,
+// distance-pass CTAs for the large-shape path).  psum_dtype: BKM_F64 when the partial sums are float64 (float64 rows, and
+// the generic kernel's GLOBAL slot whatever the rows are), else they are fp32.
+int launch_reduce_partials(const ChunkArgs& a, int sum_parts, int cnt_parts, int pin_parts, bool mstep, int psum_dtype,
                            double* sums, long long* counts, double* dist_sum, cudaStream_t s) {
   const int kd = a.k * a.d;
   int nb = (kd + 31) / 32; if (nb > 592) nb = 592; if (nb < 1) nb = 1;      // blocks of 32 outputs x 8 partial chains
-  if (dtype != BKM_F64)
+  if (psum_dtype != BKM_F64)
     reduce_partials_kernel<float><<<nb, 256, 0, s>>>((const float*)a.psum, a.pcnt, a.pin, cnt_parts, pin_parts, sum_parts,
                                                      kd, a.k, mstep, sums, counts, dist_sum, a.skip, a.first_chunk, a.counts_f64);
   else

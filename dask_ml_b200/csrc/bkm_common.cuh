@@ -108,7 +108,8 @@ struct PackHeader {
 // ---------------------------------------------------------------------------------------
 // Per-CTA partial sums: one [k*d] slot per CTA of the largest grid a CUDA-core kernel launches (8 CTAs per SM),
 // fewer when a slot is large (a kernel whose per-CTA sums occupy most of the shared memory runs 1-2 CTAs per SM), and a
-// single slot when k*d cannot be CTA-resident at all (generic kernel's GLOBAL mode: atomics into slot 0).
+// single slot when k*d cannot be CTA-resident at all (generic kernel's GLOBAL mode: float64 atomics into slot 0, so the
+// psum area always holds at least k*d doubles).
 static const int kDefaultSMs = 132;     // H100 SXM: sizing when no device is visible
 
 struct WsLayout {
@@ -139,7 +140,8 @@ static inline WsLayout ws_layout(long long n, int d, int k, int dtype, int sm_co
   // FIXED offset (independent of n): the cluster -> warp balance table of the label-indexed M-step pass survives from one
   // chunk call to the next (16-byte header {magic, k, cluster slices} + one byte per cluster, k <= 4096)
   W.off_bal = o; o = align_up(o + 16 + 4096, 256);
-  W.off_psum = o; o = align_up(o + (size_t)W.psum_slots * slot, 256);
+  const size_t psum_bytes = (size_t)W.psum_slots * slot, global_bytes = (size_t)k * d * 8;
+  W.off_psum = o; o = align_up(o + (psum_bytes > global_bytes ? psum_bytes : global_bytes), 256);
   W.off_pcnt = o; o = align_up(o + (size_t)W.part_slots * k * 4, 256);
   W.off_pin = o;  o = align_up(o + (size_t)W.part_slots * 8, 256);
   W.off_flag = o; o = align_up(o + 256, 256);          // [0] = deferred-row counter
@@ -226,7 +228,7 @@ int launch_tc2(const ChunkArgs& a, bool mstep, int sm_count, int* grid_out, cuda
 int launch_rowpass_mstep(const ChunkArgs& a, int x_dtype, int sm_count, int* parts_out, cudaStream_t s);
 int launch_rowpass_dist(const ChunkArgs& a, int x_dtype, int sm_count, int* parts_out, cudaStream_t s);
 // implemented in bkm_aux.cu
-int launch_reduce_partials(const ChunkArgs& a, int sum_parts, int cnt_parts, int pin_parts, bool mstep, int dtype,
+int launch_reduce_partials(const ChunkArgs& a, int sum_parts, int cnt_parts, int pin_parts, bool mstep, int psum_dtype,
                            double* sums, long long* counts, double* dist_sum, cudaStream_t s);
 
 }  // namespace bkm

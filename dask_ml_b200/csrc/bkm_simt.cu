@@ -13,8 +13,9 @@
 // Data movement: a tile of TILE rows is staged once in shared memory with coalesced 16-byte
 // loads; both the E-step and the M-step read it from there, so X is read from HBM exactly once
 // per Lloyd iteration.  Centres, per-CTA sums and counts live in shared memory (SMEM mode) or,
-// when k*d is too large for that, centres are read through L1 and sums go to global atomics
-// (GLOBAL mode).
+// when k*d is too large for that, centres are read through L1 and sums go to float64 global
+// atomics (GLOBAL mode: one slot adds the rows of the whole chunk, where an fp32 running sum of a
+// dominant cluster would lose its low bits).
 #include "bkm_common.cuh"
 #include <math_constants.h>
 
@@ -322,8 +323,8 @@ simt_chunk_kernel(ChunkArgs a, SimtSmem S) {
           int c = __shfl_sync(0xffffffffu, ml, b);
           const T* xr = xs + (base + b) * pitch;
           if (GLOBAL) {
-            PS* g = reinterpret_cast<PS*>(a.psum) + (size_t)c * d;
-            for (int i = lane; i < d; i += 32) atomicAdd(g + i, (PS)xr[i]);
+            double* g = reinterpret_cast<double*>(a.psum) + (size_t)c * d;
+            for (int i = lane; i < d; i += 32) atomicAdd(g + i, (double)xr[i]);
             if (lane == 0) atomicAdd(&cnts_s[c], 1);
           } else {
             PS* sr = sums_s + (size_t)c * d;
@@ -419,8 +420,9 @@ static int launch_T(const ChunkArgs& a, bool mstep, int sm_count, int* grid_out,
 #undef BKM_DISPATCH
 }
 
-// In GLOBAL mode the kernel accumulates into psum slot 0 with atomics: the caller zeroes it and
-// reduce_partials treats it as a single partial.  grid_out is returned negative in that case.
+// In GLOBAL mode the kernel accumulates into psum slot 0 with float64 atomics (fp32 inputs too): the
+// caller zeroes it and reduce_partials reads it as a single float64 partial.  grid_out is returned
+// negative in that case.
 int launch_simt(const ChunkArgs& a, bool mstep, int dtype, int sm_count, int* grid_out, cudaStream_t s) {
   int rc;
   bool global_mode;
@@ -428,7 +430,7 @@ int launch_simt(const ChunkArgs& a, bool mstep, int dtype, int sm_count, int* gr
     int J = ((a.k + 15) / 16 * 16 - a.k) <= ((a.k + 7) / 8 * 8 - a.k) ? 16 : 8;
     global_mode = simt_mode_global<float>(a.k, a.d, J, mstep);
     if (global_mode && mstep) {
-      BKM_CUDA_TRY(cudaMemsetAsync(a.psum, 0, (size_t)a.k * a.d * sizeof(float), s));
+      BKM_CUDA_TRY(cudaMemsetAsync(a.psum, 0, (size_t)a.k * a.d * sizeof(double), s));
       note_launch();
     }
     rc = launch_T<float>(a, mstep, sm_count, grid_out, s);

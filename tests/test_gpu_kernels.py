@@ -458,14 +458,26 @@ def test_baseline_size_parity(be, name, n, d, k):
         assert be.deferred_rows(n, d, k, torch.float32) < 0.01 * n
 
 
-@pytest.mark.parametrize("d,k,dtype_name", [(32, 64, "float32"), (13, 20, "float32"), (64, 256, "float32"), (128, 600, "bfloat16")])
-def test_sums_with_a_dominant_cluster_and_offset_data(be, d, k, dtype_name):
+@pytest.mark.parametrize("d,k,dtype_name,flags", [
+    pytest.param(32, 64, "float32", 0, id="32-64-float32"),
+    pytest.param(13, 20, "float32", 0, id="13-20-float32"),
+    pytest.param(64, 256, "float32", 0, id="64-256-float32"),
+    pytest.param(128, 600, "bfloat16", 0, id="128-600-bfloat16"),
+    # the generic kernel: GLOBAL mode (k * d too large for shared memory: one slot for the whole chunk), SMEM mode
+    pytest.param(128, 300, "float32", 0, id="128-300-float32-global"),
+    pytest.param(64, 512, "float32", 0, id="64-512-float32-global"),
+    pytest.param(64, 256, "float32", 1, id="64-256-float32-simt"),
+    pytest.param(64, 256, "float64", 0, id="64-256-float64-global"),
+])
+def test_sums_with_a_dominant_cluster_and_offset_data(be, d, k, dtype_name, flags):
     """The fused kernels keep per-CTA (per-warp) partial sums in fp32 and widen them to float64 once per chunk call
-    (the reference accumulates in float64, k_means.py:576).  Worst case for that: one cluster owns 90 % of 2M rows and
-    the data sit far from the origin.  The sums must still agree with the float64 sums of the SAME labels to ~1e-5 of
-    the data's magnitude (the centres move by less than 1e-3 of the cluster's standard deviation)."""
+    (the reference accumulates in float64, k_means.py:576); the generic kernel's GLOBAL mode adds the whole chunk into
+    one float64 slot.  Worst case for that: one cluster owns 90 % of 2M rows and the data sit far from the origin.  The
+    sums must still agree with the float64 sums of the SAME labels to ~1e-5 of the data's magnitude (the centres move by
+    less than 1e-3 of the cluster's standard deviation)."""
     import torch
 
+    be.flags = flags
     dtype = getattr(torch, dtype_name)
     n = 2_000_000
     g = torch.Generator(device=be.device).manual_seed(d * 1000 + k)
@@ -478,8 +490,11 @@ def test_sums_with_a_dominant_cluster_and_offset_data(be, d, k, dtype_name):
     pack = be.pack_centers(C, dtype)
     labels = be.empty((n,), torch.int32)
     sums = be.zeros((k * d,), torch.float64); counts = be.zeros((k,), torch.int64)
-    be.lloyd_chunk(x, pack, k, labels, None, sums, counts, None)
-    torch.cuda.synchronize()
+    try:
+        be.lloyd_chunk(x, pack, k, labels, None, sums, counts, None)
+        torch.cuda.synchronize()
+    finally:
+        be.flags = 0
     lab = labels.long()
     want = torch.zeros((k, d), dtype=torch.float64, device=be.device).index_add_(0, lab, X.double())
     wcnt = torch.bincount(lab, minlength=k)
