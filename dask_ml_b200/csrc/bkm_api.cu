@@ -259,7 +259,7 @@ int bkm_transform_chunk(const void* X, int64_t n, int d, int64_t ldx, int x_dtyp
     a.pack = (const unsigned char*)pack;
     a.L = pack_layout(k, d, x_dtype);
     a.k = k;
-    a.xf_out = (float*)out; a.xf_ld = ld_out; a.xf_mode = mode; a.xf_gamma = (float)gamma;
+    a.xf_out = (float*)out; a.xf_ld = ld_out; a.xf_mode = mode; a.xf_gamma = gamma;
     rc = launch_tc_transform(a, sm, (cudaStream_t)stream);
     if (rc != BKM_EALIGN && rc != BKM_EUNSUPPORTED) return rc;
     if (flags & BKM_FLAG_FORCE_TC) return rc;

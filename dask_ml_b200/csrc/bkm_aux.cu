@@ -103,7 +103,15 @@ __global__ void pack_norms_kernel(const double* __restrict__ C, unsigned char* p
 
 // scale = 2^(9 - floor(log2 max|c|)): s * max|c| in [2^9, 2^10), so -2 s c fits fp16 with a 32x margin and
 // rows of X up to ~64x the largest centre component convert without overflow (larger ones are deferred to
-// the float64 path by the kernel).  Runs first: the other pack kernels read it.
+// the float64 path by the kernel).  The exponent is clamped to [-126, 126], so that s and 1/s are normal floats: the
+// transform epilogue divides by s twice in fp32.  So the rule holds whenever max|c| >= 2^-117.
+__device__ __forceinline__ int pack_scale_exp(double max_abs_c) {
+  int e = 0;
+  if (max_abs_c > 0.0 && max_abs_c < CUDART_INF) e = 9 - ilogb(max_abs_c);
+  return e > 126 ? 126 : (e < -126 ? -126 : e);
+}
+
+// Runs first: the other pack kernels read the scale.
 __global__ void pack_scale_kernel(const double* __restrict__ C, unsigned char* pack, PackLayout L) {
   __shared__ double sm[32];
   double m = 0.0;
@@ -114,11 +122,8 @@ __global__ void pack_scale_kernel(const double* __restrict__ C, unsigned char* p
   __syncthreads();
   if (threadIdx.x == 0) {
     for (int w = 1; w < (int)(blockDim.x >> 5); ++w) m = fmax(m, sm[w]);
-    int e = 0;
-    if (m > 0.0 && m < CUDART_INF) e = 9 - ilogb(m);
-    e = e > 100 ? 100 : (e < -100 ? -100 : e);
     PackHeader* h = reinterpret_cast<PackHeader*>(pack);
-    h->scale = (float)scalbn(1.0, e);
+    h->scale = (float)scalbn(1.0, pack_scale_exp(m));
     h->pad2 = 0.f;
   }
 }
@@ -158,10 +163,7 @@ __device__ __forceinline__ void pack_fused_body(Src C, unsigned char* pack, cons
   __syncthreads();
   m = red[0];
   for (int w = 1; w < 32; ++w) m = fmax(m, red[w]);
-  int e = 0;
-  if (m > 0.0 && m < CUDART_INF) e = 9 - ilogb(m);
-  e = e > 100 ? 100 : (e < -100 ? -100 : e);
-  const double sc = scalbn(1.0, e);
+  const double sc = scalbn(1.0, pack_scale_exp(m));
   __syncthreads();
   // ---- ||c_j||^2 (one warp per centre, same summation order as pack_norms_kernel) and their maximum
   for (int j = wid; j < k; j += 32) {

@@ -103,6 +103,14 @@ struct PackHeader {
   float pad2;      // before the fp16 split, so that both fit fp16's range (exact: only exponents change)
 };
 
+// Magnitude window of the unscaled fp32 / bf16 distance arithmetic (families 0, 2 and 3): a row whose fp32
+// ||x||^2 + max ||c||^2 lies outside [2^-100, 2^100] is decided in float64 like a near-tie.  Below the window the
+// products fall into fp32's subnormals, whose absolute rounding (2^-149) exceeds the near-tie bound; above it they
+// overflow.  NaN fails the test too.
+__device__ __forceinline__ bool fp32_norm_in_window(float v) {
+  return v >= 7.888609052210118e-31f && v <= 1.2676506002282294e30f;      // 2^-100, 2^100
+}
+
 // ---------------------------------------------------------------------------------------
 // Workspace for one chunk call: per-CTA partials.  Sized for the largest grid we launch.
 // ---------------------------------------------------------------------------------------
@@ -191,7 +199,7 @@ struct ChunkArgs {
   float* xf_out;      // transform variants: output block (rows x k), row pitch xf_ld floats; mode 0 sqrt / 1 squared / 2 rbf
   long long xf_ld;
   int xf_mode;
-  float xf_gamma;
+  double xf_gamma;    // float64: the tensor path applies it as gamma / s^2, which an fp32 gamma could not carry
   const int* skip;    // nullable: device word (LoopState::done); non-zero -> every kernel of the call returns at once
   int first_chunk;    // reduce_partials overwrites the accumulators (first chunk of an iteration) instead of adding
   int counts_f64;     // the counts accumulator is float64 (one float64 buffer for the all-reduce) instead of int64

@@ -295,17 +295,18 @@ rowpass_dist_kernel(ChunkArgs a) {
     const int lbl = a.labels[row];
     const TX* xr = X + row * a.ldx;
     const float* cr = gC + (size_t)(lbl < 0 ? 0 : lbl) * d4;
-    float sacc = 0.f;
+    // float64: (x - c)^2 of bf16 rows leaves fp32's range at either end of it (|x| beyond 2^64 or below 2^-63)
+    double sacc = 0.0;
     for (int i = lane; i < d; i += 32) {
-      const float df = rp_to_float<TX>(xr[i]) - cr[i];
-      sacc = fmaf(df, df, sacc);
+      const double df = (double)rp_to_float<TX>(xr[i]) - (double)cr[i];
+      sacc = fma(df, df, sacc);
     }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) sacc += __shfl_xor_sync(0xffffffffu, sacc, o);
     if (lane == 0) {
-      const float outv = a.squared ? sacc : sqrtf(sacc);
-      dsum += (double)outv;
-      if (a.min_out) reinterpret_cast<float*>(a.min_out)[row] = outv;
+      const double outv = a.squared ? sacc : sqrt(sacc);
+      dsum += outv;
+      if (a.min_out) reinterpret_cast<float*>(a.min_out)[row] = (float)outv;
     }
   }
   if (lane == 0) red_s[warp] = dsum;

@@ -243,7 +243,8 @@ simt_chunk_kernel(ChunkArgs a, SimtSmem S) {
       }
       if (a.tau > 0.f && k > 1) {
         T bound = (T)a.tau * (xn + cnmax);
-        if (!(second - best > bound)) {          // also catches NaN
+        // near-tie, NaN, or a row outside the fp32 magnitude window (a.tau > 0: fp32 rows only)
+        if (!(second - best > bound) || !fp32_norm_in_window((float)(xn + cnmax))) {
           my_slot = atomicAdd(&misc[0], 1);
           flist[my_slot] = tid;
         }

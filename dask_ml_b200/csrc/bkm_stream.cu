@@ -218,9 +218,10 @@ stream_chunk_kernel(ChunkArgs a, StreamSmem S) {
     const float hits = h0 + h1;
     int bj = (int)((hits - 1.f) * 1024.f + 0.5f);
     double d2x = -1.0;                                    // exact float64 distance when the row took the float64 path
-    if (valid && !(hits >= 1.f && hits < 2.f) && k > 1) {
+    if (valid && (!(hits >= 1.f && hits < 2.f) || !fp32_norm_in_window(xn + cnmax)) && k > 1) {
       if (a.tau > 0.f) {
-        // near-tie (or non-finite): decide in float64 against the float64 centres, lowest index on exact ties
+        // near-tie, non-finite or outside the magnitude window: decide in float64 against the float64 centres, lowest
+        // index on exact ties
         double bd = CUDART_INF;
         bj = 0;
         for (int j = 0; j < k; ++j) {
@@ -552,7 +553,7 @@ stream2_chunk_kernel(ChunkArgs a, Stream2Smem S) {
       const float hits = h0 + h1;
       int bj = (int)((hits - 1.f) * 1024.f + 0.5f);
       const bool valid = h ? v1 : v0;
-      if (valid && !(hits >= 1.f && hits < 2.f) && k > 1) {
+      if (valid && (!(hits >= 1.f && hits < 2.f) || !fp32_norm_in_window(xn + cnmax)) && k > 1) {
         if (a.tau > 0.f) {
           double bd = CUDART_INF;
           bj = 0;

@@ -86,6 +86,8 @@ tc_chunk_kernel(ChunkArgs a, TcCfg cfg) {
   double* red_s = reinterpret_cast<double*>(smem + cfg.off_red);
   const PackHeader* hdr = reinterpret_cast<const PackHeader*>(a.pack);
   const float sc = hdr->scale;
+  const float inv_s = 1.0f / sc;                             // exact: s is a power of two, s and 1/s are normal
+  const float gs = XFORM ? (float)(a.xf_gamma * (double)inv_s * (double)inv_s) : 0.f;   // rbf: gamma / s^2
 
   // ---------------- setup: B tiles, column offsets, sums ----------------
   {
@@ -198,31 +200,34 @@ tc_chunk_kernel(ChunkArgs a, TcCfg cfg) {
       if (XFORM) {
         wg::wait_all();
         wg::pin(acc);
-        // d^2 = (acc + s^2 ||c||^2 + ||s x||^2) / s^2, clamped at 0; mode 0: sqrt, 1: squared, 2: exp(-gamma d^2)
-        const float inv_s2 = 1.0f / (sc * sc);
+        // y = acc + s^2 ||c||^2 + ||s x||^2 = s^2 d^2, clamped at 0; mode 0: sqrt(y) / s, 1: y / s / s, 2: exp(-(gamma /
+        // s^2) y).  1/s is a normal float (pack_scale_exp) but 1/s^2 need not be, so it is never formed in fp32.
+        // One copy of the store loop per mode, so that each element pays for its own mode's arithmetic only
         const bool vec_ok = ((reinterpret_cast<uintptr_t>(a.xf_out) & 7) == 0) && ((a.xf_ld & 1) == 0);
+        auto store_block = [&](auto value) {
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const long long row = row0 + rA + 8 * h;
-          if (row >= a.n) continue;
-          const float xn = h ? xn1 : xn0;
-          float* orow = a.xf_out + row * a.xf_ld;
+          for (int h = 0; h < 2; ++h) {
+            const long long row = row0 + rA + 8 * h;
+            if (row >= a.n) continue;
+            const float xn = h ? xn1 : xn0;
+            float* orow = a.xf_out + row * a.xf_ld;
 #pragma unroll
-          for (int i = 0; i < N / 8; ++i) {
-            const int col = 8 * i + c2;
-            float o[2];
+            for (int i = 0; i < N / 8; ++i) {
+              const int col = 8 * i + c2;
+              float o[2];
 #pragma unroll
-            for (int e = 0; e < 2; ++e) {
-              const float d2 = fmaxf(((acc[4 * i + 2 * h + e] + cn_s[col + e]) + xn) * inv_s2, 0.f);
-              o[e] = a.xf_mode == 0 ? sqrtf(d2) : (a.xf_mode == 1 ? d2 : __expf(-a.xf_gamma * d2));
-            }
-            if (vec_ok && col + 1 < k) __stcs(reinterpret_cast<float2*>(orow + col), make_float2(o[0], o[1]));
-            else {
-              if (col < k) orow[col] = o[0];
-              if (col + 1 < k) orow[col + 1] = o[1];
+              for (int e = 0; e < 2; ++e) o[e] = value(fmaxf((acc[4 * i + 2 * h + e] + cn_s[col + e]) + xn, 0.f));
+              if (vec_ok && col + 1 < k) __stcs(reinterpret_cast<float2*>(orow + col), make_float2(o[0], o[1]));
+              else {
+                if (col < k) orow[col] = o[0];
+                if (col + 1 < k) orow[col + 1] = o[1];
+              }
             }
           }
-        }
+        };
+        if (a.xf_mode == 0) store_block([&](float y) { return sqrtf(y) * inv_s; });
+        else if (a.xf_mode == 1) store_block([&](float y) { return (y * inv_s) * inv_s; });
+        else store_block([&](float y) { return __expf(-gs * y); });
       } else {
         // ---- arg-min, near-tie test (bound = tau (||s x||^2 + max ||s c||^2)) ----
         // columns still reach each thread in increasing order: the lowest column wins exact ties as before
@@ -270,8 +275,11 @@ tc_chunk_kernel(ChunkArgs a, TcCfg cfg) {
     if (HAS_M) {
       wg::wg_sync(1 + wgi);                                  // lab_s of the tile is complete
       if (WANT_DIST && has) {
-        // winning distance in direct form sum (x - c)^2 (fp32 centres of the pack): thread (row r, feature half hh),
-        // features visited in a per-row rotated order so that the 32 rows of a warp hit 32 different banks
+        // winning distance in direct form sum (s x - s c)^2 (fp32 centres of the pack): thread (row r, feature half
+        // hh), features visited in a per-row rotated order so that the 32 rows of a warp hit 32 different banks.  It is
+        // formed in the scaled domain, where a row that was not deferred has every |s x| < 2^16: it cannot overflow, and
+        // it does not depend on the magnitude of the data (the scale follows the centres).  The square root is taken
+        // there too, and 1/s (1/s^2) is applied in float64, so no intermediate leaves the float range
         const int r = t & 63, hh = t >> 6;
         const int lab = lab_s[r];
         float s0 = 0.f, s1 = 0.f;
@@ -280,17 +288,17 @@ tc_chunk_kernel(ChunkArgs a, TcCfg cfg) {
 #pragma unroll 8
           for (int i = 0; i < 32; i += 2) {
             const int f0 = hh * 32 + ((i + r) & 31), f1 = hh * 32 + ((i + 1 + r) & 31);
-            if (f0 < d) { const float e = xs[r * XP + f0] - cr[f0]; s0 = fmaf(e, e, s0); }
-            if (f1 < d) { const float e = xs[r * XP + f1] - cr[f1]; s1 = fmaf(e, e, s1); }
+            if (f0 < d) { const float e = fmaf(sc, xs[r * XP + f0], -(sc * cr[f0])); s0 = fmaf(e, e, s0); }
+            if (f1 < d) { const float e = fmaf(sc, xs[r * XP + f1], -(sc * cr[f1])); s1 = fmaf(e, e, s1); }
           }
         }
         dp_s[hh * TBM + r] = s0 + s1;
         wg::wg_sync(1 + wgi);
         if (t < TBM && lab >= 0) {
-          const float d2 = dp_s[t] + dp_s[TBM + t];
-          const float outv = a.squared ? d2 : sqrtf(d2);
-          dsum += (double)outv;
-          if (a.min_out) reinterpret_cast<float*>(a.min_out)[row0 + t] = outv;
+          const float y = dp_s[t] + dp_s[TBM + t];                            // s^2 d^2
+          const double outv = a.squared ? (double)y * (double)inv_s * (double)inv_s : (double)sqrtf(y) * (double)inv_s;
+          dsum += outv;
+          if (a.min_out) reinterpret_cast<float*>(a.min_out)[row0 + t] = (float)outv;
         }
       }
       if (MSTEP) {

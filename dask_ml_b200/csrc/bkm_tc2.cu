@@ -161,7 +161,7 @@ tc2_assign_kernel(ChunkArgs a, Tc2Cfg cfg) {
           const long long row = row0 + r;
           if (row >= a.n) continue;
           const float xn = xn_s[r] + xn_s[T2_BM + r];
-          const bool out_of_range = !(xn < 3.0e38f);
+          const bool out_of_range = !fp32_norm_in_window(xn + cnmax);
           const bool tie = !(b.m2 > b.m1 + a.tau * (xn + cnmax)) || out_of_range;
           const int bj = slice * NS + ((tie || b.j >= NS) ? 0 : b.j);
           if (S == 1) {
@@ -203,7 +203,7 @@ tc2_combine_kernel(ChunkArgs a, int S) {
       else second = fminf(second, r.x);
     }
     const float bound = a.tau * (xn + cnmax);
-    const bool flagged = (lab < 0 || !(second - best > bound) || !(xn < 3.0e38f)) && a.k > 1;
+    const bool flagged = (lab < 0 || !(second - best > bound) || !fp32_norm_in_window(xn + cnmax)) && a.k > 1;
     if (!flagged) {
       if (a.labels) a.labels[row] = lab < 0 ? 0 : lab;
     } else {

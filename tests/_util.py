@@ -9,6 +9,30 @@ def d2_f64(X, C):
         np.maximum((X * X).sum(1)[:, None] - 2 * X @ C.T + (C * C).sum(1)[None, :], 0)
 
 
+def grid_blobs(n, d, k_true, seed, step, bound, spread=0.6, std=0.05, return_blob=False):
+    """float64 blob rows on the grid ``step`` with |x| < ``bound``.  On a grid of 2^-12 below 2^5 (float32) or 2^-4
+    below 2^4 (bfloat16) every row, and every power-of-two multiple of it that stays a normal float, is exact in that
+    type, so results on 2^p X can be compared with results on X exactly.  ``return_blob``: also the blob of each row."""
+    rng = np.random.RandomState(seed)
+    cent = rng.uniform(-spread * bound, spread * bound, size=(k_true, d))
+    blob = rng.randint(0, k_true, size=n)
+    X = cent[blob] + rng.standard_normal((n, d)) * (std * bound)
+    X = np.clip(np.round(X / step) * step, step - bound, bound - step)
+    return (X, blob) if return_blob else X
+
+
+def blob_seeds(X, blob, k):
+    """One row of each of the first k blobs: initial centres from which Lloyd settles in a few iterations and stops on
+    a zero shift."""
+    return np.stack([X[np.nonzero(blob == j)[0][0]] for j in range(k)])
+
+
+def distinct_rows(X, k, seed):
+    """k distinct rows of X (centres that scale exactly with X)."""
+    U = np.unique(X, axis=0)
+    return U[np.random.RandomState(seed).choice(len(U), k, replace=False)]
+
+
 def assert_labels_match(got, want, X, C, rtol=1e-9, max_frac=1e-3):
     """Labels must be identical except on float64 near-ties: rows where the two chosen centres are
     equidistant to `rtol` relative to (||x||^2+||c||^2).  This is the documented tie-breaking."""
