@@ -50,6 +50,10 @@ SIGNATURES = {
     "bkm_sample_chunk": (_int, [_c_void_p, _i64, _int, _dbl, _u64, _u64, _c_void_p, _i64, _c_void_p, _c_void_p]),
     "bkm_transform_chunk": (_int, [_c_void_p, _i64, _int, _i64, _int, _c_void_p, _int, _c_void_p, _i64, _int, _dbl, _int,
                                    _c_void_p]),
+    "bkm_kernel_colsum_chunk": (_int, [_c_void_p, _i64, _int, _i64, _int, _c_void_p, _int, _dbl, _c_void_p, _c_void_p,
+                                       ctypes.c_size_t, _int, _c_void_p]),
+    "bkm_nystrom_embed_chunk": (_int, [_c_void_p, _i64, _int, _i64, _int, _c_void_p, _int, _dbl, _c_void_p, _int,
+                                       _c_void_p, _i64, _int, _c_void_p]),
     "bkm_finalize": (_int, [_c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_void_p, _int, _int, _c_void_p]),
     "bkm_check_finite": (_int, [_c_void_p, _i64, _int, _i64, _int, _c_void_p, _c_void_p]),
     "bkm_p2p_mailbox_bytes": (_int, [_int, _i64, ctypes.POINTER(ctypes.c_size_t)]),

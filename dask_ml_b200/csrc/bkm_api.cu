@@ -23,6 +23,10 @@ int launch_transform(const void* X, long long n, int d, long long ldx, int dtype
                      cudaStream_t s);
 int launch_check_finite(const void* X, long long n, int d, long long ldx, int dtype, int* flag,
                         int sm_count, cudaStream_t s);
+int launch_nystrom(const void* X, long long n, int d, long long ldx, int dtype, const void* pack, int l, double gamma,
+                   int mode, const void* W, int kw, void* out, long long ld_out, double* part, size_t part_bytes,
+                   int sm_count, int* parts_out, cudaStream_t s);
+int launch_colsum_fold(const double* part, int parts, int l, double* colsum, int first, cudaStream_t s);
 
 static std::atomic<int> g_sm_count[64];
 static int sm_count_of_current(int* out) {
@@ -265,6 +269,75 @@ int bkm_transform_chunk(const void* X, int64_t n, int d, int64_t ldx, int x_dtyp
     if (flags & BKM_FLAG_FORCE_TC) return rc;
   } else if (flags & BKM_FLAG_FORCE_TC) return BKM_EUNSUPPORTED;
   return launch_transform(X, n, d, ldx, x_dtype, pack, k, out, ld_out, mode, gamma, sm, (cudaStream_t)stream);
+}
+
+// Nystrom passes (spectral.py:237-270): fp32 rows with d <= 64, l <= 256 (and k <= 64 outputs) run on the tensor-core
+// kernel's COLSUM / EMBED epilogues; every other shape, float64 rows and unaligned fp32 rows on the CUDA-core kernel
+static ChunkArgs nystrom_args(const void* X, int64_t n, int d, int64_t ldx, const void* pack, int l, double gamma) {
+  ChunkArgs a = {};
+  a.X = X; a.n = n; a.d = d; a.ldx = ldx;
+  a.pack = (const unsigned char*)pack;
+  a.L = pack_layout(l, d, BKM_F32);
+  a.k = l;
+  a.xf_gamma = gamma;
+  return a;
+}
+
+int bkm_kernel_colsum_chunk(const void* X, int64_t n, int d, int64_t ldx, int x_dtype, const void* pack, int l,
+                            double gamma, double* colsum, void* workspace, size_t workspace_bytes, int flags,
+                            void* stream) {
+  if (n < 0 || d <= 0 || l <= 0 || ldx < d || !pack || !colsum || !workspace) return BKM_EINVAL;
+  if (x_dtype != BKM_F32 && x_dtype != BKM_F64) return BKM_EDTYPE;
+  if (n > 0 && !X) return BKM_EINVAL;
+  cudaStream_t s = (cudaStream_t)stream;
+  const int first = (flags & BKM_FLAG_FIRST_CHUNK) ? 1 : 0;
+  if (n == 0) {
+    if (first) BKM_CUDA_TRY(cudaMemsetAsync(colsum, 0, (size_t)l * sizeof(double), s));
+    return 0;
+  }
+  int sm = 0;
+  int rc = sm_count_of_current(&sm);
+  if (rc) return rc;
+  // The per-CTA partials go behind the workspace's persistent header (WsLayout::off_bal is left alone), into the
+  // per-call area of a chunk call with k = l: it holds at least the counts region, part_slots x l int32 = 4 x SMs
+  // slots of l float64, the most either kernel writes (tensor path: 2 per CTA, one CTA per SM; CUDA cores: <= 4 x SMs
+  // CTAs); launch_tc_colsum / launch_nystrom check the size they need against it.
+  const WsLayout WL = ws_layout(n, d, l, x_dtype, sm);
+  if (workspace_bytes < WL.total) return BKM_EWORKSPACE;
+  double* part = (double*)((unsigned char*)workspace + WL.off_psum);
+  const size_t part_bytes = workspace_bytes - WL.off_psum;
+  int parts = 0;
+  rc = BKM_EALIGN;
+  if (x_dtype == BKM_F32 && tc_supported(d, l, x_dtype) && !(flags & BKM_FLAG_FORCE_SIMT)) {
+    rc = launch_tc_colsum(nystrom_args(X, n, d, ldx, pack, l, gamma), part, part_bytes, sm, &parts, s);
+    if (rc != 0 && (flags & BKM_FLAG_FORCE_TC)) return rc;
+    if (rc != 0 && rc != BKM_EALIGN) return rc;
+  } else if (flags & BKM_FLAG_FORCE_TC) return BKM_EUNSUPPORTED;
+  if (rc != 0) {
+    rc = launch_nystrom(X, n, d, ldx, x_dtype, pack, l, gamma, 0, nullptr, 0, nullptr, 0, part, part_bytes, sm, &parts, s);
+    if (rc) return rc;
+  }
+  return launch_colsum_fold(part, parts, l, colsum, first, s);
+}
+
+int bkm_nystrom_embed_chunk(const void* X, int64_t n, int d, int64_t ldx, int x_dtype, const void* pack, int l,
+                            double gamma, const void* W, int k, void* out, int64_t ld_out, int flags, void* stream) {
+  if (n < 0 || d <= 0 || l <= 0 || k <= 0 || ldx < d || ld_out < k || !pack || !W) return BKM_EINVAL;
+  if (x_dtype != BKM_F32 && x_dtype != BKM_F64) return BKM_EDTYPE;
+  if (n == 0) return 0;
+  if (!X || !out) return BKM_EINVAL;
+  int sm = 0;
+  int rc = sm_count_of_current(&sm);
+  if (rc) return rc;
+  cudaStream_t s = (cudaStream_t)stream;
+  if (x_dtype == BKM_F32 && tc_supported(d, l, x_dtype) && k <= 64 && !(flags & BKM_FLAG_FORCE_SIMT)) {
+    ChunkArgs a = nystrom_args(X, n, d, ldx, pack, l, gamma);
+    a.xf_out = (float*)out; a.xf_ld = ld_out;
+    rc = launch_tc_embed(a, (const float*)W, k, sm, s);
+    if (rc != BKM_EALIGN || (flags & BKM_FLAG_FORCE_TC)) return rc;
+  } else if (flags & BKM_FLAG_FORCE_TC) return BKM_EUNSUPPORTED;
+  int parts = 0;
+  return launch_nystrom(X, n, d, ldx, x_dtype, pack, l, gamma, 1, W, k, out, ld_out, nullptr, 0, sm, &parts, s);
 }
 
 int bkm_finalize(const double* sums, const int64_t* counts, const double* centers_old,

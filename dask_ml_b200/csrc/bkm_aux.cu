@@ -726,6 +726,156 @@ int launch_transform(const void* X, long long n, int d, long long ldx, int dtype
 }
 
 // ---------------------------------------------------------------------------------------
+// Nystrom passes of SpectralClustering (spectral.py:237-282) on the CUDA cores, any shape, computed in the dtype of X:
+//   COLSUM (mode 0): part[cta][j] = sum over the CTA's rows of exp(-gamma y_ij),  y_ij = max(||x_i||^2 - 2 x_i.c_j
+//                    + ||c_j||^2, 0), accumulated in float64 (colsum_fold adds the CTAs in order), for the keep rows
+//                    j0 <= j < j0 + lb of one launch (the host launches one per block of lb keep rows)
+//   EMBED  (mode 1): out_i = e_i / ||e_i||,  e_i = sum_j exp(-gamma (y_ij - m_i)) W_j,  m_i = min_j y_ij; NaN where
+//                    gamma m_i > 745.13 (the float64 reference's kernel row is 0 there).  The l kernel values go through
+//                    shared memory lb at a time; when l > lb, a first sweep finds m_i and the second recomputes y.
+// One warp per row (rows in a fixed order per warp); lane j handles keep rows j, j + 32, ...  Per warp in shared
+// memory: the row, lb kernel values and kw outputs; COLSUM adds the warp's float64 column sums [lb].  Every sum runs
+// over j (rows) in the same order whatever lb is, so the results do not depend on the blocking.
+// ---------------------------------------------------------------------------------------
+template <typename T>
+__global__ void __launch_bounds__(256)
+nystrom_kernel(const T* __restrict__ X, long long n, int d, long long ldx, const unsigned char* __restrict__ pack,
+               PackLayout L, double gamma, int mode, const T* __restrict__ W, int kw, T* __restrict__ out,
+               long long ld_out, double* __restrict__ part, int j0, int lb) {
+  extern __shared__ __align__(16) unsigned char smem[];
+  const int l = L.k, d4 = L.d4, lane = threadIdx.x & 31, wid = threadIdx.x >> 5, nw = blockDim.x >> 5;
+  const size_t per_warp = ((size_t)(d4 + lb + kw) * sizeof(T) + 15) / 16 * 16;
+  double* cacc = reinterpret_cast<double*>(smem);                                           // [nw][lb] (COLSUM)
+  unsigned char* wbase = smem + (mode == 0 ? ((size_t)nw * lb * 8 + 15) / 16 * 16 : 0) + wid * per_warp;
+  T* xw = reinterpret_cast<T*>(wbase);                // [d4]
+  T* vw = xw + d4;                                    // [lb]
+  T* ew = vw + lb;                                    // [kw]
+  const T* C = reinterpret_cast<const T*>(pack + L.off_cT);
+  const T* cn = reinterpret_cast<const T*>(pack + L.off_cnT);
+  const T g = (T)gamma;
+  const bool one = l <= lb;                           // EMBED: every kernel value of a row fits at once
+  if (mode == 0)
+    for (int j = lane; j < lb; j += 32) cacc[wid * lb + j] = 0.0;
+  for (long long row = (long long)blockIdx.x * nw + wid; row < n; row += (long long)gridDim.x * nw) {
+    __syncwarp();
+    for (int i = lane; i < d; i += 32) xw[i] = X[row * ldx + i];
+    __syncwarp();
+    T xn = T(0);
+    for (int i = lane; i < d; i += 32) xn = fma(xw[i], xw[i], xn);
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) xn += __shfl_xor_sync(0xffffffffu, xn, o);   // the same value in every lane
+    auto y_of = [&](int j) {
+      const T* cr = C + (size_t)j * d4;
+      T acc = T(0);
+      for (int i = 0; i < d; ++i) acc = fma(xw[i], cr[i], acc);
+      const T y = xn + cn[j] - T(2) * acc;
+      return y > T(0) ? y : T(0);
+    };
+    if (mode == 0) {
+      for (int j = lane; j < lb; j += 32) cacc[wid * lb + j] += (double)exp(-g * y_of(j0 + j));
+      continue;
+    }
+    T m = T(CUDART_INF);
+    for (int j = lane; j < l; j += 32) {
+      const T y = y_of(j);
+      if (one) vw[j] = y;
+      m = y < m ? y : m;
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) { const T v = __shfl_xor_sync(0xffffffffu, m, o); m = v < m ? v : m; }
+    for (int o = lane; o < kw; o += 32) ew[o] = T(0);
+    for (int b0 = 0; b0 < l; b0 += lb) {
+      const int nb = min(lb, l - b0);
+      for (int j = lane; j < nb; j += 32) vw[j] = exp(-g * ((one ? vw[j] : y_of(b0 + j)) - m));
+      __syncwarp();
+      for (int o = lane; o < kw; o += 32) {
+        T e = ew[o];
+        for (int j = 0; j < nb; ++j) e = fma(vw[j], W[(size_t)(b0 + j) * kw + o], e);
+        ew[o] = e;
+      }
+      __syncwarp();
+    }
+    T nrm = T(0);
+    for (int o = lane; o < kw; o += 32) nrm = fma(ew[o], ew[o], nrm);
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) nrm += __shfl_xor_sync(0xffffffffu, nrm, o);
+    const T f = ((double)m * gamma > 745.13) ? T(CUDART_NAN) : T(1) / sqrt(nrm);
+    for (int o = lane; o < kw; o += 32) out[row * ld_out + o] = ew[o] * f;
+  }
+  if (mode != 0) return;
+  __syncthreads();
+  for (int j = threadIdx.x; j < lb; j += blockDim.x) {
+    double s = 0.0;
+    for (int w = 0; w < nw; ++w) s += cacc[w * lb + j];
+    part[(size_t)blockIdx.x * l + j0 + j] = s;
+  }
+}
+
+// colsum[j] (+)= sum of the partial slots p = 0, 1, ... in order (first: overwrite)
+__global__ void colsum_fold_kernel(const double* __restrict__ part, int parts, int l, double* colsum, int first) {
+  for (int j = blockIdx.x * blockDim.x + threadIdx.x; j < l; j += gridDim.x * blockDim.x) {
+    double s = 0.0;
+    for (int p = 0; p < parts; ++p) s += part[(size_t)p * l + j];
+    colsum[j] = first ? s : colsum[j] + s;
+  }
+}
+
+int launch_colsum_fold(const double* part, int parts, int l, double* colsum, int first, cudaStream_t s) {
+  colsum_fold_kernel<<<(l + 255) / 256, 256, 0, s>>>(part, parts, l, colsum, first);
+  note_launch();
+  BKM_CUDA_TRY(cudaGetLastError());
+  return 0;
+}
+
+// mode 0: column sums into part ([grid][l] float64, *parts_out = grid); mode 1: embedding rows into out.
+// Shared memory decides the warps per CTA (8 down to 1) and the block of keep rows lb (l down to 32).
+int launch_nystrom(const void* X, long long n, int d, long long ldx, int dtype, const void* pack, int l, double gamma,
+                   int mode, const void* W, int kw, void* out, long long ld_out, double* part, size_t part_bytes,
+                   int sm_count, int* parts_out, cudaStream_t s) {
+  PackLayout L = pack_layout(l, d, dtype);
+  const size_t esz = dtype == BKM_F64 ? 8 : 4;
+  auto smem_of = [&](int w, int b) {
+    return (mode == 0 ? align_up((size_t)w * b * 8, 16) : 0) + (size_t)w * align_up((size_t)(L.d4 + b + kw) * esz, 16);
+  };
+  int nw = 8, lb = l;
+  while (smem_of(nw, lb) > 200 * 1024) {
+    if (lb > 1024) lb = (lb / 2 + 31) / 32 * 32;
+    else if (nw > 1) nw >>= 1;
+    else if (lb > 32) lb = (lb / 2 + 31) / 32 * 32;
+    else break;
+  }
+  const size_t smem = smem_of(nw, lb);
+  if (smem > 227 * 1024) return BKM_EUNSUPPORTED;      // a row of X plus k outputs alone exceed shared memory
+  long long grid = (n + nw - 1) / nw;
+  if (grid > (long long)sm_count * 4) grid = (long long)sm_count * 4;
+  if (grid < 1) grid = 1;
+  if (mode == 0) {
+    if ((size_t)grid * l * 8 > part_bytes) return BKM_EWORKSPACE;
+    *parts_out = (int)grid;
+  }
+  if (dtype == BKM_F32)
+    BKM_CUDA_TRY(cudaFuncSetAttribute(nystrom_kernel<float>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  else
+    BKM_CUDA_TRY(cudaFuncSetAttribute(nystrom_kernel<double>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  // COLSUM: one launch per block of lb keep rows; EMBED: one launch (the kernel walks the blocks itself)
+  for (int j0 = 0; j0 < l; j0 += lb) {
+    const int nb = mode == 0 ? (l - j0 < lb ? l - j0 : lb) : lb;
+    if (dtype == BKM_F32)
+      nystrom_kernel<float><<<(int)grid, nw * 32, smem, s>>>((const float*)X, n, d, ldx, (const unsigned char*)pack, L,
+                                                             gamma, mode, (const float*)W, kw, (float*)out, ld_out, part,
+                                                             j0, nb);
+    else
+      nystrom_kernel<double><<<(int)grid, nw * 32, smem, s>>>((const double*)X, n, d, ldx, (const unsigned char*)pack, L,
+                                                              gamma, mode, (const double*)W, kw, (double*)out, ld_out,
+                                                              part, j0, nb);
+    note_launch();
+    BKM_CUDA_TRY(cudaGetLastError());
+    if (mode != 0) break;
+  }
+  return 0;
+}
+
+// ---------------------------------------------------------------------------------------
 // k-means|| rounds (k_means.py:423-431 / 466-469): the reference re-evaluates the distances to ALL candidates every
 // round; min_j d(x, c_j) over a growing set is the running minimum of the per-round minima.  This kernel folds the
 // minima of the new candidates into the running minimum and sums the result (the cost phi) in one pass, with a fixed

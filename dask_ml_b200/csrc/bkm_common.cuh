@@ -227,6 +227,8 @@ bool tc_supported(int d, int k, int dtype);
 int launch_tc(const ChunkArgs& a, bool mstep, int sm_count, int* grid_out, cudaStream_t s);
 int launch_tc_recheck(const ChunkArgs& a, bool mstep, int sm_count, cudaStream_t s);
 int launch_tc_transform(const ChunkArgs& a, int sm_count, cudaStream_t s);
+int launch_tc_colsum(const ChunkArgs& a, double* part, size_t part_bytes, int sm_count, int* parts_out, cudaStream_t s);
+int launch_tc_embed(const ChunkArgs& a, const float* W, int kw, int sm_count, cudaStream_t s);
 int tc_trace(long long* out, int n);
 // implemented in bkm_stream.cu
 bool stream_supported(int d, int k, int dtype);

@@ -44,6 +44,28 @@ struct TcCfg {
   uint32_t off_bhi, off_blo, off_x, off_sum, off_cn, off_cnt, off_lab, off_dp, off_red, off_cls, total;
 };
 
+// Epilogue of tc_chunk_kernel (all four share the MMAs, the tile pipeline and the A-fragment build):
+//   ARGMIN  labels / M-step (the Lloyd and assign chunk calls)
+//   XFORM   the whole (rows x k) block of distances / kernel values (bkm_transform_chunk)
+//   COLSUM  per column j of the keep set: sum over rows of exp(-gamma d^2(x, c_j)) (bkm_kernel_colsum_chunk)
+//   EMBED   per row: e = sum_j exp(-gamma (d^2(x, c_j) - min_j d^2)) W_j, written as e / ||e|| (bkm_nystrom_embed_chunk)
+enum TcEpi { EPI_ARGMIN = 0, EPI_XFORM = 1, EPI_COLSUM = 2, EPI_EMBED = 3 };
+static const int TC_EMBED_MAXK = 64;      // outputs of the EMBED epilogue (W rows are staged in shared memory)
+// gamma * min_j d^2 beyond which the float64 reference's kernel row underflows to 0 everywhere (exp(-745.14) == 0 in
+// float64): such rows are written as NaN, as the reference's 0 / 0 normalisation gives
+static const double NYS_UNDERFLOW = 745.13;
+// The Nystrom variants' configuration: per-warp column sums of a tile (COLSUM); the projection weights W [N][wp] fp32
+// (EMBED: kw outputs, row pitch wp = ceil(kw/8)*8 + 4).  A type of its own, so that the ARGMIN / XFORM variants keep
+// their parameter layout (and code) unchanged.
+struct TcCfgNys : TcCfg {
+  uint32_t off_cs, off_w;
+  int kw, wp;
+  const float* w;
+};
+template <int EPI> struct TcCfgOf { using type = TcCfg; };
+template <> struct TcCfgOf<EPI_COLSUM> { using type = TcCfgNys; };
+template <> struct TcCfgOf<EPI_EMBED> { using type = TcCfgNys; };
+
 // The deferred-row re-check reports a failed fused kernel through this word (see tc_recheck_kernel); the wgmma kernel
 // has no waits that can time out, so it stays 0 unless a debugging build sets it.
 __device__ unsigned int g_tc_abort = 0;
@@ -63,11 +85,13 @@ __device__ __forceinline__ uint32_t pack_half2(float lo, float hi) {
   return *reinterpret_cast<const uint32_t*>(&h);
 }
 
-// XFORM: the epilogue writes the whole (rows x k) block of distances / kernel values instead of the arg-min
-// (euclidean_distances, dask_ml/metrics/pairwise.py:69-97; rbf_kernel :131-139) — same MMAs, no M-step.
-template <int N, int KS, bool MSTEP, bool WANT_DIST, bool XFORM>
+// EPI (TcEpi): XFORM writes the whole (rows x k) block of distances / kernel values instead of the arg-min
+// (euclidean_distances, dask_ml/metrics/pairwise.py:69-97; rbf_kernel :131-139); COLSUM and EMBED are the two passes
+// of the Nystrom embedding (dask_ml/cluster/spectral.py:237-282).  Same MMAs, no M-step.
+template <int N, int KS, bool MSTEP, bool WANT_DIST, int EPI>
 __global__ void __launch_bounds__(TC_THREADS, 1)
-tc_chunk_kernel(ChunkArgs a, TcCfg cfg) {
+tc_chunk_kernel(ChunkArgs a, typename TcCfgOf<EPI>::type cfg) {
+  constexpr bool XFORM = EPI == EPI_XFORM;
   if (a.skip && *a.skip) return;                            // converged loop: no-op iteration
 
   extern __shared__ __align__(1024) unsigned char smem[];
@@ -87,7 +111,7 @@ tc_chunk_kernel(ChunkArgs a, TcCfg cfg) {
   const PackHeader* hdr = reinterpret_cast<const PackHeader*>(a.pack);
   const float sc = hdr->scale;
   const float inv_s = 1.0f / sc;                             // exact: s is a power of two, s and 1/s are normal
-  const float gs = XFORM ? (float)(a.xf_gamma * (double)inv_s * (double)inv_s) : 0.f;   // rbf: gamma / s^2
+  const float gs = EPI != EPI_ARGMIN ? (float)(a.xf_gamma * (double)inv_s * (double)inv_s) : 0.f;   // rbf: gamma / s^2
 
   // ---------------- setup: B tiles, column offsets, sums ----------------
   {
@@ -111,6 +135,14 @@ tc_chunk_kernel(ChunkArgs a, TcCfg cfg) {
     }
     if (MSTEP)
       for (int i = tid; i < (N + 2) * 64; i += TC_THREADS) sum_s[i] = 0.f;
+    if constexpr (EPI == EPI_EMBED) {
+      // W rows j < k (keep rows), outputs o < kw; zero elsewhere
+      float* w_s = reinterpret_cast<float*>(smem + cfg.off_w);
+      for (int i = tid; i < N * cfg.wp; i += TC_THREADS) {
+        const int j = i / cfg.wp, o = i - j * cfg.wp;
+        w_s[i] = (j < k && o < cfg.kw) ? cfg.w[(size_t)j * cfg.kw + o] : 0.f;
+      }
+    }
     wg::fence_proxy_async();                                 // generic-proxy stores -> visible to wgmma
   }
   __syncthreads();
@@ -142,6 +174,7 @@ tc_chunk_kernel(ChunkArgs a, TcCfg cfg) {
   const uint64_t dbh = wg::desc_sw128(sbase + cfg.off_bhi), dbl = wg::desc_sw128(sbase + cfg.off_blo);
   const float cnmax = (float)(hdr->cn_max * (double)sc * (double)sc);
   double dsum = 0.0;
+  double cs0 = 0.0, cs1 = 0.0;                               // COLSUM: this warpgroup's sums of columns t, t + 128
 
   load_tile(0, 0);
 #pragma unroll 1
@@ -197,7 +230,112 @@ tc_chunk_kernel(ChunkArgs a, TcCfg cfg) {
         wg::commit();
       }
 
-      if (XFORM) {
+      if constexpr (EPI == EPI_COLSUM) {
+        wg::wait_all();
+        wg::pin(acc);
+        // v = exp(-(gamma / s^2) y) of the tile's real rows; per column the warp's 16 rows are added by a fixed shuffle
+        // tree (rows rA, rA + 8 in the thread, then lanes g = 0..7), the 4 warps' sums in warp order, all in fp32; the
+        // tile's sum then goes into the thread's float64 accumulator of that column
+        const bool ok0 = row0 + rA < a.n, ok1 = row0 + rA + 8 < a.n;
+        float* cs_s = reinterpret_cast<float*>(smem + cfg.off_cs) + wgi * 4 * N;     // [4 warps][N]
+#pragma unroll
+        for (int i = 0; i < N / 8; ++i) {
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int col = 8 * i + c2 + e;
+            float v = ok0 ? __expf(-gs * fmaxf((acc[4 * i + e] + cn_s[col]) + xn0, 0.f)) : 0.f;
+            if (ok1) v += __expf(-gs * fmaxf((acc[4 * i + 2 + e] + cn_s[col]) + xn1, 0.f));
+            v += __shfl_xor_sync(0xffffffffu, v, 4);
+            v += __shfl_xor_sync(0xffffffffu, v, 8);
+            v += __shfl_xor_sync(0xffffffffu, v, 16);
+            if (g == 0) cs_s[wq * N + col] = v;
+          }
+        }
+        wg::wg_sync(1 + wgi);
+        if (t < N) cs0 += (double)(((cs_s[t] + cs_s[N + t]) + cs_s[2 * N + t]) + cs_s[3 * N + t]);
+        if (t + 128 < N) cs1 += (double)(((cs_s[t + 128] + cs_s[N + t + 128]) + cs_s[2 * N + t + 128]) + cs_s[3 * N + t + 128]);
+      } else if constexpr (EPI == EPI_EMBED) {
+        wg::wait_all();
+        wg::pin(acc);
+        // y (clamped at 0) and the row minimum m over the real columns (the quad holds a row's columns)
+        float m0 = CUDART_INF_F, m1 = CUDART_INF_F;
+#pragma unroll
+        for (int i = 0; i < N / 8; ++i) {
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int col = 8 * i + c2 + e;
+            const float y0 = fmaxf((acc[4 * i + e] + cn_s[col]) + xn0, 0.f);
+            const float y1 = fmaxf((acc[4 * i + 2 + e] + cn_s[col]) + xn1, 0.f);
+            acc[4 * i + e] = y0; acc[4 * i + 2 + e] = y1;
+            if (col < k) { m0 = fminf(m0, y0); m1 = fminf(m1, y1); }
+          }
+        }
+        m0 = fminf(m0, __shfl_xor_sync(0xffffffffu, m0, 1)); m0 = fminf(m0, __shfl_xor_sync(0xffffffffu, m0, 2));
+        m1 = fminf(m1, __shfl_xor_sync(0xffffffffu, m1, 1)); m1 = fminf(m1, __shfl_xor_sync(0xffffffffu, m1, 2));
+        // v = exp(-(gamma / s^2)(y - m)): the largest term of a row is 1, so fp32 does not underflow where the float64
+        // reference does not (the shift cancels in the normalisation)
+#pragma unroll
+        for (int i = 0; i < N / 8; ++i) {
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const bool real = 8 * i + c2 + e < k;
+            acc[4 * i + e] = real ? __expf(-gs * (acc[4 * i + e] - m0)) : 0.f;
+            acc[4 * i + 2 + e] = real ? __expf(-gs * (acc[4 * i + 2 + e] - m1)) : 0.f;
+          }
+        }
+        // e = v . W in groups of 8 outputs: per thread over its columns, then the quad's 4 partial sums (the same
+        // value lands in all 4 lanes); lane q of the quad stages outputs 2q, 2q + 1 of the group in the tile's X stage
+        // (rows of this warp only: their A fragments are built and consumed)
+        const float* w_s = reinterpret_cast<const float*>(smem + cfg.off_w);
+        float* est = reinterpret_cast<float*>(smem + cfg.off_x) + (wgi * 2 + stage) * TBM * XP;
+        const int q = lane & 3;
+        float n0 = 0.f, n1 = 0.f;
+        __syncwarp();
+#pragma unroll 1
+        for (int o0 = 0; o0 < cfg.kw; o0 += 8) {
+          float e0[8], e1[8];
+#pragma unroll
+          for (int o = 0; o < 8; ++o) { e0[o] = 0.f; e1[o] = 0.f; }
+#pragma unroll
+          for (int i = 0; i < N / 8; ++i) {
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const float* wr = w_s + (8 * i + c2 + e) * cfg.wp + o0;
+              const float4 wa = *reinterpret_cast<const float4*>(wr), wb = *reinterpret_cast<const float4*>(wr + 4);
+              const float w8[8] = {wa.x, wa.y, wa.z, wa.w, wb.x, wb.y, wb.z, wb.w};
+              const float va = acc[4 * i + e], vb = acc[4 * i + 2 + e];
+#pragma unroll
+              for (int o = 0; o < 8; ++o) { e0[o] = fmaf(va, w8[o], e0[o]); e1[o] = fmaf(vb, w8[o], e1[o]); }
+            }
+          }
+#pragma unroll
+          for (int o = 0; o < 8; ++o) {
+            e0[o] += __shfl_xor_sync(0xffffffffu, e0[o], 1); e0[o] += __shfl_xor_sync(0xffffffffu, e0[o], 2);
+            e1[o] += __shfl_xor_sync(0xffffffffu, e1[o], 1); e1[o] += __shfl_xor_sync(0xffffffffu, e1[o], 2);
+            n0 = fmaf(e0[o], e0[o], n0); n1 = fmaf(e1[o], e1[o], n1);       // outputs >= kw are 0 (W is zero padded)
+          }
+          const float2 p0 = q == 0 ? make_float2(e0[0], e0[1]) : q == 1 ? make_float2(e0[2], e0[3])
+                          : q == 2 ? make_float2(e0[4], e0[5]) : make_float2(e0[6], e0[7]);
+          const float2 p1 = q == 0 ? make_float2(e1[0], e1[1]) : q == 1 ? make_float2(e1[2], e1[3])
+                          : q == 2 ? make_float2(e1[4], e1[5]) : make_float2(e1[6], e1[7]);
+          *reinterpret_cast<float2*>(est + rA * XP + o0 + 2 * q) = p0;
+          *reinterpret_cast<float2*>(est + (rA + 8) * XP + o0 + 2 * q) = p1;
+        }
+        // per-row factor 1 / ||e||; NaN where gamma * m (unscaled, float64) is beyond the float64 reference's underflow
+        if (q == 0) {
+          const double gsd = a.xf_gamma * (double)inv_s * (double)inv_s;
+          dp_s[rA] = ((double)m0 * gsd > NYS_UNDERFLOW) ? CUDART_NAN_F : 1.0f / sqrtf(n0);
+          dp_s[rA + 8] = ((double)m1 * gsd > NYS_UNDERFLOW) ? CUDART_NAN_F : 1.0f / sqrtf(n1);
+        }
+        __syncwarp();
+        // the warp writes its 16 rows, consecutive lanes on consecutive outputs
+        const int kw = cfg.kw;
+        for (int e = lane; e < 16 * kw; e += 32) {
+          const int rr = e / kw, o = e - rr * kw, r = wq * 16 + rr;
+          const long long row = row0 + r;
+          if (row < a.n) __stcs(a.xf_out + row * a.xf_ld + o, est[r * XP + o] * dp_s[r]);
+        }
+      } else if constexpr (EPI == EPI_XFORM) {
         wg::wait_all();
         wg::pin(acc);
         // y = acc + s^2 ||c||^2 + ||s x||^2 = s^2 d^2, clamped at 0; mode 0: sqrt(y) / s, 1: y / s / s, 2: exp(-(gamma /
@@ -229,6 +367,7 @@ tc_chunk_kernel(ChunkArgs a, TcCfg cfg) {
         else if (a.xf_mode == 1) store_block([&](float y) { return (y * inv_s) * inv_s; });
         else store_block([&](float y) { return __expf(-gs * y); });
       } else {
+        static_assert(EPI == EPI_ARGMIN, "epilogue");
         // ---- arg-min, near-tie test (bound = tau (||s x||^2 + max ||s c||^2)) ----
         // columns still reach each thread in increasing order: the lowest column wins exact ties as before
         wg::Best2 b0 = wg::best2_init(), b1 = b0;
@@ -391,6 +530,13 @@ tc_chunk_kernel(ChunkArgs a, TcCfg cfg) {
       gs[i] = sum_s[c * 64 + (i - c * d)];
     }
     for (int c = tid; c < k; c += TC_THREADS) a.pcnt[(size_t)blockIdx.x * k + c] = cnt_s[c];
+  }
+  if constexpr (EPI == EPI_COLSUM) {
+    // partial column sums of warpgroup wgi of this CTA -> slot 2 * CTA + wgi (colsum_fold adds the slots in order)
+    double* part = a.pin + (size_t)(2 * blockIdx.x + wgi) * k;
+    if (t < k) part[t] = cs0;
+    if (t + 128 < k) part[t + 128] = cs1;
+    return;
   }
   red_s[tid] = dsum;
   __syncthreads();
@@ -556,15 +702,28 @@ static bool make_cfg(int d, int k, bool mstep, TcCfg* c) {
   return o <= 227u * 1024u;
 }
 
-template <int N, int KS, bool M, bool W, bool XF>
-static int launch_variant(const ChunkArgs& a, const TcCfg& cfg, int grid, cudaStream_t s) {
+static bool make_cfg_nys(int d, int k, int epi, int kw, TcCfgNys* c) {
+  make_cfg(d, k, false, c);
+  const uint32_t N = (uint32_t)wg::mma_n(c->NP);
+  uint32_t o = c->total;
+  c->off_cs = o; if (epi == EPI_COLSUM) o += 2u * 4u * N * 4u;     // per-warp column sums of a tile
+  c->kw = kw;
+  c->wp = (kw + 7) / 8 * 8 + 4;                     // 4 mod 8 floats: the quad's 4 W rows of a float4 load hit 4 bank groups
+  c->w = nullptr;
+  c->off_w = o; if (epi == EPI_EMBED) o += N * (uint32_t)c->wp * 4u;   // (every offset above is a multiple of 16)
+  c->total = o;
+  return o <= 227u * 1024u;
+}
+
+template <int N, int KS, bool M, bool W, int XF>
+static int launch_variant(const ChunkArgs& a, const typename TcCfgOf<XF>::type& cfg, int grid, cudaStream_t s) {
   auto kern = tc_chunk_kernel<N, KS, M, W, XF>;
   BKM_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cfg.total));
   kern<<<grid, TC_THREADS, cfg.total, s>>>(a, cfg);
   return 0;
 }
-template <int N, bool M, bool W, bool XF>
-static int launch_ks(const ChunkArgs& a, const TcCfg& cfg, int grid, cudaStream_t s) {
+template <int N, bool M, bool W, int XF>
+static int launch_ks(const ChunkArgs& a, const typename TcCfgOf<XF>::type& cfg, int grid, cudaStream_t s) {
   switch (cfg.KS) {
     case 1: return launch_variant<N, 1, M, W, XF>(a, cfg, grid, s);
     case 2: return launch_variant<N, 2, M, W, XF>(a, cfg, grid, s);
@@ -572,8 +731,8 @@ static int launch_ks(const ChunkArgs& a, const TcCfg& cfg, int grid, cudaStream_
     default: return launch_variant<N, 4, M, W, XF>(a, cfg, grid, s);
   }
 }
-template <bool M, bool W, bool XF>
-static int launch_n(const ChunkArgs& a, const TcCfg& cfg, int grid, cudaStream_t s) {
+template <bool M, bool W, int XF>
+static int launch_n(const ChunkArgs& a, const typename TcCfgOf<XF>::type& cfg, int grid, cudaStream_t s) {
   switch (wg::mma_n(cfg.NP)) {
     case 16: return launch_ks<16, M, W, XF>(a, cfg, grid, s);
     case 32: return launch_ks<32, M, W, XF>(a, cfg, grid, s);
@@ -598,8 +757,8 @@ int launch_tc(const ChunkArgs& a, bool mstep, int sm_count, int* grid_out, cudaS
   *grid_out = grid;
   BKM_CUDA_TRY(cudaMemsetAsync(a.defer_cnt, 0, sizeof(int), s));
   int rc;
-  if (mstep) rc = want_dist ? launch_n<true, true, false>(a, cfg, grid, s) : launch_n<true, false, false>(a, cfg, grid, s);
-  else rc = want_dist ? launch_n<false, true, false>(a, cfg, grid, s) : launch_n<false, false, false>(a, cfg, grid, s);
+  if (mstep) rc = want_dist ? launch_n<true, true, EPI_ARGMIN>(a, cfg, grid, s) : launch_n<true, false, EPI_ARGMIN>(a, cfg, grid, s);
+  else rc = want_dist ? launch_n<false, true, EPI_ARGMIN>(a, cfg, grid, s) : launch_n<false, false, EPI_ARGMIN>(a, cfg, grid, s);
   if (rc) return rc;
   note_launch(2);
   BKM_CUDA_TRY(cudaGetLastError());
@@ -611,7 +770,39 @@ int launch_tc_transform(const ChunkArgs& a, int sm_count, cudaStream_t s) {
   if ((reinterpret_cast<uintptr_t>(a.X) & 15) || (a.ldx % 4)) return BKM_EALIGN;
   TcCfg cfg;
   if (!make_cfg(a.d, a.k, false, &cfg)) return BKM_EUNSUPPORTED;
-  const int rc = launch_n<false, false, true>(a, cfg, tc_grid(a.n, sm_count), s);
+  const int rc = launch_n<false, false, EPI_XFORM>(a, cfg, tc_grid(a.n, sm_count), s);
+  if (rc) return rc;
+  note_launch();
+  BKM_CUDA_TRY(cudaGetLastError());
+  return 0;
+}
+
+// Nystrom column sums on the tensor path: per-warpgroup partials [2 * grid][k] (float64) into `part`; returns the number
+// of partial slots written, which colsum_fold adds in slot order
+int launch_tc_colsum(const ChunkArgs& a, double* part, size_t part_bytes, int sm_count, int* parts_out, cudaStream_t s) {
+  if ((reinterpret_cast<uintptr_t>(a.X) & 15) || (a.ldx % 4)) return BKM_EALIGN;
+  TcCfgNys cfg;
+  if (!make_cfg_nys(a.d, a.k, EPI_COLSUM, 0, &cfg)) return BKM_EUNSUPPORTED;
+  const int grid = tc_grid(a.n, sm_count);
+  if ((size_t)2 * grid * a.k * sizeof(double) > part_bytes) return BKM_EWORKSPACE;
+  ChunkArgs b = a;
+  b.pin = part;
+  const int rc = launch_n<false, false, EPI_COLSUM>(b, cfg, grid, s);
+  if (rc) return rc;
+  *parts_out = 2 * grid;
+  note_launch();
+  BKM_CUDA_TRY(cudaGetLastError());
+  return 0;
+}
+
+// Nystrom embedding rows on the tensor path (kw <= TC_EMBED_MAXK outputs, W fp32 [k][kw]); out = a.xf_out, pitch a.xf_ld
+int launch_tc_embed(const ChunkArgs& a, const float* W, int kw, int sm_count, cudaStream_t s) {
+  if ((reinterpret_cast<uintptr_t>(a.X) & 15) || (a.ldx % 4)) return BKM_EALIGN;
+  if (kw < 1 || kw > TC_EMBED_MAXK) return BKM_EUNSUPPORTED;
+  TcCfgNys cfg;
+  if (!make_cfg_nys(a.d, a.k, EPI_EMBED, kw, &cfg)) return BKM_EUNSUPPORTED;
+  cfg.w = W;
+  const int rc = launch_n<false, false, EPI_EMBED>(a, cfg, tc_grid(a.n, sm_count), s);
   if (rc) return rc;
   note_launch();
   BKM_CUDA_TRY(cudaGetLastError());

@@ -383,6 +383,28 @@ class CudaBackend(object):
                 self._ptr(out), out.stride(0) if n else k, int(mode), float(gamma), self.flags, self._stream()),
                 "bkm_transform_chunk")
 
+    def kernel_colsum(self, x, pack, l, gamma, colsum, first=False):
+        """colsum[j] (+)= sum_i exp(-gamma ||x_i - c_j||^2) over the rows of the chunk (float64 [l]); ``first`` overwrites.
+        The first pass of the Nystrom embedding (SpectralClustering)."""
+        n, d = x.shape
+        ws = self._workspace(n, d, l, x.dtype)
+        flags = self.flags | (_lib.FLAG_FIRST_CHUNK if first else 0)
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.bkm_kernel_colsum_chunk(
+                self._ptr(x), n, d, x.stride(0) if n else d, _DT_CODE[x.dtype], self._ptr(pack), int(l), float(gamma),
+                self._ptr(colsum), self._ptr(ws), ws.numel(), flags, self._stream()), "bkm_kernel_colsum_chunk")
+
+    def nystrom_embed(self, x, pack, l, gamma, W, out):
+        """out[i] = e_i / ||e_i||, e_i = sum_j exp(-gamma (||x_i - c_j||^2 - min_j ||x_i - c_j||^2)) W[j] — the second
+        pass of the Nystrom embedding.  ``W`` is (l, k) in the dtype of x; ``out`` (n, k) may have a padded row pitch."""
+        n, d = x.shape
+        k = int(W.shape[1])
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.bkm_nystrom_embed_chunk(
+                self._ptr(x), n, d, x.stride(0) if n else d, _DT_CODE[x.dtype], self._ptr(pack), int(l), float(gamma),
+                self._ptr(W), k, self._ptr(out), out.stride(0) if n else k, self.flags, self._stream()),
+                "bkm_nystrom_embed_chunk")
+
     def finalize(self, sums, counts, C_old, C_new, shift):
         k, d = C_old.shape
         with torch.cuda.device(self.device):

@@ -18,6 +18,8 @@
  *     k_means.py:466-491, pairwise.py:55-66
  *   metrics.euclidean_distances(X, Y)  pairwise.py:69-97          bkm_transform_chunk
  *   da.isnull(X).any(), da.isinf(X).any()  k_means.py:179-180     bkm_check_finite
+ *   pairwise_kernels(X_keep, X_rest) and the products with B of   bkm_kernel_colsum_chunk
+ *     SpectralClustering.fit, cluster/spectral.py:237-270          bkm_nystrom_embed_chunk
  *
  * Conventions
  *   - extern "C", plain pointers and sizes only; no torch / C++ types.
@@ -143,6 +145,27 @@ int bkm_min_fold_chunk(void* run_min, const void* new_min, int64_t n, int x_dtyp
 int bkm_transform_chunk(const void* X, int64_t n, int d, int64_t ldx, int x_dtype,
                         const void* pack, int k, void* out, int64_t ld_out, int mode, double gamma, int flags,
                         void* stream);
+
+/* ---- SpectralClustering: the two passes of the Nystrom embedding -------------------------------------------------
+ * replace per chunk: pairwise_kernels(X_keep, X_rest, 'rbf') and every product with B in spectral.py:237-270
+ * (A.sum(0) + B.sum(1), [A2; B2^T] . U . diag(S^-1/2) and the row normalisation of spectral.py:282).  The keep rows are
+ * an ordinary centre pack (bkm_pack_centers with k = l).  With y_ij = max(||x_i - c_j||^2, 0) computed as in
+ * bkm_transform_chunk:
+ *   bkm_kernel_colsum_chunk  colsum[j] (l, float64) = sum_i exp(-gamma y_ij); OVERWRITTEN with BKM_FLAG_FIRST_CHUNK,
+ *                            else ACCUMULATED (+=).  Rows, then per-CTA partials, are added in a fixed order:
+ *                            bit-reproducible on one device.  workspace: bkm_workspace_bytes(n, d, l, x_dtype) bytes
+ *                            (the same buffer as the chunk calls: its persistent header is left alone).
+ *   bkm_nystrom_embed_chunk  out[i][0..k) = e_i / ||e_i||, e_i = sum_j exp(-gamma (y_ij - min_j y_ij)) W[j][0..k)
+ *                            (W [l][k] row-major, x-dtype; out x-dtype with row pitch ld_out >= k).  The row shift
+ *                            cancels in the normalisation and keeps fp32 from underflowing; a row with
+ *                            gamma * min_j y_ij > 745.13 is written as NaN (the float64 reference gives 0 / 0 there).
+ * fp32 rows with d <= 64, l <= 256 (embed: k <= 64) and 16-byte rows run on the tensor-core kernel; other shapes and
+ * float64 rows on the CUDA cores (float64 throughout).  Honours BKM_FLAG_FORCE_SIMT / BKM_FLAG_FORCE_TC. */
+int bkm_kernel_colsum_chunk(const void* X, int64_t n, int d, int64_t ldx, int x_dtype, const void* pack, int l,
+                            double gamma, double* colsum, void* workspace, size_t workspace_bytes, int flags,
+                            void* stream);
+int bkm_nystrom_embed_chunk(const void* X, int64_t n, int d, int64_t ldx, int x_dtype, const void* pack, int l,
+                            double gamma, const void* W, int k, void* out, int64_t ld_out, int flags, void* stream);
 
 /* ---- centre update + shift (k_means.py:548-555), run after the cross-GPU allreduce ----
  *   C_new = sums / max(counts,1)[:,None]   (empty cluster -> zero vector, Q1)
