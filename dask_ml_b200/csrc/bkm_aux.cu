@@ -11,95 +11,23 @@ namespace bkm {
 std::atomic<long long> g_launches{0};
 
 // ---------------------------------------------------------------------------------------
-// pack_centers: float64 centres [k][d] -> every layout the kernels read (see PackLayout).
-//   cT   [k][d4]  x-dtype, zero padded          cnT  [k] x-dtype   ||c||^2 (computed in f64)
-//   c64  [k][d]   float64 copy                  cn64 [k] float64
-//   bhi  [kp][64] fp16: rn(-2 s c)              blo  [kp][64] fp16: rn(-2 s c - bhi)   (s = header scale)
-//   cn32 [kp]     fp32 ||c||^2, +inf for padded centres
+// Centre pack: float64 centres [k][d] -> every layout the kernels read (offsets: pack_layout, bkm_common.cuh).
+//   header     PackHeader: cn_max = max_j ||c_j||^2 and the scale s
+//   cT   [k][d4] x-dtype (bf16 rows: fp32), zero padded      cnT  [k] the same dtype: ||c||^2
+//   c64  [k][d]  float64 copy                                 cn64 [k] float64 ||c||^2
+// family 1 (tc_supported, bkm_tc.cu):
+//   bhi / blo [kp][64] fp16: rn(-2 s c), rn(-2 s c - bhi)     cns  [kp] fp32: rn(s^2 ||c||^2), 3e38 beyond k
+//   c64T [d][kp] float64 (re-check)
+// family 3 (tc2_shape, bkm_tc2.cu):
+//   b2hi / b2lo [kp2][dk2] bf16: rn(-2 c), rn(-2 c - b2hi)    cn2  [kp2] fp32: rn(||c||^2), 3e38 beyond k
+//   c64T2 [d][kp2] float64 (re-check)
+// Tile entries beyond (k, d) are zero.  ||c||^2 is computed once, in float64 (pack_norms); every layout rounds that.
+// The writers take the centres from a source: `C(i)` yields element i of the row-major (k, d) float64 centres.
 // ---------------------------------------------------------------------------------------
-__device__ __forceinline__ float to_tf32_rna(float x) {
-  uint32_t r;
-  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
-  return __uint_as_float(r);
-}
-
-__global__ void pack_centers_kernel(const double* __restrict__ C, unsigned char* pack, PackLayout L) {
-  const int k = L.k, d = L.d;
-  const int tid = blockIdx.x * blockDim.x + threadIdx.x;
-  const int nth = gridDim.x * blockDim.x;
-  double* c64 = reinterpret_cast<double*>(pack + L.off_c64);
-  for (int i = tid; i < k * d; i += nth) c64[i] = C[i];
-  if (L.dtype != BKM_F64) {
-    float* cT = reinterpret_cast<float*>(pack + L.off_cT);
-    for (int i = tid; i < k * L.d4; i += nth) {
-      int r = i / L.d4, c = i - r * L.d4;
-      cT[i] = c < d ? (float)C[(size_t)r * d + c] : 0.f;
-    }
-    // tensor-core operands: B = -2 s C as an fp16 pair (hi + lo carries 22 significant bits); rows/columns
-    // beyond (k, d) are zero.  Only shapes the tensor path takes (d <= 64) have room in the pack.
-    if (d <= L.dh) {
-      const double sc = (double)reinterpret_cast<const PackHeader*>(pack)->scale;
-      __half* bhi = reinterpret_cast<__half*>(pack + L.off_bhi);
-      __half* blo = reinterpret_cast<__half*>(pack + L.off_blo);
-      for (int i = tid; i < L.kp * L.dh; i += nth) {
-        int r = i / L.dh, c = i - r * L.dh;
-        __half hi = __float2half_rn(0.f), lo = hi;
-        if (r < k && c < d) {
-          const double v = -2.0 * sc * C[(size_t)r * d + c];
-          hi = __double2half(v);
-          lo = __double2half(v - (double)__half2float(hi));
-        }
-        bhi[i] = hi; blo[i] = lo;
-      }
-    }
-  } else {
-    double* cT = reinterpret_cast<double*>(pack + L.off_cT);
-    for (int i = tid; i < k * L.d4; i += nth) {
-      int r = i / L.d4, c = i - r * L.d4;
-      cT[i] = c < d ? C[(size_t)r * d + c] : 0.0;
-    }
-  }
-}
-
-// one warp per centre: ||c||^2 in float64, then block 0 computes the max.
-__global__ void pack_norms_kernel(const double* __restrict__ C, unsigned char* pack, PackLayout L) {
-  const int k = L.k, d = L.d;
-  const int lane = threadIdx.x & 31;
-  const int wid = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const int nw = (gridDim.x * blockDim.x) >> 5;
-  double* cn64 = reinterpret_cast<double*>(pack + L.off_cn64);
-  float* cn32 = reinterpret_cast<float*>(pack + L.off_cn32);
-  for (int j = wid; j < L.kp; j += nw) {
-    double s = 0.0;
-    if (j < k) for (int i = lane; i < d; i += 32) { double v = C[(size_t)j * d + i]; s = fma(v, v, s); }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-    if (lane == 0) {
-      if (j < k) {
-        cn64[j] = s;
-        if (L.dtype != BKM_F64) reinterpret_cast<float*>(pack + L.off_cnT)[j] = (float)s;
-        else reinterpret_cast<double*>(pack + L.off_cnT)[j] = s;
-      }
-      if (L.dtype != BKM_F64) {
-        cn32[j] = j < k ? (float)s : CUDART_INF_F;
-        // ||c_j||^2 as a K=8 tf32 operand row [hi, mid, lo, 0...] (hi+mid+lo == fp32 value exactly) in the
-        // canonical no-swizzle K-major layout: 8-row groups of 256 B = [8 rows x 16 B | 8 rows x 16 B].
-        float* bcn = reinterpret_cast<float*>(pack + L.off_bcn) + (j >> 3) * 64 + (j & 7) * 4;
-        float hi = 3.0e38f, mid = 0.f, lo = 0.f;
-        if (j < k) {
-          const double sc = (double)reinterpret_cast<const PackHeader*>(pack)->scale;
-          const float cf = (float)(s * sc * sc);          // the tensor path works on s X and s C
-          hi = to_tf32_rna(cf);
-          const float r1 = cf - hi;
-          mid = to_tf32_rna(r1);
-          lo = r1 - mid;
-        }
-        bcn[0] = hi; bcn[1] = mid; bcn[2] = lo; bcn[3] = 0.f;
-        bcn[32] = 0.f; bcn[33] = 0.f; bcn[34] = 0.f; bcn[35] = 0.f;
-      }
-    }
-  }
-}
+struct CentreFromMemory {
+  const double* p;
+  __device__ __forceinline__ double operator()(size_t i) const { return p[i]; }
+};
 
 // scale = 2^(9 - floor(log2 max|c|)): s * max|c| in [2^9, 2^10), so -2 s c fits fp16 with a 32x margin and
 // rows of X up to ~64x the largest centre component convert without overflow (larger ones are deferred to
@@ -111,160 +39,173 @@ __device__ __forceinline__ int pack_scale_exp(double max_abs_c) {
   return e > 126 ? 126 : (e < -126 ? -126 : e);
 }
 
-// Runs first: the other pack kernels read the scale.
-__global__ void pack_scale_kernel(const double* __restrict__ C, unsigned char* pack, PackLayout L) {
-  __shared__ double sm[32];
-  double m = 0.0;
-  for (int i = threadIdx.x; i < L.k * L.d; i += blockDim.x) m = fmax(m, fabs(C[i]));
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) m = fmax(m, __shfl_xor_sync(0xffffffffu, m, o));
-  if ((threadIdx.x & 31) == 0) sm[threadIdx.x >> 5] = m;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    for (int w = 1; w < (int)(blockDim.x >> 5); ++w) m = fmax(m, sm[w]);
-    PackHeader* h = reinterpret_cast<PackHeader*>(pack);
-    h->scale = (float)scalbn(1.0, pack_scale_exp(m));
-    h->pad2 = 0.f;
-  }
-}
-
-__global__ void pack_header_kernel(unsigned char* pack, PackLayout L) {
-  const double* cn64 = reinterpret_cast<const double*>(pack + L.off_cn64);
-  __shared__ double sm[32];
-  double m = 0.0;
-  for (int j = threadIdx.x; j < L.k; j += blockDim.x) m = fmax(m, cn64[j]);
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) m = fmax(m, __shfl_xor_sync(0xffffffffu, m, o));
-  if ((threadIdx.x & 31) == 0) sm[threadIdx.x >> 5] = m;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    for (int w = 1; w < (int)(blockDim.x >> 5); ++w) m = fmax(m, sm[w]);
-    PackHeader* h = reinterpret_cast<PackHeader*>(pack);
-    h->k = L.k; h->d = L.d; h->dtype = L.dtype; h->pad = 0; h->cn_max = m;
-  }
-}
-
-// Small (k, d) — every shape the tensor path takes — are packed by ONE kernel: each CTA recomputes the two
-// global quantities (max |c| -> scale, all ||c||^2 -> cn_max; k*d is a few thousand elements) and then writes
-// its share of every layout.  Four dependent launches cost more than the work itself.
-// The body is shared by pack_fused_kernel (centres read from memory) and finalize_step_fused_kernel (centres computed
-// on the fly from the reduced sums and counts): `C(i)` yields element i of the row-major (k, d) float64 centres.
-template <typename Src>
-__device__ __forceinline__ void pack_fused_body(Src C, unsigned char* pack, const PackLayout& L, double* cn_s) {
+// maximum of v over the CTA, in every thread
+__device__ __forceinline__ double block_max(double v) {
   __shared__ double red[32];
-  const int k = L.k, d = L.d, tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-  // ---- max |c| -> scale
-  double m = 0.0;
-#pragma unroll 8
-  for (int i = tid; i < k * d; i += 1024) m = fmax(m, fabs(C(i)));
 #pragma unroll
-  for (int o = 16; o > 0; o >>= 1) m = fmax(m, __shfl_xor_sync(0xffffffffu, m, o));
-  if (lane == 0) red[wid] = m;
+  for (int o = 16; o > 0; o >>= 1) v = fmax(v, __shfl_xor_sync(0xffffffffu, v, o));
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
   __syncthreads();
-  m = red[0];
-  for (int w = 1; w < 32; ++w) m = fmax(m, red[w]);
-  const double sc = scalbn(1.0, pack_scale_exp(m));
+  v = red[0];
+  for (int w = 1; w < (int)(blockDim.x >> 5); ++w) v = fmax(v, red[w]);
   __syncthreads();
-  // ---- ||c_j||^2 (one warp per centre, same summation order as pack_norms_kernel) and their maximum
-  for (int j = wid; j < k; j += 32) {
+  return v;
+}
+
+// ||c_j||^2 -> cn[j] for the centres j = w, w + nw, ... of warp w (of nw): lane-strided fma, then the xor-shuffle tree
+template <typename Src>
+__device__ __forceinline__ void pack_norms(Src C, const PackLayout& L, double* cn, int w, int nw) {
+  const int lane = threadIdx.x & 31;
+  for (int j = w; j < L.k; j += nw) {
     double s = 0.0;
-    for (int i = lane; i < d; i += 32) { double v = C((size_t)j * d + i); s = fma(v, v, s); }
+    for (int i = lane; i < L.d; i += 32) { const double v = C((size_t)j * L.d + i); s = fma(v, v, s); }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-    if (lane == 0) cn_s[j] = s;
-  }
-  __syncthreads();
-  double cm = 0.0;
-  for (int j = tid; j < k; j += 1024) cm = fmax(cm, cn_s[j]);
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) cm = fmax(cm, __shfl_xor_sync(0xffffffffu, cm, o));
-  if (lane == 0) red[wid] = cm;
-  __syncthreads();
-  if (blockIdx.x == 0 && tid == 0) {
-    cm = red[0];
-    for (int w = 1; w < 32; ++w) cm = fmax(cm, red[w]);
-    PackHeader* h = reinterpret_cast<PackHeader*>(pack);
-    h->k = k; h->d = d; h->dtype = L.dtype; h->pad = 0; h->cn_max = cm; h->scale = (float)sc; h->pad2 = 0.f;
-  }
-  // ---- this CTA's share of the layouts
-  const int gt = blockIdx.x * 1024 + tid, nth = gridDim.x * 1024;
-  double* c64 = reinterpret_cast<double*>(pack + L.off_c64);
-  for (int i = gt; i < k * d; i += nth) c64[i] = C(i);
-  double* cn64 = reinterpret_cast<double*>(pack + L.off_cn64);
-  if (L.dtype != BKM_F64) {
-    float* cT = reinterpret_cast<float*>(pack + L.off_cT);
-    for (int i = gt; i < k * L.d4; i += nth) {
-      int r = i / L.d4, c = i - r * L.d4;
-      cT[i] = c < d ? (float)C((size_t)r * d + c) : 0.f;
-    }
-    if (d <= L.dh) {
-      __half* bhi = reinterpret_cast<__half*>(pack + L.off_bhi);
-      __half* blo = reinterpret_cast<__half*>(pack + L.off_blo);
-      for (int i = gt; i < L.kp * L.dh; i += nth) {
-        int r = i / L.dh, c = i - r * L.dh;
-        __half hi = __float2half_rn(0.f), lo = hi;
-        if (r < k && c < d) {
-          const double v = -2.0 * sc * C((size_t)r * d + c);
-          hi = __double2half(v);
-          lo = __double2half(v - (double)__half2float(hi));
-        }
-        bhi[i] = hi; blo[i] = lo;
-      }
-    }
-    if (L.off_c64T != L.total) {
-      double* cTT = reinterpret_cast<double*>(pack + L.off_c64T);
-      for (int i = gt; i < d * L.kp; i += nth) {
-        int f = i / L.kp, j = i - f * L.kp;
-        cTT[i] = j < k ? C((size_t)j * d + f) : 0.0;
-      }
-    }
-    float* cn32 = reinterpret_cast<float*>(pack + L.off_cn32);
-    for (int j = gt; j < L.kp; j += nth) {
-      const double s = j < k ? cn_s[j] : 0.0;
-      if (j < k) { cn64[j] = s; reinterpret_cast<float*>(pack + L.off_cnT)[j] = (float)s; }
-      cn32[j] = j < k ? (float)s : CUDART_INF_F;
-      float* bcn = reinterpret_cast<float*>(pack + L.off_bcn) + (j >> 3) * 64 + (j & 7) * 4;
-      float hi = 3.0e38f, mid = 0.f, lo = 0.f;
-      if (j < k) {
-        const float cf = (float)(s * sc * sc);          // the tensor path works on s X and s C
-        hi = to_tf32_rna(cf);
-        const float r1 = cf - hi;
-        mid = to_tf32_rna(r1);
-        lo = r1 - mid;
-      }
-      bcn[0] = hi; bcn[1] = mid; bcn[2] = lo; bcn[3] = 0.f;
-      bcn[32] = 0.f; bcn[33] = 0.f; bcn[34] = 0.f; bcn[35] = 0.f;
-    }
-  } else {
-    double* cT = reinterpret_cast<double*>(pack + L.off_cT);
-    for (int i = gt; i < k * L.d4; i += nth) {
-      int r = i / L.d4, c = i - r * L.d4;
-      cT[i] = c < d ? C((size_t)r * d + c) : 0.0;
-    }
-    for (int j = gt; j < k; j += nth) { cn64[j] = cn_s[j]; reinterpret_cast<double*>(pack + L.off_cnT)[j] = cn_s[j]; }
+    if (lane == 0) cn[j] = s;
   }
 }
 
-struct CentreFromMemory {
-  const double* p;
-  __device__ __forceinline__ double operator()(size_t i) const { return p[i]; }
-};
+// max |c| over one CTA (coalesced; on the one-kernel path it also brings the centres into L1 for pack_norms)
+template <typename Src>
+__device__ __forceinline__ double pack_max_abs(Src C, const PackLayout& L) {
+  double m = 0.0;
+#pragma unroll 8
+  for (int i = threadIdx.x; i < L.k * L.d; i += blockDim.x) m = fmax(m, fabs(C(i)));
+  return block_max(m);
+}
+
+// One CTA, after every cn[j] is written: the scale from max |c| (returned) and cn_max; CTA 0 writes the header.
+__device__ __forceinline__ double pack_header(unsigned char* pack, const PackLayout& L, double max_abs,
+                                              const double* cn) {
+  const double sc = scalbn(1.0, pack_scale_exp(max_abs));
+  double cm = 0.0;
+  for (int j = threadIdx.x; j < L.k; j += blockDim.x) cm = fmax(cm, cn[j]);
+  cm = block_max(cm);
+  if (blockIdx.x == 0 && threadIdx.x == 0) {
+    PackHeader* h = reinterpret_cast<PackHeader*>(pack);
+    h->k = L.k; h->d = L.d; h->dtype = L.dtype; h->pad = 0; h->cn_max = cm; h->scale = (float)sc; h->pad2 = 0.f;
+  }
+  return sc;
+}
+
+// cT and cnT in the element type T of the rows' layouts
+template <typename T, typename Src>
+__device__ __forceinline__ void pack_rows(Src C, unsigned char* pack, const PackLayout& L, const double* cn, int gt,
+                                          int nth) {
+  T* cT = reinterpret_cast<T*>(pack + L.off_cT);
+  T* cnT = reinterpret_cast<T*>(pack + L.off_cnT);
+  for (int i = gt; i < L.k * L.d4; i += nth) {
+    const int r = i / L.d4, c = i - r * L.d4;
+    cT[i] = c < L.d ? (T)C((size_t)r * L.d + c) : T(0);
+  }
+  for (int j = gt; j < L.k; j += nth) cnT[j] = (T)cn[j];
+}
+
+// 16-bit (hi, lo) pair of v: hi + lo carries 22 (fp16) or 16 (bf16) significant bits
+__device__ __forceinline__ void split16(double v, __half& hi, __half& lo) {
+  hi = __double2half(v);
+  lo = __double2half(v - (double)__half2float(hi));
+}
+__device__ __forceinline__ void split16(double v, __nv_bfloat16& hi, __nv_bfloat16& lo) {
+  hi = __double2bfloat16(v);
+  lo = __double2bfloat16(v - (double)__bfloat162float(hi));
+}
+
+// MMA operand tiles [rows][cols] of f * C: row r = centre r, column c = feature c
+template <typename H, typename Src>
+__device__ __forceinline__ void pack_split_tiles(Src C, const PackLayout& L, H* hi, H* lo, int rows, int cols, double f,
+                                                 int gt, int nth) {
+  for (int i = gt; i < rows * cols; i += nth) {
+    const int r = i / cols, c = i - r * cols;
+    H h, l;
+    split16(r < L.k && c < L.d ? f * C((size_t)r * L.d + c) : 0.0, h, l);
+    hi[i] = h; lo[i] = l;
+  }
+}
+
+// float64 centres transposed [d][cols] (coalesced over centres for the re-check kernels)
+template <typename Src>
+__device__ __forceinline__ void pack_transposed(Src C, const PackLayout& L, double* out, int cols, int gt, int nth) {
+  for (int i = gt; i < L.d * cols; i += nth) {
+    const int f = i / cols, j = i - f * cols;
+    out[i] = j < L.k ? C((size_t)j * L.d + f) : 0.0;
+  }
+}
+
+// Every layout but the header, grid-strided, from the norms cn and the scale sc.
+template <typename Src>
+__device__ __forceinline__ void pack_layouts(Src C, unsigned char* pack, const PackLayout& L, const double* cn,
+                                             double sc) {
+  const int k = L.k, gt = blockIdx.x * blockDim.x + threadIdx.x, nth = gridDim.x * blockDim.x;
+  double* c64 = reinterpret_cast<double*>(pack + L.off_c64);
+  double* cn64 = reinterpret_cast<double*>(pack + L.off_cn64);
+  for (int i = gt; i < k * L.d; i += nth) c64[i] = C(i);
+  if (cn != cn64)                                   // the large path's pack_norms_kernel wrote them in place
+    for (int j = gt; j < k; j += nth) cn64[j] = cn[j];
+  if (L.dtype == BKM_F64) pack_rows<double>(C, pack, L, cn, gt, nth);
+  else pack_rows<float>(C, pack, L, cn, gt, nth);
+  if (L.tc) {                                       // the tensor path works on s X and s C
+    pack_split_tiles(C, L, reinterpret_cast<__half*>(pack + L.off_bhi), reinterpret_cast<__half*>(pack + L.off_blo),
+                     L.kp, 64, -2.0 * sc, gt, nth);
+    float* cns = reinterpret_cast<float*>(pack + L.off_cns);
+    for (int j = gt; j < L.kp; j += nth) cns[j] = j < k ? (float)(cn[j] * sc * sc) : 3.0e38f;
+    pack_transposed(C, L, reinterpret_cast<double*>(pack + L.off_c64T), L.kp, gt, nth);
+  }
+  if (L.tc2) {                                      // bf16 has fp32's range: no scale
+    pack_split_tiles(C, L, reinterpret_cast<__nv_bfloat16*>(pack + L.off_b2hi),
+                     reinterpret_cast<__nv_bfloat16*>(pack + L.off_b2lo), L.kp2, L.dk2, -2.0, gt, nth);
+    float* cn2 = reinterpret_cast<float*>(pack + L.off_cn2);
+    for (int j = gt; j < L.kp2; j += nth) cn2[j] = j < k ? (float)cn[j] : 3.0e38f;
+    pack_transposed(C, L, reinterpret_cast<double*>(pack + L.off_c64T2), L.kp2, gt, nth);
+  }
+}
+
+// Every CTA of one kernel computes the norms and the header quantities (k*d is a few thousand elements), then writes
+// its share of the layouts: dependent launches cost more than the repeated work.  In shared memory: cn_s [k].
+template <typename Src>
+__device__ __forceinline__ void pack_small(Src C, unsigned char* pack, const PackLayout& L, double* cn_s) {
+  const double m = pack_max_abs(C, L);
+  pack_norms(C, L, cn_s, threadIdx.x >> 5, blockDim.x >> 5);
+  __syncthreads();
+  pack_layouts(C, pack, L, cn_s, pack_header(pack, L, m, cn_s));
+}
 
 __global__ void __launch_bounds__(1024)
-pack_fused_kernel(const double* __restrict__ C, unsigned char* pack, PackLayout L) {
+pack_small_kernel(const double* __restrict__ C, unsigned char* pack, PackLayout L) {
   extern __shared__ double cn_s[];        // [k]
-  pack_fused_body(CentreFromMemory{C}, pack, L, cn_s);
+  pack_small(CentreFromMemory{C}, pack, L, cn_s);
+}
+
+// Large shapes: pack_norms_kernel writes the norms to the pack's cn64, then pack_layouts_kernel the rest; its CTA 0
+// also the header.  The layouts do not wait for the scale: only family-1 layouts use it, and those shapes are small.
+// st (nullable): the Lloyd loop of bkm_finalize_step; once it is done, its pack stays as it is.
+__global__ void __launch_bounds__(256)
+pack_norms_kernel(const double* __restrict__ C, unsigned char* pack, PackLayout L, const LoopState* st) {
+  if (st && st->done) return;
+  pack_norms(CentreFromMemory{C}, L, reinterpret_cast<double*>(pack + L.off_cn64),
+             (blockIdx.x * blockDim.x + threadIdx.x) >> 5, (gridDim.x * blockDim.x) >> 5);
+}
+
+__global__ void __launch_bounds__(1024)
+pack_layouts_kernel(const double* __restrict__ C, unsigned char* pack, PackLayout L, const LoopState* st) {
+  if (st && st->done) return;
+  const double* cn64 = reinterpret_cast<const double*>(pack + L.off_cn64);
+  if (blockIdx.x == 0) pack_header(pack, L, pack_max_abs(CentreFromMemory{C}, L), cn64);
+  pack_layouts(CentreFromMemory{C}, pack, L, cn64, 0.0);
 }
 
 // ---------------------------------------------------------------------------------------
-// One Lloyd iteration's tail in ONE kernel (small k*d, i.e. every shape of the fused chunk kernels):
+// One Lloyd iteration's tail:
 //   C' = sums / max(counts, 1)  (k_means.py:548-551, empty cluster -> zero vector)
 //   shift = ||C - C'||_F^2      (k_means.py:555)        -> LoopState.shift, hist[n_iter], n_iter += 1
-//   if shift < tol: LoopState.done = 1, C' is NOT taken over (k_means.py:558-560: break before the assignment)
-//   else: c_out = C', and the centre pack for the NEXT iteration is built from C' right here.
-// Every CTA recomputes the shift (fixed order -> the same value and the same decision everywhere) and the two global
-// quantities of the pack; centres are read from c_in and written to c_out (two buffers: no CTA reads what another one
-// writes).  red = [k*d sums | k counts as float64 | inertia] is the all-reduced buffer of the step.
+//   if shift < tol: LoopState.done = 1, C' is NOT taken over (k_means.py:558-560: break before the assignment) and
+//   the pack is left as it is
+//   else: c_out = C', and the centre pack for the NEXT iteration is built from C'.
+// Every CTA recomputes the shift (fixed order -> the same value and the same decision everywhere); centres are read
+// from c_in and written to c_out (two buffers: no CTA reads what another one writes).  red = [k*d sums | k counts as
+// float64 | inertia] is the all-reduced buffer of the step.
+// LAYOUTS (small shapes): the whole pack too (pack_small).  Otherwise (large shapes, one CTA) pack_norms_kernel and
+// pack_layouts_kernel follow, reading c_out.
 // ---------------------------------------------------------------------------------------
 struct CentreFromSums {
   const double* red;
@@ -276,13 +217,13 @@ struct CentreFromSums {
 };
 
 // STAGED: every CTA first evaluates C' = sums / max(counts, 1) ONCE into shared memory (k*d float64: 128 KB at C2) and
-// all later passes (shift, max |c|, norms, the five layouts) read that copy instead of repeating the float64 division
-// per access — the same quotient, computed once (44 -> ~15 us at k*d = 16384).
-template <bool STAGED>
+// all later passes (shift, norms, header, layouts) read that copy instead of repeating the float64 division per access — the
+// same quotient, computed once (44 -> ~15 us at k*d = 16384).
+template <bool STAGED, bool LAYOUTS>
 __global__ void __launch_bounds__(1024)
-finalize_step_fused_kernel(const double* __restrict__ red, const double* __restrict__ c_in, double* __restrict__ c_out,
-                           LoopState* st, unsigned char* pack, PackLayout L) {
-  extern __shared__ double cn_s[];        // [k] (+ [k*d] staged centres)
+finalize_step_kernel(const double* __restrict__ red, const double* __restrict__ c_in, double* __restrict__ c_out,
+                     LoopState* st, unsigned char* pack, PackLayout L) {
+  extern __shared__ double cn_s[];        // LAYOUTS: [k] (+ [k*d] staged centres)
   __shared__ double sred[32];
   if (st->done) return;
   const int k = L.k, d = L.d, kd = k * d, tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
@@ -305,8 +246,8 @@ finalize_step_fused_kernel(const double* __restrict__ red, const double* __restr
   const bool converged = shift < st->tol;
   if (!converged) {
     for (int i = blockIdx.x * 1024 + tid; i < kd; i += gridDim.x * 1024) c_out[i] = STAGED ? cmem(i) : cfs(i);
-    if (STAGED) pack_fused_body(cmem, pack, L, cn_s);
-    else pack_fused_body(cfs, pack, L, cn_s);
+    if (LAYOUTS && STAGED) pack_small(cmem, pack, L, cn_s);
+    else if (LAYOUTS) pack_small(cfs, pack, L, cn_s);
   }
   // the state is written last, by one thread of the last CTA to get here (every CTA has read st->done / st->tol)
   __shared__ bool last;
@@ -324,35 +265,6 @@ finalize_step_fused_kernel(const double* __restrict__ red, const double* __restr
   }
 }
 
-// Large k*d: single-CTA state update (shift, stop test, centre hand-over); the pack follows as separate kernels.
-__global__ void __launch_bounds__(1024)
-finalize_state_kernel(const double* __restrict__ red, const double* __restrict__ c_in, double* __restrict__ c_out,
-                      LoopState* st, int k, int d) {
-  __shared__ double sred[32];
-  if (st->done) return;
-  const int kd = k * d, tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-  const CentreFromSums cnew{red, kd, d};
-  double acc = 0.0;
-  for (int i = tid; i < kd; i += 1024) { const double df = c_in[i] - cnew(i); acc = fma(df, df, acc); }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
-  if (lane == 0) sred[wid] = acc;
-  __syncthreads();
-  double shift = 0.0;
-  for (int w = 0; w < 32; ++w) shift += sred[w];
-  const bool converged = shift < st->tol;
-  // on convergence c_out = c_in, so that the pack kernels that follow (and the host) always read c_out
-  for (int i = tid; i < kd; i += 1024) c_out[i] = converged ? c_in[i] : cnew(i);
-  __syncthreads();
-  if (tid == 0) {
-    st->shift = shift;
-    if (st->hist && st->n_iter < st->hist_cap) st->hist[st->n_iter] = shift;
-    st->n_iter += 1;
-    __threadfence();
-    if (converged) st->done = 2;       // 2: converged in THIS iteration (bkm_finalize_step's pack still runs once)
-  }
-}
-
 __global__ void loop_reset_kernel(LoopState* st, double tol, double* hist, int hist_cap) {
   st->done = 0; st->n_iter = 0; st->hist_cap = hist_cap; st->pad = 0;
   st->tol = tol; st->shift = CUDART_INF; st->hist = hist;
@@ -365,99 +277,58 @@ int launch_loop_reset(void* state, double tol, double* hist, int hist_cap, cudaS
   return 0;
 }
 
-// Layouts of the large-shape tensor path (bkm_tc2.cu), written after the float64 norms:
-//   b2hi / b2lo [kp2][dk2] bf16: rn(-2 c), rn(-2 c - hi)          (row j = centre j; rows >= k and columns >= d: zero)
-//   bcn2 [kp2] rows [hi, mid, lo, 0 | 0 0 0 0] tf32 of ||c_j||^2 in the no-swizzle K-major operand layout; rows >= k: 3e38
-//   c64T2 [d][kp2] float64 (re-check)
-__global__ void pack_tc2_kernel(const double* __restrict__ C, unsigned char* pack, PackLayout L, Tc2Geom g) {
-  const int k = L.k, d = L.d;
-  const int gt = blockIdx.x * blockDim.x + threadIdx.x, nth = gridDim.x * blockDim.x;
-  const double* cn64 = reinterpret_cast<const double*>(pack + L.off_cn64);
-  __nv_bfloat16* bhi = reinterpret_cast<__nv_bfloat16*>(pack + L.off_b2hi);
-  __nv_bfloat16* blo = reinterpret_cast<__nv_bfloat16*>(pack + L.off_b2lo);
-  for (int i = gt; i < g.kp2 * g.dk2; i += nth) {
-    const int r = i / g.dk2, c = i - r * g.dk2;
-    __nv_bfloat16 hi = __float2bfloat16_rn(0.f), lo = hi;
-    if (r < k && c < d) {
-      const double v = -2.0 * C[(size_t)r * d + c];
-      hi = __double2bfloat16(v);
-      lo = __double2bfloat16(v - (double)__bfloat162float(hi));
-    }
-    bhi[i] = hi; blo[i] = lo;
-  }
-  for (int j = gt; j < g.kp2; j += nth) {
-    float* bcn = reinterpret_cast<float*>(pack + L.off_bcn2) + (j >> 3) * 64 + (j & 7) * 4;
-    float hi = 3.0e38f, mid = 0.f, lo = 0.f;
-    if (j < k) {
-      const float cf = (float)cn64[j];
-      hi = to_tf32_rna(cf);
-      const float r1 = cf - hi;
-      mid = to_tf32_rna(r1);
-      lo = r1 - mid;
-    }
-    bcn[0] = hi; bcn[1] = mid; bcn[2] = lo; bcn[3] = 0.f;
-    bcn[32] = 0.f; bcn[33] = 0.f; bcn[34] = 0.f; bcn[35] = 0.f;
-  }
-  double* cTT = reinterpret_cast<double*>(pack + L.off_c64T2);
-  for (int i = gt; i < d * g.kp2; i += nth) {
-    const int f = i / g.kp2, j = i - f * g.kp2;
-    cTT[i] = j < k ? C[(size_t)j * d + f] : 0.0;
-  }
+// The one-kernel path: k*d up to 64 K elements (every shape of the fused chunk kernels).
+static bool pack_in_one_kernel(const PackLayout& L) { return L.k <= 2048 && (long long)L.k * L.d <= 65536; }
+
+// CTAs of a layouts pass: one per `per` elements of the largest layout, at most `cap`
+static int pack_grid(const PackLayout& L, int per, int cap) {
+  size_t n = (size_t)L.k * L.d4;
+  if (L.tc && (size_t)L.kp * 64 > n) n = (size_t)L.kp * 64;
+  if (L.tc2 && (size_t)L.kp2 * L.dk2 > n) n = (size_t)L.kp2 * L.dk2;
+  const size_t nb = (n + per - 1) / per;
+  return nb < 1 ? 1 : (nb > (size_t)cap ? cap : (int)nb);
 }
 
-static int launch_pack_tc2(const double* C, const PackLayout& L, void* pack, cudaStream_t s) {
-  if (!tc2_shape(L.d, L.k, L.dtype)) return 0;
-  const Tc2Geom g = tc2_geom(L.k, L.d);
-  int nb = (g.kp2 * g.dk2 + 1023) / 1024; if (nb > 296) nb = 296; if (nb < 1) nb = 1;
-  pack_tc2_kernel<<<nb, 256, 0, s>>>(C, (unsigned char*)pack, L, g);
-  note_launch();
+int launch_pack(const double* C, int k, int d, int dtype, void* pack, cudaStream_t s) {
+  const PackLayout L = pack_layout(k, d, dtype);
+  unsigned char* p = (unsigned char*)pack;
+  if (pack_in_one_kernel(L)) {
+    pack_small_kernel<<<pack_grid(L, 2048, 16), 1024, (size_t)k * 8, s>>>(C, p, L);
+    note_launch();
+  } else {
+    pack_norms_kernel<<<(k + 7) / 8 < 132 ? (k + 7) / 8 : 132, 256, 0, s>>>(C, p, L, nullptr);
+    pack_layouts_kernel<<<pack_grid(L, 1024, 132), 1024, 0, s>>>(C, p, L, nullptr);
+    note_launch(2);
+  }
   BKM_CUDA_TRY(cudaGetLastError());
   return 0;
 }
 
-int launch_pack(const double* C, int k, int d, int dtype, void* pack, cudaStream_t s) {
-  PackLayout L = pack_layout(k, d, dtype);
-  if (k <= 2048 && (long long)k * d <= 65536) {
-    int nb = (L.kp * L.dk + 2047) / 2048; if (nb > 16) nb = 16; if (nb < 1) nb = 1;
-    pack_fused_kernel<<<nb, 1024, (size_t)k * 8, s>>>(C, (unsigned char*)pack, L);
-    note_launch();
-    BKM_CUDA_TRY(cudaGetLastError());
-    return launch_pack_tc2(C, L, pack, s);
-  }
-  int nb = (L.kp * L.dk + 255) / 256; if (nb > 296) nb = 296; if (nb < 1) nb = 1;
-  pack_scale_kernel<<<1, 1024, 0, s>>>(C, (unsigned char*)pack, L);
-  pack_centers_kernel<<<nb, 256, 0, s>>>(C, (unsigned char*)pack, L);
-  int nb2 = (L.kp + 7) / 8; if (nb2 > 132) nb2 = 132;
-  pack_norms_kernel<<<nb2, 256, 0, s>>>(C, (unsigned char*)pack, L);
-  pack_header_kernel<<<1, 256, 0, s>>>((unsigned char*)pack, L);
-  note_launch(4);
-  BKM_CUDA_TRY(cudaGetLastError());
-  return launch_pack_tc2(C, L, pack, s);
-}
-
 int launch_finalize_step(const double* red, const double* c_in, double* c_out, void* state, int k, int d, int dtype,
                          void* pack, cudaStream_t s) {
-  PackLayout L = pack_layout(k, d, dtype);
+  const PackLayout L = pack_layout(k, d, dtype);
   LoopState* st = reinterpret_cast<LoopState*>(state);
-  if (k <= 2048 && (long long)k * d <= 65536 && !tc2_shape(d, k, dtype)) {
-    int nb = (L.kp * L.dk + 2047) / 2048; if (nb > 16) nb = 16; if (nb < 1) nb = 1;
+  unsigned char* p = (unsigned char*)pack;
+  if (pack_in_one_kernel(L)) {
+    const int nb = pack_grid(L, 2048, 16);
     const size_t staged_bytes = ((size_t)k + (size_t)k * d) * 8;
     if (staged_bytes <= 200 * 1024) {
       if (staged_bytes > 48 * 1024)
-        BKM_CUDA_TRY(cudaFuncSetAttribute(finalize_step_fused_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+        BKM_CUDA_TRY(cudaFuncSetAttribute(finalize_step_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                           (int)staged_bytes));
-      finalize_step_fused_kernel<true><<<nb, 1024, staged_bytes, s>>>(red, c_in, c_out, st, (unsigned char*)pack, L);
+      finalize_step_kernel<true, true><<<nb, 1024, staged_bytes, s>>>(red, c_in, c_out, st, p, L);
     } else {
-      finalize_step_fused_kernel<false><<<nb, 1024, (size_t)k * 8, s>>>(red, c_in, c_out, st, (unsigned char*)pack, L);
+      finalize_step_kernel<false, true><<<nb, 1024, (size_t)k * 8, s>>>(red, c_in, c_out, st, p, L);
     }
     note_launch();
-    BKM_CUDA_TRY(cudaGetLastError());
-    return 0;
+  } else {
+    finalize_step_kernel<false, false><<<1, 1024, 0, s>>>(red, c_in, c_out, st, p, L);
+    pack_norms_kernel<<<(k + 7) / 8 < 132 ? (k + 7) / 8 : 132, 256, 0, s>>>(c_out, p, L, st);
+    pack_layouts_kernel<<<pack_grid(L, 1024, 132), 1024, 0, s>>>(c_out, p, L, st);
+    note_launch(3);
   }
-  finalize_state_kernel<<<1, 1024, 0, s>>>(red, c_in, c_out, st, k, d);
-  note_launch();
   BKM_CUDA_TRY(cudaGetLastError());
-  return launch_pack(c_out, k, d, dtype, pack, s);
+  return 0;
 }
 
 // ---------------------------------------------------------------------------------------

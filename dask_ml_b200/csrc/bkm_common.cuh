@@ -46,22 +46,29 @@ static inline bool tc2_shape(int d, int k, int dtype) {
   return dtype == BKM_BF16 && d >= 1 && d <= 128 && k >= 1 && k <= 4096;      // <= 16 cluster slices in the M-step row pass
 }
 
+// fp32 input with d <= 64 and k <= 256: the tensor-core kernel of bkm_tc.cu (implemented there)
+bool tc_supported(int d, int k, int dtype);
+
 // ---------------------------------------------------------------------------------------
 // Centre pack: one device buffer holding every layout of the (k,d) centres the kernels use.
-// Built by pack_centers_kernel from the float64 centres (reference keeps centres in f64:
-// dask_ml/cluster/k_means.py:551-552).
+// Built from the float64 centres (reference keeps centres in f64: dask_ml/cluster/k_means.py:551-552) by
+// bkm_pack_centers / bkm_finalize_step (bkm_aux.cu, which lists the layouts).  A shape's pack holds the layouts of the
+// kernels that can read it: every shape has the four plain ones, tc_supported shapes the family-1 operands and
+// tc2_shape shapes the family-3 operands.
 // ---------------------------------------------------------------------------------------
 struct PackLayout {
   int k, d, dtype;
   int d4;      // d rounded up to a multiple of 4 (SIMT row pitch, zero padded)
   int kp;      // k rounded up to a multiple of 16 (MMA N granularity)
-  int dk;      // d rounded up to a multiple of 32 (one 128-byte swizzle atom of fp32 per K-block)
-  int dh;      // row length of the fp16 MMA operand tiles: 64 halves = one 128-byte swizzle atom (d <= 64)
+  bool tc;     // family-1 operands present (tc_supported)
+  bool tc2;    // family-3 operands present (tc2_shape)
+  int kp2, dk2;  // family-3 operand tiles: rows (all centre slices) x 16-bit columns (Tc2Geom)
   size_t esz;  // sizeof(T)
-  size_t off_cT, off_cnT, off_c64, off_cn64, off_bhi, off_blo, off_cn32, off_bcn, off_c64T, total;
-  // large-shape tensor path (tc2_shape): fp16 (hi, lo) operand tiles [kp2][dk2], ||c||^2 operand rows [kp2][8] tf32,
-  // float64 centres transposed [d][kp2]
-  size_t off_b2hi, off_b2lo, off_bcn2, off_c64T2;
+  size_t off_cT, off_cnT, off_c64, off_cn64, total;
+  // family 1: fp16 (hi, lo) operand tiles [kp][64], s^2 ||c||^2 [kp] fp32, float64 centres transposed [d][kp]
+  size_t off_bhi, off_blo, off_cns, off_c64T;
+  // family 3: bf16 (hi, lo) operand tiles [kp2][dk2], ||c||^2 [kp2] fp32, float64 centres transposed [d][kp2]
+  size_t off_b2hi, off_b2lo, off_cn2, off_c64T2;
 };
 
 static inline PackLayout pack_layout(int k, int d, int dtype) {
@@ -69,26 +76,29 @@ static inline PackLayout pack_layout(int k, int d, int dtype) {
   L.k = k; L.d = d; L.dtype = dtype;
   L.d4 = (d + 3) / 4 * 4;
   L.kp = (k + 15) / 16 * 16;
-  L.dk = (d + 31) / 32 * 32;
-  L.dh = 64;
+  L.tc = tc_supported(d, k, dtype);
+  L.tc2 = tc2_shape(d, k, dtype);
   L.esz = dtype == BKM_F64 ? 8 : 4;                // bf16 input: the fp32 layouts (the kernels widen the rows)
   size_t o = 256;  // header
   L.off_cT = o;   o = align_up(o + (size_t)k * L.d4 * L.esz, 256);
   L.off_cnT = o;  o = align_up(o + (size_t)k * L.esz, 256);
   L.off_c64 = o;  o = align_up(o + (size_t)k * d * 8, 256);
   L.off_cn64 = o; o = align_up(o + (size_t)k * 8, 256);
-  L.off_bhi = o;  o = align_up(o + (size_t)L.kp * L.dh * 2, 256);   // fp16 tiles (tensor path, d <= 64)
-  L.off_blo = o;  o = align_up(o + (size_t)L.kp * L.dh * 2, 256);
-  L.off_cn32 = o; o = align_up(o + (size_t)L.kp * 4, 256);
-  L.off_bcn = o;  o = align_up(o + (size_t)L.kp * 32, 256);   // ||c||^2 as an MMA operand tile (see bkm_tc.cu)
-  // float64 centres transposed [d][kp] for the float64 re-check of the tensor path (coalesced over centres)
-  L.off_c64T = o; if (dtype == BKM_F32 && d <= 64 && k <= 256) o = align_up(o + (size_t)d * L.kp * 8, 256);
-  L.off_b2hi = L.off_b2lo = L.off_bcn2 = L.off_c64T2 = o;
-  if (tc2_shape(d, k, dtype)) {
+  L.off_bhi = L.off_blo = L.off_cns = L.off_c64T = o;
+  if (L.tc) {
+    L.off_bhi = o;  o = align_up(o + (size_t)L.kp * 64 * 2, 256);    // 64 halves = one 128-byte swizzle atom per row
+    L.off_blo = o;  o = align_up(o + (size_t)L.kp * 64 * 2, 256);
+    L.off_cns = o;  o = align_up(o + (size_t)L.kp * 4, 256);
+    L.off_c64T = o; o = align_up(o + (size_t)d * L.kp * 8, 256);     // float64 re-check, coalesced over centres
+  }
+  L.kp2 = L.dk2 = 0;
+  L.off_b2hi = L.off_b2lo = L.off_cn2 = L.off_c64T2 = o;
+  if (L.tc2) {
     const Tc2Geom g = tc2_geom(k, d);
+    L.kp2 = g.kp2; L.dk2 = g.dk2;
     L.off_b2hi = o;  o = align_up(o + (size_t)g.kp2 * g.dk2 * 2, 1024);
     L.off_b2lo = o;  o = align_up(o + (size_t)g.kp2 * g.dk2 * 2, 1024);
-    L.off_bcn2 = o;  o = align_up(o + (size_t)g.kp2 * 32, 256);
+    L.off_cn2 = o;   o = align_up(o + (size_t)g.kp2 * 4, 256);
     L.off_c64T2 = o; o = align_up(o + (size_t)d * g.kp2 * 8, 256);
   }
   L.total = o;
@@ -223,7 +233,6 @@ struct LoopState {
 // implemented in bkm_simt.cu
 int launch_simt(const ChunkArgs& a, bool mstep, int dtype, int sm_count, int* grid_out, cudaStream_t s);
 // implemented in bkm_tc.cu
-bool tc_supported(int d, int k, int dtype);
 int launch_tc(const ChunkArgs& a, bool mstep, int sm_count, int* grid_out, cudaStream_t s);
 int launch_tc_recheck(const ChunkArgs& a, bool mstep, int sm_count, cudaStream_t s);
 int launch_tc_transform(const ChunkArgs& a, int sm_count, cudaStream_t s);

@@ -125,12 +125,9 @@ tc_chunk_kernel(ChunkArgs a, typename TcCfgOf<EPI>::type cfg) {
       *reinterpret_cast<uint4*>(smem + cfg.off_bhi + wg::sw128_chunk(r, q)) = h;
       *reinterpret_cast<uint4*>(smem + cfg.off_blo + wg::sw128_chunk(r, q)) = l;
     }
-    // s^2 ||c_j||^2 from the pack's exact 3-way split [hi, mid, lo] (hi + mid + lo == the fp32 value)
-    const float* bcn = reinterpret_cast<const float*>(a.pack + a.L.off_bcn);
+    const float* cns = reinterpret_cast<const float*>(a.pack + a.L.off_cns);
     for (int j = tid; j < N; j += TC_THREADS) {
-      float v = 3.0e38f;
-      if (j < a.L.kp) { const float* p = bcn + (j >> 3) * 64 + (j & 7) * 4; v = (p[0] + p[1]) + p[2]; }
-      cn_s[j] = v;
+      cn_s[j] = j < a.L.kp ? cns[j] : 3.0e38f;
       cnt_s[j] = 0;
     }
     if (MSTEP)

@@ -66,13 +66,8 @@ tc2_assign_kernel(ChunkArgs a, Tc2Cfg cfg) {
       if (r < NS) val = (v ? glo : ghi)[(size_t)(slice * NS + r) * rq + kb * 8 + q];
       *reinterpret_cast<uint4*>(smem + cfg.off_b + (uint32_t)(v * KB + kb) * btile + wg::sw128_chunk(r, q)) = val;
     }
-    // ||c_j||^2 from the pack's exact 3-way split [hi, mid, lo] (hi + mid + lo == the fp32 value)
-    const float* bcn = reinterpret_cast<const float*>(a.pack + a.L.off_bcn2);
-    for (int j = tid; j < N; j += T2_THREADS) {
-      float v = 3.0e38f;
-      if (j < NS) { const int jg = slice * NS + j; const float* p = bcn + (jg >> 3) * 64 + (jg & 7) * 4; v = (p[0] + p[1]) + p[2]; }
-      cn_s[j] = v;
-    }
+    const float* cn2 = reinterpret_cast<const float*>(a.pack + a.L.off_cn2);
+    for (int j = tid; j < N; j += T2_THREADS) cn_s[j] = j < NS ? cn2[slice * NS + j] : 3.0e38f;
     wg::fence_proxy_async();                                 // generic-proxy stores -> visible to wgmma
   }
   __syncthreads();
