@@ -45,6 +45,8 @@ SIGNATURES = {
     "bkm_loop_reset": (_int, [_c_void_p, _dbl, _c_void_p, _int, _c_void_p]),
     "bkm_finalize_step": (_int, [_c_void_p, _c_void_p, _c_void_p, _c_void_p, _int, _int, _int, _c_void_p,
                                  ctypes.c_size_t, _c_void_p]),
+    "bkm_minibatch_step": (_int, [_c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_void_p, _int, _int, _int, _c_void_p,
+                                  ctypes.c_size_t, _c_void_p]),
     "bkm_assign_chunk": (_int, [_c_void_p, _i64, _int, _i64, _int, _c_void_p, _int, _c_void_p, _c_void_p,
                                 _int, _c_void_p, _c_void_p, ctypes.c_size_t, _int, _c_void_p]),
     "bkm_sample_chunk": (_int, [_c_void_p, _i64, _int, _dbl, _u64, _u64, _c_void_p, _i64, _c_void_p, _c_void_p]),

@@ -14,6 +14,8 @@ int launch_min_fold(void* run_min, const void* new_min, long long n, int dtype, 
 int launch_loop_reset(void* state, double tol, double* hist, int hist_cap, cudaStream_t s);
 int launch_finalize_step(const double* red, const double* c_in, double* c_out, void* state, int k, int d, int dtype,
                          void* pack, cudaStream_t s);
+int launch_minibatch_step(const double* red, const double* c_in, const double* w_in, double* c_out, double* w_out,
+                          int k, int d, int dtype, void* pack, cudaStream_t s);
 int launch_finalize(const double* sums, const long long* counts, const double* Cold, double* Cnew,
                     double* shift, int k, int d, cudaStream_t s);
 int launch_sample(const void* d2, long long n, int dtype, double eop, uint64_t seed, uint64_t off,
@@ -390,6 +392,18 @@ int bkm_finalize_step(const double* reduced, const double* centers_in, double* c
   if (pack_bytes < pack_layout(k, d, x_dtype).total) return BKM_EWORKSPACE;
   if (((uintptr_t)pack & 255) || ((uintptr_t)loop_state & 7)) return BKM_EALIGN;
   return launch_finalize_step(reduced, centers_in, centers_out, loop_state, k, d, x_dtype, pack, (cudaStream_t)stream);
+}
+
+int bkm_minibatch_step(const double* reduced, const double* centers_in, const double* weights_in, double* centers_out,
+                       double* weights_out, int k, int d, int x_dtype, void* pack, size_t pack_bytes, void* stream) {
+  if (!reduced || !centers_in || !weights_in || !centers_out || !weights_out || !pack || k <= 0 || d <= 0)
+    return BKM_EINVAL;
+  if (centers_in == centers_out || weights_in == weights_out) return BKM_EINVAL;
+  if (!dtype_ok(x_dtype)) return BKM_EDTYPE;
+  if (pack_bytes < pack_layout(k, d, x_dtype).total) return BKM_EWORKSPACE;
+  if ((uintptr_t)pack & 255) return BKM_EALIGN;
+  return launch_minibatch_step(reduced, centers_in, weights_in, centers_out, weights_out, k, d, x_dtype, pack,
+                               (cudaStream_t)stream);
 }
 
 int bkm_check_finite(const void* X, int64_t n, int d, int64_t ldx, int x_dtype, int* flag,

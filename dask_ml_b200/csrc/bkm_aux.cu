@@ -332,6 +332,81 @@ int launch_finalize_step(const double* red, const double* c_in, double* c_out, v
 }
 
 // ---------------------------------------------------------------------------------------
+// One mini-batch step (scikit-learn's _minibatch_update_dense, sklearn/cluster/_k_means_minibatch.pyx), after the fused
+// E+M pass over the batch left red = [k*d sums S | k counts n as float64 | inertia]:
+//   c_out[j] = (c_in[j] * w_in[j] + S[j]) * (1 / (w_in[j] + n[j]))   where n[j] > 0, else c_in[j]
+//   w_out[j] = w_in[j] + n[j]
+// and the centre pack of c_out.  The products and sums are explicit round-to-nearest intrinsics: the expression is
+// scikit-learn's, evaluated in float64 without FMA contraction.  Centres and weight sums are read from the *_in
+// buffers and written to the *_out ones (ping-pong), so no CTA reads what another one writes.
+// LAYOUTS (small shapes): every CTA also builds the whole pack (pack_small).  Otherwise pack_norms_kernel and
+// pack_layouts_kernel follow, reading c_out.
+// ---------------------------------------------------------------------------------------
+struct CentreFromMinibatch {
+  const double* red;
+  const double* c;
+  const double* w;
+  int kd, d;
+  __device__ __forceinline__ double operator()(size_t i) const {
+    const int j = (int)(i / (size_t)d);
+    const double n = red[kd + j];
+    if (!(n > 0.0)) return c[i];
+    const double alpha = __ddiv_rn(1.0, __dadd_rn(w[j], n));
+    return __dmul_rn(__dadd_rn(__dmul_rn(c[i], w[j]), red[i]), alpha);
+  }
+};
+
+// STAGED: every CTA evaluates the new centres once into shared memory ([k] norms + [k*d] centres), as
+// finalize_step_kernel does; the pack passes then read that copy.
+template <bool STAGED, bool LAYOUTS>
+__global__ void __launch_bounds__(1024)
+minibatch_step_kernel(const double* __restrict__ red, const double* __restrict__ c_in, const double* __restrict__ w_in,
+                      double* __restrict__ c_out, double* __restrict__ w_out, unsigned char* pack, PackLayout L) {
+  extern __shared__ double cn_s[];        // LAYOUTS: [k] (+ [k*d] staged centres)
+  const int k = L.k, kd = k * L.d, tid = threadIdx.x;
+  const CentreFromMinibatch cmb{red, c_in, w_in, kd, L.d};
+  double* cs = cn_s + k;
+  if (STAGED) {
+    for (int i = tid; i < kd; i += blockDim.x) cs[i] = cmb(i);
+    __syncthreads();
+  }
+  const CentreFromMemory cmem{cs};
+  const int gt = blockIdx.x * blockDim.x + tid, nth = gridDim.x * blockDim.x;
+  for (int i = gt; i < kd; i += nth) c_out[i] = STAGED ? cmem(i) : cmb(i);
+  for (int j = gt; j < k; j += nth) w_out[j] = __dadd_rn(w_in[j], red[kd + j]);
+  if (LAYOUTS && STAGED) pack_small(cmem, pack, L, cn_s);
+  else if (LAYOUTS) pack_small(cmb, pack, L, cn_s);
+}
+
+int launch_minibatch_step(const double* red, const double* c_in, const double* w_in, double* c_out, double* w_out,
+                          int k, int d, int dtype, void* pack, cudaStream_t s) {
+  const PackLayout L = pack_layout(k, d, dtype);
+  unsigned char* p = (unsigned char*)pack;
+  if (pack_in_one_kernel(L)) {
+    const int nb = pack_grid(L, 2048, 16);
+    const size_t staged_bytes = ((size_t)k + (size_t)k * d) * 8;
+    if (staged_bytes <= 200 * 1024) {
+      if (staged_bytes > 48 * 1024)
+        BKM_CUDA_TRY(cudaFuncSetAttribute(minibatch_step_kernel<true, true>,
+                                          cudaFuncAttributeMaxDynamicSharedMemorySize, (int)staged_bytes));
+      minibatch_step_kernel<true, true><<<nb, 1024, staged_bytes, s>>>(red, c_in, w_in, c_out, w_out, p, L);
+    } else {
+      minibatch_step_kernel<false, true><<<nb, 1024, (size_t)k * 8, s>>>(red, c_in, w_in, c_out, w_out, p, L);
+    }
+    note_launch();
+  } else {
+    const long long kd = (long long)k * d;
+    const int nb = (int)((kd + 1023) / 1024 < 132 ? (kd + 1023) / 1024 : 132);
+    minibatch_step_kernel<false, false><<<nb, 1024, 0, s>>>(red, c_in, w_in, c_out, w_out, p, L);
+    pack_norms_kernel<<<(k + 7) / 8 < 132 ? (k + 7) / 8 : 132, 256, 0, s>>>(c_out, p, L, nullptr);
+    pack_layouts_kernel<<<pack_grid(L, 1024, 132), 1024, 0, s>>>(c_out, p, L, nullptr);
+    note_launch(3);
+  }
+  BKM_CUDA_TRY(cudaGetLastError());
+  return 0;
+}
+
+// ---------------------------------------------------------------------------------------
 // reduce_partials: fold the per-CTA partials of one chunk into the float64 accumulators in a
 // FIXED order (CTA 0,1,2,...), so a chunk's contribution is bit-reproducible run to run.
 // ---------------------------------------------------------------------------------------

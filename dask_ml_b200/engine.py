@@ -349,6 +349,15 @@ class CudaBackend(object):
                                                   k, d, _DT_CODE[dtype], self._ptr(pack), pack.numel(), self._stream()),
                        "bkm_finalize_step")
 
+    def minibatch_step(self, red, c_in, w_in, c_out, w_out, pack, dtype):
+        """One mini-batch centre update from ``red = [k*d sums | k counts | inertia]`` of the batch: c_out, w_out and the
+        pack of c_out (scikit-learn's _minibatch_update_dense, in float64)."""
+        k, d = c_in.shape
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.bkm_minibatch_step(self._ptr(red), self._ptr(c_in), self._ptr(w_in), self._ptr(c_out),
+                                                   self._ptr(w_out), k, d, _DT_CODE[dtype], self._ptr(pack), pack.numel(),
+                                                   self._stream()), "bkm_minibatch_step")
+
     def assign_chunk(self, x, pack, k, labels, min_dist, squared, dist_sum):
         n, d = x.shape
         ws = self._workspace(n, d, k, x.dtype)
@@ -463,10 +472,14 @@ class StreamedChunks(object):
         return len(self.parts)
 
     def __iter__(self):
+        return self.iter_order(range(len(self.parts)))
+
+    def iter_order(self, order):
+        """Iterate the parts in ``order`` (a sequence of part indices), with the same double buffering."""
         be = self.backend
         if be.device.type != "cuda":
-            for p in self.parts:
-                yield p
+            for i in order:
+                yield self.parts[i]
             return
         if self._bufs is None:
             rows = max(self.sizes) if self.sizes else 1
@@ -479,8 +492,9 @@ class StreamedChunks(object):
             self._copy_stream = torch.cuda.Stream(device=be.device)
         main = torch.cuda.current_stream(be.device)
         consumed = [None, None]
-        for i, p in enumerate(self.parts):
-            slot = i & 1
+        for pos, i in enumerate(order):
+            p = self.parts[i]
+            slot = pos & 1
             m = int(p.shape[0])
             with torch.cuda.stream(self._copy_stream):
                 if consumed[slot] is not None:

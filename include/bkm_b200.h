@@ -192,6 +192,18 @@ int bkm_loop_reset(void* loop_state, double tol, double* shift_hist, int hist_ca
 int bkm_finalize_step(const double* reduced, const double* centers_in, double* centers_out, void* loop_state,
                       int k, int d, int x_dtype, void* pack, size_t pack_bytes, void* stream);
 
+/* ---- one mini-batch k-means step: replaces scikit-learn's _minibatch_update_dense -------------------------------
+ * (sklearn/cluster/_k_means_minibatch.pyx, called by MiniBatchKMeans.partial_fit through _mini_batch_step) on the
+ * result of one bkm_lloyd_chunk pass over the batch with BKM_FLAG_FIRST_CHUNK | BKM_FLAG_COUNTS_F64:
+ *   reduced = [k*d sums S | k counts n as float64 | inertia]
+ *   centers_out[j] = (centers_in[j] * weights_in[j] + S[j]) * (1 / (weights_in[j] + n[j]))   if n[j] > 0
+ *                  = centers_in[j]                                                          otherwise
+ *   weights_out[j] = weights_in[j] + n[j]
+ * evaluated in float64 without FMA contraction, and `pack` rebuilt from centers_out (the bytes bkm_pack_centers
+ * writes for them).  centers_in != centers_out and weights_in != weights_out: ping-pong buffers. */
+int bkm_minibatch_step(const double* reduced, const double* centers_in, const double* weights_in, double* centers_out,
+                       double* weights_out, int k, int d, int x_dtype, void* pack, size_t pack_bytes, void* stream);
+
 /* ---- datasets.make_blobs, one block on the device (dask_ml/datasets.py:178-189) ---------------------------------
  * The reference generates every block independently from (centres, cluster_std, seed = block index) with
  * sklearn.datasets.make_blobs; this is the device-side equivalent of ONE block: label_i ~ U{0..k-1}, row_i =
