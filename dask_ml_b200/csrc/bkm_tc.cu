@@ -18,8 +18,9 @@
 //   3 KS wgmma.m64nNk16 (KS = ceil(d/16), a template parameter so that they issue back to back) with B
 //   (= -2 s C as fp16 hi / lo, SWIZZLE_128B K-major) resident in shared memory; N = 256 runs as two column halves in
 //   two commit groups;
-//   the arg-min epilogue from the register accumulators (best, second best, near-tie test), over the first column
-//   half while the tensor cores compute the second;
+//   the arg-min epilogue from the register accumulators in two passes (the row minimum, then the count and index
+//   of the columns within the near-tie bound of it), the first pass over the first column half while the tensor
+//   cores compute the second;
 //   the winning distance in direct form (x - c)^2 in fp32, and the M-step.
 // The M-step adds the tile's rows in row order into the CTA's sums; the two warpgroups take turns (named barriers),
 // so every cluster's sum is formed in one fixed order and the sums are bit-reproducible.  Each sums element has one
@@ -366,36 +367,43 @@ tc_chunk_kernel(ChunkArgs a, typename TcCfgOf<EPI>::type cfg) {
       } else {
         static_assert(EPI == EPI_ARGMIN, "epilogue");
         // ---- arg-min, near-tie test (bound = tau (||s x||^2 + max ||s c||^2)) ----
-        // columns still reach each thread in increasing order: the lowest column wins exact ties as before
-        wg::Best2 b0 = wg::best2_init(), b1 = b0;
+        // pass 1: the values in place and the row minimum m, over the first column half while the second computes
+        float m[2] = {CUDART_INF_F, CUDART_INF_F};
         if constexpr (NH == 2) {
           float(&a0)[NC / 2] = *reinterpret_cast<float(*)[NC / 2]>(acc);
           float(&a1)[NC / 2] = *reinterpret_cast<float(*)[NC / 2]>(acc + NC / 2);
           wg::wait_1();                                      // first column half done, second still running
           wg::pin(a0);
-          wg::best2_cols<NC>(a0, cn_s, 0, lane, b0, b1);
+          wg::min_cols<NC>(a0, cn_s, 0, lane, m);
           wg::wait_all();
           wg::pin(a1);
-          wg::best2_cols<NC>(a1, cn_s, NC, lane, b0, b1);
+          wg::min_cols<NC>(a1, cn_s, NC, lane, m);
         } else {
           wg::wait_all();
           wg::pin(acc);
-          wg::best2_cols<N>(acc, cn_s, 0, lane, b0, b1);
+          wg::min_cols<N>(acc, cn_s, 0, lane, m);
         }
-        wg::best2_quad_merge(b0, b1);
+        wg::min_quad_merge(m);
+        // pass 2: count and index sum of the columns with value <= thr = m + bound (tau >= 0; xn >= 0 or NaN)
+        const float thr[2] = {m[0] + a.tau * (xn0 + cnmax), m[1] + a.tau * (xn1 + cnmax)};
+        float hits[2];
+        wg::hit_cols<N>(acc, thr, hits);
+        wg::hit_quad_merge(hits, lane);
         if ((lane & 3) == 0) {
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
-            const wg::Best2 b = h ? b1 : b0;
             const float xn = h ? xn1 : xn0;
             const int r = rA + 8 * h;
             const long long row = row0 + r;
             // an entry beyond fp16's range (|s x| >= 65504 => xn >= 4.29e9) or a non-finite one: float64 path
             const bool out_of_range = !(xn < 4.29e9f);
-            const bool tie = !(b.m2 > b.m1 + a.tau * (xn + cnmax)) || out_of_range;
+            // a near-tie iff the second best is <= thr, i.e. iff not exactly one column is <= thr; a thr that is +inf
+            // or NaN makes every row a near-tie, as the comparison with the second best does
+            const bool tie = !(hits[h] >= 1.f && hits[h] < 2.f) || !(thr[h] < CUDART_INF_F) || out_of_range;
+            const int j = (int)((hits[h] - 1.f) * 1024.f);  // the arg-min when exactly one column is <= thr
             const bool valid = row < a.n;
             const bool flagged = valid && tie && k > 1;
-            const int bj = (tie || b.j >= k) ? 0 : b.j;
+            const int bj = (tie || j >= k) ? 0 : j;
             if (valid && !flagged && a.labels) a.labels[row] = bj;
             if (flagged) {
               // deferred: tc_recheck_kernel decides this row in float64 and adds its M-step contribution

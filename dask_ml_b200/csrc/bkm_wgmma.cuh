@@ -10,6 +10,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <math_constants.h>
+#include "bkm_ptx.cuh"
 
 namespace bkm {
 namespace wg {
@@ -173,6 +174,69 @@ __device__ __forceinline__ void tile_best2(const float (&d)[N / 2], const float*
   r1 = r0;
   best2_cols<N>(d, cn, 0, lane, r0, r1);
   best2_quad_merge(r0, r1);
+}
+
+// Arg-min epilogue in two passes, for a caller that needs the best column and whether another column lies within a
+// bound of it, but not the second-best value itself.  Pass 1 (min_cols, min_quad_merge) gives the row minimum m; the
+// caller forms thr = m + bound; pass 2 (hit_cols, hit_quad_merge) counts the columns with value <= thr and sums their
+// indices.  When thr is finite and the bound is >= 0, exactly one column qualifies iff the second best of the row is
+// > thr, and that column is the arg-min.  NaN values are skipped by both passes, as best2_add skips them.
+//
+// Pass 1: forms the value d[..] + cn[j] of columns j0 .. j0 + N - 1 of the thread's two rows IN PLACE and folds their
+// minima into m[0], m[1], in four independent chains per row (fminf returns the other operand of a NaN).
+template <int N>
+__device__ __forceinline__ void min_cols(float (&d)[N / 2], const float* cn, int j0, int lane, float (&m)[2]) {
+  static_assert(N >= 16, "the chains start from columns i = 0, 1");
+  const int c2 = j0 + (lane & 3) * 2;
+  float p[2][4];                                     // [row][column parity + 2 (i parity)]
+#pragma unroll
+  for (int i = 0; i < N / 8; ++i) {
+    const float2 cv = *reinterpret_cast<const float2*>(cn + 8 * i + c2);
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      d[4 * i + e] += (e & 1) ? cv.y : cv.x;
+      float& c = p[e >> 1][2 * (i & 1) + (e & 1)];
+      c = i < 2 ? d[4 * i + e] : fminf(c, d[4 * i + e]);
+    }
+  }
+#pragma unroll
+  for (int h = 0; h < 2; ++h) m[h] = fminf(m[h], fminf(fminf(p[h][0], p[h][1]), fminf(p[h][2], p[h][3])));
+}
+// minimum over the four lanes of the quad: every lane ends with its rows' minima over all the columns
+__device__ __forceinline__ void min_quad_merge(float (&m)[2]) {
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    m[h] = fminf(m[h], __shfl_xor_sync(0xffffffffu, m[h], 1));
+    m[h] = fminf(m[h], __shfl_xor_sync(0xffffffffu, m[h], 2));
+  }
+}
+// Pass 2 over the values of all N columns (formed by min_cols) of the thread's two rows: hits[h] = the sum over the
+// columns j with value <= t[h] of 1 + j / 1024, without the lane's column offset 2 (lane % 4) in j, which
+// hit_quad_merge adds: each column then costs one FSET (0 for NaN) and one FFMA with an immediate.  Every partial sum
+// is a multiple of 2^-10 below 2^9, so it is exact in any order.  Two chains per row.
+template <int N>
+__device__ __forceinline__ void hit_cols(const float (&d)[N / 2], const float (&t)[2], float (&hits)[2]) {
+  float c[2][2] = {{0.f, 0.f}, {0.f, 0.f}};         // [row][column parity]
+#pragma unroll
+  for (int i = 0; i < N / 8; ++i)
+#pragma unroll
+    for (int e = 0; e < 4; ++e)
+      c[e >> 1][e & 1] = fmaf(ptx::fset_le(d[4 * i + e], t[e >> 1]), 1.f + (float)(8 * i + (e & 1)) * 0.0009765625f, c[e >> 1][e & 1]);
+#pragma unroll
+  for (int h = 0; h < 2; ++h) hits[h] = c[h][0] + c[h][1];
+}
+// Adds the lane's column offset, then sums over the quad: every lane ends with its rows' totals.  A lane with one hit
+// holds a value in [1, 1.25) (its index part is < 256 / 1024), so floor() is its hit count; a lane with more hits
+// gets some offset >= 0 and stays >= 2.  So the total lies in [1, 2) iff exactly one column of the row is <= t, and then
+// it is 1 + (that column) / 1024.
+__device__ __forceinline__ void hit_quad_merge(float (&hits)[2], int lane) {
+  const float c2 = (float)((lane & 3) * 2) * 0.0009765625f;
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    hits[h] = fmaf(c2, floorf(hits[h]), hits[h]);
+    hits[h] += __shfl_xor_sync(0xffffffffu, hits[h], 1);
+    hits[h] += __shfl_xor_sync(0xffffffffu, hits[h], 2);
+  }
 }
 
 // named barrier of one warpgroup (ids 1.. : id 0 is __syncthreads)
