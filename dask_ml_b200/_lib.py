@@ -56,6 +56,11 @@ SIGNATURES = {
                                        ctypes.c_size_t, _int, _c_void_p]),
     "bkm_nystrom_embed_chunk": (_int, [_c_void_p, _i64, _int, _i64, _int, _c_void_p, _int, _dbl, _c_void_p, _int,
                                        _c_void_p, _i64, _int, _c_void_p]),
+    "bkm_gram_workspace_bytes": (_int, [_i64, _int, _szp]),
+    "bkm_gram_chunk": (_int, [_c_void_p, _i64, _int, _i64, _int, _c_void_p, _c_void_p, _c_void_p, _c_void_p,
+                              ctypes.c_size_t, _int, _c_void_p]),
+    "bkm_project_chunk": (_int, [_c_void_p, _i64, _int, _i64, _int, _c_void_p, _c_void_p, _int, _c_void_p, _i64, _int,
+                                 _c_void_p, _i64, _int, _c_void_p]),
     "bkm_finalize": (_int, [_c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_void_p, _int, _int, _c_void_p]),
     "bkm_check_finite": (_int, [_c_void_p, _i64, _int, _i64, _int, _c_void_p, _c_void_p]),
     "bkm_p2p_mailbox_bytes": (_int, [_int, _i64, ctypes.POINTER(ctypes.c_size_t)]),

@@ -403,6 +403,42 @@ class CudaBackend(object):
                 self._ptr(x), n, d, x.stride(0) if n else d, _DT_CODE[x.dtype], self._ptr(pack), int(l), float(gamma),
                 self._ptr(colsum), self._ptr(ws), ws.numel(), flags, self._stream()), "bkm_kernel_colsum_chunk")
 
+    def gram_chunk(self, x, shift, colsum, gram, first=False):
+        """colsum (+)= sum_i (x_i - shift) and gram (+)= sum_i (x_i - shift)(x_i - shift)^T over the rows of the chunk
+        (float64 [d] and [d, d] on the device); ``first`` overwrites.  The fit pass of PCA / TruncatedSVD."""
+        n, d = x.shape
+        nb = ctypes.c_size_t(0)
+        _lib.check(self.lib.bkm_gram_workspace_bytes(int(n), int(d), ctypes.byref(nb)), "bkm_gram_workspace_bytes")
+        ws = self._ws.get("gram")
+        if ws is None or ws.numel() < nb.value:
+            ws = torch.empty(max(int(nb.value), 256), dtype=torch.uint8, device=self.device)
+            self._ws["gram"] = ws
+        flags = self.flags | (_lib.FLAG_FIRST_CHUNK if first else 0)
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.bkm_gram_chunk(
+                self._ptr(x), n, d, x.stride(0) if n else d, _DT_CODE[x.dtype], self._ptr(shift), self._ptr(colsum),
+                self._ptr(gram), self._ptr(ws), ws.numel(), flags, self._stream()), "bkm_gram_chunk")
+
+    def project_chunk(self, x, shift, W, out=None, colmax=None, row_offset=0):
+        """out = (x - shift) W^T (``W`` float64 (k, d), ``shift`` float64 (d,) or None, ``out`` (n, k) float32 / float64
+        with any row pitch, or None) and, into ``colmax`` (float64 (k, 4) records, see ``colmax_new``), per column
+        the largest |out_ij| with its lowest global row ``row_offset + i`` and its signed value."""
+        n, d = x.shape
+        k = int(W.shape[0])
+        odt = _DT_CODE[out.dtype] if out is not None else _lib.BKM_F64
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.bkm_project_chunk(
+                self._ptr(x), n, d, x.stride(0) if n else d, _DT_CODE[x.dtype], self._ptr(shift), self._ptr(W), k,
+                self._ptr(out), (out.stride(0) if n else k) if out is not None else k, odt, self._ptr(colmax),
+                int(row_offset), self.flags, self._stream()), "bkm_project_chunk")
+
+    def colmax_new(self, k):
+        """k empty arg-max records {absmax = -1, row = -1, value = 0, lock = 0} for ``project_chunk``."""
+        rec = torch.zeros((k, 4), dtype=torch.float64)
+        rec[:, 0] = -1.0
+        rec[:, 1:2].view(torch.int64).fill_(-1)
+        return rec.to(self.device)
+
     def nystrom_embed(self, x, pack, l, gamma, W, out):
         """out[i] = e_i / ||e_i||, e_i = sum_j exp(-gamma (||x_i - c_j||^2 - min_j ||x_i - c_j||^2)) W[j] — the second
         pass of the Nystrom embedding.  ``W`` is (l, k) in the dtype of x; ``out`` (n, k) may have a padded row pitch."""

@@ -20,6 +20,8 @@
  *   da.isnull(X).any(), da.isinf(X).any()  k_means.py:179-180     bkm_check_finite
  *   pairwise_kernels(X_keep, X_rest) and the products with B of   bkm_kernel_colsum_chunk
  *     SpectralClustering.fit, cluster/spectral.py:237-270          bkm_nystrom_embed_chunk
+ *   da.linalg.svd(X) + svd_flip of PCA / TruncatedSVD             bkm_gram_chunk + bkm_project_chunk
+ *     decomposition/pca.py, truncated_svd.py
  *
  * Conventions
  *   - extern "C", plain pointers and sizes only; no torch / C++ types.
@@ -166,6 +168,27 @@ int bkm_kernel_colsum_chunk(const void* X, int64_t n, int d, int64_t ldx, int x_
                             void* stream);
 int bkm_nystrom_embed_chunk(const void* X, int64_t n, int d, int64_t ldx, int x_dtype, const void* pack, int l,
                             double gamma, const void* W, int k, void* out, int64_t ld_out, int flags, void* stream);
+
+/* ---- PCA / TruncatedSVD: the two passes over row chunks (replace da.linalg.svd / svd_flip of
+ * dask_ml/decomposition/pca.py and truncated_svd.py by a float64 Gram matrix and its eigendecomposition) -------------
+ * Both widen the rows to float64, subtract the shift and multiply on the fp64 tensor cores (DMMA), so for every input
+ * dtype the results are float64 sums of exact float64 products.  Any d, any row pitch ldx >= d.
+ *   bkm_gram_chunk     colsum [d]    (+)= sum_i (x_i - shift)
+ *                      gram   [d][d] (+)= sum_i (x_i - shift)(x_i - shift)^T   (full symmetric matrix, row-major)
+ *                      OVERWRITTEN with BKM_FLAG_FIRST_CHUNK, else ACCUMULATED.  shift [d] float64 (device).  Per-CTA
+ *                      partials are added in a fixed order: two calls with the same inputs give the same bits.
+ *                      workspace: bkm_gram_workspace_bytes(n, d) bytes, any content.
+ *   bkm_project_chunk  out [n][ldo] = (x - shift) W^T, out_dtype BKM_F32 or BKM_F64 (out nullable; shift nullable:
+ *                      no shift), W [k][d] float64 row-major.  colmax (nullable) [k] records of 32 bytes
+ *                      {double absmax, int64 row, double value, uint64 lock}: per column j the largest |out_ij| over
+ *                      the chunk, its lowest GLOBAL row (row_offset + i) and the signed value, folded into the record
+ *                      (larger |value| wins, equal |value| -> lower row).  Initialise records to {-1, -1, 0, 0}. */
+int bkm_gram_workspace_bytes(int64_t n, int d, size_t* out);
+int bkm_gram_chunk(const void* X, int64_t n, int d, int64_t ldx, int x_dtype, const double* shift, double* colsum,
+                   double* gram, void* workspace, size_t ws_bytes, int flags, void* stream);
+int bkm_project_chunk(const void* X, int64_t n, int d, int64_t ldx, int x_dtype, const double* shift,
+                      const double* W, int k, void* out, int64_t ldo, int out_dtype, void* colmax, int64_t row_offset,
+                      int flags, void* stream);
 
 /* ---- centre update + shift (k_means.py:548-555), run after the cross-GPU allreduce ----
  *   C_new = sums / max(counts,1)[:,None]   (empty cluster -> zero vector, Q1)
