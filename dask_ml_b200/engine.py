@@ -439,6 +439,40 @@ class CudaBackend(object):
         rec[:, 1:2].view(torch.int64).fill_(-1)
         return rec.to(self.device)
 
+    def class_moments_chunk(self, x, cls, K, sums, counts=None, theta=None, first=False):
+        """GaussianNB's fit passes over the rows of one chunk, by int32 class index ``cls`` (indices outside [0, K) are
+        skipped): without ``theta``, sums (K, d) (+)= per-class row sums and counts (K,) (+)= per-class rows; with
+        ``theta`` (float64 (K, d)), sums (+)= per-class sums of (x - theta_c)^2.  float64 on the device; ``first``
+        overwrites."""
+        n, d = x.shape
+        nb = ctypes.c_size_t(0)
+        _lib.check(self.lib.bkm_nb_workspace_bytes(int(n), int(d), int(K), ctypes.byref(nb)), "bkm_nb_workspace_bytes")
+        ws = self._ws.get("nb")
+        if ws is None or ws.numel() < nb.value:
+            ws = torch.empty(max(int(nb.value), 256), dtype=torch.uint8, device=self.device)
+            self._ws["nb"] = ws
+        flags = self.flags | (_lib.FLAG_FIRST_CHUNK if first else 0)
+        mode = 0 if theta is None else 1
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.bkm_class_moments_chunk(
+                self._ptr(x), n, d, x.stride(0) if n else d, _DT_CODE[x.dtype], self._ptr(cls), int(K), mode,
+                self._ptr(theta), self._ptr(sums), self._ptr(counts), self._ptr(ws), ws.numel(), flags,
+                self._stream()), "bkm_class_moments_chunk")
+
+    def nb_jll_chunk(self, x, theta, inv_sigma, logc, labels=None, out=None, exp_out=False, n_deferred=None):
+        """GaussianNB's predict pass over one chunk: ``labels`` (int32 (n,)) the arg-max of the joint log-likelihood
+        and / or ``out`` (float64 (n, K), any row pitch) its log-softmax, exponentiated with ``exp_out``.  ``theta``,
+        ``inv_sigma`` float64 (K, d), ``logc`` float64 (K,) on the device; ``n_deferred`` (int32 (1,)) counts the fp32
+        rows re-decided in float64."""
+        n, d = x.shape
+        K = int(theta.shape[0])
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.bkm_nb_jll_chunk(
+                self._ptr(x), n, d, x.stride(0) if n else d, _DT_CODE[x.dtype], self._ptr(theta), self._ptr(inv_sigma),
+                self._ptr(logc), K, self._ptr(labels), self._ptr(out),
+                (out.stride(0) if n else K) if out is not None else K, int(bool(exp_out)), self._ptr(n_deferred),
+                self.flags, self._stream()), "bkm_nb_jll_chunk")
+
     def nystrom_embed(self, x, pack, l, gamma, W, out):
         """out[i] = e_i / ||e_i||, e_i = sum_j exp(-gamma (||x_i - c_j||^2 - min_j ||x_i - c_j||^2)) W[j] — the second
         pass of the Nystrom embedding.  ``W`` is (l, k) in the dtype of x; ``out`` (n, k) may have a padded row pitch."""

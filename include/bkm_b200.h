@@ -22,6 +22,8 @@
  *     SpectralClustering.fit, cluster/spectral.py:237-270          bkm_nystrom_embed_chunk
  *   da.linalg.svd(X) + svd_flip of PCA / TruncatedSVD             bkm_gram_chunk + bkm_project_chunk
  *     decomposition/pca.py, truncated_svd.py
+ *   X[y == c].mean(0) / .var(0) and _joint_log_likelihood of      bkm_class_moments_chunk + bkm_nb_jll_chunk
+ *     GaussianNB, naive_bayes.py:32-122
  *
  * Conventions
  *   - extern "C", plain pointers and sizes only; no torch / C++ types.
@@ -189,6 +191,31 @@ int bkm_gram_chunk(const void* X, int64_t n, int d, int64_t ldx, int x_dtype, co
 int bkm_project_chunk(const void* X, int64_t n, int d, int64_t ldx, int x_dtype, const double* shift,
                       const double* W, int k, void* out, int64_t ldo, int out_dtype, void* colmax, int64_t row_offset,
                       int flags, void* stream);
+
+/* ---- GaussianNB: the fit passes and the predict pass over row chunks (replace the per-class X[y == c].mean / .var
+ * and the K stacked elementwise passes of _joint_log_likelihood in dask_ml/naive_bayes.py) ---------------------------
+ *   bkm_class_moments_chunk  cls [n] int32 class indices; rows with cls outside [0, K) are left out of every sum.
+ *                      mode 0: sums [K][d] (+)= sum of the rows of class c, counts [K] float64 (+)= their number
+ *                      mode 1: sums [K][d] (+)= sum of (x - theta_c)^2 over the rows of class c (theta [K][d] float64;
+ *                              counts unused)
+ *                      OVERWRITTEN with BKM_FLAG_FIRST_CHUNK, else ACCUMULATED.  float64 accumulators in a fixed order
+ *                      (per-CTA row groups, then groups, then row splits): two calls with the same inputs give the
+ *                      same bits.  workspace: bkm_nb_workspace_bytes(n, d, K) bytes, any content.
+ *   bkm_nb_jll_chunk   jll_ic = logc_c - 1/2 sum_j (x_ij - theta_cj)^2 inv_sigma_cj (theta, inv_sigma [K][d], logc [K]
+ *                      float64; all finite except logc, where NaN marks a class whose log-likelihood is NaN).
+ *                      labels [n] (nullable): arg-max over c, lowest c on exact ties, the first NaN class if any.
+ *                      out [n][ldo] float64 (nullable): jll - (log sum_c exp(jll - max) + max), exponentiated when
+ *                      exp_out; a row with any NaN jll is NaN throughout.  fp32 / bf16 rows are computed in fp32; a row
+ *                      whose best class is not ahead of every other class by the fp32 error bound is re-decided in
+ *                      float64 (skipped with BKM_FLAG_NO_RECHECK) and counted into n_deferred (int32, nullable,
+ *                      ACCUMULATED).  float64 rows are computed in float64.  Any d, any row pitch ldx >= d. */
+int bkm_nb_workspace_bytes(int64_t n, int d, int K, size_t* out);
+int bkm_class_moments_chunk(const void* X, int64_t n, int d, int64_t ldx, int x_dtype, const int32_t* cls, int K,
+                            int mode, const double* theta, double* sums, double* counts, void* workspace,
+                            size_t ws_bytes, int flags, void* stream);
+int bkm_nb_jll_chunk(const void* X, int64_t n, int d, int64_t ldx, int x_dtype, const double* theta,
+                     const double* inv_sigma, const double* logc, int K, int32_t* labels, double* out, int64_t ldo,
+                     int exp_out, int* n_deferred, int flags, void* stream);
 
 /* ---- centre update + shift (k_means.py:548-555), run after the cross-GPU allreduce ----
  *   C_new = sums / max(counts,1)[:,None]   (empty cluster -> zero vector, Q1)
