@@ -66,6 +66,11 @@ SIGNATURES = {
                                        _c_void_p, _c_void_p, ctypes.c_size_t, _int, _c_void_p]),
     "bkm_nb_jll_chunk": (_int, [_c_void_p, _i64, _int, _i64, _int, _c_void_p, _c_void_p, _c_void_p, _int, _c_void_p,
                                 _c_void_p, _i64, _int, _c_void_p, _int, _c_void_p]),
+    "bkm_glm_workspace_bytes": (_int, [_i64, _int, _szp]),
+    "bkm_glm_pass_chunk": (_int, [_c_void_p, _i64, _int, _i64, _int, _c_void_p, _c_void_p, _int, _int, _c_void_p,
+                                  _c_void_p, _c_void_p, _c_void_p, _c_void_p, ctypes.c_size_t, _int, _c_void_p]),
+    "bkm_gram_weighted_chunk": (_int, [_c_void_p, _i64, _int, _i64, _int, _c_void_p, _c_void_p, _c_void_p,
+                                       ctypes.c_size_t, _int, _c_void_p]),
     "bkm_finalize": (_int, [_c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_void_p, _int, _int, _c_void_p]),
     "bkm_check_finite": (_int, [_c_void_p, _i64, _int, _i64, _int, _c_void_p, _c_void_p]),
     "bkm_p2p_mailbox_bytes": (_int, [_int, _i64, ctypes.POINTER(ctypes.c_size_t)]),

@@ -90,6 +90,7 @@ struct GramArgs {
   long long rows_per_split;
   int first;
   int bulk;
+  const double* w;         // WEIGHTED: the row weights [n]
 };
 
 template <typename T>
@@ -100,7 +101,9 @@ static size_t gram_smem_bytes() {
          + 16;                               // two mbarriers
 }
 
-template <typename T>
+// WEIGHTED: G (+)= sum_i w_i x_i x_i^T, no shift and no column sums.  The weight scales the block-j operand tile as it
+// is widened, so the diagonal tiles convert their one staged block twice (block i plain, block j weighted).
+template <typename T, bool WEIGHTED = false>
 __global__ void __launch_bounds__(kThreads) gram_kernel(GramArgs a) {
   extern __shared__ __align__(128) unsigned char smem[];
   double* Fi = reinterpret_cast<double*>(smem);
@@ -118,8 +121,9 @@ __global__ void __launch_bounds__(kThreads) gram_kernel(GramArgs a) {
   const bool diag = bi == bj;
   const int f0i = bi * GB, f0j = bj * GB;
   const int wi = min(GB, d - f0i), wj = min(GB, d - f0j);
-  double* Fj = diag ? Fi : Fi + GR * GP;
+  double* Fj = (diag && !WEIGHTED) ? Fi : Fi + GR * GP;
   const int nblk = diag ? 1 : 2;
+  const int ncvt = WEIGHTED ? 2 : nblk;         // operand tiles converted per staged tile
 
   const long long rb = (long long)split * a.rows_per_split;
   const long long re = min(a.n, rb + a.rows_per_split);
@@ -173,11 +177,11 @@ __global__ void __launch_bounds__(kThreads) gram_kernel(GramArgs a) {
     if (a.bulk) mbar_wait(bar0 + 8u * st, (uint32_t)((t >> 1) & 1));
     __syncthreads();                            // the previous tile's MMAs are done with Fi / Fj
 #pragma unroll 1
-    for (int b = 0; b < nblk; ++b) {
+    for (int b = 0; b < ncvt; ++b) {
       double* F = b ? Fj : Fi;
       const int f0 = b ? f0j : f0i, w = b ? wj : wi;
-      const T* rs = raw + (size_t)(st * 2 + b) * GR * GB;
-      const double sh = cf < w ? a.shift[f0 + cf] : 0.0;
+      const T* rs = raw + (size_t)(st * 2 + (WEIGHTED && diag ? 0 : b)) * GR * GB;
+      const double sh = WEIGHTED ? 0.0 : (cf < w ? a.shift[f0 + cf] : 0.0);
 #pragma unroll 4
       for (int e = tid; e < GR * GB; e += kThreads) {
         const int r = e >> 6;
@@ -185,9 +189,10 @@ __global__ void __launch_bounds__(kThreads) gram_kernel(GramArgs a) {
         if (r < rows && cf < w) {
           const T x = a.bulk ? rs[r * GB + cf] : X[(r0 + r) * a.ldx + f0 + cf];
           v = to_f64(x) - sh;
+          if (WEIGHTED && b) v *= a.w[r0 + r];
         }
         F[r * GP + cf] = v;
-        if (diag) csum += v;
+        if (diag && !WEIGHTED) csum += v;
       }
     }
     __syncthreads();
@@ -226,7 +231,7 @@ __global__ void __launch_bounds__(kThreads) gram_kernel(GramArgs a) {
     P[(r + 8) * GB + c] = acc[nt][2];
     P[(r + 8) * GB + c + 1] = acc[nt][3];
   }
-  if (diag) {
+  if (diag && !WEIGHTED) {
     cred[(tid >> 6) * GB + cf] = csum;
     __syncthreads();
     if (tid < GB)
@@ -258,7 +263,7 @@ __global__ void __launch_bounds__(kThreads) gram_kernel(GramArgs a) {
       *gji = u;
     }
   }
-  if (diag && tid < wi) {
+  if (diag && !WEIGHTED && tid < wi) {
     double v = 0.0;
     for (int s = 0; s < a.splits; ++s) v += __ldcg(a.cpart + ((size_t)bi * a.splits + s) * GB + tid);
     a.colsum[f0i + tid] = a.first ? v : a.colsum[f0i + tid] + v;
@@ -435,11 +440,11 @@ static int sm_count(int* out) {
   return 0;
 }
 
-template <typename T>
+template <typename T, bool WEIGHTED = false>
 static int launch_gram(const GramArgs& a, int pairs, int splits, cudaStream_t s) {
   const size_t sm = gram_smem_bytes<T>();
-  BKM_CUDA_TRY(cudaFuncSetAttribute(gram_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
-  gram_kernel<T><<<dim3(pairs, splits), kThreads, sm, s>>>(a);
+  BKM_CUDA_TRY(cudaFuncSetAttribute(gram_kernel<T, WEIGHTED>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
+  gram_kernel<T, WEIGHTED><<<dim3(pairs, splits), kThreads, sm, s>>>(a);
   BKM_CUDA_TRY(cudaGetLastError());
   note_launch();
   return 0;
@@ -466,6 +471,27 @@ static int launch_project(const ProjArgs& a, int sms, cudaStream_t s) {
   return launch_project_nt<T, 4>(a, sms, s);
 }
 
+template <bool WEIGHTED>
+static int gram_run(const void* X, int64_t n, int d, int64_t ldx, int x_dtype, const double* shift, double* colsum,
+                    double* gram, const double* w, const GramGeom& G, void* workspace, int flags, void* stream) {
+  cudaStream_t s = (cudaStream_t)stream;
+  unsigned char* ws = reinterpret_cast<unsigned char*>(workspace);
+  BKM_CUDA_TRY(cudaMemsetAsync(ws + G.off_ticket, 0, (size_t)G.pairs * 4, s));
+  const size_t es = esize(x_dtype);
+  GramArgs a;
+  a.X = X; a.n = n; a.d = d; a.ldx = ldx; a.shift = shift; a.colsum = colsum; a.gram = gram; a.w = w;
+  a.part = reinterpret_cast<double*>(ws + G.off_part);
+  a.cpart = reinterpret_cast<double*>(ws + G.off_cpart);
+  a.ticket = reinterpret_cast<unsigned int*>(ws + G.off_ticket);
+  a.nb = G.nb; a.splits = G.splits; a.rows_per_split = G.rows_per_split;
+  a.first = (flags & BKM_FLAG_FIRST_CHUNK) ? 1 : 0;
+  // bulk copies need 16-byte aligned sources and sizes: base, row pitch and (for the last block) the row width
+  a.bulk = n > 0 && ((uintptr_t)X % 16 == 0) && ((ldx * es) % 16 == 0) && ((d * es) % 16 == 0);
+  if (x_dtype == BKM_F32) return launch_gram<float, WEIGHTED>(a, G.pairs, G.splits, s);
+  if (x_dtype == BKM_F64) return launch_gram<double, WEIGHTED>(a, G.pairs, G.splits, s);
+  return launch_gram<__nv_bfloat16, WEIGHTED>(a, G.pairs, G.splits, s);
+}
+
 }  // namespace
 }  // namespace bkm
 
@@ -489,22 +515,20 @@ extern "C" int bkm_gram_chunk(const void* X, int64_t n, int d, int64_t ldx, int 
   if (rc) return rc;
   const GramGeom G = gram_geom(n, d, sms);
   if (ws_bytes < G.total) return BKM_EWORKSPACE;
-  cudaStream_t s = (cudaStream_t)stream;
-  unsigned char* ws = reinterpret_cast<unsigned char*>(workspace);
-  BKM_CUDA_TRY(cudaMemsetAsync(ws + G.off_ticket, 0, (size_t)G.pairs * 4, s));
-  const size_t es = esize(x_dtype);
-  GramArgs a;
-  a.X = X; a.n = n; a.d = d; a.ldx = ldx; a.shift = shift; a.colsum = colsum; a.gram = gram;
-  a.part = reinterpret_cast<double*>(ws + G.off_part);
-  a.cpart = reinterpret_cast<double*>(ws + G.off_cpart);
-  a.ticket = reinterpret_cast<unsigned int*>(ws + G.off_ticket);
-  a.nb = G.nb; a.splits = G.splits; a.rows_per_split = G.rows_per_split;
-  a.first = (flags & BKM_FLAG_FIRST_CHUNK) ? 1 : 0;
-  // bulk copies need 16-byte aligned sources and sizes: base, row pitch and (for the last block) the row width
-  a.bulk = n > 0 && ((uintptr_t)X % 16 == 0) && ((ldx * es) % 16 == 0) && ((d * es) % 16 == 0);
-  if (x_dtype == BKM_F32) return launch_gram<float>(a, G.pairs, G.splits, s);
-  if (x_dtype == BKM_F64) return launch_gram<double>(a, G.pairs, G.splits, s);
-  return launch_gram<__nv_bfloat16>(a, G.pairs, G.splits, s);
+  return gram_run<false>(X, n, d, ldx, x_dtype, shift, colsum, gram, nullptr, G, workspace, flags, stream);
+}
+
+extern "C" int bkm_gram_weighted_chunk(const void* X, int64_t n, int d, int64_t ldx, int x_dtype, const double* w,
+                                       double* gram, void* workspace, size_t ws_bytes, int flags, void* stream) {
+  if (n < 0 || d <= 0 || ldx < d || !gram || !workspace) return BKM_EINVAL;
+  if (n > 0 && (!X || !w)) return BKM_EINVAL;
+  if (!dtype_ok(x_dtype)) return BKM_EDTYPE;
+  int sms = 0;
+  const int rc = sm_count(&sms);
+  if (rc) return rc;
+  const GramGeom G = gram_geom(n, d, sms);
+  if (ws_bytes < G.total) return BKM_EWORKSPACE;
+  return gram_run<true>(X, n, d, ldx, x_dtype, nullptr, nullptr, gram, w, G, workspace, flags, stream);
 }
 
 extern "C" int bkm_project_chunk(const void* X, int64_t n, int d, int64_t ldx, int x_dtype, const double* shift,

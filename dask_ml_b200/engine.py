@@ -209,6 +209,14 @@ class CudaBackend(object):
             self._ws["buf"] = ws
         return ws
 
+    def _scratch(self, key, nbytes):
+        """A grow-only device buffer of at least ``nbytes`` per key (the workspace of one kind of pass)."""
+        ws = self._ws.get(key)
+        if ws is None or ws.numel() < nbytes:
+            ws = torch.empty(max(int(nbytes), 256), dtype=torch.uint8, device=self.device)
+            self._ws[key] = ws
+        return ws
+
     def kernel_family(self, d, k, dtype):
         return self.lib.bkm_kernel_family(d, k, _DT_CODE[dtype], self.flags)
 
@@ -409,10 +417,7 @@ class CudaBackend(object):
         n, d = x.shape
         nb = ctypes.c_size_t(0)
         _lib.check(self.lib.bkm_gram_workspace_bytes(int(n), int(d), ctypes.byref(nb)), "bkm_gram_workspace_bytes")
-        ws = self._ws.get("gram")
-        if ws is None or ws.numel() < nb.value:
-            ws = torch.empty(max(int(nb.value), 256), dtype=torch.uint8, device=self.device)
-            self._ws["gram"] = ws
+        ws = self._scratch("gram", nb.value)
         flags = self.flags | (_lib.FLAG_FIRST_CHUNK if first else 0)
         with torch.cuda.device(self.device):
             _lib.check(self.lib.bkm_gram_chunk(
@@ -447,10 +452,7 @@ class CudaBackend(object):
         n, d = x.shape
         nb = ctypes.c_size_t(0)
         _lib.check(self.lib.bkm_nb_workspace_bytes(int(n), int(d), int(K), ctypes.byref(nb)), "bkm_nb_workspace_bytes")
-        ws = self._ws.get("nb")
-        if ws is None or ws.numel() < nb.value:
-            ws = torch.empty(max(int(nb.value), 256), dtype=torch.uint8, device=self.device)
-            self._ws["nb"] = ws
+        ws = self._scratch("nb", nb.value)
         flags = self.flags | (_lib.FLAG_FIRST_CHUNK if first else 0)
         mode = 0 if theta is None else 1
         with torch.cuda.device(self.device):
@@ -472,6 +474,38 @@ class CudaBackend(object):
                 self._ptr(logc), K, self._ptr(labels), self._ptr(out),
                 (out.stride(0) if n else K) if out is not None else K, int(bool(exp_out)), self._ptr(n_deferred),
                 self.flags, self._stream()), "bkm_nb_jll_chunk")
+
+    def glm_pass_chunk(self, x, y, beta, family, mode, grad=None, hrow=None, w=None, out=None, first=False):
+        """The fused pass of the linear models over one chunk (float64 arithmetic): eta = x . beta[:d] + beta[d] with
+        ``family`` 0 logistic, 1 normal, 2 poisson.  ``mode`` 0: grad (d + 2,) (+)= [sum r x | sum r | loss];
+        1: the same, w (n,) = the Newton weights and hrow (d + 1,) (+)= [sum w x | sum w]; 2: out (n,) float64 = mu;
+        3: out (n,) uint8 = mu > 0.5.  ``y`` float64 (n,) (modes 0 and 1), ``beta`` float64 (d + 1,) on the device;
+        ``first`` overwrites."""
+        n, d = x.shape
+        ws = None
+        if mode in (0, 1):
+            nb = ctypes.c_size_t(0)
+            _lib.check(self.lib.bkm_glm_workspace_bytes(int(n), int(d), ctypes.byref(nb)), "bkm_glm_workspace_bytes")
+            ws = self._scratch("glm", nb.value)
+        flags = self.flags | (_lib.FLAG_FIRST_CHUNK if first else 0)
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.bkm_glm_pass_chunk(
+                self._ptr(x), n, d, x.stride(0) if n else d, _DT_CODE[x.dtype], self._ptr(y), self._ptr(beta),
+                int(family), int(mode), self._ptr(grad), self._ptr(hrow), self._ptr(w), self._ptr(out), self._ptr(ws),
+                ws.numel() if ws is not None else 0, flags, self._stream()), "bkm_glm_pass_chunk")
+
+    def gram_weighted_chunk(self, x, w, gram, first=False):
+        """gram (+)= sum_i w_i x_i x_i^T over the rows of the chunk (``w`` float64 (n,), ``gram`` float64 (d, d) on the
+        device): the Hessian block of a Newton step.  ``first`` overwrites."""
+        n, d = x.shape
+        nb = ctypes.c_size_t(0)
+        _lib.check(self.lib.bkm_gram_workspace_bytes(int(n), int(d), ctypes.byref(nb)), "bkm_gram_workspace_bytes")
+        ws = self._scratch("gram", nb.value)
+        flags = self.flags | (_lib.FLAG_FIRST_CHUNK if first else 0)
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.bkm_gram_weighted_chunk(
+                self._ptr(x), n, d, x.stride(0) if n else d, _DT_CODE[x.dtype], self._ptr(w), self._ptr(gram),
+                self._ptr(ws), ws.numel(), flags, self._stream()), "bkm_gram_weighted_chunk")
 
     def nystrom_embed(self, x, pack, l, gamma, W, out):
         """out[i] = e_i / ||e_i||, e_i = sum_j exp(-gamma (||x_i - c_j||^2 - min_j ||x_i - c_j||^2)) W[j] — the second

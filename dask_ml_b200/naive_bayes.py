@@ -32,10 +32,10 @@ from .chunked import ChunkedArray, _is_torch, as_chunked, block_to_numpy, is_das
 from .decomposition.pca import _device_data
 
 
-def _y_flat(y):
+def _y_flat(y, who="GaussianNB.fit"):
     """y (numpy, torch on any device, ChunkedArray or dask array, any chunking) -> one flat numpy array or tensor."""
     if y is None:
-        raise ValueError("GaussianNB.fit needs the labels y; got None")
+        raise ValueError("%s needs the labels y; got None" % who)
     if isinstance(y, ChunkedArray):
         blocks = y.blocks
     elif is_dask_array(y):

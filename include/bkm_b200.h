@@ -24,6 +24,9 @@
  *     decomposition/pca.py, truncated_svd.py
  *   X[y == c].mean(0) / .var(0) and _joint_log_likelihood of      bkm_class_moments_chunk + bkm_nb_jll_chunk
  *     GaussianNB, naive_bayes.py:32-122
+ *   dask_glm's per-iteration X.dot(beta), family loglike /        bkm_glm_pass_chunk + bkm_gram_weighted_chunk
+ *     gradient / hessian of LogisticRegression, LinearRegression,
+ *     PoissonRegression, linear_model/glm.py:169-362
  *
  * Conventions
  *   - extern "C", plain pointers and sizes only; no torch / C++ types.
@@ -216,6 +219,30 @@ int bkm_class_moments_chunk(const void* X, int64_t n, int d, int64_t ldx, int x_
 int bkm_nb_jll_chunk(const void* X, int64_t n, int d, int64_t ldx, int x_dtype, const double* theta,
                      const double* inv_sigma, const double* logc, int K, int32_t* labels, double* out, int64_t ldo,
                      int exp_out, int* n_deferred, int flags, void* stream);
+
+/* ---- LogisticRegression / LinearRegression / PoissonRegression: the per-iteration passes of the solvers (replace
+ * dask_glm's X.dot(beta) and the family's loglike / gradient / hessian, linear_model/glm.py) ------------------------
+ *   bkm_glm_pass_chunk  eta_i = x_i . beta[0:d] + beta[d]  (beta [d + 1] float64; rows widened to float64, float64
+ *                      arithmetic).  family 0 logistic (mu = sigmoid(eta), loss = softplus(eta) - y eta, r = mu - y,
+ *                      w = mu (1 - mu)), 1 normal (mu = eta, loss = (y - eta)^2, r = 2 (mu - y), w = 2), 2 poisson
+ *                      (mu = exp(eta), loss = mu - y eta, r = mu - y, w = mu; exp overflows to +inf above 709.78).
+ *                      mode 0 (gradient): grad [d + 2] (+)= [sum r_i x_i | sum r_i | sum loss_i]   (y [n] float64)
+ *                      mode 1 (Newton):   the same, and w [n] = w_i, hrow [d + 1] (+)= [sum w_i x_i | sum w_i]
+ *                      mode 2 (predict):  out [n] float64 = mu_i          mode 3 (labels): out [n] uint8 = mu_i > 0.5
+ *                      (the predict modes take no y and accumulate nothing).  OVERWRITTEN with BKM_FLAG_FIRST_CHUNK,
+ *                      else ACCUMULATED.  Per-CTA partials are added in a fixed order (no float atomics): two calls
+ *                      with the same inputs give the same bits.  Any d, any row pitch ldx >= d.  One launch.
+ *                      workspace: bkm_glm_workspace_bytes(n, d) bytes, any content (unused by the predict modes).
+ *   bkm_gram_weighted_chunk  gram [d][d] (+)= sum_i w_i x_i x_i^T (w [n] float64; full symmetric matrix), the
+ *                      Hessian block of a Newton step.  The kernel of bkm_gram_chunk without shift and column sums,
+ *                      the weight applied to one operand as the rows are widened; same order guarantee.
+ *                      workspace: bkm_gram_workspace_bytes(n, d) bytes. */
+int bkm_glm_workspace_bytes(int64_t n, int d, size_t* out);
+int bkm_glm_pass_chunk(const void* X, int64_t n, int d, int64_t ldx, int x_dtype, const double* y, const double* beta,
+                       int family, int mode, double* grad, double* hrow, double* w, void* out, void* workspace,
+                       size_t ws_bytes, int flags, void* stream);
+int bkm_gram_weighted_chunk(const void* X, int64_t n, int d, int64_t ldx, int x_dtype, const double* w, double* gram,
+                            void* workspace, size_t ws_bytes, int flags, void* stream);
 
 /* ---- centre update + shift (k_means.py:548-555), run after the cross-GPU allreduce ----
  *   C_new = sums / max(counts,1)[:,None]   (empty cluster -> zero vector, Q1)
