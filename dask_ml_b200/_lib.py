@@ -71,6 +71,15 @@ SIGNATURES = {
                                   _c_void_p, _c_void_p, _c_void_p, _c_void_p, ctypes.c_size_t, _int, _c_void_p]),
     "bkm_gram_weighted_chunk": (_int, [_c_void_p, _i64, _int, _i64, _int, _c_void_p, _c_void_p, _c_void_p,
                                        ctypes.c_size_t, _int, _c_void_p]),
+    "bkm_colstats_workspace_bytes": (_int, [_i64, _int, _szp]),
+    "bkm_colstats_chunk": (_int, [_c_void_p, _i64, _int, _i64, _int, _c_void_p, _c_void_p, _c_void_p, _c_void_p,
+                                  ctypes.c_size_t, _int, _c_void_p]),
+    "bkm_radix_state_bytes": (_int, [_int, _int, _szp]),
+    "bkm_radix_hist_chunk": (_int, [_c_void_p, _i64, _int, _i64, _int, _c_void_p, _int, _int, _c_void_p, _int,
+                                    _c_void_p]),
+    "bkm_radix_select_step": (_int, [_c_void_p, _c_void_p, _int, _int, _int, _int, _c_void_p, _c_void_p]),
+    "bkm_affine_chunk": (_int, [_c_void_p, _i64, _int, _i64, _int, _c_void_p, _c_void_p, _int, _int, _c_void_p, _i64,
+                                _int, _c_void_p]),
     "bkm_finalize": (_int, [_c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_void_p, _int, _int, _c_void_p]),
     "bkm_check_finite": (_int, [_c_void_p, _i64, _int, _i64, _int, _c_void_p, _c_void_p]),
     "bkm_p2p_mailbox_bytes": (_int, [_int, _i64, ctypes.POINTER(ctypes.c_size_t)]),

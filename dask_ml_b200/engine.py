@@ -268,21 +268,29 @@ class CudaBackend(object):
             t = torch.from_numpy(a)
         t = t.to(device=self.device, dtype=dtype, non_blocking=True)
         if t.dim() == 2 and dtype == torch.bfloat16 and t.shape[0] > 0 and (t.shape[1] % 8 or t.stride(0) % 8 or t.stride(1) != 1):
-            # bf16 rows are read by TMA: 16-byte row pitch = a multiple of 8 elements (zero padded view)
-            n, d = t.shape
-            buf = torch.zeros((n, (d + 7) // 8 * 8), dtype=dtype, device=self.device)
-            buf[:, :d] = t
-            return buf[:, :d]
+            buf = self.rows_buffer(t.shape[0], t.shape[1], dtype)
+            buf.copy_(t)
+            return buf
         if t.dim() == 2 and dtype == torch.bfloat16:
             return t
         if t.dim() == 2 and dtype == torch.float32 and t.shape[1] % 4 and t.shape[1] <= 64 and t.shape[0] > 0:
+            buf = self.rows_buffer(t.shape[0], t.shape[1], dtype)
+            buf.copy_(t)
+            return buf
+        return t.contiguous()
+
+    def rows_buffer(self, n, d, dtype):
+        """An (n, d) device block with the row pitch ``to_device`` gives rows of ``dtype``."""
+        pitch = d
+        if n > 0 and dtype == torch.bfloat16 and d % 8:
+            pitch = (d + 7) // 8 * 8             # bf16 rows are read by TMA: a 16-byte row pitch
+        elif n > 0 and dtype == torch.float32 and d % 4 and d <= 64:
             # The tensor path reads row tiles with TMA, which needs a 16-byte row pitch: rows are stored with the
             # pitch rounded up to 4 floats (zero padded) and handed on as a (n, d) view of that buffer.
-            n, d = t.shape
-            buf = torch.zeros((n, (d + 3) // 4 * 4), dtype=dtype, device=self.device)
-            buf[:, :d] = t
-            return buf[:, :d]
-        return t.contiguous()
+            pitch = (d + 3) // 4 * 4
+        if pitch == d:
+            return torch.empty((n, d), dtype=dtype, device=self.device)
+        return torch.zeros((n, pitch), dtype=dtype, device=self.device)[:, :d]
 
     def empty(self, shape, dtype):
         return torch.empty(shape, dtype=dtype, device=self.device)
@@ -506,6 +514,57 @@ class CudaBackend(object):
             _lib.check(self.lib.bkm_gram_weighted_chunk(
                 self._ptr(x), n, d, x.stride(0) if n else d, _DT_CODE[x.dtype], self._ptr(w), self._ptr(gram),
                 self._ptr(ws), ws.numel(), flags, self._stream()), "bkm_gram_weighted_chunk")
+
+    def colstats_chunk(self, x, shift, acc, minmax, first=False):
+        """The scalers' statistics pass over one chunk, float64 on the device: acc (5, d) (+)= [sum (x - shift) |
+        sum (x - shift)^2 over the finite x | NaN count | +inf count | -inf count] and minmax (2, d) = [min | max] over
+        the non-NaN x, folded.  ``shift`` float64 (d,) or None; ``first`` overwrites."""
+        n, d = x.shape
+        nb = ctypes.c_size_t(0)
+        _lib.check(self.lib.bkm_colstats_workspace_bytes(int(n), int(d), ctypes.byref(nb)),
+                   "bkm_colstats_workspace_bytes")
+        ws = self._scratch("colstats", nb.value)
+        flags = self.flags | (_lib.FLAG_FIRST_CHUNK if first else 0)
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.bkm_colstats_chunk(
+                self._ptr(x), n, d, x.stride(0) if n else d, _DT_CODE[x.dtype], self._ptr(shift), self._ptr(acc),
+                self._ptr(minmax), self._ptr(ws), ws.numel(), flags, self._stream()), "bkm_colstats_chunk")
+
+    def radix_state_new(self, d, T):
+        """Device state of one radix selection of T order statistics in each of d columns (``radix_select_step``)."""
+        nb = ctypes.c_size_t(0)
+        _lib.check(self.lib.bkm_radix_state_bytes(int(d), int(T), ctypes.byref(nb)), "bkm_radix_state_bytes")
+        return torch.zeros(int(nb.value), dtype=torch.uint8, device=self.device)
+
+    def radix_hist_chunk(self, x, state, T, rnd, hist, first=False):
+        """hist (d, T, 256) float64 (+)= the round-``rnd`` digit counts of the chunk's keys under each target's prefix;
+        ``first`` zeroes hist first."""
+        n, d = x.shape
+        flags = self.flags | (_lib.FLAG_FIRST_CHUNK if first else 0)
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.bkm_radix_hist_chunk(
+                self._ptr(x), n, d, x.stride(0) if n else d, _DT_CODE[x.dtype], self._ptr(state), int(T), int(rnd),
+                self._ptr(hist), flags, self._stream()), "bkm_radix_hist_chunk")
+
+    def radix_select_step(self, hist, state, d, T, rnd, dtype, q):
+        """Extend each target's key prefix by the digit that holds its rank (after the round's all-reduce of hist);
+        ``q`` the T / 2 quantiles in [0, 1]."""
+        qh = (ctypes.c_double * len(q))(*[float(v) for v in q])
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.bkm_radix_select_step(self._ptr(hist), self._ptr(state), int(d), int(T), int(rnd),
+                                                      _DT_CODE[dtype], ctypes.cast(qh, ctypes.c_void_p),
+                                                      self._stream()), "bkm_radix_select_step")
+
+    def affine_chunk(self, x, a, b, op1, op2, out):
+        """out = op2(op1(x, a), b) per element (op1: 0 none, 1 subtract a, 2 multiply by a; op2: 0 none, 1 divide by b,
+        2 add b), each step rounded once in out's dtype.  ``a``, ``b`` float64 (d,) or None; ``out`` (n, d) float32 /
+        float64, any row pitch."""
+        n, d = x.shape
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.bkm_affine_chunk(
+                self._ptr(x), n, d, x.stride(0) if n else d, _DT_CODE[x.dtype], self._ptr(a), self._ptr(b), int(op1),
+                int(op2), self._ptr(out), out.stride(0) if n else d, _DT_CODE[out.dtype], self._stream()),
+                "bkm_affine_chunk")
 
     def nystrom_embed(self, x, pack, l, gamma, W, out):
         """out[i] = e_i / ||e_i||, e_i = sum_j exp(-gamma (||x_i - c_j||^2 - min_j ||x_i - c_j||^2)) W[j] — the second

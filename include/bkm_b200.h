@@ -27,6 +27,9 @@
  *   dask_glm's per-iteration X.dot(beta), family loglike /        bkm_glm_pass_chunk + bkm_gram_weighted_chunk
  *     gradient / hessian of LogisticRegression, LinearRegression,
  *     PoissonRegression, linear_model/glm.py:169-362
+ *   X.mean(0) / .var(0) / .min(0) / .max(0), da.percentile and       bkm_colstats_chunk, bkm_radix_hist_chunk +
+ *     the elementwise transforms of StandardScaler, MinMaxScaler,    bkm_radix_select_step, bkm_affine_chunk
+ *     RobustScaler, preprocessing/data.py:24-221
  *
  * Conventions
  *   - extern "C", plain pointers and sizes only; no torch / C++ types.
@@ -243,6 +246,45 @@ int bkm_glm_pass_chunk(const void* X, int64_t n, int d, int64_t ldx, int x_dtype
                        size_t ws_bytes, int flags, void* stream);
 int bkm_gram_weighted_chunk(const void* X, int64_t n, int d, int64_t ldx, int x_dtype, const double* w, double* gram,
                             void* workspace, size_t ws_bytes, int flags, void* stream);
+
+/* ---- StandardScaler / MinMaxScaler / RobustScaler: the fit passes and the transform pass over row chunks (replace
+ * X.mean(0), X.var(0), X.min(0), X.max(0), da.percentile per column and the elementwise (X - m) / s of
+ * dask_ml/preprocessing/data.py) ---------------------------------------------------------------------------------------
+ *   bkm_colstats_chunk   per column j, in float64: acc [5][d] (+)= [sum (x - shift_j) | sum (x - shift_j)^2 over the
+ *                        finite x | number of NaN | of +inf | of -inf]; minmax [2][d] = [min | max] over the non-NaN x
+ *                        (+inf / -inf when there is none), folded with min / max.  shift [d] float64, nullable.
+ *                        OVERWRITTEN with BKM_FLAG_FIRST_CHUNK, else ACCUMULATED.  CTA partials are folded in a fixed
+ *                        order: two calls with the same inputs give the same bits.  One launch.
+ *                        workspace: bkm_colstats_workspace_bytes(n, d) bytes, any content.
+ *   bkm_radix_hist_chunk + bkm_radix_select_step   exact order statistics per column, T (even, <= 6) target ranks per
+ *                        column: for target t the ranks floor(v) + (t & 1) of numpy's 'linear' virtual index
+ *                        v = (m - 1) q[t / 2] over the m non-NaN values (both the last value when v >= m - 1, both
+ *                        the first when v < 0).  Values map to order-preserving unsigned keys of 16 (bf16), 32 (fp32)
+ *                        or 64 (fp64) bits, selected 8 bits per round: 2, 4 or 8 rounds.  Round r:
+ *                          every chunk: bkm_radix_hist_chunk(..., state, T, r, hist) histograms the next digit of the
+ *                            keys that carry each target's prefix (NaN rows skipped); hist [d][T][256] float64 counts,
+ *                            ZEROED with BKM_FLAG_FIRST_CHUNK (set it on the first chunk of every round), else
+ *                            ACCUMULATED.  Counts are integers: the sums are exact whatever the order, and all-reduce.
+ *                          then: bkm_radix_select_step(hist, state, d, T, r, x_dtype, q_host) extends each target's
+ *                            prefix by one digit on the device (round 0 also derives the ranks and sets nvalid).
+ *                        state: bkm_radix_state_bytes(d, T) bytes, any content before round 0; after the last round
+ *                        state [d][T] holds records of 32 bytes {uint64 key, double rank, double nvalid, int32 slot,
+ *                        int32 pad}: `key` is the key of the target's order statistic, `nvalid` the column's non-NaN
+ *                        count.  q_host [T / 2] float64 quantiles in [0, 1] (host memory, read at the call).
+ *   bkm_affine_chunk     out [n][ld_out] = op2(op1(x, a), b) per element, op1: 0 none, 1 x - a_j, 2 x * a_j;
+ *                        op2: 0 none, 1 / b_j, 2 + b_j (a, b [d] float64, values of the output dtype).  out_dtype
+ *                        BKM_F32 (x fp32 or bf16) or BKM_F64; every operation is rounded once in the output dtype
+ *                        (no FMA contraction), which is numpy's two-step expression.  Any ldx >= d, ld_out >= d. */
+int bkm_colstats_workspace_bytes(int64_t n, int d, size_t* out);
+int bkm_colstats_chunk(const void* X, int64_t n, int d, int64_t ldx, int x_dtype, const double* shift, double* acc,
+                       double* minmax, void* workspace, size_t ws_bytes, int flags, void* stream);
+int bkm_radix_state_bytes(int d, int T, size_t* out);
+int bkm_radix_hist_chunk(const void* X, int64_t n, int d, int64_t ldx, int x_dtype, const void* state, int T, int round,
+                         double* hist, int flags, void* stream);
+int bkm_radix_select_step(double* hist, void* state, int d, int T, int round, int x_dtype, const double* q_host,
+                          void* stream);
+int bkm_affine_chunk(const void* X, int64_t n, int d, int64_t ldx, int x_dtype, const double* a, const double* b,
+                     int op1, int op2, void* out, int64_t ld_out, int out_dtype, void* stream);
 
 /* ---- centre update + shift (k_means.py:548-555), run after the cross-GPU allreduce ----
  *   C_new = sums / max(counts,1)[:,None]   (empty cluster -> zero vector, Q1)
