@@ -80,6 +80,12 @@ SIGNATURES = {
     "bkm_radix_select_step": (_int, [_c_void_p, _c_void_p, _int, _int, _int, _int, _c_void_p, _c_void_p]),
     "bkm_affine_chunk": (_int, [_c_void_p, _i64, _int, _i64, _int, _c_void_p, _c_void_p, _int, _int, _c_void_p, _i64,
                                 _int, _c_void_p]),
+    "bkm_quantile_state_bytes": (_int, [_int, _int, _szp]),
+    "bkm_quantile_hist_chunk": (_int, [_c_void_p, _i64, _int, _i64, _int, _c_void_p, _int, _int, _c_void_p, _int,
+                                       _c_void_p]),
+    "bkm_quantile_select_step": (_int, [_c_void_p, _c_void_p, _int, _int, _int, _int, _c_void_p, _c_void_p]),
+    "bkm_quantile_transform_chunk": (_int, [_c_void_p, _i64, _int, _i64, _int, _c_void_p, _c_void_p, _int, _int, _int,
+                                            _dbl, _dbl, _c_void_p, _i64, _c_void_p]),
     "bkm_finalize": (_int, [_c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_void_p, _int, _int, _c_void_p]),
     "bkm_check_finite": (_int, [_c_void_p, _i64, _int, _i64, _int, _c_void_p, _c_void_p]),
     "bkm_p2p_mailbox_bytes": (_int, [_int, _i64, ctypes.POINTER(ctypes.c_size_t)]),

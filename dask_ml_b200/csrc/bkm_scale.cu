@@ -19,33 +19,13 @@
 //   bkm_affine_chunk       out = op2(op1(x, a), b), each operation rounded once in the output's dtype (__fsub_rn,
 //                          __fdiv_rn, __dmul_rn, ...): no FMA contraction, so the result equals numpy's two-step
 //                          expression bit for bit.
-#include "bkm_common.cuh"
-#include <cuda_bf16.h>
+#include "bkm_select.cuh"
 #include <math_constants.h>
 
 namespace bkm {
 namespace {
 
-constexpr int kThreads = 256;
 constexpr int kMaxTargets = 6;
-
-__device__ __forceinline__ double widen(float v) { return (double)v; }
-__device__ __forceinline__ double widen(double v) { return v; }
-__device__ __forceinline__ double widen(__nv_bfloat16 v) { return (double)__bfloat162float(v); }
-
-// column-pass geometry shared by the stats and affine kernels: CB columns per pass (a multiple of 32, at most
-// kThreads), G = kThreads / CB interleaved row groups
-__host__ __device__ __forceinline__ int col_block(int d) { return min(kThreads, (d + 31) / 32 * 32); }
-
-static int sm_count(int* out) {
-  int dev = 0;
-  BKM_CUDA_TRY(cudaGetDevice(&dev));
-  BKM_CUDA_TRY(cudaDeviceGetAttribute(out, cudaDevAttrMultiProcessorCount, dev));
-  return 0;
-}
-
-static bool dtype_ok(int t) { return t == BKM_F32 || t == BKM_F64 || t == BKM_BF16; }
-static size_t elem_size(int t) { return t == BKM_F64 ? 8 : (t == BKM_F32 ? 4 : 2); }
 
 // ============================================ column statistics ============================================
 enum { ST_SUM = 0, ST_SQ, ST_NAN, ST_PINF, ST_NINF, ST_MIN, ST_MAX, ST_N };
@@ -178,31 +158,6 @@ __global__ void __launch_bounds__(kThreads) colstats_kernel(StatsArgs a) {
 }
 
 // ============================================ radix select ============================================
-// Per (column, target) state, 32 bytes; the host reads `prefix` (the full key after the last round) and `nvalid`.
-struct SelState {
-  unsigned long long prefix;
-  double rank;             // the target's rank among the keys that carry `prefix`
-  double nvalid;           // non-NaN values of the column (set by round 0)
-  int slot;                // the first target with the same prefix: whose histogram this target reads
-  int pad;
-};
-
-__device__ __forceinline__ unsigned long long radix_key(float v) {
-  const unsigned u = __float_as_uint(v);
-  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-}
-__device__ __forceinline__ unsigned long long radix_key(double v) {
-  const unsigned long long u = (unsigned long long)__double_as_longlong(v);
-  return (u & 0x8000000000000000ull) ? ~u : (u | 0x8000000000000000ull);
-}
-__device__ __forceinline__ unsigned long long radix_key(__nv_bfloat16 v) {
-  const unsigned u = (unsigned)__bfloat16_as_ushort(v);
-  return (u & 0x8000u) ? (~u & 0xffffu) : (u | 0x8000u);
-}
-__device__ __forceinline__ bool is_nan(float v) { return v != v; }
-__device__ __forceinline__ bool is_nan(double v) { return v != v; }
-__device__ __forceinline__ bool is_nan(__nv_bfloat16 v) { return __hisnan(v); }
-
 struct HistArgs {
   const void* X;
   long long n;

@@ -33,11 +33,12 @@ from ..cluster.k_means import _NONFINITE_MSG
 SHIFT_ROWS = 65536      # rows of rank 0 whose mean is the shift of the Gram pass
 
 
-def _device_data(X):
+def _device_data(X, allow_nonfinite=False):
     """Validated input -> DeviceData (what KMeans accepts: ndarray, DataFrame, torch, ChunkedArray, dask arrays,
     ``host_resident``).  Non-finite values are detected from the Gram pass itself (a NaN or inf row makes G
     non-finite), so the fit reads X twice, not three times; only when G is non-finite is X scanned, to tell NaN / inf
-    from finite values whose squares overflow float64 (``gram_pass``)."""
+    from finite values whose squares overflow float64 (``gram_pass``).  ``allow_nonfinite`` accepts NaN and inf in
+    numpy input too, for estimators that define a result for them."""
     try:
         import pandas as pd
 
@@ -49,7 +50,8 @@ def _device_data(X):
         raise TypeError("Cannot fit on dask.dataframe due to unknown partition lengths.")
     if isinstance(X, DeviceData):
         return X
-    X = check_array(X, accept_dask_dataframe=False, accept_unknown_chunks=False, accept_sparse=False)
+    finite = {"ensure_all_finite": False} if allow_nonfinite else {}
+    X = check_array(X, accept_dask_dataframe=False, accept_unknown_chunks=False, accept_sparse=False, **finite)
     return _km._to_device_data(X, check_finite=False)
 
 

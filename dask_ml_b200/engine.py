@@ -555,6 +555,41 @@ class CudaBackend(object):
                                                       _DT_CODE[dtype], ctypes.cast(qh, ctypes.c_void_p),
                                                       self._stream()), "bkm_radix_select_step")
 
+    def quantile_state_new(self, d, n_q):
+        """Device state of one selection of the 2 ``n_q`` QuantileTransformer order statistics in each of d columns
+        (``quantile_select_step``); column j's record starts at byte j * (16 + 80 n_q)."""
+        nb = ctypes.c_size_t(0)
+        _lib.check(self.lib.bkm_quantile_state_bytes(int(d), int(n_q), ctypes.byref(nb)), "bkm_quantile_state_bytes")
+        return torch.zeros(int(nb.value), dtype=torch.uint8, device=self.device)
+
+    def quantile_hist_chunk(self, x, state, n_q, rnd, hist, first=False):
+        """hist (d, min(2 n_q, 256^rnd), 256) float64 (+)= the round-``rnd`` digit counts of the chunk's keys under each
+        live prefix; ``first`` zeroes hist first."""
+        n, d = x.shape
+        flags = self.flags | (_lib.FLAG_FIRST_CHUNK if first else 0)
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.bkm_quantile_hist_chunk(
+                self._ptr(x), n, d, x.stride(0) if n else d, _DT_CODE[x.dtype], self._ptr(state), int(n_q), int(rnd),
+                self._ptr(hist), flags, self._stream()), "bkm_quantile_hist_chunk")
+
+    def quantile_select_step(self, hist, state, d, n_q, rnd, dtype, qf):
+        """Extend each distinct rank's key prefix by one digit and build the next live list (after the round's
+        all-reduce of hist); ``qf`` float64 (n_q,) ascending quantiles in [0, 1] on the device."""
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.bkm_quantile_select_step(self._ptr(hist), self._ptr(state), int(d), int(n_q), int(rnd),
+                                                         _DT_CODE[dtype], self._ptr(qf), self._stream()),
+                       "bkm_quantile_select_step")
+
+    def quantile_transform_chunk(self, x, qT, ref, inverse, distribution, clip_lo, clip_hi, out):
+        """QuantileTransformer's per-element pass: ``qT`` float64 (d, n_q) quantiles per column, ``ref`` float64
+        (n_q,), ``distribution`` 0 uniform / 1 normal; ``out`` float64 (n, d), any row pitch."""
+        n, d = x.shape
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.bkm_quantile_transform_chunk(
+                self._ptr(x), n, d, x.stride(0) if n else d, _DT_CODE[x.dtype], self._ptr(qT), self._ptr(ref),
+                int(ref.shape[0]), int(bool(inverse)), int(distribution), float(clip_lo), float(clip_hi),
+                self._ptr(out), out.stride(0) if n else d, self._stream()), "bkm_quantile_transform_chunk")
+
     def affine_chunk(self, x, a, b, op1, op2, out):
         """out = op2(op1(x, a), b) per element (op1: 0 none, 1 subtract a, 2 multiply by a; op2: 0 none, 1 divide by b,
         2 add b), each step rounded once in out's dtype.  ``a``, ``b`` float64 (d,) or None; ``out`` (n, d) float32 /

@@ -1,3 +1,3 @@
-from .data import MinMaxScaler, RobustScaler, StandardScaler
+from .data import MinMaxScaler, QuantileTransformer, RobustScaler, StandardScaler
 
-__all__ = ["StandardScaler", "MinMaxScaler", "RobustScaler"]
+__all__ = ["StandardScaler", "MinMaxScaler", "RobustScaler", "QuantileTransformer"]

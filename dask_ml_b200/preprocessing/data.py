@@ -1,6 +1,8 @@
-"""StandardScaler, MinMaxScaler and RobustScaler with the dask_ml.preprocessing API, executed by the H100 engine.
+"""StandardScaler, MinMaxScaler, RobustScaler and QuantileTransformer with the dask_ml.preprocessing API, executed by
+the H100 engine.
 
-Mirrors dask_ml/preprocessing/data.py:24-221 (reference @ 0310a90).  Each class subclasses scikit-learn's, as the
+Mirrors dask_ml/preprocessing/data.py:24-312 (reference @ 0310a90); QuantileTransformer's passes are described in
+DESIGN.md, "The passes of QuantileTransformer".  Each class subclasses scikit-learn's, as the
 reference does, and accepts what PCA accepts.  The passes (DESIGN.md, "The passes of the scalers"):
 
     fit, Standard / MinMax (bkm_colstats_chunk, one read of X, float64), with a shift s shared by every rank:
@@ -279,3 +281,134 @@ class RobustScaler(_DeviceFitTransform, skdata.RobustScaler):
         check_is_fitted(self, ["center_", "scale_"])
         return affine(X, self.scale_ if self.with_scaling else None, self.center_ if self.with_centering else None,
                       OP1_MUL, OP2_ADD)
+
+
+# ------------------------------------------------ QuantileTransformer ------------------------------------------------
+# one selection's per-column record (include/bkm_b200.h): header, then 2 n_q SELECT_RECORDs, then 2 n_q live prefixes
+QUANTILE_HEAD = np.dtype([("nvalid", "<f8"), ("R", "<i4"), ("L", "<i4")])
+HIST_BUDGET = 512 << 20          # bytes of one round's [columns][live slots][256] float64 histogram: larger d * n_q
+                                 # runs in column groups, each of which reads X once per round
+DISTRIBUTIONS = {"uniform": 0, "normal": 1}
+
+
+def _order_stat_ranks(nvalid, qf):
+    """The floor / floor + 1 ranks of numpy's 'linear' virtual index (nvalid - 1) qf, as the selection derives them on
+    the device: (lo, hi), each (d, len(qf)) float64."""
+    nv = np.asarray(nvalid, dtype=np.float64)[:, None]
+    vi = (nv - 1.0) * qf[None, :]
+    lo, hi = np.floor(vi), np.floor(vi) + 1.0
+    top, neg = vi >= nv - 1.0, vi < 0.0
+    lo, hi = np.where(top, nv - 1.0, lo), np.where(top, nv - 1.0, hi)
+    lo, hi = np.where(neg, 0.0, lo), np.where(neg, 0.0, hi)
+    empty = np.broadcast_to(nv <= 0.0, vi.shape)
+    return np.where(empty, 0.0, lo), np.where(empty, 0.0, hi)
+
+
+def quantiles_exact(X, references):
+    """np.percentile(column, references * 100) of every whole column over every row of every rank, exact for any
+    chunking or rank split: (len(references), d) float64, NaN for a column that holds a NaN."""
+    be, comm, d = X.backend, X.comm, X.d
+    nq = len(references)
+    q = np.asarray(references, dtype=np.float64) * 100
+    qf = np.true_divide(q, 100.0)
+    qf_dev = torch.as_tensor(np.ascontiguousarray(qf)).to(be.device)
+    rounds = RADIX_ROUNDS[X.dtype]
+    stride = 16 + 80 * nq
+    state = be.quantile_state_new(d, nq)
+    widest = min(2 * nq, 256 ** (rounds - 1))
+    group = max(1, min(d, HIST_BUDGET // (widest * 256 * 8)))
+    hist = be.empty((group * widest * 256,), torch.float64)
+    for j0 in range(0, d, group):
+        j1 = min(d, j0 + group)
+        st = state[j0 * stride: j1 * stride]
+        for rnd in range(rounds):
+            h = hist[: (j1 - j0) * min(2 * nq, 256 ** rnd) * 256]
+            for i, x in enumerate(X.chunks):
+                be.quantile_hist_chunk(x[:, j0:j1], st, nq, rnd, h, first=i == 0)
+            comm.allreduce_sum_(h)
+            be.quantile_select_step(h, st, j1 - j0, nq, rnd, X.dtype, qf_dev)
+    raw = state.cpu().numpy().reshape(d, stride)
+    head = np.ascontiguousarray(raw[:, :16]).view(QUANTILE_HEAD)[:, 0]
+    rec = np.ascontiguousarray(raw[:, 16: 16 + 64 * nq]).view(SELECT_RECORD)
+    n = X.n_global
+    if n == 0:
+        return np.full((nq, d), np.nan)
+    lo, hi = _order_stat_ranks(head["nvalid"], qf)
+    keys = np.empty((2, d, nq), dtype=np.uint64)
+    for j in range(d):
+        distinct = np.unique(np.concatenate([lo[j], hi[j]]))
+        assert len(distinct) == head["R"][j], (j, len(distinct), head["R"][j])
+        keys[0, j] = rec["key"][j, np.searchsorted(distinct, lo[j])]
+        keys[1, j] = rec["key"][j, np.searchsorted(distinct, hi[j])]
+    vals = keys_to_values(keys, X.dtype)
+    P = percentile_from_order_stats(vals[0], vals[1], n, q, X.np_dtype)
+    P[head["nvalid"] < n] = np.nan                      # a NaN in the column: numpy gives NaN
+    return np.ascontiguousarray(np.asarray(P, dtype=np.float64).T)
+
+
+def quantile_transform(X, quantiles, references, inverse, distribution):
+    """The reference's _transform_col on every column (forward, or inverse) -> device-resident float64 ChunkedArray,
+    rows with the pitch ``CudaBackend.to_device`` gives."""
+    from scipy import stats
+
+    be = X.backend
+    qT = torch.as_tensor(np.ascontiguousarray(np.asarray(quantiles, dtype=np.float64).T)).to(be.device)
+    ref = torch.as_tensor(np.ascontiguousarray(references, dtype=np.float64)).to(be.device)
+    dist = stats.norm if distribution == "normal" else stats.uniform
+    eps = skdata.BOUNDS_THRESHOLD - np.spacing(1)
+    lo, hi = (0.0, 0.0) if inverse else (float(dist.ppf(eps)), float(dist.ppf(1 - eps)))
+    blocks = []
+    for x in X.chunks:
+        o = be.rows_buffer(int(x.shape[0]), X.d, torch.float64)
+        be.quantile_transform_chunk(x, qT, ref, inverse, DISTRIBUTIONS[distribution], lo, hi, o)
+        blocks.append(o)
+    return ChunkedArray(blocks)
+
+
+class _Rows(object):
+    """Device rows as scikit-learn's fit sees them: an object with a shape."""
+
+    def __init__(self, data):
+        self.data = data
+        self.shape = (data.n_global, data.d)
+
+
+class QuantileTransformer(skdata.QuantileTransformer):
+    """Transforms features using quantile information.
+
+    The quantiles are exact: ``quantiles_[:, j]`` equals ``np.percentile(X[:, j], references_ * 100)`` over every row
+    (``subsample`` is ignored, as in dask_ml).  Outputs are device-resident float64 ChunkedArrays.  The scikit-learn
+    docstring follows.
+    """
+
+    __doc__ = __doc__ + "\n".join(skdata.QuantileTransformer.__doc__.split("\n")[1:])
+
+    def _check_inputs(self, X, in_fit, accept_sparse_negative=False, copy=False):
+        """X -> device rows; scikit-learn's checks run on a 5-row sample of X's dtype, as in dask_ml."""
+        from scipy import sparse
+
+        if sparse.issparse(X):
+            raise NotImplementedError("QuantileTransformer does not accept sparse input")
+        X = _device_data(X, allow_nonfinite=True)           # NaN and inf have defined results (as in dask_ml)
+        sample = np.random.RandomState(0).uniform(size=(5, X.d)).astype(X.np_dtype)
+        super(QuantileTransformer, self)._check_inputs(sample, in_fit, accept_sparse_negative=accept_sparse_negative)
+        return _Rows(X)
+
+    def fit_transform(self, X, y=None, **fit_params):
+        """fit, then transform, with X uploaded once: a device-resident float64 ChunkedArray."""
+        X = _device_data(X, allow_nonfinite=True)
+        return self.fit(X, y).transform(X)
+
+    def _sparse_fit(self, X, random_state):
+        raise NotImplementedError
+
+    def _dense_fit(self, X, random_state):
+        self.quantiles_ = quantiles_exact(X.data, self.references_)
+
+    def _transform(self, X, inverse=False):
+        return quantile_transform(X.data, self.quantiles_, self.references_, inverse, self.output_distribution)
+
+    def inverse_transform(self, X):
+        """Back-projection to the original space: a device-resident float64 ChunkedArray."""
+        check_is_fitted(self)
+        return self._transform(self._check_inputs(X, in_fit=False), inverse=True)

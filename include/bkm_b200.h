@@ -30,6 +30,9 @@
  *   X.mean(0) / .var(0) / .min(0) / .max(0), da.percentile and       bkm_colstats_chunk, bkm_radix_hist_chunk +
  *     the elementwise transforms of StandardScaler, MinMaxScaler,    bkm_radix_select_step, bkm_affine_chunk
  *     RobustScaler, preprocessing/data.py:24-221
+ *   da.percentile at every reference and the per-column np.interp,   bkm_quantile_hist_chunk +
+ *     ppf and cdf of QuantileTransformer, preprocessing/data.py:       bkm_quantile_select_step,
+ *     224-312                                                          bkm_quantile_transform_chunk
  *
  * Conventions
  *   - extern "C", plain pointers and sizes only; no torch / C++ types.
@@ -285,6 +288,46 @@ int bkm_radix_select_step(double* hist, void* state, int d, int T, int round, in
                           void* stream);
 int bkm_affine_chunk(const void* X, int64_t n, int d, int64_t ldx, int x_dtype, const double* a, const double* b,
                      int op1, int op2, void* out, int64_t ld_out, int out_dtype, void* stream);
+
+/* ---- QuantileTransformer: the fit selection and the transform pass over row chunks (replace da.percentile per
+ * column at every reference and the per-column np.interp / ppf / cdf of dask_ml/preprocessing/data.py:224-312) ------
+ *   bkm_quantile_hist_chunk + bkm_quantile_select_step   exact order statistics per column at T = 2 n_q target ranks:
+ *                        for quantile i the ranks floor(v) and floor(v) + 1 of numpy's 'linear' virtual index
+ *                        v = (m - 1) qf[i] over the m non-NaN values (both m - 1 when v >= m - 1), with the keys and
+ *                        rounds of bkm_radix_hist_chunk.  The selection works on the column's sorted distinct ranks;
+ *                        their prefixes after round r form a sorted, duplicate-free live list of
+ *                        L <= cap(r) = min(T, 256^r) entries.  Round r:
+ *                          every chunk: bkm_quantile_hist_chunk(..., state, n_q, r, hist) counts the next digit of the
+ *                            keys whose prefix is live (NaN rows skipped); hist [d][cap(r)][256] float64 counts,
+ *                            ZEROED with BKM_FLAG_FIRST_CHUNK (set it on the first chunk of every round), else
+ *                            ACCUMULATED.  Counts are integers: the sums are exact whatever the order, and all-reduce.
+ *                          then: bkm_quantile_select_step(hist, state, d, n_q, r, x_dtype, qf) extends each distinct
+ *                            rank's prefix by one digit and builds the next live list, one CTA per column; round 0
+ *                            also derives the ranks.  It overwrites hist.
+ *                        qf [n_q] float64 ascending quantiles in [0, 1] (device memory).
+ *                        state: bkm_quantile_state_bytes(d, n_q) bytes, any content before round 0.  Column j's record
+ *                        starts at byte j * (16 + 80 n_q): {double nvalid, int32 R, int32 L}, then T records of 32 bytes
+ *                        {uint64 key, double rank, double nvalid, int32 slot, int32 pad} whose first R hold the distinct
+ *                        ranks in ascending order (after the last round `key` is the key of that order statistic), then
+ *                        T uint64 live prefixes.  The caller may run column groups as views: X + j0, state + j0 stride.
+ *   bkm_quantile_transform_chunk   out [n][ld_out] float64 per element, with the quantiles q = quantiles[j][0, n_q)
+ *                        (float64, ascending, one row per column) and the references r [n_q] of column j:
+ *                          forward (inverse 0): y = 0.5 (interp(x, q, r) - interp(-x, -q[::-1], -r[::-1])); y = 1 where
+ *                            x + 1e-7 > q[n_q - 1], then y = 0 where x - 1e-7 < q[0] (that test in X's dtype: float32 for
+ *                            fp32 and bf16 rows); out = clip(ppf(y), clip_lo, clip_hi);
+ *                          inverse (inverse 1): c = cdf(x); out = interp(c, r, q), then q[n_q - 1] where c + 1e-7 > 1,
+ *                            then q[0] where c - 1e-7 < 0;
+ *                        interp is numpy's, every operation rounded once in float64; distribution 0 uniform (ppf the
+ *                        identity on [0, 1], cdf a clip to [0, 1]), 1 normal (normcdfinv / normcdf).  NaN x gives NaN
+ *                        (n_q > 1).  Any ldx >= d, ld_out >= d; the input is only read. */
+int bkm_quantile_state_bytes(int d, int n_q, size_t* out);
+int bkm_quantile_hist_chunk(const void* X, int64_t n, int d, int64_t ldx, int x_dtype, const void* state, int n_q,
+                            int round, double* hist, int flags, void* stream);
+int bkm_quantile_select_step(double* hist, void* state, int d, int n_q, int round, int x_dtype, const double* qf,
+                             void* stream);
+int bkm_quantile_transform_chunk(const void* X, int64_t n, int d, int64_t ldx, int x_dtype, const double* quantiles,
+                                 const double* references, int n_q, int inverse, int distribution, double clip_lo,
+                                 double clip_hi, double* out, int64_t ld_out, void* stream);
 
 /* ---- centre update + shift (k_means.py:548-555), run after the cross-GPU allreduce ----
  *   C_new = sums / max(counts,1)[:,None]   (empty cluster -> zero vector, Q1)
