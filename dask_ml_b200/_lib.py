@@ -41,6 +41,8 @@ SIGNATURES = {
     "bkm_min_fold_chunk": (_int, [_c_void_p, _c_void_p, _i64, _int, _c_void_p, _c_void_p]),
     "bkm_make_blobs_chunk": (_int, [_c_void_p, _c_void_p, _i64, _int, _i64, _int, _c_void_p, _c_void_p, _int, _u64,
                                     _c_void_p]),
+    "bkm_make_glm_chunk": (_int, [_c_void_p, _c_void_p, _i64, _int, _i64, _int, _i64, _int, _c_void_p, _int, _int,
+                                  _dbl, _dbl, _u64, _c_void_p, _c_void_p]),
     "bkm_loop_state_bytes": (_int, [_szp]),
     "bkm_loop_reset": (_int, [_c_void_p, _dbl, _c_void_p, _int, _c_void_p]),
     "bkm_finalize_step": (_int, [_c_void_p, _c_void_p, _c_void_p, _c_void_p, _int, _int, _int, _c_void_p,

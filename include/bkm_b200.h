@@ -33,6 +33,10 @@
  *   da.percentile at every reference and the per-column np.interp,   bkm_quantile_hist_chunk +
  *     ppf and cdf of QuantileTransformer, preprocessing/data.py:       bkm_quantile_select_step,
  *     224-312                                                          bkm_quantile_transform_chunk
+ *   rng.normal X, X[:, idx].dot(beta[idx]) or da.dot(X, coef), then    bkm_make_glm_chunk
+ *     rng.random < sigmoid(z), + noise, rng.poisson(exp(z)) of
+ *     make_classification / make_regression / make_counts,
+ *     datasets.py:24-73, 205-378
  *
  * Conventions
  *   - extern "C", plain pointers and sizes only; no torch / C++ types.
@@ -374,6 +378,37 @@ int bkm_minibatch_step(const double* reduced, const double* centers_in, const do
  * X [n][ldx] x-dtype out, y [n] int64 out (nullable); centers [k][d] and cluster_std [k] float64 on the device. */
 int bkm_make_blobs_chunk(void* X, int64_t* y, int64_t n, int d, int64_t ldx, int x_dtype, const double* centers,
                          const double* cluster_std, int k, uint64_t seed, void* stream);
+
+/* ---- datasets.make_classification / make_regression / make_counts, one block on the device ----------------------
+ * (dask_ml/datasets.py:24-73, 205-378).  The reference's dask streams cannot be reproduced, so the package defines its
+ * own, and dask_ml_b200.datasets restates it in numpy for device=None (the two give the same X to rounding of the
+ * math library and the same y except where it sits within ~1e-12 of a decision):
+ *   host parameter draws, numpy RandomState rng (sklearn.utils.check_random_state(random_state)), in this order:
+ *     make_regression:              coef from sklearn.datasets.make_regression(n_samples=<first block>, ..., rng),
+ *                                   then key;
+ *     make_classification / counts: key, then idx = rng.choice(n_features, n_informative) (with replacement),
+ *                                   then beta = (rng.random_sample(n_features) - 1) * scale;
+ *     key = the first 8 bytes (little-endian uint64) of rng.bytes(624 * 4).
+ *   per-element draws: w = Philox4x32-10(key, counter = (row lo, row hi, j, tag)), row = the GLOBAL row index:
+ *     tag 0  X[row, 2p], X[row, 2p+1] (j = p): u1 = (w0 + 1) / 2^32, u2 = w1 / 2^32, r = sqrt(-2 log u1),
+ *            r * cospi(2 u2), r * sinpi(2 u2)   (the Box-Muller of bkm_make_blobs_chunk)
+ *     tag 1  response uniforms (j = attempt): U = ((w0 >> 5) 2^26 + (w1 >> 6)) / 2^53, V = the same of (w2, w3)
+ *     tag 2  noise normal of target t (j = t): the cosine normal of (w0, w1)
+ *   z[t] = sum over the list, in list order, of x_f * c[f, t], x_f the value AS STORED in X's dtype, in float64 with
+ *          correctly rounded steps (no FMA), starting from 0.0
+ *   family 0 logistic:  y = U < 1 / (1 + exp(-z))                                   int64 [n]
+ *   family 1 normal:    y[t] = (z[t] + bias) (+ noise * N_t if noise > 0)             float64 [n][n_targets]
+ *   family 2 poisson:   y ~ numpy's legacy Poisson of lam = exp(z) (multiplication method for lam < 10, PTRS with
+ *                       numpy's loggam for lam >= 10), each loop turn / attempt taking counter j = 0, 1, ...; a rate
+ *                       that numpy rejects (NaN or above its lam maximum 9.223372006484771e18) ORs 1 into *flag and
+ *                       writes y = 0                                                    int64 [n]
+ * X [n][ldx] x-dtype out (BKM_F32 / BKM_F64); y out as above; row0 = the global index of the block's first row;
+ * info [m][1 + n_targets] float64: the feature index, then its coefficient for every target (n_targets = 1 for
+ * families 0 and 2); flag int32 (needed for family 2).  One launch: every X element is written once, and the
+ * informative normals of a row are recomputed from their counters for z, so X is never read back. */
+int bkm_make_glm_chunk(void* X, void* y, int64_t n, int d, int64_t ldx, int x_dtype, int64_t row0, int family,
+                       const double* info, int m, int n_targets, double bias, double noise, uint64_t key, int* flag,
+                       void* stream);
 
 /* ---- NaN/inf scan of a chunk (k_means.py:179-180): sets *flag (int32) nonzero -------- */
 int bkm_check_finite(const void* X, int64_t n, int d, int64_t ldx, int x_dtype,
