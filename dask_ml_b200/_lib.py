@@ -14,6 +14,15 @@ BKM_F32 = 0
 BKM_F64 = 1
 BKM_BF16 = 2
 
+# further operand types of bkm_metric_chunk
+BKM_M_F16 = 3
+BKM_M_I32 = 4
+BKM_M_I64 = 5
+BKM_M_U8 = 6
+METRIC_EQ = 0
+METRIC_ERR = 1
+METRIC_LOGLOSS = 2
+
 FLAG_FORCE_SIMT = 1
 FLAG_FORCE_TC = 2
 FLAG_NO_RECHECK = 4
@@ -88,6 +97,11 @@ SIGNATURES = {
     "bkm_quantile_select_step": (_int, [_c_void_p, _c_void_p, _int, _int, _int, _int, _c_void_p, _c_void_p]),
     "bkm_quantile_transform_chunk": (_int, [_c_void_p, _i64, _int, _i64, _int, _c_void_p, _c_void_p, _int, _int, _int,
                                             _dbl, _dbl, _c_void_p, _i64, _c_void_p]),
+    "bkm_split_indices_chunk": (_int, [_u64, _i64, _i64, _i64, _i64, _c_void_p, _c_void_p]),
+    "bkm_gather_rows_chunk": (_int, [_c_void_p, _i64, _i64, _i64, _c_void_p, _i64, _i64, _c_void_p, _i64, _c_void_p]),
+    "bkm_metric_workspace_bytes": (_int, [_i64, _int, _int, _szp]),
+    "bkm_metric_chunk": (_int, [_c_void_p, _int, _c_void_p, _int, _c_void_p, _i64, _int, _int, _c_void_p, _dbl,
+                                _c_void_p, _c_void_p, ctypes.c_size_t, _int, _c_void_p]),
     "bkm_finalize": (_int, [_c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_void_p, _int, _int, _c_void_p]),
     "bkm_check_finite": (_int, [_c_void_p, _i64, _int, _i64, _int, _c_void_p, _c_void_p]),
     "bkm_p2p_mailbox_bytes": (_int, [_int, _i64, ctypes.POINTER(ctypes.c_size_t)]),

@@ -22,6 +22,8 @@ from .chunked import ChunkedArray, block_dtype, _is_torch
 
 _NP_TO_TORCH = {np.dtype("float32"): torch.float32, np.dtype("float64"): torch.float64}
 _DT_CODE = {torch.float32: _lib.BKM_F32, torch.float64: _lib.BKM_F64, torch.bfloat16: _lib.BKM_BF16}
+_METRIC_CODE = {**_DT_CODE, torch.float16: _lib.BKM_M_F16, torch.int32: _lib.BKM_M_I32, torch.int64: _lib.BKM_M_I64,
+                torch.bool: _lib.BKM_M_U8, torch.uint8: _lib.BKM_M_U8}
 
 
 def out_dtype(x_dtype):
@@ -600,6 +602,58 @@ class CudaBackend(object):
                 self._ptr(x), n, d, x.stride(0) if n else d, _DT_CODE[x.dtype], self._ptr(a), self._ptr(b), int(op1),
                 int(op2), self._ptr(out), out.stride(0) if n else d, _DT_CODE[out.dtype], self._stream()),
                 "bkm_affine_chunk")
+
+    def split_indices_chunk(self, seed, c, start, count, offset):
+        """int64 (count,) on the device: ``offset + pi_seed(start + i)``, the split permutation of a block of ``c`` rows
+        (include/bkm_b200.h) at positions [start, start + count)."""
+        out = torch.empty(int(count), dtype=torch.int64, device=self.device)
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.bkm_split_indices_chunk(int(seed), int(c), int(start), int(count), int(offset),
+                                                        self._ptr(out), self._stream()), "bkm_split_indices_chunk")
+        return out
+
+    def gather_rows_chunk(self, src, idx, idx_offset=0):
+        """``src[idx - idx_offset]`` for a 1-D or 2-D device block of any dtype (rows are copied as bytes; a row pitch
+        is honoured, other strides are made contiguous first).  ``idx`` int64 on the device, every value of
+        ``idx - idx_offset`` in [0, len(src)): the caller's duty, the kernel does not check."""
+        if src.dim() == 2 and src.shape[0] > 1 and (src.stride(1) != 1 or src.stride(0) < src.shape[1]):
+            src = src.contiguous()
+        elif src.dim() == 1 and src.shape[0] > 1 and src.stride(0) != 1:
+            src = src.contiguous()
+        idx = idx.contiguous()
+        n, count = int(src.shape[0]), int(idx.shape[0])
+        out = torch.empty((count,) + tuple(src.shape[1:]), dtype=src.dtype, device=self.device)
+        esz = src.element_size()
+        row_bytes = esz * (int(src.shape[1]) if src.dim() == 2 else 1)
+        if count == 0 or row_bytes == 0:
+            return out
+        if n == 0:
+            raise IndexError("cannot gather rows of an empty block")
+        ld_src = src.stride(0) * esz if (src.dim() == 2 and n > 1) else row_bytes
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.bkm_gather_rows_chunk(self._ptr(src), n, row_bytes, ld_src, self._ptr(idx),
+                                                      int(idx_offset), count, self._ptr(out), row_bytes,
+                                                      self._stream()), "bkm_gather_rows_chunk")
+        return out
+
+    def metric_chunk(self, a, b, mode, acc, w=None, shift=None, eps=0.0, first=False):
+        """One chunk of a scoring reduction (bkm_metric_chunk), float64 on the device.  ``a``, ``b`` contiguous (n,) or
+        (n, m) device blocks of any of the types below; ``w`` float64 (n,) or None; ``acc`` float64: METRIC_EQ (2,)
+        [sum w [rows equal] | sum w], METRIC_ERR (4, m) [sum (b - a)^2 | sum |b - a| | sum (a - shift) | sum (a - shift)^2]
+        with ``shift`` float64 (m,), METRIC_LOGLOSS (2,) [sum -w log q[a] | sum w] with ``a`` int32 class indices and
+        ``b`` (n,) or (n, K) probabilities clipped to [eps, 1 - eps] and renormalised.  ``first`` overwrites acc."""
+        n = int(b.shape[0])
+        m = int(b.shape[1]) if b.dim() == 2 else 1
+        nb = ctypes.c_size_t(0)
+        _lib.check(self.lib.bkm_metric_workspace_bytes(n, m, int(mode), ctypes.byref(nb)),
+                   "bkm_metric_workspace_bytes")
+        ws = self._scratch("metric", nb.value)
+        flags = _lib.FLAG_FIRST_CHUNK if first else 0
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.bkm_metric_chunk(
+                self._ptr(a), _METRIC_CODE[a.dtype], self._ptr(b), _METRIC_CODE[b.dtype], self._ptr(w), n, m, int(mode),
+                self._ptr(shift), float(eps), self._ptr(acc), self._ptr(ws), ws.numel(), flags, self._stream()),
+                "bkm_metric_chunk")
 
     def nystrom_embed(self, x, pack, l, gamma, W, out):
         """out[i] = e_i / ||e_i||, e_i = sum_j exp(-gamma (||x_i - c_j||^2 - min_j ||x_i - c_j||^2)) W[j] — the second

@@ -37,6 +37,12 @@
  *     rng.random < sigmoid(z), + noise, rng.poisson(exp(z)) of
  *     make_classification / make_regression / make_counts,
  *     datasets.py:24-73, 205-378
+ *   check_random_state(seed).permutation(n) and x[idx] per block of    bkm_split_indices_chunk +
+ *     ShuffleSplit / train_test_split, model_selection/_split.py:        bkm_gather_rows_chunk
+ *     68-89, 321-360
+ *   the elementwise graphs and reductions of accuracy_score,           bkm_metric_chunk
+ *     log_loss, mean_squared_error, mean_absolute_error, r2_score,
+ *     metrics/classification.py:11-150, metrics/regression.py:8-92
  *
  * Conventions
  *   - extern "C", plain pointers and sizes only; no torch / C++ types.
@@ -60,6 +66,9 @@ extern "C" {
 #endif
 
 #define BKM_VERSION 200
+/* Entry points added since BKM_VERSION 200 without changing an existing one raise the minor number:
+ * 1 = bkm_split_indices_chunk, bkm_gather_rows_chunk, bkm_metric_workspace_bytes, bkm_metric_chunk */
+#define BKM_VERSION_MINOR 1
 
 /* element types of X */
 #define BKM_F32 0
@@ -409,6 +418,74 @@ int bkm_make_blobs_chunk(void* X, int64_t* y, int64_t n, int d, int64_t ldx, int
 int bkm_make_glm_chunk(void* X, void* y, int64_t n, int d, int64_t ldx, int x_dtype, int64_t row0, int family,
                        const double* info, int m, int n_targets, double bias, double noise, uint64_t key, int* flag,
                        void* stream);
+
+/* ---- train_test_split / ShuffleSplit: the passes over one row block (replace, per block,
+ * check_random_state(seed).permutation(n) and x[idx] of dask_ml/model_selection/_split.py:68-89, 321-360) -----------
+ * The split permutation.  numpy's Mersenne-Twister Fisher-Yates is serial, so the package defines its own permutation
+ * of a block of c rows (1 <= c <= 2^31), a keyed bijection pi_seed : [0, c) -> [0, c) that is evaluated per position;
+ * dask_ml_b200.model_selection restates it in numpy (permutation_indices), bit for bit:
+ *   domain    w = max(1, ceil(ceil(log2 c) / 2)); the network permutes the 2w-bit values [0, 4^w), 4^w < 4c
+ *   keys      for round r = 0 .. BKM_SPLIT_ROUNDS - 1 (64-bit wrapping arithmetic, the splitmix64 finaliser):
+ *               z = seed + (r + 1) * BKM_SPLIT_KEY_STEP;  z = (z ^ (z >> 30)) * BKM_SPLIT_KEY_MUL1;
+ *               z = (z ^ (z >> 27)) * BKM_SPLIT_KEY_MUL2;  z = z ^ (z >> 31);  k0_r = low 32 bits, k1_r = high 32 bits
+ *   network   v = (L << w) | R;  every round, in order:  x = R ^ k0_r (32 bits);  p = x * BKM_SPLIT_ROUND_MUL (64 bits);
+ *               f = (p >> 32) ^ (low 32 bits of p) ^ k1_r;  f = (f ^ (f >> 16)) * BKM_SPLIT_ROUND_MIX (32 bits);
+ *               f = f ^ (f >> 15);  (L, R) <- (R, L ^ (f >> (32 - w)))
+ *             a balanced Feistel network with Philox's multiply-hi/lo round function and a multiply-xorshift
+ *             finaliser (the top w bits of the product alone are close to affine in R): a bijection of [0, 4^w)
+ *   walk      pi_seed(i): v = i; do v = network(v) while v >= c.  The cycle of the network through a value below c
+ *             returns to a value below c, so the walk ends; fewer than 4 applications are expected.
+ * BKM_SPLIT_ROUNDS: a network on 2 or 4 bits has few round functions to choose from and mixes slowly whatever the
+ * hash; 12 is the count at which the position-uniformity and pair-independence tests of
+ * tests/test_model_selection_host.py pass (6 rounds fail them), and at which 10^6 seeds show no bias above 1e-3
+ * relative for c = 3, 5, 8.
+ *   bkm_split_indices_chunk  idx_out[i] = offset + pi_seed(start + i) for i < count (start + count <= c).  One launch.
+ *   bkm_gather_rows_chunk    out row i = src row (idx[i] - idx_offset) for i < count.  Typeless: a row is row_bytes
+ *                            bytes, pitches are in bytes, so rows of any dtype and 1-D arrays (row_bytes = the element
+ *                            size) go through it.  Copies in units of 16 bytes when both base addresses, both pitches
+ *                            and row_bytes allow, else 8, 4, 2 or 1.  An index outside [0, n_src) is a caller error
+ *                            that is NOT detected (a build with -DBKM_DEBUG asserts on it).  One launch. */
+#define BKM_SPLIT_ROUNDS    12
+#define BKM_SPLIT_KEY_STEP  0x9E3779B97F4A7C15ull
+#define BKM_SPLIT_KEY_MUL1  0xBF58476D1CE4E5B9ull
+#define BKM_SPLIT_KEY_MUL2  0x94D049BB133111EBull
+#define BKM_SPLIT_ROUND_MUL 0xD2511F53u
+#define BKM_SPLIT_ROUND_MIX 0x7FEB352Du
+int bkm_split_indices_chunk(uint64_t seed, int64_t c, int64_t start, int64_t count, int64_t offset, int64_t* idx_out,
+                            void* stream);
+int bkm_gather_rows_chunk(const void* src, int64_t n_src, int64_t row_bytes, int64_t ld_src_bytes, const int64_t* idx,
+                          int64_t idx_offset, int64_t count, void* out, int64_t ld_out_bytes, void* stream);
+
+/* ---- accuracy_score / log_loss / mean_squared_error / mean_absolute_error / r2_score: one reduction pass over a
+ * pair of row chunks (replace the elementwise graphs and reductions of dask_ml/metrics/classification.py:11-150 and
+ * regression.py:8-92) ------------------------------------------------------------------------------------------------
+ *   bkm_metric_chunk   a, b: (n, m) contiguous row-major operands (m = 1 for 1-D), each of its own element type
+ *                      (BKM_F32, BKM_F64, BKM_BF16 or one of the BKM_M_* codes below); w [n] float64 row weights,
+ *                      nullable (all 1).  One read of both, float64 arithmetic.
+ *                      BKM_METRIC_EQ       acc [2] (+)= [sum_i w_i [a_ij == b_ij for all j] | sum_i w_i]; two integer
+ *                                          operands are compared as int64, any other pair as float64
+ *                      BKM_METRIC_ERR      acc [4][m] (+)= per column j [sum (b - a)^2 | sum |b - a| | sum (a - shift_j)
+ *                                          | sum (a - shift_j)^2]; shift [m] float64 (device, nullable: 0); w unused
+ *                      BKM_METRIC_LOGLOSS  a [n] int32 class index; b (n, m) probabilities, or m = 1: the probability
+ *                                          of class 1 (then the row is [1 - b, b]).  q = clip(p, eps, 1 - eps),
+ *                                          acc [2] (+)= [sum_i -w_i log(q_i[a_i] / sum_j q_ij) | sum_i w_i]; a class
+ *                                          index outside the row makes the first sum NaN
+ *                      OVERWRITTEN with BKM_FLAG_FIRST_CHUNK, else ACCUMULATED.  Threads add their rows in row order,
+ *                      the row groups of a CTA and then the CTA partials are folded in a fixed order (no float
+ *                      atomics): two calls with the same inputs give the same bits.  NaN operands propagate as in the
+ *                      same float64 expression in numpy.  One launch.
+ *                      workspace: bkm_metric_workspace_bytes(n, m, mode) bytes, any content. */
+#define BKM_M_F16 3
+#define BKM_M_I32 4
+#define BKM_M_I64 5
+#define BKM_M_U8  6   /* bool and uint8 */
+#define BKM_METRIC_EQ      0
+#define BKM_METRIC_ERR     1
+#define BKM_METRIC_LOGLOSS 2
+int bkm_metric_workspace_bytes(int64_t n, int m, int mode, size_t* out);
+int bkm_metric_chunk(const void* a, int a_dtype, const void* b, int b_dtype, const double* w, int64_t n, int m,
+                     int mode, const double* shift, double eps, double* acc, void* workspace, size_t ws_bytes,
+                     int flags, void* stream);
 
 /* ---- NaN/inf scan of a chunk (k_means.py:179-180): sets *flag (int32) nonzero -------- */
 int bkm_check_finite(const void* X, int64_t n, int d, int64_t ldx, int x_dtype,
