@@ -97,6 +97,20 @@ SIGNATURES = {
     "bkm_quantile_select_step": (_int, [_c_void_p, _c_void_p, _int, _int, _int, _int, _c_void_p, _c_void_p]),
     "bkm_quantile_transform_chunk": (_int, [_c_void_p, _i64, _int, _i64, _int, _c_void_p, _c_void_p, _int, _int, _int,
                                             _dbl, _dbl, _c_void_p, _i64, _c_void_p]),
+    "bkm_impute_stats_workspace_bytes": (_int, [_i64, _int, _szp]),
+    "bkm_impute_stats_chunk": (_int, [_c_void_p, _i64, _int, _i64, _int, _int, _dbl, _c_void_p, _c_void_p, _c_void_p,
+                                      ctypes.c_size_t, _int, _c_void_p]),
+    "bkm_quantile_hist_masked_chunk": (_int, [_c_void_p, _i64, _int, _i64, _int, _dbl, _c_void_p, _int, _int,
+                                              _c_void_p, _int, _c_void_p]),
+    "bkm_mode_count_chunk": (_int, [_c_void_p, _i64, _int, _i64, _int, _int, _dbl, _c_void_p, _c_void_p, _c_void_p,
+                                    _i64, _int, _c_void_p]),
+    "bkm_mode_best_workspace_bytes": (_int, [_int, _i64, _szp]),
+    "bkm_mode_best": (_int, [_c_void_p, _c_void_p, _c_void_p, _int, _i64, _c_void_p, _c_void_p, _c_void_p, _c_void_p,
+                             ctypes.c_size_t, _c_void_p]),
+    "bkm_mode_compact": (_int, [_c_void_p, _c_void_p, _c_void_p, _int, _c_void_p, _c_void_p, _c_void_p]),
+    "bkm_mode_merge": (_int, [_c_void_p, _i64, _c_void_p, _c_void_p, _c_void_p, _int, _i64, _c_void_p]),
+    "bkm_impute_chunk": (_int, [_c_void_p, _i64, _int, _i64, _int, _int, _dbl, _c_void_p, _c_void_p, _int, _int, _int,
+                                _int, _c_void_p, _i64, _int, _c_void_p, _c_void_p]),
     "bkm_split_indices_chunk": (_int, [_u64, _i64, _i64, _i64, _i64, _c_void_p, _c_void_p]),
     "bkm_gather_rows_chunk": (_int, [_c_void_p, _i64, _i64, _i64, _c_void_p, _i64, _i64, _c_void_p, _i64, _c_void_p]),
     "bkm_metric_workspace_bytes": (_int, [_i64, _int, _int, _szp]),

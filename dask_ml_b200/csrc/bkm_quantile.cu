@@ -15,6 +15,8 @@
 //                      for its digit, the extended prefix, and the next live list by adjacent-unique compaction (the
 //                      ranks are sorted, so their prefixes are).  Round 0 first derives the ranks from the column's
 //                      non-NaN count and merges the floor / floor + 1 lists into the distinct sorted ranks.
+//   bkm_quantile_hist_masked_chunk   the same count with the values equal to a numeric missing value skipped too, so
+//       the non-NaN count the select step derives in round 0 is the non-missing count (SimpleImputer's median).
 //   bkm_quantile_transform_chunk   per element, in float64: numpy's interp (restated branch by branch, every operation
 //       rounded once: no FMA contraction), the reference's +-1e-7 bounds test in X's dtype, then the output
 //       distribution's ppf and the clip (forward), or its cdf first (inverse).  A CTA stages one sector of columns'
@@ -71,6 +73,7 @@ struct QHistArgs {
   long long cap;           // slots per column of the histogram: live_cap(nq, round)
   int stage;               // round >= 1: the CTA's live lists are staged in shared memory
   double* hist;            // [d][cap][256]
+  double miss;             // MASKED: values equal to it (after widening to float64) are skipped
 };
 
 // the index of `v` in the sorted, duplicate-free list[0, L), or -1
@@ -85,7 +88,7 @@ __device__ __forceinline__ int find_live(P list, int L, K v) {
   return (lo < L && (K)list[lo] == v) ? lo : -1;
 }
 
-template <typename T>
+template <typename T, bool MASKED>
 __global__ void __launch_bounds__(kThreads) quantile_hist_kernel(QHistArgs a) {
   typedef typename KeyOf<T>::type K;
   extern __shared__ __align__(16) unsigned char q_smem[];
@@ -134,7 +137,7 @@ __global__ void __launch_bounds__(kThreads) quantile_hist_kernel(QHistArgs a) {
       }
 #pragma unroll
       for (int u = 0; u < U; ++u) {
-        if (r + (long long)u * RL < re && !is_nan(v[u])) {
+        if (r + (long long)u * RL < re && !is_nan(v[u]) && !(MASKED && widen(v[u]) == a.miss)) {
           const unsigned long long key = radix_key(v[u]);
           const unsigned digit = (unsigned)(key >> sh) & 255u;
           if (a.round == 0) {
@@ -468,7 +471,7 @@ __global__ void __launch_bounds__(kThreads) quantile_transform_kernel(QTransform
 
 constexpr size_t kStageBytes = 96 * 1024;    // two CTAs per SM
 
-template <typename T>
+template <typename T, bool MASKED>
 static int launch_qhist(QHistArgs a, int sms, cudaStream_t s) {
   constexpr int CS = 32 / sizeof(T);
   typedef typename KeyOf<T>::type K;
@@ -478,7 +481,7 @@ static int launch_qhist(QHistArgs a, int sms, cudaStream_t s) {
     a.stage = 1;
     smem = (size_t)CS * a.cap * sizeof(K);
   }
-  BKM_CUDA_TRY(cudaFuncSetAttribute(quantile_hist_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+  BKM_CUDA_TRY(cudaFuncSetAttribute(quantile_hist_kernel<T, MASKED>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                     (int)kStageBytes));
   const int gy = (a.d + CS - 1) / CS;
   const int per_sm = smem <= 24 * 1024 ? 8 : (smem <= 48 * 1024 ? 4 : 2);
@@ -486,7 +489,7 @@ static int launch_qhist(QHistArgs a, int sms, cudaStream_t s) {
   const long long most = (a.n + (kThreads / CS) * 16 - 1) / ((kThreads / CS) * 16);   // >= 16 rows per thread
   if (gx > most) gx = most;
   if (gx < 1) gx = 1;
-  quantile_hist_kernel<T><<<dim3((unsigned)gx, (unsigned)gy), kThreads, smem, s>>>(a);
+  quantile_hist_kernel<T, MASKED><<<dim3((unsigned)gx, (unsigned)gy), kThreads, smem, s>>>(a);
   BKM_CUDA_TRY(cudaGetLastError());
   note_launch();
   return 0;
@@ -527,8 +530,8 @@ extern "C" int bkm_quantile_state_bytes(int d, int n_q, size_t* out) {
   return 0;
 }
 
-extern "C" int bkm_quantile_hist_chunk(const void* X, int64_t n, int d, int64_t ldx, int x_dtype, const void* state,
-                                       int n_q, int round, double* hist, int flags, void* stream) {
+static int quantile_hist(const void* X, int64_t n, int d, int64_t ldx, int x_dtype, const void* state, int n_q,
+                         int round, double* hist, int flags, void* stream, bool masked, double miss) {
   if (n < 0 || d <= 0 || ldx < d || !state || !hist || n_q <= 0 || round < 0) return BKM_EINVAL;
   if (n > 0 && !X) return BKM_EINVAL;
   if (!dtype_ok(x_dtype)) return BKM_EDTYPE;
@@ -547,9 +550,27 @@ extern "C" int bkm_quantile_hist_chunk(const void* X, int64_t n, int d, int64_t 
   a.cap = cap;
   a.stage = 0;
   a.hist = hist;
-  if (x_dtype == BKM_F32) return launch_qhist<float>(a, sms, s);
-  if (x_dtype == BKM_F64) return launch_qhist<double>(a, sms, s);
-  return launch_qhist<__nv_bfloat16>(a, sms, s);
+  a.miss = miss;
+  if (masked) {
+    if (x_dtype == BKM_F32) return launch_qhist<float, true>(a, sms, s);
+    if (x_dtype == BKM_F64) return launch_qhist<double, true>(a, sms, s);
+    return launch_qhist<__nv_bfloat16, true>(a, sms, s);
+  }
+  if (x_dtype == BKM_F32) return launch_qhist<float, false>(a, sms, s);
+  if (x_dtype == BKM_F64) return launch_qhist<double, false>(a, sms, s);
+  return launch_qhist<__nv_bfloat16, false>(a, sms, s);
+}
+
+extern "C" int bkm_quantile_hist_chunk(const void* X, int64_t n, int d, int64_t ldx, int x_dtype, const void* state,
+                                       int n_q, int round, double* hist, int flags, void* stream) {
+  return quantile_hist(X, n, d, ldx, x_dtype, state, n_q, round, hist, flags, stream, false, 0.0);
+}
+
+extern "C" int bkm_quantile_hist_masked_chunk(const void* X, int64_t n, int d, int64_t ldx, int x_dtype,
+                                              double miss_value, const void* state, int n_q, int round, double* hist,
+                                              int flags, void* stream) {
+  if (miss_value != miss_value) return BKM_EINVAL;          // NaN is skipped by bkm_quantile_hist_chunk already
+  return quantile_hist(X, n, d, ldx, x_dtype, state, n_q, round, hist, flags, stream, true, miss_value);
 }
 
 extern "C" int bkm_quantile_select_step(double* hist, void* state, int d, int n_q, int round, int x_dtype,

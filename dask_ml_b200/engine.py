@@ -592,6 +592,87 @@ class CudaBackend(object):
                 int(ref.shape[0]), int(bool(inverse)), int(distribution), float(clip_lo), float(clip_hi),
                 self._ptr(out), out.stride(0) if n else d, self._stream()), "bkm_quantile_transform_chunk")
 
+    def impute_stats_chunk(self, x, miss_is_nan, miss, shift, acc, first=False):
+        """SimpleImputer's statistics pass over one chunk, float64 on the device: acc (4, d) (+)= [missing count | NaN
+        count | inf count | sum (x - shift) over the non-missing finite x].  ``miss`` a value of X's dtype (ignored
+        with ``miss_is_nan``); ``shift`` float64 (d,) or None; ``first`` overwrites."""
+        n, d = x.shape
+        nb = ctypes.c_size_t(0)
+        _lib.check(self.lib.bkm_impute_stats_workspace_bytes(int(n), int(d), ctypes.byref(nb)),
+                   "bkm_impute_stats_workspace_bytes")
+        ws = self._scratch("impute_stats", nb.value)
+        flags = self.flags | (_lib.FLAG_FIRST_CHUNK if first else 0)
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.bkm_impute_stats_chunk(
+                self._ptr(x), n, d, x.stride(0) if n else d, _DT_CODE[x.dtype], int(bool(miss_is_nan)), float(miss),
+                self._ptr(shift), self._ptr(acc), self._ptr(ws), ws.numel(), flags, self._stream()),
+                "bkm_impute_stats_chunk")
+
+    def quantile_hist_masked_chunk(self, x, miss, state, n_q, rnd, hist, first=False):
+        """``quantile_hist_chunk`` with the elements equal to ``miss`` (a number, not NaN) skipped as well."""
+        n, d = x.shape
+        flags = self.flags | (_lib.FLAG_FIRST_CHUNK if first else 0)
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.bkm_quantile_hist_masked_chunk(
+                self._ptr(x), n, d, x.stride(0) if n else d, _DT_CODE[x.dtype], float(miss), self._ptr(state),
+                int(n_q), int(rnd), self._ptr(hist), flags, self._stream()), "bkm_quantile_hist_masked_chunk")
+
+    def mode_count_chunk(self, x, miss_is_nan, miss, keys, counts, off, total, first=False):
+        """Count the distinct non-missing values of each column of ``x`` (a group of g columns) into the hash tables
+        ``keys`` / ``counts`` (uint64 as int64 (total,)), column j owning slots [off[j], off[j + 1]) (``off`` int64
+        (g + 1,) on the device); ``first`` resets the tables."""
+        n, g = x.shape
+        flags = self.flags | (_lib.FLAG_FIRST_CHUNK if first else 0)
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.bkm_mode_count_chunk(
+                self._ptr(x), n, g, x.stride(0) if n else g, _DT_CODE[x.dtype], int(bool(miss_is_nan)), float(miss),
+                self._ptr(keys), self._ptr(counts), self._ptr(off), int(total), flags, self._stream()),
+                "bkm_mode_count_chunk")
+
+    def mode_best(self, keys, counts, off, g, total):
+        """(best_key int64 (g,) holding uint64 keys, best_count float64 (g,), distinct float64 (g,)) on the device: per
+        column the largest count, the smallest key among equal counts (``total`` the tables' slots)."""
+        key = torch.empty(g, dtype=torch.int64, device=self.device)
+        cnt = torch.empty(g, dtype=torch.float64, device=self.device)
+        nd = torch.empty(g, dtype=torch.float64, device=self.device)
+        nb = ctypes.c_size_t(0)
+        _lib.check(self.lib.bkm_mode_best_workspace_bytes(int(g), int(total), ctypes.byref(nb)),
+                   "bkm_mode_best_workspace_bytes")
+        ws = self._scratch("mode_best", nb.value)
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.bkm_mode_best(self._ptr(keys), self._ptr(counts), self._ptr(off), int(g), int(total),
+                                              self._ptr(key), self._ptr(cnt), self._ptr(nd), self._ptr(ws), ws.numel(),
+                                              self._stream()), "bkm_mode_best")
+        return key, cnt, nd
+
+    def mode_compact(self, keys, counts, off, g, entries):
+        """The occupied slots of the tables as rows {column, key >> 32, key & 0xffffffff, count} of ``entries``
+        (float64 (m, 4), m at least the number of occupied slots)."""
+        cursor = torch.empty(1, dtype=torch.int64, device=self.device)
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.bkm_mode_compact(self._ptr(keys), self._ptr(counts), self._ptr(off), int(g),
+                                                 self._ptr(entries), self._ptr(cursor), self._stream()),
+                       "bkm_mode_compact")
+
+    def mode_merge(self, entries, keys, counts, off, g, total):
+        """Reset the tables and add every row of ``entries`` (float64 (m, 4)) with a non-zero count."""
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.bkm_mode_merge(self._ptr(entries), int(entries.shape[0]), self._ptr(keys),
+                                               self._ptr(counts), self._ptr(off), int(g), int(total), self._stream()),
+                       "bkm_mode_merge")
+
+    def impute_chunk(self, x, miss_is_nan, miss, stats, cols, n_keep, n_ind, n_check, inverse, out, invalid=None):
+        """SimpleImputer's fill pass (or its inverse) over one chunk into ``out`` (any row pitch, X's dtype; float32
+        for bf16 rows): see include/bkm_b200.h.  ``stats`` float64 (d,), ``cols`` int32 on the device; ``invalid``
+        float64 (2,) (+)= the NaN and inf counts of the elements read."""
+        n, d = x.shape
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.bkm_impute_chunk(
+                self._ptr(x), n, d, x.stride(0) if n else d, _DT_CODE[x.dtype], int(bool(miss_is_nan)), float(miss),
+                self._ptr(stats), self._ptr(cols), int(n_keep), int(n_ind), int(n_check), int(bool(inverse)),
+                self._ptr(out), out.stride(0) if n else int(out.shape[1]), _DT_CODE[out.dtype], self._ptr(invalid),
+                self._stream()), "bkm_impute_chunk")
+
     def affine_chunk(self, x, a, b, op1, op2, out):
         """out = op2(op1(x, a), b) per element (op1: 0 none, 1 subtract a, 2 multiply by a; op2: 0 none, 1 divide by b,
         2 add b), each step rounded once in out's dtype.  ``a``, ``b`` float64 (d,) or None; ``out`` (n, d) float32 /

@@ -304,14 +304,13 @@ def _order_stat_ranks(nvalid, qf):
     return np.where(empty, 0.0, lo), np.where(empty, 0.0, hi)
 
 
-def quantiles_exact(X, references):
-    """np.percentile(column, references * 100) of every whole column over every row of every rank, exact for any
-    chunking or rank split: (len(references), d) float64, NaN for a column that holds a NaN."""
+def order_statistics(X, qf, missing=None):
+    """The order statistics of every whole column at the floor / floor + 1 ranks of numpy's 'linear' virtual index
+    (m - 1) qf over its m valid values, exact for any chunking or rank split: (lo, hi) of X's host dtype and m, each
+    (d, len(qf)) / (d,).  Valid means not NaN and, with a number ``missing``, not equal to it (the masked count)."""
     be, comm, d = X.backend, X.comm, X.d
-    nq = len(references)
-    q = np.asarray(references, dtype=np.float64) * 100
-    qf = np.true_divide(q, 100.0)
-    qf_dev = torch.as_tensor(np.ascontiguousarray(qf)).to(be.device)
+    nq = len(qf)
+    qf_dev = torch.as_tensor(np.ascontiguousarray(qf, dtype=np.float64)).to(be.device)
     rounds = RADIX_ROUNDS[X.dtype]
     stride = 16 + 80 * nq
     state = be.quantile_state_new(d, nq)
@@ -324,15 +323,15 @@ def quantiles_exact(X, references):
         for rnd in range(rounds):
             h = hist[: (j1 - j0) * min(2 * nq, 256 ** rnd) * 256]
             for i, x in enumerate(X.chunks):
-                be.quantile_hist_chunk(x[:, j0:j1], st, nq, rnd, h, first=i == 0)
+                if missing is None:
+                    be.quantile_hist_chunk(x[:, j0:j1], st, nq, rnd, h, first=i == 0)
+                else:
+                    be.quantile_hist_masked_chunk(x[:, j0:j1], missing, st, nq, rnd, h, first=i == 0)
             comm.allreduce_sum_(h)
             be.quantile_select_step(h, st, j1 - j0, nq, rnd, X.dtype, qf_dev)
     raw = state.cpu().numpy().reshape(d, stride)
     head = np.ascontiguousarray(raw[:, :16]).view(QUANTILE_HEAD)[:, 0]
     rec = np.ascontiguousarray(raw[:, 16: 16 + 64 * nq]).view(SELECT_RECORD)
-    n = X.n_global
-    if n == 0:
-        return np.full((nq, d), np.nan)
     lo, hi = _order_stat_ranks(head["nvalid"], qf)
     keys = np.empty((2, d, nq), dtype=np.uint64)
     for j in range(d):
@@ -341,8 +340,22 @@ def quantiles_exact(X, references):
         keys[0, j] = rec["key"][j, np.searchsorted(distinct, lo[j])]
         keys[1, j] = rec["key"][j, np.searchsorted(distinct, hi[j])]
     vals = keys_to_values(keys, X.dtype)
-    P = percentile_from_order_stats(vals[0], vals[1], n, q, X.np_dtype)
-    P[head["nvalid"] < n] = np.nan                      # a NaN in the column: numpy gives NaN
+    return vals[0], vals[1], np.asarray(head["nvalid"], dtype=np.float64)
+
+
+def quantiles_exact(X, references):
+    """np.percentile(column, references * 100) of every whole column over every row of every rank, exact for any
+    chunking or rank split: (len(references), d) float64, NaN for a column that holds a NaN."""
+    d = X.d
+    nq = len(references)
+    q = np.asarray(references, dtype=np.float64) * 100
+    qf = np.true_divide(q, 100.0)
+    lo, hi, nvalid = order_statistics(X, qf)
+    n = X.n_global
+    if n == 0:
+        return np.full((nq, d), np.nan)
+    P = percentile_from_order_stats(lo, hi, n, q, X.np_dtype)
+    P[nvalid < n] = np.nan                              # a NaN in the column: numpy gives NaN
     return np.ascontiguousarray(np.asarray(P, dtype=np.float64).T)
 
 

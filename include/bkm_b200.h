@@ -43,6 +43,10 @@
  *   the elementwise graphs and reductions of accuracy_score,           bkm_metric_chunk
  *     log_loss, mean_squared_error, mean_absolute_error, r2_score,
  *     metrics/classification.py:11-150, metrics/regression.py:8-92
+ *   scikit-learn's SimpleImputer._dense_fit / transform /             bkm_impute_stats_chunk,
+ *     inverse_transform behind dask_ml/impute.py (np.ma.mean,            bkm_quantile_hist_masked_chunk,
+ *     np.ma.median, the per-column mode, the masked fill and the          bkm_mode_*, bkm_impute_chunk
+ *     indicator columns)
  *
  * Conventions
  *   - extern "C", plain pointers and sizes only; no torch / C++ types.
@@ -67,8 +71,10 @@ extern "C" {
 
 #define BKM_VERSION 200
 /* Entry points added since BKM_VERSION 200 without changing an existing one raise the minor number:
- * 1 = bkm_split_indices_chunk, bkm_gather_rows_chunk, bkm_metric_workspace_bytes, bkm_metric_chunk */
-#define BKM_VERSION_MINOR 1
+ * 1 = bkm_split_indices_chunk, bkm_gather_rows_chunk, bkm_metric_workspace_bytes, bkm_metric_chunk
+ * 2 = bkm_impute_stats_workspace_bytes, bkm_impute_stats_chunk, bkm_quantile_hist_masked_chunk, bkm_mode_count_chunk,
+ *     bkm_mode_best_workspace_bytes, bkm_mode_best, bkm_mode_compact, bkm_mode_merge, bkm_impute_chunk */
+#define BKM_VERSION_MINOR 2
 
 /* element types of X */
 #define BKM_F32 0
@@ -486,6 +492,63 @@ int bkm_metric_workspace_bytes(int64_t n, int m, int mode, size_t* out);
 int bkm_metric_chunk(const void* a, int a_dtype, const void* b, int b_dtype, const double* w, int64_t n, int m,
                      int mode, const double* shift, double eps, double* acc, void* workspace, size_t ws_bytes,
                      int flags, void* stream);
+
+/* ---- SimpleImputer: the fit statistics and the fill pass over row chunks (replace scikit-learn's _dense_fit, transform
+ * and inverse_transform, which dask_ml/impute.py calls for numpy input) -------------------------------------------------
+ * The missing value is passed as (miss_is_nan, miss_value): NaN when miss_is_nan = 1 (miss_value is then ignored, NaN
+ * allowed), else every x with (double)x == miss_value (miss_value a value of X's dtype; +0.0 and -0.0 both match 0).
+ *   bkm_impute_stats_chunk   acc [4][d] float64 per column: [missing count | NaN count | inf count | sum (x - shift_j)
+ *                        over the non-missing finite x]; shift [d] float64 (device, nullable: 0).  OVERWRITTEN with
+ *                        BKM_FLAG_FIRST_CHUNK, else ACCUMULATED; CTA partials are folded in a fixed order (no float
+ *                        atomics): two calls with the same inputs give the same bits.  workspace:
+ *                        bkm_impute_stats_workspace_bytes(n, d) bytes, any content.
+ *   bkm_quantile_hist_masked_chunk   bkm_quantile_hist_chunk with the x == miss_value rows skipped as well (miss_value
+ *                        not NaN), so that the select step's nvalid is the non-missing count.  Same state, rounds and
+ *                        bkm_quantile_select_step.
+ *   bkm_mode_count_chunk     per column j of a group of g columns, the count of every distinct non-missing, non-NaN
+ *                        value, by its order-preserving key (the keys of bkm_quantile_hist_chunk: 16, 32 or 64 bits in a
+ *                        uint64, -0.0 counted as +0.0), in an open-addressing table: keys / counts [total_slots] uint64,
+ *                        column j owning slots [slot_off[j], slot_off[j + 1]) (slot_off [g + 1] int64, device), a power of
+ *                        two (or zero) at least twice the values the column can receive, so that no table fills.  Empty
+ *                        slots hold the key ~0 (a NaN pattern).  With BKM_FLAG_FIRST_CHUNK the tables are reset first,
+ *                        else counts are ACCUMULATED.  Counts are integers: exact in any order.  X + j0 with ldx runs
+ *                        a column group as a view.
+ *   bkm_mode_best        per column: best_key [g] uint64 and best_count [g] float64 of the entry of largest count, the
+ *                        smallest key among equal counts (count 0: no value), and distinct [g] float64 the number of
+ *                        occupied slots.  The order is total: the result does not depend on the table layout.  Several
+ *                        CTAs share a column's table (slices, then a fold of their partials).  workspace:
+ *                        bkm_mode_best_workspace_bytes(g, total_slots) bytes, any content.
+ *   bkm_mode_compact     every occupied slot as a row of entries [*][4] float64 {column, key >> 32, key & 0xffffffff,
+ *                        count}, rows in no particular order; *cursor (uint64, device) ends at the number of rows.
+ *   bkm_mode_merge       resets the tables, then adds every row of entries [n_entries][4] with count > 0 to its
+ *                        column's table (rows with count 0 are skipped: the zero padding of gathered slices).
+ *   bkm_impute_chunk     forward (inverse 0): out [n][ld_out] in out_dtype (X's dtype; BKM_F32 for bf16 rows), columns
+ *                        o < n_keep: x[:, cols[o]] with its missing elements replaced by (out_dtype)stats[cols[o]];
+ *                        then n_ind indicator columns: 1 where x[:, cols[o]] is missing, else 0; then n_check input
+ *                        columns cols[o] that are only validated.  invalid [2] float64 (nullable) (+)= the NaN and inf
+ *                        counts of the filled and validated columns.  inverse (inverse 1): n_keep = n_ind = the output
+ *                        width, cols [2 n_keep]: out[:, o] = x[:, cols[o]] (0 when cols[o] = -1), then miss_value where
+ *                        x[:, cols[n_keep + o]] != 0 (cols[n_keep + o] >= 0).  One read of X, one write of out; any
+ *                        ldx >= d, ld_out >= the output width; the input is only read. */
+int bkm_impute_stats_workspace_bytes(int64_t n, int d, size_t* out);
+int bkm_impute_stats_chunk(const void* X, int64_t n, int d, int64_t ldx, int x_dtype, int miss_is_nan, double miss_value,
+                           const double* shift, double* acc, void* workspace, size_t ws_bytes, int flags, void* stream);
+int bkm_quantile_hist_masked_chunk(const void* X, int64_t n, int d, int64_t ldx, int x_dtype, double miss_value,
+                                   const void* state, int n_q, int round, double* hist, int flags, void* stream);
+int bkm_mode_count_chunk(const void* X, int64_t n, int g, int64_t ldx, int x_dtype, int miss_is_nan, double miss_value,
+                         unsigned long long* keys, unsigned long long* counts, const int64_t* slot_off,
+                         int64_t total_slots, int flags, void* stream);
+int bkm_mode_best_workspace_bytes(int g, int64_t total_slots, size_t* out);
+int bkm_mode_best(const unsigned long long* keys, const unsigned long long* counts, const int64_t* slot_off, int g,
+                  int64_t total_slots, unsigned long long* best_key, double* best_count, double* distinct,
+                  void* workspace, size_t ws_bytes, void* stream);
+int bkm_mode_compact(const unsigned long long* keys, const unsigned long long* counts, const int64_t* slot_off, int g,
+                     double* entries, unsigned long long* cursor, void* stream);
+int bkm_mode_merge(const double* entries, int64_t n_entries, unsigned long long* keys, unsigned long long* counts,
+                   const int64_t* slot_off, int g, int64_t total_slots, void* stream);
+int bkm_impute_chunk(const void* X, int64_t n, int d, int64_t ldx, int x_dtype, int miss_is_nan, double miss_value,
+                     const double* stats, const int* cols, int n_keep, int n_ind, int n_check, int inverse, void* out,
+                     int64_t ld_out, int out_dtype, double* invalid, void* stream);
 
 /* ---- NaN/inf scan of a chunk (k_means.py:179-180): sets *flag (int32) nonzero -------- */
 int bkm_check_finite(const void* X, int64_t n, int d, int64_t ldx, int x_dtype,
