@@ -22,6 +22,10 @@ BKM_M_U8 = 6
 METRIC_EQ = 0
 METRIC_ERR = 1
 METRIC_LOGLOSS = 2
+ENCODE_CODES = 0
+ENCODE_DENSE = 1
+ENCODE_CSR = 2
+ENCODE_KEEP = 8
 
 FLAG_FORCE_SIMT = 1
 FLAG_FORCE_TC = 2
@@ -111,6 +115,12 @@ SIGNATURES = {
     "bkm_mode_merge": (_int, [_c_void_p, _i64, _c_void_p, _c_void_p, _c_void_p, _int, _i64, _c_void_p]),
     "bkm_impute_chunk": (_int, [_c_void_p, _i64, _int, _i64, _int, _int, _dbl, _c_void_p, _c_void_p, _int, _int, _int,
                                 _int, _c_void_p, _i64, _int, _c_void_p, _c_void_p]),
+    "bkm_distinct_chunk": (_int, [_c_void_p, _i64, _int, _i64, _int, _c_void_p, _c_void_p, _c_void_p, _i64, _c_void_p,
+                                  _int, _c_void_p]),
+    "bkm_encode_chunk": (_int, [_c_void_p, _i64, _int, _i64, _int, _c_void_p, _c_void_p, _i64, _int, _c_void_p, _i64,
+                                _int, _c_void_p, _c_void_p, _c_void_p]),
+    "bkm_decode_chunk": (_int, [_c_void_p, _i64, _int, _i64, _int, _c_void_p, _c_void_p, _int, _c_void_p, _i64,
+                                _c_void_p, _c_void_p]),
     "bkm_split_indices_chunk": (_int, [_u64, _i64, _i64, _i64, _i64, _c_void_p, _c_void_p]),
     "bkm_gather_rows_chunk": (_int, [_c_void_p, _i64, _i64, _i64, _c_void_p, _i64, _i64, _c_void_p, _i64, _c_void_p]),
     "bkm_metric_workspace_bytes": (_int, [_i64, _int, _int, _szp]),

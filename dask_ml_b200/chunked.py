@@ -23,7 +23,9 @@ if torch is not None:
     _TORCH_TO_NP = {
         torch.float32: np.dtype("float32"), torch.float64: np.dtype("float64"),
         torch.float16: np.dtype("float16"), torch.int32: np.dtype("int32"),
-        torch.int64: np.dtype("int64"), torch.bool: np.dtype("bool"),
+        torch.int64: np.dtype("int64"), torch.bool: np.dtype("bool"), torch.uint8: np.dtype("uint8"),
+        torch.int8: np.dtype("int8"), torch.int16: np.dtype("int16"), torch.uint16: np.dtype("uint16"),
+        torch.uint32: np.dtype("uint32"),
         # numpy has no bfloat16: a bf16 block presents itself as float32 to numpy consumers (it is widened on
         # the way out) and stays bf16 on the device (the large-shape tensor path multiplies the rows as stored)
         torch.bfloat16: np.dtype("float32"),
@@ -34,7 +36,19 @@ def block_dtype(b):
     return _TORCH_TO_NP[b.dtype] if _is_torch(b) else np.dtype(b.dtype)
 
 
+def is_sparse_csr_block(b):
+    return _is_torch(b) and b.layout == torch.sparse_csr
+
+
 def block_to_numpy(b):
+    """A block as numpy; a torch sparse CSR block (OneHotEncoder's sparse output) as a scipy.sparse.csr_matrix."""
+    if is_sparse_csr_block(b):
+        import scipy.sparse
+
+        b = b.detach().cpu()
+        vals = b.values()
+        vals = (vals.float() if vals.dtype == torch.bfloat16 else vals).numpy()
+        return scipy.sparse.csr_matrix((vals, b.col_indices().numpy(), b.crow_indices().numpy()), shape=tuple(b.shape))
     if _is_torch(b):
         b = b.detach()
         if b.dtype == torch.bfloat16:
@@ -97,7 +111,13 @@ class ChunkedArray(object):
     # -- materialisation ---------------------------------------------------------------
     def compute(self):
         parts = [block_to_numpy(b) for b in self.blocks]
-        return parts[0] if len(parts) == 1 else np.concatenate(parts, axis=0)
+        if len(parts) == 1:
+            return parts[0]
+        if any(is_sparse_csr_block(b) for b in self.blocks):
+            import scipy.sparse
+
+            return scipy.sparse.vstack(parts, format="csr")
+        return np.concatenate(parts, axis=0)
 
     def __array__(self, dtype=None, copy=None):
         a = self.compute()

@@ -139,18 +139,6 @@ __global__ void __launch_bounds__(kThreads) impute_stats_kernel(IStatsArgs a) {
 }
 
 // ============================================ mode ============================================
-constexpr unsigned long long kEmpty = ~0ull;       // a NaN pattern: never a key of an inserted value
-constexpr int kTileRows = 256;
-
-__device__ __forceinline__ unsigned long long mix64(unsigned long long k) {
-  k ^= k >> 33;
-  k *= 0xff51afd7ed558ccdull;
-  k ^= k >> 33;
-  k *= 0xc4ceb9fe1a85ec53ull;
-  k ^= k >> 33;
-  return k;
-}
-
 // add `cnt` to the entry of `key` in the table keys / counts [cap] (cap a power of two, never full)
 __device__ __forceinline__ void table_add(unsigned long long* keys, unsigned long long* counts, long long cap,
                                           unsigned long long key, unsigned long long cnt) {

@@ -55,5 +55,19 @@ __device__ __forceinline__ bool is_nan(float v) { return v != v; }
 __device__ __forceinline__ bool is_nan(double v) { return v != v; }
 __device__ __forceinline__ bool is_nan(__nv_bfloat16 v) { return __hisnan(v); }
 
+// Open-addressing key tables of the mode (bkm_impute.cu) and distinct-value (bkm_encode.cu) passes: the empty slot
+// marker (a NaN pattern for float keys; the key of INT64_MAX for int64 keys) and the slot hash.
+constexpr unsigned long long kEmpty = ~0ull;
+constexpr int kTileRows = 256;     // rows of X a CTA stages per tile
+
+__device__ __forceinline__ unsigned long long mix64(unsigned long long k) {
+  k ^= k >> 33;
+  k *= 0xff51afd7ed558ccdull;
+  k ^= k >> 33;
+  k *= 0xc4ceb9fe1a85ec53ull;
+  k ^= k >> 33;
+  return k;
+}
+
 }  // namespace
 }  // namespace bkm

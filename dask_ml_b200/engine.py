@@ -24,6 +24,10 @@ _NP_TO_TORCH = {np.dtype("float32"): torch.float32, np.dtype("float64"): torch.f
 _DT_CODE = {torch.float32: _lib.BKM_F32, torch.float64: _lib.BKM_F64, torch.bfloat16: _lib.BKM_BF16}
 _METRIC_CODE = {**_DT_CODE, torch.float16: _lib.BKM_M_F16, torch.int32: _lib.BKM_M_I32, torch.int64: _lib.BKM_M_I64,
                 torch.bool: _lib.BKM_M_U8, torch.uint8: _lib.BKM_M_U8}
+# element types of the encoders' passes (X, one-hot outputs and codes)
+_ENC_CODE = {torch.float32: _lib.BKM_F32, torch.float64: _lib.BKM_F64, torch.bfloat16: _lib.BKM_BF16,
+             torch.int32: _lib.BKM_M_I32, torch.int64: _lib.BKM_M_I64, torch.bool: _lib.BKM_M_U8,
+             torch.uint8: _lib.BKM_M_U8}
 
 
 def out_dtype(x_dtype):
@@ -672,6 +676,43 @@ class CudaBackend(object):
                 self._ptr(stats), self._ptr(cols), int(n_keep), int(n_ind), int(n_check), int(bool(inverse)),
                 self._ptr(out), out.stride(0) if n else int(out.shape[1]), _DT_CODE[out.dtype], self._ptr(invalid),
                 self._stream()), "bkm_impute_chunk")
+
+    def distinct_chunk(self, x, keys, counts, off, total, state, first=False):
+        """Record the distinct keys of each column of ``x`` (a group of g columns, any element type of
+        ``ENCODE_DTYPES``) in the tables ``keys`` / ``counts`` (uint64 as int64 (total,)), column j owning slots
+        [off[j], off[j + 1]); ``state`` int64 (2, g) on the device (+)= [occupied slots | status bits: 1 overflow,
+        2 holds INT64_MAX]; ``first`` resets tables and state."""
+        n, g = x.shape
+        flags = self.flags | (_lib.FLAG_FIRST_CHUNK if first else 0)
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.bkm_distinct_chunk(
+                self._ptr(x), n, g, x.stride(0) if n else g, _ENC_CODE[x.dtype], self._ptr(keys), self._ptr(counts),
+                self._ptr(off), int(total), self._ptr(state), flags, self._stream()), "bkm_distinct_chunk")
+
+    def encode_chunk(self, x, cat_keys, cat_off, n_cats, layout, out, unknown, indices=None):
+        """One read of ``x`` (n, d): codes, a dense one-hot block or the CSR indices / data of every element, by its
+        column's sorted key list (``cat_keys`` int64 holding uint64 keys, ``cat_off`` int64 (d + 1,) on the device).
+        ``unknown`` uint64 as int64 (1 + d + d * ENCODE_KEEP,) (+)= the unknown-key counts and kept keys."""
+        n, d = x.shape
+        if layout == _lib.ENCODE_DENSE:
+            ld = int(n_cats)
+        else:
+            ld = out.stride(0) if layout == _lib.ENCODE_CODES and n else d
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.bkm_encode_chunk(
+                self._ptr(x), n, d, x.stride(0) if n else d, _ENC_CODE[x.dtype], self._ptr(cat_keys),
+                self._ptr(cat_off), int(n_cats), int(layout), self._ptr(out), ld, _ENC_CODE[out.dtype],
+                self._ptr(indices), self._ptr(unknown), self._stream()), "bkm_encode_chunk")
+
+    def decode_chunk(self, codes, cat_vals, cat_off, out, unknown):
+        """out (n, d) = cat_vals[cat_off[j] + codes[:, j]] (``codes`` int32 / int64 (n, d), ``cat_vals`` any dtype of
+        1, 2, 4 or 8 bytes, ``out`` of the same dtype); codes outside [0, K_j) add to ``unknown``."""
+        n, d = codes.shape
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.bkm_decode_chunk(
+                self._ptr(codes), n, d, codes.stride(0) if n else d, _ENC_CODE[codes.dtype], self._ptr(cat_vals),
+                self._ptr(cat_off), cat_vals.element_size(), self._ptr(out), out.stride(0) if n else d,
+                self._ptr(unknown), self._stream()), "bkm_decode_chunk")
 
     def affine_chunk(self, x, a, b, op1, op2, out):
         """out = op2(op1(x, a), b) per element (op1: 0 none, 1 subtract a, 2 multiply by a; op2: 0 none, 1 divide by b,

@@ -1,3 +1,5 @@
+from ._encoders import OneHotEncoder
 from .data import MinMaxScaler, QuantileTransformer, RobustScaler, StandardScaler
+from .label import LabelEncoder
 
-__all__ = ["StandardScaler", "MinMaxScaler", "RobustScaler", "QuantileTransformer"]
+__all__ = ["StandardScaler", "MinMaxScaler", "RobustScaler", "QuantileTransformer", "LabelEncoder", "OneHotEncoder"]

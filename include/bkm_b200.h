@@ -47,6 +47,9 @@
  *     inverse_transform behind dask_ml/impute.py (np.ma.mean,            bkm_quantile_hist_masked_chunk,
  *     np.ma.median, the per-column mode, the masked fill and the          bkm_mode_*, bkm_impute_chunk
  *     indicator columns)
+ *   da.unique / np.searchsorted / the sparse one-hot blocks of         bkm_distinct_chunk (+ bkm_mode_compact /
+ *     LabelEncoder and OneHotEncoder, preprocessing/label.py:14-302,     bkm_mode_merge / bkm_mode_best),
+ *     preprocessing/_encoders.py:18-244                                 bkm_encode_chunk, bkm_decode_chunk
  *
  * Conventions
  *   - extern "C", plain pointers and sizes only; no torch / C++ types.
@@ -73,8 +76,9 @@ extern "C" {
 /* Entry points added since BKM_VERSION 200 without changing an existing one raise the minor number:
  * 1 = bkm_split_indices_chunk, bkm_gather_rows_chunk, bkm_metric_workspace_bytes, bkm_metric_chunk
  * 2 = bkm_impute_stats_workspace_bytes, bkm_impute_stats_chunk, bkm_quantile_hist_masked_chunk, bkm_mode_count_chunk,
- *     bkm_mode_best_workspace_bytes, bkm_mode_best, bkm_mode_compact, bkm_mode_merge, bkm_impute_chunk */
-#define BKM_VERSION_MINOR 2
+ *     bkm_mode_best_workspace_bytes, bkm_mode_best, bkm_mode_compact, bkm_mode_merge, bkm_impute_chunk
+ * 3 = bkm_distinct_chunk, bkm_encode_chunk, bkm_decode_chunk */
+#define BKM_VERSION_MINOR 3
 
 /* element types of X */
 #define BKM_F32 0
@@ -549,6 +553,47 @@ int bkm_mode_merge(const double* entries, int64_t n_entries, unsigned long long*
 int bkm_impute_chunk(const void* X, int64_t n, int d, int64_t ldx, int x_dtype, int miss_is_nan, double miss_value,
                      const double* stats, const int* cols, int n_keep, int n_ind, int n_check, int inverse, void* out,
                      int64_t ld_out, int out_dtype, double* invalid, void* stream);
+
+/* ---- LabelEncoder / OneHotEncoder: the categories of every column and the encoding passes (replace da.unique,
+ * np.searchsorted and the per-block sparse one-hot matrices of dask_ml/preprocessing/label.py and _encoders.py) --------
+ * Element types of X: BKM_F32, BKM_F64, BKM_BF16, BKM_M_I32, BKM_M_I64, BKM_M_U8 (bool and uint8).  Every value has an
+ * order-preserving 64-bit key: floats the radix key of bkm_quantile_hist_chunk with -0.0 folded to +0.0 and every NaN
+ * mapped to the key of the canonical quiet NaN (so NaN is one key, the largest); int32 / int64 the value with its sign
+ * bit flipped; uint8 the value.
+ *   bkm_distinct_chunk   per column j of a group of g columns, every distinct key, in an open-addressing table of the
+ *                        layout of bkm_mode_count_chunk: keys / counts [total_slots] uint64, column j owning slots
+ *                        [slot_off[j], slot_off[j + 1]) (a power of two), empty slots ~0, count 1 for a present key (so
+ *                        bkm_mode_compact, bkm_mode_merge and bkm_mode_best's distinct count apply unchanged).
+ *                        state [2][g] uint64: [occupied slots | status bits]; status 1 = OVERFLOW (the occupancy passed
+ *                        half the capacity or a probe chain passed 1024 slots: the column's table is incomplete, grow it
+ *                        and run the group again), 2 = MARKER (the column holds the key ~0, i.e. INT64_MAX, which the
+ *                        tables cannot store).  With BKM_FLAG_FIRST_CHUNK the tables and state are reset first, else
+ *                        ACCUMULATED.  X + j0 with ldx runs a column group as a view.
+ *   bkm_encode_chunk     cat_keys [n_cats] uint64: column j's sorted keys at [cat_off[j], cat_off[j + 1]) (cat_off [d + 1]
+ *                        int64, device).  The code of x[i, j] is the position of its key in its column's list.
+ *                        layout CODES: out [n][ld_out >= d] int64 codes (-1 for an unknown key; out_dtype ignored).
+ *                        layout DENSE: out [n][n_cats] (ld_out == n_cats, 16-byte aligned) in out_dtype (BKM_F64,
+ *                        BKM_F32, BKM_M_I64, BKM_M_I32, BKM_M_U8): 1 at column cat_off[j] + code of every j, 0 elsewhere,
+ *                        every element written once; d <= 2048.  layout CSR: indices [n d] int64 = cat_off[j] + code
+ *                        (-1 for an unknown key) at i d + j, out [n d] ones in out_dtype.  unknown [1 + d + d
+ *                        BKM_ENCODE_KEEP] uint64 (+)= [elements with an unknown key | per column: their count | per
+ *                        column: up to BKM_ENCODE_KEEP of their keys, in no particular order]; the caller zeroes it.
+ *   bkm_decode_chunk     codes [n][ldc] int32 / int64 (BKM_M_I32 / BKM_M_I64) -> out [n][ld_out] elements of elem_bytes
+ *                        (1, 2, 4, 8): out[i, j] = cat_vals[cat_off[j] + codes[i, j]]; a code outside [0, K_j) writes
+ *                        zero bytes and adds to unknown (as above, the code kept as the key). */
+#define BKM_ENCODE_CODES 0
+#define BKM_ENCODE_DENSE 1
+#define BKM_ENCODE_CSR   2
+#define BKM_ENCODE_KEEP  8
+int bkm_distinct_chunk(const void* X, int64_t n, int g, int64_t ldx, int x_dtype, unsigned long long* keys,
+                       unsigned long long* counts, const int64_t* slot_off, int64_t total_slots, unsigned long long* state,
+                       int flags, void* stream);
+int bkm_encode_chunk(const void* X, int64_t n, int d, int64_t ldx, int x_dtype, const unsigned long long* cat_keys,
+                     const int64_t* cat_off, int64_t n_cats, int layout, void* out, int64_t ld_out, int out_dtype,
+                     int64_t* indices, unsigned long long* unknown, void* stream);
+int bkm_decode_chunk(const void* codes, int64_t n, int d, int64_t ldc, int code_dtype, const void* cat_vals,
+                     const int64_t* cat_off, int elem_bytes, void* out, int64_t ld_out, unsigned long long* unknown,
+                     void* stream);
 
 /* ---- NaN/inf scan of a chunk (k_means.py:179-180): sets *flag (int32) nonzero -------- */
 int bkm_check_finite(const void* X, int64_t n, int d, int64_t ldx, int x_dtype,
