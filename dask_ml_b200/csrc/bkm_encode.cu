@@ -1,14 +1,6 @@
-// bkm_encode.cu — the passes of LabelEncoder and OneHotEncoder over row chunks (sm_90a).
+// bkm_encode.cu — the passes of LabelEncoder and OneHotEncoder over row chunks (sm_90a).  The categories come from the
+// per-column key tables of bkm_keys.cu (bkm_distinct_chunk).
 //
-//   bkm_distinct_chunk   per column of a group, every distinct value's order-preserving 64-bit key in an
-//                        open-addressing table (the layout of the mode tables of bkm_impute.cu, so that
-//                        bkm_mode_compact / bkm_mode_merge / bkm_mode_best serve it unchanged).  Tables start small: a
-//                        column whose occupancy passes half its capacity, or whose probe chain passes kMaxProbe, is
-//                        flagged and the host grows it and runs the group again.  A CTA stages 256 rows x one 32-byte
-//                        sector of columns in shared memory; a warp takes 32 values of one column, lanes with equal keys
-//                        merge through __match_any_sync, and the leader looks the key up in a per-CTA, per-column
-//                        direct-mapped cache of keys already in the table (shared memory) before it probes global
-//                        memory: a column of few distinct values costs about one global lookup per value per CTA.
 //   bkm_encode_chunk     one read of X: each element's key is looked up by binary search in its column's sorted key
 //                        list (staged in shared memory when every list fits, else read through L2) and written as a
 //                        code (CODES), a CSR index and one (CSR), or a one-hot row (DENSE: the CTA's tile of rows is
@@ -22,140 +14,8 @@
 namespace bkm {
 namespace {
 
-constexpr int kMaxProbe = 1024;          // probe chain bound of the distinct tables
-constexpr int kFilterSlots = 4096;       // per CTA, shared between the columns of a sector
 constexpr int kDenseRowsMax = 256;       // rows per tile of the one-hot writer
 constexpr int kPosInts = 2048;           // the tile's positions (rows x d ints) in shared memory
-
-// ---- the keys: order-preserving, -0.0 folded to +0.0, every NaN one key (the canonical quiet NaN's, the largest) ----
-__device__ __forceinline__ unsigned long long enc_key(float v) {
-  if (v != v) return 0xFFC00000ull;
-  return v == 0.0f ? 0x80000000ull : radix_key(v);
-}
-__device__ __forceinline__ unsigned long long enc_key(double v) {
-  if (v != v) return 0xFFF8000000000000ull;
-  return v == 0.0 ? 0x8000000000000000ull : radix_key(v);
-}
-__device__ __forceinline__ unsigned long long enc_key(__nv_bfloat16 v) {
-  if (__hisnan(v)) return 0xFFC0ull;
-  return __bfloat162float(v) == 0.0f ? 0x8000ull : radix_key(v);
-}
-__device__ __forceinline__ unsigned long long enc_key(int v) { return (unsigned long long)((unsigned)v ^ 0x80000000u); }
-__device__ __forceinline__ unsigned long long enc_key(long long v) {
-  return (unsigned long long)v ^ 0x8000000000000000ull;
-}
-__device__ __forceinline__ unsigned long long enc_key(unsigned char v) { return (unsigned long long)v; }
-
-static bool enc_dtype_ok(int t) {
-  return t == BKM_F32 || t == BKM_F64 || t == BKM_BF16 || t == BKM_M_I32 || t == BKM_M_I64 || t == BKM_M_U8;
-}
-
-// ============================================ distinct keys ============================================
-enum { ST_OVERFLOW = 1, ST_MARKER = 2 };
-
-struct DistinctArgs {
-  const void* X;
-  long long n;
-  int g;
-  long long ldx;
-  unsigned long long* keys;
-  unsigned long long* counts;
-  const long long* off;
-  unsigned long long* occupied;    // [g]
-  unsigned long long* status;      // [g]
-};
-
-// true when `key` is in (or was added to) the table; false when the column overflowed
-__device__ __forceinline__ bool table_insert(const DistinctArgs& a, int j, long long o, long long cap,
-                                             unsigned long long key) {
-  unsigned long long* keys = a.keys + o;
-  unsigned long long h = mix64(key) & (unsigned long long)(cap - 1);
-  const int bound = cap < kMaxProbe ? (int)cap : kMaxProbe;
-  for (int p = 0; p < bound; ++p) {
-    unsigned long long cur = __ldcg(keys + h);
-    if (cur == kEmpty) {
-      cur = atomicCAS(keys + h, kEmpty, key);
-      if (cur == kEmpty) {
-        a.counts[o + h] = 1ull;
-        const unsigned long long occ = atomicAdd(a.occupied + j, 1ull) + 1ull;
-        if (2 * occ > (unsigned long long)cap) atomicOr(a.status + j, (unsigned long long)ST_OVERFLOW);
-        return true;
-      }
-    }
-    if (cur == key) return true;
-    h = (h + 1) & (unsigned long long)(cap - 1);
-  }
-  atomicOr(a.status + j, (unsigned long long)ST_OVERFLOW);
-  return false;
-}
-
-template <typename T>
-__global__ void __launch_bounds__(kThreads) distinct_kernel(DistinctArgs a) {
-  constexpr int CS = 32 / sizeof(T);                         // columns per CTA: one 32-byte sector of a row
-  constexpr int FS = kFilterSlots / CS;                      // cache slots per column
-  __shared__ T s_tile[kTileRows * CS];
-  __shared__ unsigned long long s_filter[kFilterSlots];
-  __shared__ long long s_off[CS + 1];
-  const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
-  const T* X = reinterpret_cast<const T*>(a.X);
-  const long long tiles = (a.n + kTileRows - 1) / kTileRows;
-  const long long per = (tiles + gridDim.x - 1) / gridDim.x;
-  const long long tb = (long long)blockIdx.x * per, te = min(tiles, tb + per);
-#pragma unroll 1
-  for (int jb = blockIdx.y * CS; jb < a.g; jb += gridDim.y * CS) {
-    const int nc = min(CS, a.g - jb);
-    __syncthreads();
-    if (tid <= CS) s_off[tid] = a.off[min(jb + tid, a.g)];
-    for (int e = tid; e < kFilterSlots; e += kThreads) s_filter[e] = kEmpty;
-#pragma unroll 1
-    for (long long t = tb; t < te; ++t) {
-      const long long r0 = t * kTileRows;
-      __syncthreads();
-      for (int e = tid; e < kTileRows * CS; e += kThreads) {
-        const int r = e / CS, c = e - r * CS;
-        if (r0 + r < a.n && c < nc) s_tile[e] = X[(r0 + r) * a.ldx + jb + c];
-      }
-      __syncthreads();
-      // tasks: (column c, 32 rows), warp-uniform
-      for (int task = w; task < CS * (kTileRows / 32); task += kThreads / 32) {
-        const int c = task % CS, rs = (task / CS) * 32;
-        if (c >= nc) continue;
-        const int j = jb + c;
-        const long long o = s_off[c], cap = s_off[c + 1] - o;
-        unsigned long long st = lane == 0 ? __ldcg(a.status + j) : 0ull;
-        st = __shfl_sync(0xffffffffu, st, 0);
-        if (cap == 0 || (st & ST_OVERFLOW)) continue;                       // this group runs again
-        const bool ok = r0 + rs + lane < a.n;
-        const unsigned act = __ballot_sync(0xffffffffu, ok);
-        if (!ok) continue;
-        const unsigned long long key = enc_key(s_tile[(rs + lane) * CS + c]);
-        const unsigned peers = __match_any_sync(act, key);
-        if ((peers & ((1u << lane) - 1u)) != 0u) continue;
-        if (key == kEmpty) {                                 // INT64_MAX: the table's empty marker, kept as a flag
-          if (!(__ldcg(a.status + j) & ST_MARKER)) atomicOr(a.status + j, (unsigned long long)ST_MARKER);
-          continue;
-        }
-        volatile unsigned long long* slot = s_filter + c * FS + (int)((mix64(key) >> 40) & (FS - 1));
-        if (*slot == key) continue;
-        if (table_insert(a, j, o, cap, key)) *slot = key;
-      }
-    }
-  }
-}
-
-template <typename T>
-static int launch_distinct(const DistinctArgs& a, int sms, cudaStream_t s) {
-  constexpr int CS = 32 / sizeof(T);
-  const int gy = (a.g + CS - 1) / CS < 65535 ? (a.g + CS - 1) / CS : 65535;
-  const long long tiles = (a.n + kTileRows - 1) / kTileRows;
-  long long gx = ((long long)8 * sms + gy - 1) / gy;
-  if (gx > tiles) gx = tiles;
-  if (gx < 1) gx = 1;
-  distinct_kernel<T><<<dim3((unsigned)gx, (unsigned)gy), kThreads, 0, s>>>(a);
-  BKM_CUDA_TRY(cudaGetLastError());
-  note_launch();
-  return 0;
-}
 
 // ============================================ encode ============================================
 struct EncodeArgs {
@@ -341,38 +201,6 @@ __global__ void __launch_bounds__(kThreads) decode_kernel(DecodeArgs a) {
 }  // namespace bkm
 
 using namespace bkm;
-
-extern "C" int bkm_distinct_chunk(const void* X, int64_t n, int g, int64_t ldx, int x_dtype, unsigned long long* keys,
-                                  unsigned long long* counts, const int64_t* slot_off, int64_t total_slots,
-                                  unsigned long long* state, int flags, void* stream) {
-  if (n < 0 || g <= 0 || ldx < g || total_slots < 0 || !slot_off || !state) return BKM_EINVAL;
-  if (total_slots > 0 && (!keys || !counts)) return BKM_EINVAL;
-  if (n > 0 && !X) return BKM_EINVAL;
-  if (!enc_dtype_ok(x_dtype)) return BKM_EDTYPE;
-  cudaStream_t s = (cudaStream_t)stream;
-  if (flags & BKM_FLAG_FIRST_CHUNK) {
-    if (total_slots > 0) {
-      BKM_CUDA_TRY(cudaMemsetAsync(keys, 0xff, (size_t)total_slots * 8, s));
-      BKM_CUDA_TRY(cudaMemsetAsync(counts, 0, (size_t)total_slots * 8, s));
-    }
-    BKM_CUDA_TRY(cudaMemsetAsync(state, 0, (size_t)g * 16, s));
-  }
-  if (n == 0 || total_slots == 0) return 0;
-  int sms = 0;
-  const int rc = sm_count(&sms);
-  if (rc) return rc;
-  DistinctArgs a;
-  a.X = X; a.n = n; a.g = g; a.ldx = ldx; a.keys = keys; a.counts = counts;
-  a.off = reinterpret_cast<const long long*>(slot_off); a.occupied = state; a.status = state + g;
-  switch (x_dtype) {
-    case BKM_F32: return launch_distinct<float>(a, sms, s);
-    case BKM_F64: return launch_distinct<double>(a, sms, s);
-    case BKM_BF16: return launch_distinct<__nv_bfloat16>(a, sms, s);
-    case BKM_M_I32: return launch_distinct<int>(a, sms, s);
-    case BKM_M_I64: return launch_distinct<long long>(a, sms, s);
-    default: return launch_distinct<unsigned char>(a, sms, s);
-  }
-}
 
 extern "C" int bkm_encode_chunk(const void* X, int64_t n, int d, int64_t ldx, int x_dtype,
                                 const unsigned long long* cat_keys, const int64_t* cat_off, int64_t n_cats, int layout,

@@ -32,6 +32,7 @@ from sklearn.utils._mask import _get_mask
 from sklearn.utils._missing import is_pandas_na, is_scalar_nan
 from sklearn.utils.validation import check_is_fitted
 
+from . import _keytables
 from .chunked import ChunkedArray
 from .decomposition.pca import SHIFT_ROWS, _device_data, _on_rank0
 from .preprocessing.data import keys_to_values, order_statistics
@@ -39,18 +40,10 @@ from .preprocessing.data import keys_to_values, order_statistics
 STRATEGIES = ["mean", "median", "most_frequent", "constant"]
 MODE_BUDGET = 1 << 30        # bytes of one column group's hash tables (plus, with several ranks, its gathered lists):
                              # wider data runs in column groups, each of which reads its columns of X once
-_KEY_BITS = {torch.bfloat16: 16, torch.float32: 32, torch.float64: 64}
 
 
 def _missing_is_nan(missing_values):
     return is_scalar_nan(missing_values) or is_pandas_na(missing_values)
-
-
-def _table_slots(m, dtype):
-    """Hash table capacity for a column that receives ``m`` values: a power of two >= twice the distinct values it can
-    hold (at most 2^16 for bf16 rows), 0 for none."""
-    m = min(int(m), 1 << _KEY_BITS[dtype])
-    return 0 if m <= 0 else 1 << (2 * m - 1).bit_length()
 
 
 def _shift(X, miss_is_nan, miss):
@@ -87,7 +80,7 @@ def mode_statistics(X, miss_is_nan, miss, local_valid, global_valid):
     for a zero), NaN for a column without one: float64 numpy."""
     be, comm, d = X.backend, X.comm, X.d
     world = comm.world
-    cost = [16 * _table_slots(m, X.dtype) + (32 * int(m) if world > 1 else 0) for m in global_valid]
+    cost = [16 * _keytables.capacity(m, X.dtype) + (32 * int(m) if world > 1 else 0) for m in global_valid]
     groups, j0 = [], 0
     while j0 < d:                        # identical on every rank: the costs come from global counts
         j1, used = j0 + 1, cost[j0]
@@ -99,33 +92,15 @@ def mode_statistics(X, miss_is_nan, miss, local_valid, global_valid):
     best_key = np.zeros(d, dtype=np.uint64)
     best_cnt = np.zeros(d)
 
-    def tables(caps):
-        off = np.concatenate([[0], np.cumsum(caps)]).astype(np.int64)
-        total = int(off[-1])
-        keys = be.empty((max(total, 1),), torch.int64)
-        counts = be.empty((max(total, 1),), torch.int64)
-        return keys, counts, torch.as_tensor(off).to(be.device), total
-
     for j0, j1 in groups:
         g = j1 - j0
-        keys, counts, off, total = tables([_table_slots(m, X.dtype) for m in local_valid[j0:j1]])
+        tables = _keytables.alloc(be, [_keytables.capacity(m, X.dtype) for m in local_valid[j0:j1]])
+        keys, counts, off, total = tables
         for i, x in enumerate(X.chunks):
             be.mode_count_chunk(x[:, j0:j1], miss_is_nan, miss, keys, counts, off, total, first=i == 0)
         key, cnt, nd = be.mode_best(keys, counts, off, g, total)
         if world > 1:
-            lens = be.zeros((world, g), torch.float64)
-            lens[comm.rank] = nd
-            comm.allreduce_sum_(lens.view(-1))
-            L = lens.cpu().numpy()
-            per_rank = L.sum(1).astype(np.int64)
-            start, E = int(per_rank[: comm.rank].sum()), int(per_rank.sum())
-            entries = be.zeros((max(E, 1), 4), torch.float64)
-            if per_rank[comm.rank] > 0:
-                be.mode_compact(keys, counts, off, g, entries[start: start + int(per_rank[comm.rank])])
-            comm.allreduce_sum_(entries.view(-1))     # every rank's slice, exact: integers below 2^53
-            keys, counts, off, total = tables([_table_slots(m, X.dtype) for m in L.sum(0)])
-            be.mode_merge(entries[:E], keys, counts, off, g, total)
-            key, cnt, nd = be.mode_best(keys, counts, off, g, total)
+            _, (key, cnt, nd), _ = _keytables.merge_ranks(be, comm, tables, g, X.dtype, nd)
         best_key[j0:j1] = key.cpu().numpy().view(np.uint64)
         best_cnt[j0:j1] = cnt.cpu().numpy()
     vals = np.asarray(keys_to_values(best_key, X.dtype), dtype=np.float64)

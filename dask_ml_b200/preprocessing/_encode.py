@@ -18,7 +18,7 @@ float32 by torch before the pass (exact); the categories are mapped back to the 
 import numpy as np
 import torch
 
-from .. import _lib
+from .. import _keytables, _lib
 from ..chunked import ChunkedArray, _is_torch, block_dtype, is_dask_dataframe
 from ..cluster import k_means as _km
 from ..engine import DeviceData
@@ -33,8 +33,6 @@ _NATIVE = (torch.float32, torch.float64, torch.bfloat16, torch.int32, torch.int6
 _WIDEN = {torch.int8: torch.int32, torch.int16: torch.int32, torch.float16: torch.float32}
 _NP_WIDEN = {np.dtype("int8"): torch.int32, np.dtype("int16"): torch.int32, np.dtype("uint16"): torch.int32,
              np.dtype("uint32"): torch.int64, np.dtype("float16"): torch.float32}
-_KEY_BITS = {torch.bfloat16: 16, torch.float32: 32, torch.float64: 64, torch.int32: 32, torch.int64: 64,
-             torch.uint8: 8, torch.bool: 1}
 _NAN_KEY = {torch.bfloat16: 0xFFC0, torch.float32: 0xFFC00000, torch.float64: 0xFFF8000000000000}
 _I64_MIN = -(1 << 63)
 
@@ -124,7 +122,7 @@ def host_keys(values, tdt):
             u = f.view(np.uint32).astype(np.uint64)
         else:
             u = (f.view(np.uint32) >> np.uint32(16)).astype(np.uint64)
-        bits = _KEY_BITS[tdt]
+        bits = _keytables.KEY_BITS[tdt]
         sign = np.uint64(1 << (bits - 1))
         mask = np.uint64((1 << bits) - 1) if bits < 64 else np.uint64(0xFFFFFFFFFFFFFFFF)
         k = np.where(u & sign, ~u & mask, u | sign)
@@ -151,23 +149,6 @@ def key_values(keys, tdt, hdt):
     return vals.astype(hdt)
 
 
-def _pow2(m):
-    return 1 << max(1, (int(m) - 1).bit_length())
-
-
-def _limit(rows, tdt):
-    """A table capacity that cannot overflow: a power of two >= twice the values the column can hold."""
-    return _pow2(2 * max(1, min(int(rows), 1 << _KEY_BITS[tdt])))
-
-
-def _tables(be, caps):
-    off = np.concatenate([[0], np.cumsum(caps)]).astype(np.int64)
-    total = int(off[-1])
-    keys = be.empty((max(total, 1),), torch.int64)
-    counts = be.empty((max(total, 1),), torch.int64)
-    return keys, counts, torch.as_tensor(off).to(be.device), total
-
-
 def _entry_keys(entries):
     """(column, key int64 holding the uint64 key) of compacted rows {column, key >> 32, key & 0xffffffff, count}."""
     e = entries.to(torch.int64)
@@ -178,10 +159,10 @@ def _group_keys(X, j0, j1):
     """Every distinct key of columns [j0, j1) over every rank: (column within the group, key) int64 device tensors,
     unsorted."""
     be, comm, g = X.backend, X.comm, j1 - j0
-    limit = _limit(X.n_local, X.dtype)
+    limit = _keytables.capacity(max(1, X.n_local), X.dtype)         # a table that cannot overflow
     caps = np.full(g, min(INITIAL_SLOTS, limit), dtype=np.int64)
     while True:
-        keys, counts, off, total = _tables(be, caps)
+        keys, counts, off, total = _keytables.alloc(be, caps)
         state = be.zeros((2, g), torch.int64)
         for i, x in enumerate(X.chunks):
             be.distinct_chunk(x[:, j0:j1], keys, counts, off, total, state, first=i == 0)
@@ -192,22 +173,9 @@ def _group_keys(X, j0, j1):
         caps[over] = np.where(caps[over] < limit, np.minimum(caps[over] * GROWTH, limit), caps[over] * 2)
     occupied, marker = st[0], (st[1] & 2) != 0
     if comm.world > 1:
-        lens = be.zeros((comm.world, 2 * g), torch.float64)
-        lens[comm.rank, :g] = torch.as_tensor(occupied, dtype=torch.float64)
-        lens[comm.rank, g:] = torch.as_tensor(marker, dtype=torch.float64)
-        comm.allreduce_sum_(lens.view(-1))
-        L = lens.cpu().numpy()
-        per_rank = L[:, :g].sum(1).astype(np.int64)
-        start, E = int(per_rank[: comm.rank].sum()), int(per_rank.sum())
-        entries = be.zeros((max(E, 1), 4), torch.float64)
-        if per_rank[comm.rank] > 0:
-            be.mode_compact(keys, counts, off, g, entries[start: start + int(per_rank[comm.rank])])
-        comm.allreduce_sum_(entries.view(-1))      # every rank's slice, exact: integers below 2^53
-        merged = [0 if m == 0 else _pow2(2 * m) for m in L[:, :g].sum(0)]
-        keys, counts, off, total = _tables(be, merged)
-        be.mode_merge(entries[:E], keys, counts, off, g, total)
-        nd = be.mode_best(keys, counts, off, g, total)[2]
-        occupied, marker = nd.cpu().numpy().astype(np.int64), L[:, g:].sum(0) > 0
+        (keys, counts, off, total), (_, _, nd), marker = _keytables.merge_ranks(
+            be, comm, (keys, counts, off, total), g, X.dtype, occupied, marker)
+        occupied = nd.cpu().numpy().astype(np.int64)
     E = int(occupied.sum())
     entries = be.zeros((max(E, 1), 4), torch.float64)
     if E:
@@ -224,7 +192,7 @@ def fit_keys(X):
     """(cat_keys, counts): every column's sorted distinct keys, concatenated (int64 device tensor holding uint64 keys),
     and the number of categories of every column (numpy int64).  Identical on every rank."""
     be, d = X.backend, X.d
-    per_col = 16 * min(INITIAL_SLOTS, _limit(X.n_local, X.dtype))
+    per_col = 16 * min(INITIAL_SLOTS, _keytables.capacity(max(1, X.n_local), X.dtype))
     step = max(1, ENCODE_BUDGET // per_col)      # the same on every rank: columns are grouped by the first tables
     cols, keys = [], []
     for j0 in range(0, d, step):

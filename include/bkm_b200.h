@@ -497,6 +497,32 @@ int bkm_metric_chunk(const void* a, int a_dtype, const void* b, int b_dtype, con
                      int mode, const double* shift, double eps, double* acc, void* workspace, size_t ws_bytes,
                      int flags, void* stream);
 
+/* ---- Per-column key tables: SimpleImputer's most-frequent counts and the encoders' categories ------------------------
+ * A group of g columns owns keys / counts [total_slots] uint64, column j owning slots [slot_off[j], slot_off[j + 1])
+ * (slot_off [g + 1] int64, device), a power of two (or zero).  Empty slots hold the key ~0 (a NaN pattern).  X + j0
+ * with ldx runs a column group as a view.  Every value has an order-preserving 64-bit key: floats the radix key of
+ * bkm_quantile_hist_chunk (16, 32 or 64 bits in a uint64) with -0.0 folded to +0.0 and every NaN mapped to the key of
+ * the canonical quiet NaN (so NaN is one key, the largest); int32 / int64 the value with its sign bit flipped; uint8 the
+ * value.  The tables are filled by bkm_mode_count_chunk (SimpleImputer) and bkm_distinct_chunk (the encoders); a
+ * table's content is a set of keys with integer counts.
+ *   bkm_mode_best        per column: best_key [g] uint64 and best_count [g] float64 of the entry of largest count, the
+ *                        smallest key among equal counts (count 0: no value), and distinct [g] float64 the number of
+ *                        occupied slots.  The order is total: the result does not depend on the table layout.  Several
+ *                        CTAs share a column's table (slices, then a fold of their partials).  workspace:
+ *                        bkm_mode_best_workspace_bytes(g, total_slots) bytes, any content.
+ *   bkm_mode_compact     every occupied slot as a row of entries [*][4] float64 {column, key >> 32, key & 0xffffffff,
+ *                        count}, rows in no particular order; *cursor (uint64, device) ends at the number of rows.
+ *   bkm_mode_merge       resets the tables, then adds every row of entries [n_entries][4] with count > 0 to its
+ *                        column's table (rows with count 0 are skipped: the zero padding of gathered slices). */
+int bkm_mode_best_workspace_bytes(int g, int64_t total_slots, size_t* out);
+int bkm_mode_best(const unsigned long long* keys, const unsigned long long* counts, const int64_t* slot_off, int g,
+                  int64_t total_slots, unsigned long long* best_key, double* best_count, double* distinct,
+                  void* workspace, size_t ws_bytes, void* stream);
+int bkm_mode_compact(const unsigned long long* keys, const unsigned long long* counts, const int64_t* slot_off, int g,
+                     double* entries, unsigned long long* cursor, void* stream);
+int bkm_mode_merge(const double* entries, int64_t n_entries, unsigned long long* keys, unsigned long long* counts,
+                   const int64_t* slot_off, int g, int64_t total_slots, void* stream);
+
 /* ---- SimpleImputer: the fit statistics and the fill pass over row chunks (replace scikit-learn's _dense_fit, transform
  * and inverse_transform, which dask_ml/impute.py calls for numpy input) -------------------------------------------------
  * The missing value is passed as (miss_is_nan, miss_value): NaN when miss_is_nan = 1 (miss_value is then ignored, NaN
@@ -510,22 +536,10 @@ int bkm_metric_chunk(const void* a, int a_dtype, const void* b, int b_dtype, con
  *                        not NaN), so that the select step's nvalid is the non-missing count.  Same state, rounds and
  *                        bkm_quantile_select_step.
  *   bkm_mode_count_chunk     per column j of a group of g columns, the count of every distinct non-missing, non-NaN
- *                        value, by its order-preserving key (the keys of bkm_quantile_hist_chunk: 16, 32 or 64 bits in a
- *                        uint64, -0.0 counted as +0.0), in an open-addressing table: keys / counts [total_slots] uint64,
- *                        column j owning slots [slot_off[j], slot_off[j + 1]) (slot_off [g + 1] int64, device), a power of
- *                        two (or zero) at least twice the values the column can receive, so that no table fills.  Empty
- *                        slots hold the key ~0 (a NaN pattern).  With BKM_FLAG_FIRST_CHUNK the tables are reset first,
- *                        else counts are ACCUMULATED.  Counts are integers: exact in any order.  X + j0 with ldx runs
- *                        a column group as a view.
- *   bkm_mode_best        per column: best_key [g] uint64 and best_count [g] float64 of the entry of largest count, the
- *                        smallest key among equal counts (count 0: no value), and distinct [g] float64 the number of
- *                        occupied slots.  The order is total: the result does not depend on the table layout.  Several
- *                        CTAs share a column's table (slices, then a fold of their partials).  workspace:
- *                        bkm_mode_best_workspace_bytes(g, total_slots) bytes, any content.
- *   bkm_mode_compact     every occupied slot as a row of entries [*][4] float64 {column, key >> 32, key & 0xffffffff,
- *                        count}, rows in no particular order; *cursor (uint64, device) ends at the number of rows.
- *   bkm_mode_merge       resets the tables, then adds every row of entries [n_entries][4] with count > 0 to its
- *                        column's table (rows with count 0 are skipped: the zero padding of gathered slices).
+ *                        value, by its key, in the per-column key tables (above), each a power of two (or zero) at least
+ *                        twice the values the column can receive, so that no table fills.  With BKM_FLAG_FIRST_CHUNK
+ *                        the tables are reset first, else counts are ACCUMULATED.  Counts are integers: exact in any
+ *                        order.  The best entry, compaction and multi-rank merge are bkm_mode_best / _compact / _merge.
  *   bkm_impute_chunk     forward (inverse 0): out [n][ld_out] in out_dtype (X's dtype; BKM_F32 for bf16 rows), columns
  *                        o < n_keep: x[:, cols[o]] with its missing elements replaced by (out_dtype)stats[cols[o]];
  *                        then n_ind indicator columns: 1 where x[:, cols[o]] is missing, else 0; then n_check input
@@ -542,33 +556,21 @@ int bkm_quantile_hist_masked_chunk(const void* X, int64_t n, int d, int64_t ldx,
 int bkm_mode_count_chunk(const void* X, int64_t n, int g, int64_t ldx, int x_dtype, int miss_is_nan, double miss_value,
                          unsigned long long* keys, unsigned long long* counts, const int64_t* slot_off,
                          int64_t total_slots, int flags, void* stream);
-int bkm_mode_best_workspace_bytes(int g, int64_t total_slots, size_t* out);
-int bkm_mode_best(const unsigned long long* keys, const unsigned long long* counts, const int64_t* slot_off, int g,
-                  int64_t total_slots, unsigned long long* best_key, double* best_count, double* distinct,
-                  void* workspace, size_t ws_bytes, void* stream);
-int bkm_mode_compact(const unsigned long long* keys, const unsigned long long* counts, const int64_t* slot_off, int g,
-                     double* entries, unsigned long long* cursor, void* stream);
-int bkm_mode_merge(const double* entries, int64_t n_entries, unsigned long long* keys, unsigned long long* counts,
-                   const int64_t* slot_off, int g, int64_t total_slots, void* stream);
 int bkm_impute_chunk(const void* X, int64_t n, int d, int64_t ldx, int x_dtype, int miss_is_nan, double miss_value,
                      const double* stats, const int* cols, int n_keep, int n_ind, int n_check, int inverse, void* out,
                      int64_t ld_out, int out_dtype, double* invalid, void* stream);
 
 /* ---- LabelEncoder / OneHotEncoder: the categories of every column and the encoding passes (replace da.unique,
  * np.searchsorted and the per-block sparse one-hot matrices of dask_ml/preprocessing/label.py and _encoders.py) --------
- * Element types of X: BKM_F32, BKM_F64, BKM_BF16, BKM_M_I32, BKM_M_I64, BKM_M_U8 (bool and uint8).  Every value has an
- * order-preserving 64-bit key: floats the radix key of bkm_quantile_hist_chunk with -0.0 folded to +0.0 and every NaN
- * mapped to the key of the canonical quiet NaN (so NaN is one key, the largest); int32 / int64 the value with its sign
- * bit flipped; uint8 the value.
- *   bkm_distinct_chunk   per column j of a group of g columns, every distinct key, in an open-addressing table of the
- *                        layout of bkm_mode_count_chunk: keys / counts [total_slots] uint64, column j owning slots
- *                        [slot_off[j], slot_off[j + 1]) (a power of two), empty slots ~0, count 1 for a present key (so
- *                        bkm_mode_compact, bkm_mode_merge and bkm_mode_best's distinct count apply unchanged).
+ * Element types of X: BKM_F32, BKM_F64, BKM_BF16, BKM_M_I32, BKM_M_I64, BKM_M_U8 (bool and uint8).  Values are
+ * compared by their keys (the per-column key tables, above).
+ *   bkm_distinct_chunk   per column j of a group of g columns, every distinct key, count 1, in the per-column key
+ *                        tables (above); bkm_mode_compact, bkm_mode_merge and bkm_mode_best's distinct count read them.
  *                        state [2][g] uint64: [occupied slots | status bits]; status 1 = OVERFLOW (the occupancy passed
  *                        half the capacity or a probe chain passed 1024 slots: the column's table is incomplete, grow it
  *                        and run the group again), 2 = MARKER (the column holds the key ~0, i.e. INT64_MAX, which the
  *                        tables cannot store).  With BKM_FLAG_FIRST_CHUNK the tables and state are reset first, else
- *                        ACCUMULATED.  X + j0 with ldx runs a column group as a view.
+ *                        ACCUMULATED.
  *   bkm_encode_chunk     cat_keys [n_cats] uint64: column j's sorted keys at [cat_off[j], cat_off[j + 1]) (cat_off [d + 1]
  *                        int64, device).  The code of x[i, j] is the position of its key in its column's list.
  *                        layout CODES: out [n][ld_out >= d] int64 codes (-1 for an unknown key; out_dtype ignored).

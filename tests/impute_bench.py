@@ -59,7 +59,7 @@ def main():
     assert torch.cuda.is_available(), "impute_bench needs a GPU"
     from dask_ml_b200.engine import DeviceData
     from dask_ml_b200.cluster import k_means as km
-    from dask_ml_b200 import impute
+    from dask_ml_b200 import _keytables, impute
 
     name = torch.cuda.get_device_name()
     try:
@@ -106,7 +106,7 @@ def main():
             else:
                 Y = X
             yd = DeviceData([Y[i:i + (1 << 21)] for i in range(0, n, 1 << 21)], be)
-            cost = [16 * impute._table_slots(m, dt) for m in valid]
+            cost = [16 * _keytables.capacity(m, dt) for m in valid]
             gw, used = 1, cost[0]
             while gw < d and used + cost[gw] <= impute.MODE_BUDGET:
                 used += cost[gw]

@@ -257,19 +257,20 @@ def test_one_category_and_empty_blocks(cpu_backend):
     np.testing.assert_array_equal(le.classes_, [3])
 
 
-def test_table_growth(cpu_backend, monkeypatch):
+def test_table_growth_steps(cpu_backend, monkeypatch):
+    from dask_ml_b200 import _keytables
     from dask_ml_b200.preprocessing import _encode
 
     X = np.stack([np.arange(3000) % 1500, np.arange(3000) % 3], axis=1).astype(np.int64)
     calls = []
-    grow = _encode._tables
+    grow = _keytables.alloc
 
     def tables(be, caps):
         calls.append(list(caps))
         return grow(be, caps)
 
     monkeypatch.setattr(_encode, "INITIAL_SLOTS", 4)
-    monkeypatch.setattr(_encode, "_tables", tables)
+    monkeypatch.setattr(_keytables, "alloc", tables)
     check_onehot(X, 700)
     # x8 per step: the 3-value column grows once (4 -> 32), the 1500-value one up to its cap (2 x 3000 rows -> 8192)
     assert calls[:5] == [[4, 4], [32, 32], [256, 32], [2048, 32], [8192, 32]]

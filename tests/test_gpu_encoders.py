@@ -135,6 +135,52 @@ def test_growth_many_distinct():
     np.testing.assert_array_equal(codes, np.searchsorted(le.classes_, y))
 
 
+def _table_entries(be, keys, counts, off, g, rows):
+    """{(column, key): count} of the occupied slots of the tables (at most ``rows`` of them)."""
+    e = be.zeros((rows, 4), torch.float64)
+    be.mode_compact(keys, counts, off, g, e)
+    e = e.cpu().numpy()
+    return {(int(c), (int(hi) << 32) | int(lo)): int(n) for c, hi, lo, n in e[e[:, 3] > 0]}
+
+
+@pytest.mark.parametrize("dt", ["f32", "f64", "bf16"])
+def test_count_and_distinct_passes_share_keys(dt):
+    """SimpleImputer's count pass (NaN missing) and the encoders' distinct pass put the same keys in the tables for
+    the same columns of signed zeros, infinities, subnormals, NaN and repeats; the counts are torch.unique's, with
+    -0.0 counted as +0.0."""
+    from dask_ml_b200 import _keytables
+    from dask_ml_b200.cluster import k_means as km
+    from dask_ml_b200.preprocessing._encode import host_keys
+
+    tdt = DTYPES[dt]
+    tiny = float(torch.finfo(tdt).smallest_normal)
+    pool = np.array([0.0, -0.0, 1.0, -1.0, 1.5, -2.25, np.inf, -np.inf, np.nan, tiny / 2, -tiny / 2, tiny / 4, tiny])
+    rng = np.random.RandomState(7)
+    n, g = 5000, 3
+    idx = np.minimum(rng.geometric(0.25, (n, g)) - 1, len(pool) - 1)
+    idx[: len(pool)] = np.arange(len(pool))[:, None]
+    X = torch.as_tensor(pool[rng.permutation(idx)]).to(tdt).cuda()
+    be = km._get_backend()
+    keys, counts, off, total = _keytables.alloc(be, [_keytables.capacity(n, tdt)] * g)
+    be.mode_count_chunk(X, True, float("nan"), keys, counts, off, total, first=True)
+    counted = _table_entries(be, keys, counts, off, g, n * g)
+    state = be.zeros((2, g), torch.int64)
+    be.distinct_chunk(X, keys, counts, off, total, state, first=True)
+    assert not (state[1].cpu().numpy() & 1).any()
+    distinct = _table_entries(be, keys, counts, off, g, n * g)
+    want = {}
+    for j in range(g):
+        col = X[:, j].double()
+        u, c = torch.unique(col[~torch.isnan(col)], return_counts=True)
+        for k, m in zip(host_keys(u.cpu().numpy(), tdt), c.cpu().numpy()):
+            want[(j, int(k))] = want.get((j, int(k)), 0) + int(m)
+    assert counted == want
+    nan_key = int(host_keys(np.array([np.nan]), tdt)[0])
+    assert {k for k in distinct if k[1] != nan_key} == set(want)
+    assert {k for k in distinct if k[1] == nan_key} == {(j, nan_key) for j in range(g)}
+    assert set(distinct.values()) == {1}
+
+
 def test_unknown_after_multi_chunk_transform():
     from dask_ml_b200.preprocessing import LabelEncoder, OneHotEncoder
 
