@@ -26,6 +26,7 @@ ENCODE_CODES = 0
 ENCODE_DENSE = 1
 ENCODE_CSR = 2
 ENCODE_KEEP = 8
+TEXT_NORM = {None: 0, "l1": 1, "l2": 2}
 
 FLAG_FORCE_SIMT = 1
 FLAG_FORCE_TC = 2
@@ -121,6 +122,14 @@ SIGNATURES = {
                                 _int, _c_void_p, _c_void_p, _c_void_p]),
     "bkm_decode_chunk": (_int, [_c_void_p, _i64, _int, _i64, _int, _c_void_p, _c_void_p, _int, _c_void_p, _i64,
                                 _c_void_p, _c_void_p]),
+    "bkm_text_workspace_bytes": (_int, [_i64, _i64, _i64, _szp]),
+    "bkm_text_tokens_chunk": (_int, [_c_void_p, _i64, _c_void_p, _i64, _int, _int, _c_void_p, _i64, _c_void_p,
+                                     _c_void_p, _c_void_p, _c_void_p, ctypes.c_size_t, _c_void_p]),
+    "bkm_text_hash_chunk": (_int, [_c_void_p, _i64, _c_void_p, _c_void_p, _c_void_p, _i64, _i64, _i64, _int, _int,
+                                   _int, _i64, _int, _int, _int, _int, _c_void_p, _c_void_p, _c_void_p, _c_void_p,
+                                   _c_void_p, ctypes.c_size_t, _c_void_p]),
+    "bkm_text_write_chunk": (_int, [_c_void_p, _c_void_p, _c_void_p, _c_void_p, _i64, _int, _c_void_p, _c_void_p,
+                                    _int, _c_void_p]),
     "bkm_split_indices_chunk": (_int, [_u64, _i64, _i64, _i64, _i64, _c_void_p, _c_void_p]),
     "bkm_gather_rows_chunk": (_int, [_c_void_p, _i64, _i64, _i64, _c_void_p, _i64, _i64, _c_void_p, _i64, _c_void_p]),
     "bkm_metric_workspace_bytes": (_int, [_i64, _int, _int, _szp]),

@@ -714,6 +714,48 @@ class CudaBackend(object):
                 self._ptr(cat_off), cat_vals.element_size(), self._ptr(out), out.stride(0) if n else d,
                 self._ptr(unknown), self._stream()), "bkm_decode_chunk")
 
+    def _text_workspace(self, n_bytes, n_docs, n_pairs):
+        nb = ctypes.c_size_t(0)
+        _lib.check(self.lib.bkm_text_workspace_bytes(int(n_bytes), int(n_docs), int(n_pairs), ctypes.byref(nb)),
+                   "bkm_text_workspace_bytes")
+        return self._scratch("text", nb.value)
+
+    def text_tokens_chunk(self, buf, doc_off, min_n, max_n, tok_start, tok_off, pair_off, totals):
+        """HashingVectorizer's token pass over the documents packed in ``buf`` (uint8, each document ending in a byte
+        that is not a word character, document i at [doc_off[i], doc_off[i + 1])): ``tok_start`` int64 (at least
+        len(buf) // 3 + 1,) the tokens' byte positions, ``tok_off`` / ``pair_off`` int64 (n + 1,) each document's first
+        token and first n-gram of length in [min_n, max_n]; ``totals`` int64 (3,) [0:2] = the token and n-gram counts."""
+        nb, n = int(buf.numel()), int(doc_off.numel()) - 1
+        ws = self._text_workspace(nb, n, 0)
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.bkm_text_tokens_chunk(
+                self._ptr(buf), nb, self._ptr(doc_off), n, int(min_n), int(max_n), self._ptr(tok_start),
+                int(tok_start.numel()), self._ptr(tok_off), self._ptr(pair_off), self._ptr(totals), self._ptr(ws),
+                ws.numel(), self._stream()), "bkm_text_tokens_chunk")
+
+    def text_hash_chunk(self, buf, tok_start, tok_off, pair_off, n_tokens, n_pairs, min_n, max_n, lowercase,
+                        n_features, alternate_sign, binary, norm, dtype, keys, indptr, scale, totals):
+        """Hash every n-gram into ``keys`` (int32 (n_pairs,) holding uint32 2 column + negative sign, sorted per
+        document); ``indptr`` int64 (n + 1,) the CSR row offsets and ``scale`` float64 (n,) the row divisors (0: none)
+        of the output in ``dtype`` (torch float32 / float64) with ``norm`` None / 'l1' / 'l2'; totals[2] = stored
+        entries."""
+        nb, n = int(buf.numel()), int(pair_off.numel()) - 1
+        ws = self._text_workspace(nb, n, n_pairs)
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.bkm_text_hash_chunk(
+                self._ptr(buf), nb, self._ptr(tok_start), self._ptr(tok_off), self._ptr(pair_off), n, int(n_tokens),
+                int(n_pairs), int(min_n), int(max_n), int(bool(lowercase)), int(n_features), int(bool(alternate_sign)),
+                int(bool(binary)), _lib.TEXT_NORM[norm], _DT_CODE[dtype], self._ptr(keys), self._ptr(indptr),
+                self._ptr(scale), self._ptr(totals), self._ptr(ws), ws.numel(), self._stream()), "bkm_text_hash_chunk")
+
+    def text_write_chunk(self, keys, pair_off, indptr, scale, binary, indices, data):
+        """Write the CSR ``indices`` int64 and ``data`` (float32 / float64) of every stored entry."""
+        n = int(pair_off.numel()) - 1
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.bkm_text_write_chunk(
+                self._ptr(keys), self._ptr(pair_off), self._ptr(indptr), self._ptr(scale), n, int(bool(binary)),
+                self._ptr(indices), self._ptr(data), _DT_CODE[data.dtype], self._stream()), "bkm_text_write_chunk")
+
     def affine_chunk(self, x, a, b, op1, op2, out):
         """out = op2(op1(x, a), b) per element (op1: 0 none, 1 subtract a, 2 multiply by a; op2: 0 none, 1 divide by b,
         2 add b), each step rounded once in out's dtype.  ``a``, ``b`` float64 (d,) or None; ``out`` (n, d) float32 /

@@ -50,6 +50,9 @@
  *   da.unique / np.searchsorted / the sparse one-hot blocks of         bkm_distinct_chunk (+ bkm_mode_compact /
  *     LabelEncoder and OneHotEncoder, preprocessing/label.py:14-302,     bkm_mode_merge / bkm_mode_best),
  *     preprocessing/_encoders.py:18-244                                 bkm_encode_chunk, bkm_decode_chunk
+ *   sklearn HashingVectorizer.transform per block of a 1-D dask array  bkm_text_tokens_chunk +
+ *     of documents, feature_extraction/text.py:9-80 (tokenise, hash,     bkm_text_hash_chunk +
+ *     sum duplicates, binary, normalize)                                 bkm_text_write_chunk
  *
  * Conventions
  *   - extern "C", plain pointers and sizes only; no torch / C++ types.
@@ -77,8 +80,9 @@ extern "C" {
  * 1 = bkm_split_indices_chunk, bkm_gather_rows_chunk, bkm_metric_workspace_bytes, bkm_metric_chunk
  * 2 = bkm_impute_stats_workspace_bytes, bkm_impute_stats_chunk, bkm_quantile_hist_masked_chunk, bkm_mode_count_chunk,
  *     bkm_mode_best_workspace_bytes, bkm_mode_best, bkm_mode_compact, bkm_mode_merge, bkm_impute_chunk
- * 3 = bkm_distinct_chunk, bkm_encode_chunk, bkm_decode_chunk */
-#define BKM_VERSION_MINOR 3
+ * 3 = bkm_distinct_chunk, bkm_encode_chunk, bkm_decode_chunk
+ * 4 = bkm_text_workspace_bytes, bkm_text_tokens_chunk, bkm_text_hash_chunk, bkm_text_write_chunk */
+#define BKM_VERSION_MINOR 4
 
 /* element types of X */
 #define BKM_F32 0
@@ -596,6 +600,46 @@ int bkm_encode_chunk(const void* X, int64_t n, int d, int64_t ldx, int x_dtype, 
 int bkm_decode_chunk(const void* codes, int64_t n, int d, int64_t ldc, int code_dtype, const void* cat_vals,
                      const int64_t* cat_off, int elem_bytes, void* out, int64_t ld_out, unsigned long long* unknown,
                      void* stream);
+
+/* ---- HashingVectorizer: the document-term matrix of one block of ASCII documents (replaces scikit-learn's
+ * HashingVectorizer.transform, which dask_ml/feature_extraction/text.py maps over the blocks) --------------------------
+ * buf [n_bytes] uint8 holds the documents back to back, document i at [doc_off[i], doc_off[i + 1]) (doc_off [n_docs + 1]
+ * int64, device, doc_off[n_docs] = n_bytes), each ENDING in a byte that is not a word character (the caller appends one,
+ * e.g. '\n'), so that no token spans two documents.  Word characters are [A-Za-z0-9_]; a token is a maximal run of two
+ * or more of them (scikit-learn's default token_pattern on ASCII text), lowercased A-Z when `lowercase`; an n-gram is n
+ * consecutive tokens of one document joined by one space, min_n <= n <= max_n (1 <= min_n).  An n-gram's hash h is
+ * MurmurHash3 x86_32 with seed 0 over its bytes, as int32; its column is |h| % n_features (for h = -2^31:
+ * (2^31 - 1 - (n_features - 1)) % n_features) and its sign -1 when alternate_sign and h < 0, else +1.  A row's value in
+ * a column is the sum of the signs of its n-grams there, zeros kept (1 for every stored column when `binary`); with
+ * norm BKM_TEXT_NORM_L1 / _L2 the row is divided by sum |v| / sqrt(sum v^2), accumulated in float64 (the squares rounded
+ * to out_dtype first) and divided in float64 before the rounding to out_dtype, unless the sum is 0.  This is
+ * scikit-learn 1.9's arithmetic (_hashing_fast.pyx, sum_duplicates, sparsefuncs_fast.pyx) bit for bit, for float32
+ * while no value passes 2^24.
+ *   bkm_text_workspace_bytes  workspace of the two calls below: (n_bytes, n_docs, 0) for bkm_text_tokens_chunk,
+ *                        (n_bytes, n_docs, n_pairs) for bkm_text_hash_chunk; n_pairs <= INT_MAX.
+ *   bkm_text_tokens_chunk  tok_start [tok_cap >= n_bytes / 3 + 1] int64 = the byte position of every token, ascending;
+ *                        tok_off [n_docs + 1] int64 = each document's first token (tok_off[n_docs] = the token count);
+ *                        pair_off [n_docs + 1] int64 = each document's first n-gram (the exclusive scan of the n-gram
+ *                        counts); totals[0] = tokens, totals[1] = n-grams (int64, device).
+ *   bkm_text_hash_chunk  keys [n_pairs] uint32 = 2 column + (1 for sign -1) of every n-gram, sorted within each
+ *                        document; indptr [n_docs + 1] int64 = the CSR row offsets; scale [n_docs] float64 = each row's
+ *                        divisor (0: not divided); totals[2] = stored entries.  n_tokens, n_pairs: totals[0], totals[1].
+ *   bkm_text_write_chunk indices [totals[2]] int64, ascending within a row, and data [totals[2]] in out_dtype (BKM_F32 or
+ *                        BKM_F64) of every stored entry. */
+#define BKM_TEXT_NORM_NONE 0
+#define BKM_TEXT_NORM_L1   1
+#define BKM_TEXT_NORM_L2   2
+int bkm_text_workspace_bytes(int64_t n_bytes, int64_t n_docs, int64_t n_pairs, size_t* out);
+int bkm_text_tokens_chunk(const uint8_t* buf, int64_t n_bytes, const int64_t* doc_off, int64_t n_docs, int min_n,
+                          int max_n, int64_t* tok_start, int64_t tok_cap, int64_t* tok_off, int64_t* pair_off,
+                          int64_t* totals, void* workspace, size_t ws_bytes, void* stream);
+int bkm_text_hash_chunk(const uint8_t* buf, int64_t n_bytes, const int64_t* tok_start, const int64_t* tok_off,
+                        const int64_t* pair_off, int64_t n_docs, int64_t n_tokens, int64_t n_pairs, int min_n, int max_n,
+                        int lowercase, int64_t n_features, int alternate_sign, int binary, int norm, int out_dtype,
+                        uint32_t* keys, int64_t* indptr, double* scale, int64_t* totals, void* workspace,
+                        size_t ws_bytes, void* stream);
+int bkm_text_write_chunk(const uint32_t* keys, const int64_t* pair_off, const int64_t* indptr, const double* scale,
+                         int64_t n_docs, int binary, int64_t* indices, void* data, int out_dtype, void* stream);
 
 /* ---- NaN/inf scan of a chunk (k_means.py:179-180): sets *flag (int32) nonzero -------- */
 int bkm_check_finite(const void* X, int64_t n, int d, int64_t ldx, int x_dtype,
