@@ -87,6 +87,20 @@ SIGNATURES = {
                                   _c_void_p, _c_void_p, _c_void_p, _c_void_p, ctypes.c_size_t, _int, _c_void_p]),
     "bkm_gram_weighted_chunk": (_int, [_c_void_p, _i64, _int, _i64, _int, _c_void_p, _c_void_p, _c_void_p,
                                        ctypes.c_size_t, _int, _c_void_p]),
+    "bkm_glm_csr_workspace_bytes": (_int, [_i64, _szp]),
+    "bkm_glm_csr_pass_chunk": (_int, [_c_void_p, _c_void_p, _c_void_p, _int, _i64, _int, _i64, _c_void_p, _c_void_p,
+                                      _int, _int, _c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_void_p,
+                                      ctypes.c_size_t, _int, _c_void_p]),
+    "bkm_csr_transpose_workspace_bytes": (_int, [_i64, _int, _i64, _szp, _szp]),
+    "bkm_csr_transpose_chunk": (_int, [_c_void_p, _c_void_p, _c_void_p, _int, _i64, _int, _i64, _c_void_p, _c_void_p,
+                                       _c_void_p, _c_void_p, ctypes.c_size_t, _c_void_p, ctypes.c_size_t, _c_void_p]),
+    "bkm_csc_matvec_workspace_bytes": (_int, [_int, _i64, _szp]),
+    "bkm_csc_matvec_chunk": (_int, [_c_void_p, _c_void_p, _c_void_p, _int, _int, _i64, _c_void_p, _c_void_p,
+                                    _c_void_p, _c_void_p, _c_void_p, _c_void_p, ctypes.c_size_t, _int, _c_void_p]),
+    "bkm_gram_weighted_csr_workspace_bytes": (_int, [_int, _i64, _szp]),
+    "bkm_gram_weighted_csr_chunk": (_int, [_c_void_p, _c_void_p, _c_void_p, _int, _i64, _int, _i64, _c_void_p,
+                                           _c_void_p, _c_void_p, _c_void_p, _i64, _c_void_p, _c_void_p, _c_void_p,
+                                           ctypes.c_size_t, _int, _c_void_p]),
     "bkm_colstats_workspace_bytes": (_int, [_i64, _int, _szp]),
     "bkm_colstats_chunk": (_int, [_c_void_p, _i64, _int, _i64, _int, _c_void_p, _c_void_p, _c_void_p, _c_void_p,
                                   ctypes.c_size_t, _int, _c_void_p]),

@@ -521,6 +521,79 @@ class CudaBackend(object):
                 self._ptr(x), n, d, x.stride(0) if n else d, _DT_CODE[x.dtype], self._ptr(w), self._ptr(gram),
                 self._ptr(ws), ws.numel(), flags, self._stream()), "bkm_gram_weighted_chunk")
 
+    def glm_csr_pass_chunk(self, blk, d, y, beta, family, mode, r=None, w=None, grad=None, hrow=None, out=None,
+                           first=False):
+        """``glm_pass_chunk`` on one CSR block ``blk`` = (crow int64 (n + 1,), col int64 (nnz,), val float32 / float64
+        (nnz,), n) of d columns.  Modes 0 and 1 write r (n,) (and w (n,)) float64 for ``csc_matvec_chunk`` and set
+        grad[d:d + 2] = [sum r | loss] (and hrow[d] = sum w); modes 2 and 3 write ``out`` as the dense pass does."""
+        crow, col, val, n = blk
+        ws = None
+        if mode in (0, 1):
+            nb = ctypes.c_size_t(0)
+            _lib.check(self.lib.bkm_glm_csr_workspace_bytes(int(n), ctypes.byref(nb)), "bkm_glm_csr_workspace_bytes")
+            ws = self._scratch("glm_csr", nb.value)
+        flags = self.flags | (_lib.FLAG_FIRST_CHUNK if first else 0)
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.bkm_glm_csr_pass_chunk(
+                self._ptr(crow), self._ptr(col), self._ptr(val), _DT_CODE[val.dtype], int(n), int(d), int(col.numel()),
+                self._ptr(y), self._ptr(beta), int(family), int(mode), self._ptr(r), self._ptr(w), self._ptr(grad),
+                self._ptr(hrow), self._ptr(out), self._ptr(ws), ws.numel() if ws is not None else 0, flags,
+                self._stream()), "bkm_glm_csr_pass_chunk")
+
+    def csr_transpose_chunk(self, blk, d):
+        """The CSC of one CSR block: (colptr int64 (d + 1,), rows int32 (nnz,) ascending within each column, vals
+        (nnz,) in the block's dtype, plan int64), plan[:4] = [non-canonical flag | segments | Gram slots | longest
+        column] (include/bkm_b200.h)."""
+        crow, col, val, n = blk
+        nnz = int(col.numel())
+        wb, pb = ctypes.c_size_t(0), ctypes.c_size_t(0)
+        _lib.check(self.lib.bkm_csr_transpose_workspace_bytes(int(n), int(d), nnz, ctypes.byref(wb), ctypes.byref(pb)),
+                   "bkm_csr_transpose_workspace_bytes")
+        ws = self._scratch("csr_transpose", wb.value)
+        colptr = torch.empty(int(d) + 1, dtype=torch.int64, device=self.device)
+        rows = torch.empty(nnz, dtype=torch.int32, device=self.device)
+        vals = torch.empty(nnz, dtype=val.dtype, device=self.device)
+        plan = torch.empty((pb.value + 7) // 8, dtype=torch.int64, device=self.device)
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.bkm_csr_transpose_chunk(
+                self._ptr(crow), self._ptr(col), self._ptr(val), _DT_CODE[val.dtype], int(n), int(d), nnz,
+                self._ptr(colptr), self._ptr(rows), self._ptr(vals), self._ptr(plan), plan.numel() * 8, self._ptr(ws),
+                ws.numel(), self._stream()), "bkm_csr_transpose_chunk")
+        return colptr, rows, vals, plan
+
+    def csc_matvec_chunk(self, csc, d, v1, out1, v2=None, out2=None, first=False):
+        """out1[:d] (+)= X^T v1 (and out2[:d] (+)= X^T v2) over the transpose ``csc`` of one block, each column's
+        entries added in ascending row order.  ``first`` overwrites."""
+        colptr, rows, vals, plan = csc
+        nnz = int(rows.numel())
+        nb = ctypes.c_size_t(0)
+        _lib.check(self.lib.bkm_csc_matvec_workspace_bytes(int(d), nnz, ctypes.byref(nb)),
+                   "bkm_csc_matvec_workspace_bytes")
+        ws = self._scratch("csc_matvec", nb.value)
+        flags = self.flags | (_lib.FLAG_FIRST_CHUNK if first else 0)
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.bkm_csc_matvec_chunk(
+                self._ptr(colptr), self._ptr(rows), self._ptr(vals), _DT_CODE[vals.dtype], int(d), nnz, self._ptr(plan),
+                self._ptr(v1), self._ptr(v2), self._ptr(out1), self._ptr(out2), self._ptr(ws), ws.numel(), flags,
+                self._stream()), "bkm_csc_matvec_chunk")
+
+    def gram_weighted_csr_chunk(self, blk, csc, d, w, gram, n_slots, first=False):
+        """gram (d, d) (+)= sum_i w_i x_i x_i^T over one CSR block and its transpose; ``n_slots`` = plan[2] of the
+        transpose (read once per fit).  ``first`` overwrites."""
+        crow, col, val, n = blk
+        colptr, rows, vals, plan = csc
+        nb = ctypes.c_size_t(0)
+        _lib.check(self.lib.bkm_gram_weighted_csr_workspace_bytes(int(d), int(n_slots), ctypes.byref(nb)),
+                   "bkm_gram_weighted_csr_workspace_bytes")
+        ws = self._scratch("gram_csr", nb.value)
+        flags = self.flags | (_lib.FLAG_FIRST_CHUNK if first else 0)
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.bkm_gram_weighted_csr_chunk(
+                self._ptr(crow), self._ptr(col), self._ptr(val), _DT_CODE[val.dtype], int(n), int(d),
+                int(col.numel()), self._ptr(colptr), self._ptr(rows), self._ptr(vals), self._ptr(plan), int(n_slots),
+                self._ptr(w), self._ptr(gram), self._ptr(ws), ws.numel(), flags, self._stream()),
+                "bkm_gram_weighted_csr_chunk")
+
     def colstats_chunk(self, x, shift, acc, minmax, first=False):
         """The scalers' statistics pass over one chunk, float64 on the device: acc (5, d) (+)= [sum (x - shift) |
         sum (x - shift)^2 over the finite x | NaN count | +inf count | -inf count] and minmax (2, d) = [min | max] over

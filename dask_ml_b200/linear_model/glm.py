@@ -16,23 +16,34 @@ Each evaluation is one device pass per chunk and one all-reduce:
     Newton pass   (bkm_glm_pass_chunk mode 1, then      [sum r x | sum r | loss], w_i,
                    bkm_gram_weighted_chunk with w_i):   [sum w x | sum w], sum w x x^T      all-reduce of [H | g | loss]
 
+Sparse X (a ChunkedArray of torch sparse CSR blocks, one torch CSR tensor, or any scipy.sparse matrix) runs the same
+solvers on the same objective; only the per-block calls change (``_SparsePasses``):
+
+    gradient pass (bkm_glm_csr_pass_chunk mode 0, then bkm_csc_matvec_chunk with r_i over the block's transpose)
+    Newton pass   (mode 1, the column pass with r_i and w_i, then bkm_gram_weighted_csr_chunk with w_i)
+
+The transpose of each block is built on the first evaluation of a fit and kept for it.
+
 The solvers run on the host in float64 (DESIGN.md A22): 'newton' (unregularised, Cholesky, least squares when it
 fails, the step halved until the loss passes an Armijo test, stop at max |delta| < tol), 'lbfgs' (scipy's fmin_l_bfgs_b, pgtol = tol), 'gradient_descent' (unregularised,
 Armijo backtracking, stop when the relative decrease of the loss is below tol), 'proximal_grad' (backtracking on the
 quadratic bound, stop at max |delta beta| < tol (1 + max |beta|)).  'admm' is a documented deviation: penalised Newton
-for l2, 'proximal_grad' for l1 -- the exact optimum that the reference's consensus ADMM approximates.
+for l2, 'proximal_grad' for l1 -- the exact optimum that the reference's consensus ADMM approximates.  On sparse X with
+more than ``SPARSE_NEWTON_MAX_P`` coefficients the (p, p) Hessian is not formed: 'newton' raises, and l2 'admm' runs
+'lbfgs' on the same objective (pgtol = tol).
 
 Unregularised logistic regression on separable data has no finite optimum: the coefficients grow until max_iter, as in
 the reference.
 """
 import numpy as np
 import scipy.linalg
+import scipy.sparse
 import torch
 from scipy.optimize import fmin_l_bfgs_b
 from sklearn.base import BaseEstimator
 from sklearn.exceptions import NotFittedError
 
-from ..chunked import ChunkedArray, _is_torch
+from ..chunked import ChunkedArray, _is_torch, is_sparse_csr_block
 from ..cluster.k_means import _NONFINITE_MSG
 from ..decomposition.pca import _device_data
 from ..naive_bayes import _y_flat
@@ -40,6 +51,91 @@ from ..naive_bayes import _y_flat
 LOGISTIC, NORMAL, POISSON = 0, 1, 2                # the kernel's family codes
 _GRAD, _NEWTON, _PREDICT, _LABEL = 0, 1, 2, 3      # and its modes
 _SOLVERS = {"admm", "proximal_grad", "lbfgs", "newton", "gradient_descent"}
+SPARSE_NEWTON_MAX_P = 4096                         # the largest p = d (+ 1) whose Hessian sparse input forms
+
+
+class _SparseData(object):
+    """Sparse CSR row blocks on the device: ``blocks`` = [(crow int64, col int64, val float32 / float64, n)], with what
+    ``_y_chunks`` and the passes read of ``DeviceData``.  ``transposes()`` builds each block's CSC once."""
+
+    def __init__(self, blocks, d, backend, comm=None):
+        from ..engine import Comm
+
+        self.blocks, self.d, self.backend = blocks, int(d), backend
+        self.comm = comm or Comm()
+        self.chunk_rows = [int(b[3]) for b in blocks]
+        self.n_local = int(sum(self.chunk_rows))
+        self.chunk_offsets = np.cumsum([0] + self.chunk_rows)
+        self._csc = None
+        self.n_slots = None
+
+    def transposes(self):
+        """The blocks' transposes, built on first use.  Their checks are read here, once: a block whose column indices
+        are not strictly increasing within each row (or not in [0, d)) raises ValueError on every rank."""
+        if self._csc is None:
+            be = self.backend
+            csc = [be.csr_transpose_chunk(b, self.d) for b in self.blocks]
+            status = torch.stack([c[3][:4] for c in csc]).cpu().numpy()
+            bad = [i for i in range(len(csc)) if status[i, 0] != 0]
+            flag = torch.tensor([float(len(bad))], dtype=torch.float64, device=be.device)
+            self.comm.allreduce_sum_(flag)
+            if float(flag.item()) != 0.0:
+                where = ("block %d" % bad[0]) if bad else "a block of another rank"
+                raise ValueError("Sparse input must be canonical CSR: the column indices of %s are not strictly "
+                                 "increasing within each row, or not in [0, %d)" % (where, self.d))
+            self.n_slots = [int(v) for v in status[:, 2]]
+            self._csc = csc
+        return self._csc
+
+
+def _sparse_values(v):
+    """float32 / float64 values as they are; integer and bool values widened once to float64."""
+    if v.dtype in (torch.float32, torch.float64):
+        return v
+    if v.dtype == torch.bool or not (v.dtype.is_floating_point or v.dtype.is_complex):
+        return v.to(torch.float64)
+    raise TypeError("Sparse input values of dtype %s are not supported: use float32, float64, an integer type or "
+                    "bool" % (v.dtype,))
+
+
+def _sparse_data(X):
+    """Sparse X -> ``_SparseData``, or None for every other input.  Accepted: a ChunkedArray whose blocks are all torch
+    sparse CSR tensors (device or host), one torch sparse CSR tensor, or a scipy.sparse matrix of any format (made
+    canonical CSR on the host and uploaded as one block)."""
+    if isinstance(X, ChunkedArray):
+        sp = [is_sparse_csr_block(b) for b in X.blocks]
+        if not any(sp):
+            return None
+        if not all(sp):
+            raise TypeError("A ChunkedArray that mixes dense and sparse CSR blocks is not supported")
+        blocks = X.blocks
+    elif _is_torch(X) and X.layout == torch.sparse_csr:
+        blocks = [X]
+    elif scipy.sparse.issparse(X):
+        m = scipy.sparse.csr_matrix(X, copy=True)
+        m.sum_duplicates()
+        m.sort_indices()
+        v = torch.from_numpy(np.ascontiguousarray(m.data))
+        blocks = [(torch.from_numpy(m.indptr.astype(np.int64)), torch.from_numpy(m.indices.astype(np.int64)), v,
+                   m.shape)]
+    else:
+        return None
+    from ..cluster import k_means as _km
+
+    be = _km._get_backend()
+    out = []
+    for b in blocks:
+        if isinstance(b, tuple):
+            crow, col, val, shape = b
+        else:
+            crow, col, val, shape = b.crow_indices(), b.col_indices(), b.values(), tuple(b.shape)
+        if len(shape) != 2:
+            raise ValueError("Expected a 2-D sparse matrix, got shape %s" % (tuple(shape),))
+        val = _sparse_values(val)
+        crow = crow.to(device=be.device, dtype=torch.int64).contiguous()
+        col = col.to(device=be.device, dtype=torch.int64).contiguous()
+        out.append((crow, col, val.to(device=be.device).contiguous(), int(shape[0])))
+    return _SparseData(out, int(shape[1]), be)
 
 
 def _y_chunks(y, X, who):
@@ -70,6 +166,10 @@ class _Passes(object):
         full[: self.p] = b
         return torch.as_tensor(full).to(self.be.device)
 
+    def _scanned(self):
+        """The 2-D parts of X that the non-finite scan reads, one per y chunk."""
+        return self.X.chunks
+
     def _check(self, vals):
         """The first evaluation is at beta = 0, where every term is finite for finite X and y: a non-finite result
         there is a NaN or inf in X or y.  X is scanned only then, as PCA does."""
@@ -80,7 +180,7 @@ class _Passes(object):
             return
         be = self.be
         flag = torch.zeros(1, dtype=torch.float64, device=be.device)
-        for x, y in zip(self.X.chunks, self.ys):
+        for x, y in zip(self._scanned(), self.ys):
             flag += be.check_finite([x]).to(torch.float64)
             flag += (~torch.isfinite(y)).any().to(torch.float64)
         self.comm.allreduce_sum_(flag)
@@ -113,6 +213,63 @@ class _Passes(object):
             w = self.wbuf[: int(x.shape[0])]
             be.glm_pass_chunk(x, self.ys[i], bd, self.family, _NEWTON, grad=grad, hrow=hrow, w=w, first=i == 0)
             be.gram_weighted_chunk(x, w, G, first=i == 0)
+        self.comm.allreduce_sum_(red)
+        h = red.cpu().numpy()
+        self._check(h)
+        H = np.empty((d + 1, d + 1))
+        H[:d, :d] = h[: d * d].reshape(d, d)
+        H[d, :d] = H[:d, d] = h[d * d: d * d + d]
+        H[d, d] = h[d * d + d]
+        g = h[d * d + d + 1:]
+        return float(g[d + 1]), g[: self.p].copy(), H[: self.p, : self.p].copy()
+
+
+class _SparsePasses(_Passes):
+    """``_Passes`` on sparse CSR blocks: the same evaluations, reduction buffers and all-reduces, each block's terms
+    from the CSR row pass, the column pass over its transpose and (Newton) the sparse weighted Gram."""
+
+    def __init__(self, X, ys, family, fit_intercept):
+        super(_SparsePasses, self).__init__(X, ys, family, fit_intercept)
+        self.rbuf = None
+
+    def _scanned(self):
+        return [b[2].view(-1, 1) for b in self.X.blocks]
+
+    def _bufs(self, newton):
+        rows = max([1] + self.X.chunk_rows)
+        if self.rbuf is None:
+            self.rbuf = self.be.empty((rows,), torch.float64)
+        if newton and self.wbuf is None:
+            self.wbuf = self.be.empty((rows,), torch.float64)
+
+    def grad(self, b):
+        d, be = self.d, self.be
+        bd = self._beta(b)
+        csc = self.X.transposes()
+        self._bufs(False)
+        red = be.zeros((d + 2,), torch.float64)
+        for i, blk in enumerate(self.X.blocks):
+            r = self.rbuf[: blk[3]]
+            be.glm_csr_pass_chunk(blk, d, self.ys[i], bd, self.family, _GRAD, r=r, grad=red, first=i == 0)
+            be.csc_matvec_chunk(csc[i], d, r, red, first=i == 0)
+        self.comm.allreduce_sum_(red)
+        h = red.cpu().numpy()
+        self._check(h)
+        return float(h[d + 1]), h[: self.p].copy()
+
+    def newton(self, b):
+        d, be = self.d, self.be
+        bd = self._beta(b)
+        csc = self.X.transposes()
+        self._bufs(True)
+        red = be.zeros((d * d + 2 * d + 3,), torch.float64)
+        G, hrow, grad = red[: d * d].view(d, d), red[d * d: d * d + d + 1], red[d * d + d + 1:]
+        for i, blk in enumerate(self.X.blocks):
+            r, w = self.rbuf[: blk[3]], self.wbuf[: blk[3]]
+            be.glm_csr_pass_chunk(blk, d, self.ys[i], bd, self.family, _NEWTON, r=r, w=w, grad=grad, hrow=hrow,
+                                  first=i == 0)
+            be.csc_matvec_chunk(csc[i], d, r, grad, v2=w, out2=hrow, first=i == 0)
+            be.gram_weighted_csr_chunk(blk, csc[i], d, w, G, self.X.n_slots[i], first=i == 0)
         self.comm.allreduce_sum_(red)
         h = red.cpu().numpy()
         self._check(h)
@@ -292,13 +449,26 @@ class _GLM(BaseEstimator):
         return kw
 
     def fit(self, X, y=None):
-        """Fit the model on the training data.  X: every input KMeans takes (``host_resident`` included); y: numpy,
-        torch, ``ChunkedArray`` or dask, chunked any way."""
+        """Fit the model on the training data.  X: every input KMeans takes (``host_resident`` included), or sparse X
+        (a ChunkedArray of torch sparse CSR blocks, a torch CSR tensor, a scipy.sparse matrix); y: numpy, torch,
+        ``ChunkedArray`` or dask, chunked any way."""
         kw = self._get_solver_kwargs()
-        X = _device_data(X)
+        Xs = _sparse_data(X)
+        X = Xs if Xs is not None else _device_data(X)
         ys = _y_chunks(y, X, type(self).__name__ + ".fit")
-        P = _Passes(X, ys, self._family, self.fit_intercept)
-        self._coef = np.asarray(_SOLVER_FNS[self.solver](P, **kw), dtype=np.float64)
+        solver = _SOLVER_FNS[self.solver]
+        if Xs is None:
+            P = _Passes(X, ys, self._family, self.fit_intercept)
+        else:
+            P = _SparsePasses(X, ys, self._family, self.fit_intercept)
+            if P.p > SPARSE_NEWTON_MAX_P:
+                if self.solver == "newton":
+                    raise ValueError("solver='newton' needs the (p, p) Hessian, which is too large for sparse input "
+                                     "with p = %d > %d coefficients; use 'lbfgs', 'gradient_descent' or "
+                                     "'proximal_grad'" % (P.p, SPARSE_NEWTON_MAX_P))
+                if self.solver == "admm" and kw.get("regularizer") != "l1":
+                    solver = lbfgs                   # the same l2 objective without the Hessian (pgtol = tol)
+        self._coef = np.asarray(solver(P, **kw), dtype=np.float64)
         if self.fit_intercept:
             self.coef_ = self._coef[:-1]
             self.intercept_ = float(self._coef[-1])
@@ -312,7 +482,8 @@ class _GLM(BaseEstimator):
         if getattr(self, "_coef", None) is None:
             raise NotFittedError("This %s instance is not fitted yet. Call 'fit' with appropriate arguments before "
                                  "using this estimator." % type(self).__name__)
-        X = _device_data(X)
+        Xs = _sparse_data(X)
+        X = Xs if Xs is not None else _device_data(X)
         be, d = X.backend, X.d
         if d != len(self.coef_):
             raise ValueError("X has %d features, but %s is expecting %d features as input"
@@ -321,10 +492,13 @@ class _GLM(BaseEstimator):
         beta[: len(self._coef)] = self._coef
         bd = torch.as_tensor(beta).to(be.device)
         outs = []
-        for x in X.chunks:
-            n = int(x.shape[0])
+        for x in (X.blocks if Xs is not None else X.chunks):
+            n = int(x[3]) if Xs is not None else int(x.shape[0])
             o = be.empty((n,), torch.float64 if mode == _PREDICT else torch.uint8)
-            be.glm_pass_chunk(x, None, bd, self._family, mode, out=o)
+            if Xs is not None:
+                be.glm_csr_pass_chunk(x, d, None, bd, self._family, mode, out=o)
+            else:
+                be.glm_pass_chunk(x, None, bd, self._family, mode, out=o)
             outs.append(o if mode == _PREDICT else o.view(torch.bool))
         return X, outs
 

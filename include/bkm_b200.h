@@ -27,6 +27,9 @@
  *   dask_glm's per-iteration X.dot(beta), family loglike /        bkm_glm_pass_chunk + bkm_gram_weighted_chunk
  *     gradient / hessian of LogisticRegression, LinearRegression,
  *     PoissonRegression, linear_model/glm.py:169-362
+ *   the same per-iteration terms on sparse CSR blocks, which the      bkm_glm_csr_pass_chunk, bkm_csr_transpose_chunk,
+ *     reference cannot take (linear_model/utils.py:34-53 appends a    bkm_csc_matvec_chunk,
+ *     dense ones column to every block)                               bkm_gram_weighted_csr_chunk
  *   X.mean(0) / .var(0) / .min(0) / .max(0), da.percentile and       bkm_colstats_chunk, bkm_radix_hist_chunk +
  *     the elementwise transforms of StandardScaler, MinMaxScaler,    bkm_radix_select_step, bkm_affine_chunk
  *     RobustScaler, preprocessing/data.py:24-221
@@ -81,8 +84,11 @@ extern "C" {
  * 2 = bkm_impute_stats_workspace_bytes, bkm_impute_stats_chunk, bkm_quantile_hist_masked_chunk, bkm_mode_count_chunk,
  *     bkm_mode_best_workspace_bytes, bkm_mode_best, bkm_mode_compact, bkm_mode_merge, bkm_impute_chunk
  * 3 = bkm_distinct_chunk, bkm_encode_chunk, bkm_decode_chunk
- * 4 = bkm_text_workspace_bytes, bkm_text_tokens_chunk, bkm_text_hash_chunk, bkm_text_write_chunk */
-#define BKM_VERSION_MINOR 4
+ * 4 = bkm_text_workspace_bytes, bkm_text_tokens_chunk, bkm_text_hash_chunk, bkm_text_write_chunk
+ * 5 = bkm_glm_csr_workspace_bytes, bkm_glm_csr_pass_chunk, bkm_csr_transpose_workspace_bytes, bkm_csr_transpose_chunk,
+ *     bkm_csc_matvec_workspace_bytes, bkm_csc_matvec_chunk, bkm_gram_weighted_csr_workspace_bytes,
+ *     bkm_gram_weighted_csr_chunk */
+#define BKM_VERSION_MINOR 5
 
 /* element types of X */
 #define BKM_F32 0
@@ -276,6 +282,49 @@ int bkm_glm_pass_chunk(const void* X, int64_t n, int d, int64_t ldx, int x_dtype
                        size_t ws_bytes, int flags, void* stream);
 int bkm_gram_weighted_chunk(const void* X, int64_t n, int d, int64_t ldx, int x_dtype, const double* w, double* gram,
                             void* workspace, size_t ws_bytes, int flags, void* stream);
+
+/* ---- The same passes on one sparse CSR block: crow [n + 1] int64 row pointers, col [nnz] int64 column indices, val
+ * [nnz] values of val_dtype BKM_F32 or BKM_F64, widened to float64.  Every sum runs in a fixed order (no float atomics):
+ * two calls with the same inputs give the same bits.  ---------------------------------------------------------------
+ *   bkm_glm_csr_pass_chunk  eta_i = sum_k val_k beta[col_k] + beta[d], the families and modes of bkm_glm_pass_chunk.
+ *                      Modes 0 / 1 write r [n] = r_i (and w [n] = w_i) for the column pass and set grad[d] = sum r_i,
+ *                      grad[d + 1] = sum loss_i (and hrow[d] = sum w_i); grad[0:d] and hrow[0:d] are the column pass's.
+ *                      Modes 2 / 3 write out as bkm_glm_pass_chunk.  Rows without entries are legal.  Column indices
+ *                      outside [0, d) are skipped.  OVERWRITTEN with BKM_FLAG_FIRST_CHUNK, else ACCUMULATED.  One launch.
+ *                      workspace: bkm_glm_csr_workspace_bytes(n) bytes, any content.
+ *   bkm_csr_transpose_chunk  the block's CSC: colptr [d + 1] int64, rows [nnz] int32 (strictly ascending within each
+ *                      column), vals [nnz] in val_dtype; n, nnz < 2^31 (else BKM_EUNSUPPORTED).  plan: int64 [status (4) |
+ *                      the column segments that the two calls below read], status = [nonzero when a column index is
+ *                      outside [0, d), not strictly above its predecessor in the row, or crow is not a valid row pointer
+ *                      array | segments | Gram slots (n_slots below) | longest column].  plan_bytes and the workspace
+ *                      (any content) from bkm_csr_transpose_workspace_bytes.  A CUB radix sort and five small launches.
+ *   bkm_csc_matvec_chunk  out1[j] (+)= sum over column j's entries, in ascending row order, of v1[row] val (and out2 from
+ *                      v2 when v2 is not null): the first d entries of grad / hrow.  A column of more than 2048 entries
+ *                      is summed in segments whose partials are added in segment order.  One launch.  workspace:
+ *                      bkm_csc_matvec_workspace_bytes(d, nnz) bytes, any content.
+ *   bkm_gram_weighted_csr_chunk  gram [d][d] (+)= sum_i w_i x_i x_i^T (w [n] float64; the full matrix), each term
+ *                      (w_i x_ij) x_ik, for d <= 12288 (else BKM_EUNSUPPORTED).  Column j's entries are walked in row order
+ *                      in runs of up to 64 Ki entries; the runs of a longer column are added in run order.  One launch.
+ *                      The work is sum_i nnz_i^2.  workspace: bkm_gram_weighted_csr_workspace_bytes(d, n_slots) bytes,
+ *                      any content, n_slots = status[2] of the block's plan. */
+int bkm_glm_csr_workspace_bytes(int64_t n, size_t* out);
+int bkm_glm_csr_pass_chunk(const int64_t* crow, const int64_t* col, const void* val, int val_dtype, int64_t n, int d,
+                           int64_t nnz, const double* y, const double* beta, int family, int mode, double* r, double* w,
+                           double* grad, double* hrow, void* out, void* workspace, size_t ws_bytes, int flags,
+                           void* stream);
+int bkm_csr_transpose_workspace_bytes(int64_t n, int d, int64_t nnz, size_t* ws_bytes, size_t* plan_bytes);
+int bkm_csr_transpose_chunk(const int64_t* crow, const int64_t* col, const void* val, int val_dtype, int64_t n, int d,
+                            int64_t nnz, int64_t* colptr, int32_t* rows, void* vals, int64_t* plan, size_t plan_bytes,
+                            void* workspace, size_t ws_bytes, void* stream);
+int bkm_csc_matvec_workspace_bytes(int d, int64_t nnz, size_t* out);
+int bkm_csc_matvec_chunk(const int64_t* colptr, const int32_t* rows, const void* vals, int val_dtype, int d,
+                         int64_t nnz, const int64_t* plan, const double* v1, const double* v2, double* out1,
+                         double* out2, void* workspace, size_t ws_bytes, int flags, void* stream);
+int bkm_gram_weighted_csr_workspace_bytes(int d, int64_t n_slots, size_t* out);
+int bkm_gram_weighted_csr_chunk(const int64_t* crow, const int64_t* col, const void* val, int val_dtype, int64_t n,
+                                int d, int64_t nnz, const int64_t* colptr, const int32_t* rows, const void* vals,
+                                const int64_t* plan, int64_t n_slots, const double* w, double* gram, void* workspace,
+                                size_t ws_bytes, int flags, void* stream);
 
 /* ---- StandardScaler / MinMaxScaler / RobustScaler: the fit passes and the transform pass over row chunks (replace
  * X.mean(0), X.var(0), X.min(0), X.max(0), da.percentile per column and the elementwise (X - m) / s of
