@@ -101,6 +101,11 @@ SIGNATURES = {
     "bkm_gram_weighted_csr_chunk": (_int, [_c_void_p, _c_void_p, _c_void_p, _int, _i64, _int, _i64, _c_void_p,
                                            _c_void_p, _c_void_p, _c_void_p, _i64, _c_void_p, _c_void_p, _c_void_p,
                                            ctypes.c_size_t, _int, _c_void_p]),
+    "bkm_csr_panel_chunk": (_int, [_c_void_p, _c_void_p, _c_void_p, _int, _i64, _int, _i64, _c_void_p, _int, _c_void_p,
+                                   _i64, _int, _c_void_p, _i64, _c_void_p]),
+    "bkm_csc_panel_workspace_bytes": (_int, [_int, _i64, _int, _szp]),
+    "bkm_csc_panel_chunk": (_int, [_c_void_p, _c_void_p, _c_void_p, _int, _int, _i64, _c_void_p, _c_void_p, _int,
+                                   _c_void_p, _c_void_p, ctypes.c_size_t, _int, _c_void_p]),
     "bkm_colstats_workspace_bytes": (_int, [_i64, _int, _szp]),
     "bkm_colstats_chunk": (_int, [_c_void_p, _i64, _int, _i64, _int, _c_void_p, _c_void_p, _c_void_p, _c_void_p,
                                   ctypes.c_size_t, _int, _c_void_p]),

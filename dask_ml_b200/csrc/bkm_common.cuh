@@ -20,6 +20,30 @@ inline void note_launch(int n = 1) { g_launches.fetch_add(n, std::memory_order_r
 
 static inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 
+// Column record of the signed arg-max epilogues (bkm_project_chunk, bkm_csr_panel_chunk): the largest |t|, its lowest
+// global row, the signed value, and a lock word.  Ordered by (|t| descending, row ascending): every update order ends
+// on the same record.
+struct ColMax {
+  double absmax;
+  long long row;
+  double value;
+  unsigned long long lock;
+};
+
+__device__ __forceinline__ bool colmax_beats(double a, long long ra, double b, long long rb) {
+  return a > b || (a == b && ra < rb);
+}
+
+// one CTA's best candidate of a column folded into its global record under the record's lock
+__device__ __forceinline__ void colmax_fold(ColMax* rec, double a, long long row, double v) {
+  while (atomicCAS(&rec->lock, 0ull, 1ull) != 0ull) { }
+  __threadfence();
+  volatile ColMax* vr = rec;
+  if (colmax_beats(a, row, vr->absmax, vr->row)) { vr->absmax = a; vr->row = row; vr->value = v; }
+  __threadfence();
+  atomicExch(&rec->lock, 0ull);
+}
+
 // ---------------------------------------------------------------------------------------
 // Geometry of the large-shape tensor path (bkm_tc2.cu): the k centres are cut into S slices of NS <= 256 (one slice
 // per CTA, resident in shared memory), the features into KB blocks of 64 16-bit values (one 128-byte swizzle atom).

@@ -23,6 +23,7 @@
 //                step).  The warp copies are added in warp order; a column of several runs goes through slots folded
 //                in run order by the last run to finish.
 #include "bkm_common.cuh"
+#include "bkm_csc_plan.cuh"
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
 
@@ -31,19 +32,13 @@ namespace {
 
 constexpr int kThreads = 256;
 constexpr int kWarps = kThreads / 32;
-constexpr long long SEG = 2048;        // entries per column segment (column pass)
 constexpr long long GS = 32;           // segments per Gram run: a Gram CTA walks up to 64 Ki entries of its column
 constexpr int kGramSmem = 96 * 1024;   // shared memory of a Gram CTA: the warps' copies of one Gram row
 
 enum { GLM_GRAD = 0, GLM_NEWTON = 1, GLM_PREDICT = 2, GLM_LABEL = 3 };
-// plan layout (int64): [status (4) | seg_off (d + 1) | gseg_off (d + 1) | seg_col (int32, seg_cap(d, nnz))]
-// status = [non-canonical flag | segments T | Gram slots | longest column]
-enum { ST_BAD = 0, ST_SEGS = 1, ST_SLOTS = 2, ST_MAXLEN = 3, ST_N = 4 };
 
 __device__ __forceinline__ double to_f64(float v) { return (double)v; }
 __device__ __forceinline__ double to_f64(double v) { return v; }
-
-static long long seg_cap(int d, long long nnz) { return (long long)d + nnz / SEG + 1; }
 
 // (mu, loss, r, w) of one row: the families of bkm_glm.cu
 __device__ __forceinline__ void family_terms(int family, double eta, double y, double& mu, double& loss, double& r,

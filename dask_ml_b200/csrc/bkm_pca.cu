@@ -272,20 +272,7 @@ __global__ void __launch_bounds__(kThreads) gram_kernel(GramArgs a) {
 }
 
 // ------------------------------------------------------------------------------------------------------- project
-// Column record of the arg-max epilogue (the layout of bkm_project_chunk's colmax): the largest |t|, its lowest global
-// row, the signed value, and a lock word.  Ordered by (|t| descending, row ascending): every update order ends on the
-// same record.
-struct ColMax {
-  double absmax;
-  long long row;
-  double value;
-  unsigned long long lock;
-};
-
-__device__ __forceinline__ bool beats(double a, long long ra, double b, long long rb) {
-  return a > b || (a == b && ra < rb);
-}
-
+// The arg-max epilogue folds into ColMax records (bkm_common.cuh).
 struct ProjArgs {
   const void* X;
   long long n;
@@ -385,7 +372,7 @@ __global__ void __launch_bounds__(kThreads) project_kernel(ProjArgs a) {
             else
               reinterpret_cast<float*>(a.out)[(r0 + r) * a.ldo + c0 + c] = (float)v;
           }
-          if (a.colmax && beats(fabs(v), grow, babs[nt][j], brow[nt][j])) {
+          if (a.colmax && colmax_beats(fabs(v), grow, babs[nt][j], brow[nt][j])) {
             babs[nt][j] = fabs(v); brow[nt][j] = grow; bval[nt][j] = v;
           }
         }
@@ -405,7 +392,7 @@ __global__ void __launch_bounds__(kThreads) project_kernel(ProjArgs a) {
         const double oa = __shfl_xor_sync(0xffffffffu, babs[nt][j], off);
         const long long orow = __shfl_xor_sync(0xffffffffu, brow[nt][j], off);
         const double ov = __shfl_xor_sync(0xffffffffu, bval[nt][j], off);
-        if (beats(oa, orow, babs[nt][j], brow[nt][j])) { babs[nt][j] = oa; brow[nt][j] = orow; bval[nt][j] = ov; }
+        if (colmax_beats(oa, orow, babs[nt][j], brow[nt][j])) { babs[nt][j] = oa; brow[nt][j] = orow; bval[nt][j] = ov; }
       }
       if (g == 0) {
         const int c = nh * NT * 8 + nt * 8 + 2 * tq + j;
@@ -417,16 +404,8 @@ __global__ void __launch_bounds__(kThreads) project_kernel(ProjArgs a) {
     double ba = r_abs[0][tid], bv = r_val[0][tid];
     long long br = r_row[0][tid];
     for (int m = 1; m < 4; ++m)
-      if (beats(r_abs[m][tid], r_row[m][tid], ba, br)) { ba = r_abs[m][tid]; br = r_row[m][tid]; bv = r_val[m][tid]; }
-    if (ba >= 0.0) {
-      ColMax* rec = a.colmax + c0 + tid;
-      while (atomicCAS(&rec->lock, 0ull, 1ull) != 0ull) { }
-      __threadfence();
-      volatile ColMax* vr = rec;
-      if (beats(ba, br, vr->absmax, vr->row)) { vr->absmax = ba; vr->row = br; vr->value = bv; }
-      __threadfence();
-      atomicExch(&rec->lock, 0ull);
-    }
+      if (colmax_beats(r_abs[m][tid], r_row[m][tid], ba, br)) { ba = r_abs[m][tid]; br = r_row[m][tid]; bv = r_val[m][tid]; }
+    if (ba >= 0.0) colmax_fold(a.colmax + c0 + tid, ba, br, bv);
   }
 }
 

@@ -384,6 +384,32 @@ def _generate(sizes, d, dtype, family, info, key, device, n_targets=1, bias=0.0,
     return ChunkedArray(Xs), ChunkedArray(ys)
 
 
+def _normal_panel(key, m, d, device):
+    """Rows 0 .. m - 1 of the stream's X under ``key`` as a float64 (m, d) tensor on ``device``: ``bkm_make_glm_chunk``
+    on a CUDA device, the numpy restatement ``_x_block`` otherwise (the two agree to rounding of the math library).
+    TruncatedSVD's Gaussian test matrix on sparse X."""
+    import torch
+
+    device = torch.device(device)
+    if device.type != "cuda":
+        return torch.from_numpy(_x_block(key, 0, m, d, np.float64))
+    import ctypes
+
+    from . import _lib
+    from .engine import CudaBackend
+
+    be = CudaBackend(device)
+    X = torch.empty((m, d), dtype=torch.float64, device=device)
+    y = torch.empty((m,), dtype=torch.int64, device=device)       # the (unused) logistic response of the same call
+    if m:
+        with torch.cuda.device(device):
+            _lib.check(be.lib.bkm_make_glm_chunk(
+                ctypes.c_void_p(X.data_ptr()), ctypes.c_void_p(y.data_ptr()), m, d, d, _lib.BKM_F64, 0, _LOGISTIC,
+                None, 0, 1, 0.0, 0.0, key, None, ctypes.c_void_p(torch.cuda.current_stream(device).cuda_stream)),
+                "bkm_make_glm_chunk")
+    return X
+
+
 def make_counts(n_samples=1000, n_features=100, n_informative=2, scale=1.0, chunks=100, random_state=None,
                 device=None, dtype=None):
     """A dummy dataset for modelling count data (datasets.py:24-73): X i.i.d. N(0, 1), y ~ Poisson(exp(z)) with

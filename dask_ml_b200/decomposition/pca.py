@@ -138,6 +138,13 @@ def project_pass(X, shift, W, out_dtype=None, signs=True):
             outs.append(o)
     if not signs:
         return outs, None
+    return outs, colmax_signs(comm, rec)
+
+
+def colmax_signs(comm, rec):
+    """Per column, the sign (-1 or +1) of the value of largest magnitude in the arg-max records ``rec`` (``colmax_new``)
+    of every rank, the lowest global row winning ties: one gather across ranks."""
+    k = int(rec.shape[0])
     r = rec.cpu()
     local = (r[:, 0].numpy().copy(), r[:, 1].contiguous().view(torch.int64).numpy().copy(), r[:, 2].numpy().copy())
     parts = comm.allgather_obj(local)
@@ -149,7 +156,7 @@ def project_pass(X, shift, W, out_dtype=None, signs=True):
         best_abs = np.where(take, a, best_abs)
         best_row = np.where(take, row, best_row)
         best_val = np.where(take, v, best_val)
-    return outs, np.where(best_val < 0, -1.0, 1.0)
+    return np.where(best_val < 0, -1.0, 1.0)
 
 
 def negate_columns(outs, signs):

@@ -594,6 +594,37 @@ class CudaBackend(object):
                 self._ptr(w), self._ptr(gram), self._ptr(ws), ws.numel(), flags, self._stream()),
                 "bkm_gram_weighted_csr_chunk")
 
+    def csr_panel_chunk(self, blk, d, W, out=None, colmax=None, row_offset=0):
+        """out = X W over one CSR block ``blk`` of d columns (``W`` float64 (d, l) row-major, ``out`` (n, l) float32 /
+        float64 with any row pitch, or None), each element adding its row's entries in column order, and, into
+        ``colmax`` (``colmax_new(l)`` records), per column the largest |out_ij| with its lowest global row
+        ``row_offset + i`` and its signed value."""
+        crow, col, val, n = blk
+        l = int(W.shape[1])
+        odt = _DT_CODE[out.dtype] if out is not None else _lib.BKM_F64
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.bkm_csr_panel_chunk(
+                self._ptr(crow), self._ptr(col), self._ptr(val), _DT_CODE[val.dtype], int(n), int(d), int(col.numel()),
+                self._ptr(W), l, self._ptr(out), (out.stride(0) if n else l) if out is not None else l, odt,
+                self._ptr(colmax), int(row_offset), self._stream()), "bkm_csr_panel_chunk")
+
+    def csc_panel_chunk(self, csc, d, P, out, first=False):
+        """out (d, l) (+)= X^T P over the transpose ``csc`` of one block (``P`` float64 (n, l) row-major, ``out`` float64
+        (d, l) contiguous), each column's entries added in ascending row order.  ``first`` overwrites."""
+        colptr, rows, vals, plan = csc
+        nnz = int(rows.numel())
+        l = int(out.shape[1])
+        nb = ctypes.c_size_t(0)
+        _lib.check(self.lib.bkm_csc_panel_workspace_bytes(int(d), nnz, l, ctypes.byref(nb)),
+                   "bkm_csc_panel_workspace_bytes")
+        ws = self._scratch("csc_panel", nb.value)
+        flags = self.flags | (_lib.FLAG_FIRST_CHUNK if first else 0)
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.bkm_csc_panel_chunk(
+                self._ptr(colptr), self._ptr(rows), self._ptr(vals), _DT_CODE[vals.dtype], int(d), nnz, self._ptr(plan),
+                self._ptr(P), l, self._ptr(out), self._ptr(ws), ws.numel(), flags, self._stream()),
+                "bkm_csc_panel_chunk")
+
     def colstats_chunk(self, x, shift, acc, minmax, first=False):
         """The scalers' statistics pass over one chunk, float64 on the device: acc (5, d) (+)= [sum (x - shift) |
         sum (x - shift)^2 over the finite x | NaN count | +inf count | -inf count] and minmax (2, d) = [min | max] over

@@ -30,6 +30,9 @@
  *   the same per-iteration terms on sparse CSR blocks, which the      bkm_glm_csr_pass_chunk, bkm_csr_transpose_chunk,
  *     reference cannot take (linear_model/utils.py:34-53 appends a    bkm_csc_matvec_chunk,
  *     dense ones column to every block)                               bkm_gram_weighted_csr_chunk
+ *   da.linalg.svd_compressed's X.dot(omega), X.T.dot(q) and the        bkm_csr_panel_chunk, bkm_csc_panel_chunk
+ *     projection of TruncatedSVD on sparse CSR blocks, which the
+ *     reference densifies (decomposition/truncated_svd.py)
  *   X.mean(0) / .var(0) / .min(0) / .max(0), da.percentile and       bkm_colstats_chunk, bkm_radix_hist_chunk +
  *     the elementwise transforms of StandardScaler, MinMaxScaler,    bkm_radix_select_step, bkm_affine_chunk
  *     RobustScaler, preprocessing/data.py:24-221
@@ -87,8 +90,9 @@ extern "C" {
  * 4 = bkm_text_workspace_bytes, bkm_text_tokens_chunk, bkm_text_hash_chunk, bkm_text_write_chunk
  * 5 = bkm_glm_csr_workspace_bytes, bkm_glm_csr_pass_chunk, bkm_csr_transpose_workspace_bytes, bkm_csr_transpose_chunk,
  *     bkm_csc_matvec_workspace_bytes, bkm_csc_matvec_chunk, bkm_gram_weighted_csr_workspace_bytes,
- *     bkm_gram_weighted_csr_chunk */
-#define BKM_VERSION_MINOR 5
+ *     bkm_gram_weighted_csr_chunk
+ * 6 = bkm_csr_panel_chunk, bkm_csc_panel_workspace_bytes, bkm_csc_panel_chunk */
+#define BKM_VERSION_MINOR 6
 
 /* element types of X */
 #define BKM_F32 0
@@ -325,6 +329,30 @@ int bkm_gram_weighted_csr_chunk(const int64_t* crow, const int64_t* col, const v
                                 int d, int64_t nnz, const int64_t* colptr, const int32_t* rows, const void* vals,
                                 const int64_t* plan, int64_t n_slots, const double* w, double* gram, void* workspace,
                                 size_t ws_bytes, int flags, void* stream);
+
+/* ---- TruncatedSVD on sparse CSR blocks: the products of a block with a dense float64 panel (replace da.linalg's
+ * svd_compressed power iterations X (X^T Q) and the projection X V^T, which the reference runs on dense blocks) --------
+ * The block is given as for the linear models above (crow / col / val, or its transpose from bkm_csr_transpose_chunk).
+ * Values are widened to float64; every sum runs in a fixed order (no float atomics): two calls with the same inputs give
+ * the same bits.
+ *   bkm_csr_panel_chunk  out [n][ldo] = X W, W [p][l] float64 row-major, out_dtype BKM_F32 or BKM_F64, any l >= 1.
+ *                      Each out_ic adds row i's entries in stored order (ascending column for a canonical block) by fma;
+ *                      column indices outside [0, p) are skipped.  colmax (nullable) [l] records of bkm_project_chunk's
+ *                      format: per column the largest |out_ic| with its lowest GLOBAL row (row_offset + i) and the signed
+ *                      value, folded into the record.  out nullable (the epilogue only).  One launch, no workspace.
+ *   bkm_csc_panel_chunk  out [p][l] (+)= X^T P, P [n][l] float64 row-major, over the block's transpose and its plan:
+ *                      each out_jc adds column j's entries in ascending row order; a column of more than 2048 entries is
+ *                      summed in segments whose partials are added in segment order by the last segment to finish.
+ *                      OVERWRITTEN with BKM_FLAG_FIRST_CHUNK, else ACCUMULATED.  One launch.  workspace:
+ *                      bkm_csc_panel_workspace_bytes(p, nnz, l) bytes, any content: 2 (nnz / 2048 + 1) l float64 segment
+ *                      partials, then p uint32 tickets (cleared by the call). */
+int bkm_csr_panel_chunk(const int64_t* crow, const int64_t* col, const void* val, int val_dtype, int64_t n, int p,
+                        int64_t nnz, const double* W, int l, void* out, int64_t ldo, int out_dtype, void* colmax,
+                        int64_t row_offset, void* stream);
+int bkm_csc_panel_workspace_bytes(int p, int64_t nnz, int l, size_t* out);
+int bkm_csc_panel_chunk(const int64_t* colptr, const int32_t* rows, const void* vals, int val_dtype, int p,
+                        int64_t nnz, const int64_t* plan, const double* P, int l, double* out, void* workspace,
+                        size_t ws_bytes, int flags, void* stream);
 
 /* ---- StandardScaler / MinMaxScaler / RobustScaler: the fit passes and the transform pass over row chunks (replace
  * X.mean(0), X.var(0), X.min(0), X.max(0), da.percentile per column and the elementwise (X - m) / s of
