@@ -31,7 +31,7 @@ int launch_nystrom(const void* X, long long n, int d, long long ldx, int dtype, 
 int launch_colsum_fold(const double* part, int parts, int l, double* colsum, int first, cudaStream_t s);
 
 static std::atomic<int> g_sm_count[64];
-static int sm_count_of_current(int* out) {
+int sm_count(int* out) {
   int dev = 0;
   BKM_CUDA_TRY(cudaGetDevice(&dev));
   if (dev < 0 || dev >= 64) return BKM_EINVAL;
@@ -44,14 +44,12 @@ static int sm_count_of_current(int* out) {
   return 0;
 }
 
+static std::atomic<long long> g_fallbacks{0};   // chunk calls that left their shape's kernel family for the generic kernel
+
 // Near-tie margin coefficient: a row is re-evaluated in float64 when
 //   second_best - best <= tau * (||x||^2 + max_j ||c_j||^2).
 // fp32 dot products of length d carry a rounding error of about sqrt(d)*2^-24 relative to
 // sum|x_i c_i| <= (||x||^2+||c||^2)/2; both distances and the -2 factor give the constant.
-static bool dtype_ok(int x_dtype) { return x_dtype == BKM_F32 || x_dtype == BKM_F64 || x_dtype == BKM_BF16; }
-
-static std::atomic<long long> g_fallbacks{0};   // chunk calls that left their shape's kernel family for the generic kernel
-
 static float tau_for(int d, int dtype, int flags, int family) {
   if (dtype == BKM_F64 || (flags & BKM_FLAG_NO_RECHECK)) return 0.f;
   const float eps = 1.0f / 16777216.0f;   // 2^-24
@@ -82,7 +80,7 @@ static int chunk_common(const void* X, long long n, int d, long long ldx, int x_
   if (n == 0) return 0;
   if (!X) return BKM_EINVAL;
   int sm = 0;
-  int rc = sm_count_of_current(&sm);
+  int rc = sm_count(&sm);
   if (rc) return rc;
   WsLayout W = ws_layout(n, d, k, x_dtype, sm);
   if (ws_bytes < W.total) return BKM_EWORKSPACE;
@@ -215,9 +213,7 @@ int bkm_pack_centers(const double* centers64, int k, int d, int x_dtype, void* p
 int bkm_workspace_bytes(int64_t n, int d, int k, int x_dtype, size_t* out) {
   if (k <= 0 || d <= 0 || n < 0 || !out) return BKM_EINVAL;
   if (!dtype_ok(x_dtype)) return BKM_EDTYPE;
-  int sm = 0;
-  if (sm_count_of_current(&sm)) sm = kDefaultSMs;       // no device (CPU-side sizing): the H100 SXM figure
-  *out = ws_layout(n, d, k, x_dtype, sm).total;
+  *out = ws_layout(n, d, k, x_dtype, sm_count_or_default()).total;
   return 0;
 }
 
@@ -256,7 +252,7 @@ int bkm_transform_chunk(const void* X, int64_t n, int d, int64_t ldx, int x_dtyp
   if (n == 0) return 0;
   if (!X || !out) return BKM_EINVAL;
   int sm = 0;
-  int rc = sm_count_of_current(&sm);
+  int rc = sm_count(&sm);
   if (rc) return rc;
   // fp32, d <= 64, k <= 256: the tensor-core kernel with the transform epilogue (callers cut wider Y into column blocks)
   if (x_dtype == BKM_F32 && tc_supported(d, k, x_dtype) && !(flags & BKM_FLAG_FORCE_SIMT)) {
@@ -298,7 +294,7 @@ int bkm_kernel_colsum_chunk(const void* X, int64_t n, int d, int64_t ldx, int x_
     return 0;
   }
   int sm = 0;
-  int rc = sm_count_of_current(&sm);
+  int rc = sm_count(&sm);
   if (rc) return rc;
   // The per-CTA partials go behind the workspace's persistent header (WsLayout::off_bal is left alone), into the
   // per-call area of a chunk call with k = l: it holds at least the counts region, part_slots x l int32 = 4 x SMs
@@ -329,7 +325,7 @@ int bkm_nystrom_embed_chunk(const void* X, int64_t n, int d, int64_t ldx, int x_
   if (n == 0) return 0;
   if (!X || !out) return BKM_EINVAL;
   int sm = 0;
-  int rc = sm_count_of_current(&sm);
+  int rc = sm_count(&sm);
   if (rc) return rc;
   cudaStream_t s = (cudaStream_t)stream;
   if (x_dtype == BKM_F32 && tc_supported(d, l, x_dtype) && k <= 64 && !(flags & BKM_FLAG_FORCE_SIMT)) {
@@ -355,7 +351,7 @@ int bkm_min_fold_chunk(void* run_min, const void* new_min, int64_t n, int x_dtyp
   if (n == 0) return 0;
   if (!run_min) return BKM_EINVAL;
   int sm = 0;
-  int rc = sm_count_of_current(&sm);
+  int rc = sm_count(&sm);
   if (rc) return rc;
   return launch_min_fold(run_min, new_min, n, x_dtype, phi_acc, sm, (cudaStream_t)stream);
 }
@@ -367,7 +363,7 @@ int bkm_make_blobs_chunk(void* X, int64_t* y, int64_t n, int d, int64_t ldx, int
   if (n == 0) return 0;
   if (!X) return BKM_EINVAL;
   int sm = 0;
-  int rc = sm_count_of_current(&sm);
+  int rc = sm_count(&sm);
   if (rc) return rc;
   return launch_make_blobs(X, (long long*)y, n, d, ldx, x_dtype, centers, cluster_std, k, seed, sm, (cudaStream_t)stream);
 }
@@ -413,7 +409,7 @@ int bkm_check_finite(const void* X, int64_t n, int d, int64_t ldx, int x_dtype, 
   if (n == 0) return 0;
   if (!X) return BKM_EINVAL;
   int sm = 0;
-  int rc = sm_count_of_current(&sm);
+  int rc = sm_count(&sm);
   if (rc) return rc;
   return launch_check_finite(X, n, d, ldx, x_dtype, flag, sm, (cudaStream_t)stream);
 }
@@ -428,9 +424,7 @@ void bkm_debug_reset(void) { bkm::tc_abort_reset(); }
 int bkm_debug_deferred_rows(const void* workspace, int64_t n, int d, int k, int x_dtype, int* count_host) {
   if (!workspace || !count_host || n < 0 || d <= 0 || k <= 0) return BKM_EINVAL;
   if (!dtype_ok(x_dtype)) return BKM_EDTYPE;
-  int sm = 0;
-  if (sm_count_of_current(&sm)) sm = kDefaultSMs;
-  WsLayout W = ws_layout(n, d, k, x_dtype, sm);
+  WsLayout W = ws_layout(n, d, k, x_dtype, sm_count_or_default());
   BKM_CUDA_TRY(cudaMemcpy(count_host, (const unsigned char*)workspace + W.off_flag, sizeof(int), cudaMemcpyDeviceToHost));
   return 0;
 }

@@ -20,6 +20,56 @@ inline void note_launch(int n = 1) { g_launches.fetch_add(n, std::memory_order_r
 
 static inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 
+static const int kDefaultSMs = 132;     // H100 SXM: sizing when no device is visible
+
+// SM count of the current device, cached per device (defined in bkm_api.cu)
+int sm_count(int* out);
+// ... or kDefaultSMs when there is no device: for the *_workspace_bytes sizing, which must answer without one
+static inline int sm_count_or_default() {
+  int sms = 0;
+  if (sm_count(&sms) != 0 || sms <= 0) sms = kDefaultSMs;
+  return sms;
+}
+
+// the dense input dtypes of the row-chunk passes, and their element sizes
+static inline bool dtype_ok(int t) { return t == BKM_F32 || t == BKM_F64 || t == BKM_BF16; }
+static inline size_t elem_size(int t) { return t == BKM_F64 ? 8 : (t == BKM_F32 ? 4 : 2); }
+
+// Last-CTA election of a deterministic fold.  Every CTA calls it after writing its partial; the one that arrives last
+// of `arrivals` gets true (block-uniform) and, after the fences, sees every other CTA's partial.  The caller folds the
+// partials in its own fixed order and resets the ticket.  The second barrier carries the result to every thread, so the
+// election needs no shared memory.
+__device__ __forceinline__ bool last_block(unsigned* ticket, unsigned arrivals) {
+  __threadfence();
+  __syncthreads();
+  const bool mine = threadIdx.x == 0 && atomicAdd(ticket, 1u) == arrivals - 1;
+  const bool last = __syncthreads_or(mine);
+  if (last) __threadfence();
+  return last;
+}
+
+// last_block for one warp (warp-uniform): every lane fences its own writes before lane 0 takes the ticket.
+__device__ __forceinline__ bool last_warp(unsigned* ticket, unsigned arrivals) {
+  __threadfence();
+  __syncwarp();
+  int last = 0;
+  if ((threadIdx.x & 31) == 0) last = atomicAdd(ticket, 1u) == arrivals - 1;
+  last = __shfl_sync(0xffffffffu, last, 0);
+  if (last) __threadfence();
+  return last;
+}
+
+// Workspace of a one-ticket last_block fold: `grid` CTA partials of `per_cta` doubles, then 256 bytes for the ticket
+static inline size_t partials_bytes(long long grid, size_t per_cta) {
+  return align_up((size_t)grid * per_cta * 8, 256) + 256;
+}
+// ... carved from `ws` of `bytes` = partials_bytes(...) bytes, the ticket zeroed on the stream
+static inline cudaError_t carve_partials(void* ws, size_t bytes, double** part, unsigned** ticket, cudaStream_t s) {
+  *part = reinterpret_cast<double*>(ws);
+  *ticket = reinterpret_cast<unsigned*>(reinterpret_cast<unsigned char*>(ws) + bytes - 256);
+  return cudaMemsetAsync(*ticket, 0, 4, s);
+}
+
 // Column record of the signed arg-max epilogues (bkm_project_chunk, bkm_csr_panel_chunk): the largest |t|, its lowest
 // global row, the signed value, and a lock word.  Ordered by (|t| descending, row ascending): every update order ends
 // on the same record.
@@ -152,8 +202,6 @@ __device__ __forceinline__ bool fp32_norm_in_window(float v) {
 // fewer when a slot is large (a kernel whose per-CTA sums occupy most of the shared memory runs 1-2 CTAs per SM), and a
 // single slot when k*d cannot be CTA-resident at all (generic kernel's GLOBAL mode: float64 atomics into slot 0, so the
 // psum area always holds at least k*d doubles).
-static const int kDefaultSMs = 132;     // H100 SXM: sizing when no device is visible
-
 struct WsLayout {
   size_t off_bal, off_psum, off_pcnt, off_pin, off_flag, off_defer, off_rec, off_lab, off_bin, off_binoff, total;
   size_t psum_esz;

@@ -207,13 +207,6 @@ int launch_gen(const GenArgs& a, int family, int grid, cudaStream_t s) {
   return 0;
 }
 
-int sm_count(int* out) {
-  int dev = 0;
-  BKM_CUDA_TRY(cudaGetDevice(&dev));
-  BKM_CUDA_TRY(cudaDeviceGetAttribute(out, cudaDevAttrMultiProcessorCount, dev));
-  return 0;
-}
-
 }  // namespace
 }  // namespace bkm
 
@@ -236,7 +229,7 @@ extern "C" int bkm_make_glm_chunk(void* X, void* y, int64_t n, int d, int64_t ld
   GenArgs a;
   a.X = X; a.y = y; a.n = n; a.d = d; a.ldx = ldx; a.row0 = row0; a.info = info; a.m = m; a.nt = n_targets;
   a.bias = bias; a.noise = noise; a.key = key; a.flag = flag;
-  const size_t es = x_dtype == BKM_F64 ? 8 : 4;
+  const size_t es = elem_size(x_dtype);
   a.vec = (d % 2 == 0) && (ldx % 2 == 0) && ((uintptr_t)X % (2 * es) == 0);
   if (x_dtype == BKM_F32) return launch_gen<float>(a, family, (int)grid, (cudaStream_t)stream);
   return launch_gen<double>(a, family, (int)grid, (cudaStream_t)stream);

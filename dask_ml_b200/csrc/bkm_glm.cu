@@ -103,7 +103,6 @@ __global__ void __launch_bounds__(kThreads, 3) glm_pass_kernel(GlmArgs a) {
   __shared__ double s_r[TR], s_w[TR];
   __shared__ double s_fold[kThreads * 2];
   __shared__ double s_warp[kWarps][RW][3];
-  __shared__ int s_last;
 
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int d = a.d;
@@ -252,12 +251,7 @@ __global__ void __launch_bounds__(kThreads, 3) glm_pass_kernel(GlmArgs a) {
     part[d + 1] = sl;
     part[2 * d + 2] = sw;
   }
-  __threadfence();
-  __syncthreads();
-  if (tid == 0) s_last = atomicAdd(a.ticket, 1u) == gridDim.x - 1;
-  __syncthreads();
-  if (!s_last) return;
-  __threadfence();
+  if (!last_block(a.ticket, gridDim.x)) return;
 
   // ---- the last CTA: the CTA partials in CTA order ----
   const int m = newton ? P : d + 2;
@@ -271,8 +265,6 @@ __global__ void __launch_bounds__(kThreads, 3) glm_pass_kernel(GlmArgs a) {
   if (tid == 0) *a.ticket = 0u;
 }
 
-static bool dtype_ok(int t) { return t == BKM_F32 || t == BKM_F64 || t == BKM_BF16; }
-
 static int glm_grid(long long n, int sms) {
   const long long tiles = (n + TR - 1) / TR;
   long long g = 3LL * sms;                      // three CTAs per SM: all resident at once (launch bounds)
@@ -281,16 +273,7 @@ static int glm_grid(long long n, int sms) {
   return (int)g;
 }
 
-static size_t glm_ws(long long n, int d, int sms) {
-  return align_up((size_t)glm_grid(n, sms) * (2 * (size_t)d + 3) * 8, 256) + 256;
-}
-
-static int sm_count(int* out) {
-  int dev = 0;
-  BKM_CUDA_TRY(cudaGetDevice(&dev));
-  BKM_CUDA_TRY(cudaDeviceGetAttribute(out, cudaDevAttrMultiProcessorCount, dev));
-  return 0;
-}
+static size_t glm_ws(long long n, int d, int sms) { return partials_bytes(glm_grid(n, sms), 2 * (size_t)d + 3); }
 
 template <typename T>
 static int launch_glm(const GlmArgs& a, int grid, cudaStream_t s) {
@@ -307,9 +290,7 @@ using namespace bkm;
 
 extern "C" int bkm_glm_workspace_bytes(int64_t n, int d, size_t* out) {
   if (!out || n < 0 || d <= 0) return BKM_EINVAL;
-  int sms = 0;
-  if (sm_count(&sms) != 0 || sms <= 0) sms = kDefaultSMs;
-  *out = glm_ws(n, d, sms);
+  *out = glm_ws(n, d, sm_count_or_default());
   return 0;
 }
 
@@ -334,16 +315,14 @@ extern "C" int bkm_glm_pass_chunk(const void* X, int64_t n, int d, int64_t ldx, 
   a.X = X; a.n = n; a.d = d; a.ldx = ldx; a.y = y; a.beta = beta; a.family = family; a.mode = mode;
   a.grad = grad; a.hrow = hrow; a.w = w; a.out = out;
   a.first = (flags & BKM_FLAG_FIRST_CHUNK) ? 1 : 0;
-  const size_t es = x_dtype == BKM_F64 ? 8 : (x_dtype == BKM_F32 ? 4 : 2);
+  const size_t es = elem_size(x_dtype);
   a.vec = n > 0 && ((uintptr_t)X % 16 == 0) && ((ldx * es) % 16 == 0) && ((d * es) % 16 == 0);
   a.part = nullptr;
   a.ticket = nullptr;
   if (accumulate) {
-    if (ws_bytes < glm_ws(n, d, sms)) return BKM_EWORKSPACE;
-    unsigned char* ws = reinterpret_cast<unsigned char*>(workspace);
-    a.part = reinterpret_cast<double*>(ws);
-    a.ticket = reinterpret_cast<unsigned int*>(ws + glm_ws(n, d, sms) - 256);
-    BKM_CUDA_TRY(cudaMemsetAsync(a.ticket, 0, 4, s));
+    const size_t need = glm_ws(n, d, sms);
+    if (ws_bytes < need) return BKM_EWORKSPACE;
+    BKM_CUDA_TRY(carve_partials(workspace, need, &a.part, &a.ticket, s));
   }
   if (x_dtype == BKM_F32) return launch_glm<float>(a, grid, s);
   if (x_dtype == BKM_F64) return launch_glm<double>(a, grid, s);

@@ -88,7 +88,6 @@ struct RowArgs {
 template <typename T, int G>
 __global__ void __launch_bounds__(kThreads, 4) csr_row_kernel(RowArgs a) {
   __shared__ double s_warp[kWarps][3];
-  __shared__ int s_last;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int sub = lane & (G - 1);
   const T* val = reinterpret_cast<const T*>(a.val);
@@ -149,12 +148,7 @@ __global__ void __launch_bounds__(kThreads, 4) csr_row_kernel(RowArgs a) {
     for (int k = 0; k < kWarps; ++k) v += s_warp[k][tid];
     a.part[(size_t)blockIdx.x * 3 + tid] = v;
   }
-  __threadfence();
-  __syncthreads();
-  if (tid == 0) s_last = atomicAdd(a.ticket, 1u) == gridDim.x - 1;
-  __syncthreads();
-  if (!s_last) return;
-  __threadfence();
+  if (!last_block(a.ticket, gridDim.x)) return;
   if (tid < 3 && (tid < 2 || a.mode == GLM_NEWTON)) {
     double v = 0.0;
     for (unsigned c = 0; c < gridDim.x; ++c) v += __ldcg(a.part + (size_t)c * 3 + tid);
@@ -177,20 +171,7 @@ static int row_group(long long n, long long nnz) {
   return mean <= 6.0 ? 4 : mean <= 12.0 ? 8 : mean <= 24.0 ? 16 : 32;
 }
 
-static int sm_count(int* out) {
-  int dev = 0;
-  BKM_CUDA_TRY(cudaGetDevice(&dev));
-  BKM_CUDA_TRY(cudaDeviceGetAttribute(out, cudaDevAttrMultiProcessorCount, dev));
-  return 0;
-}
-
-static int sms_or_default() {
-  int sms = 0;
-  if (sm_count(&sms) != 0 || sms <= 0) sms = kDefaultSMs;
-  return sms;
-}
-
-static size_t row_ws(int sms) { return align_up((size_t)4 * sms * 3 * 8, 256) + 256; }
+static size_t row_ws(int sms) { return partials_bytes(4LL * sms, 3); }
 
 template <typename T>
 static int launch_row(const RowArgs& a, int G, int grid, cudaStream_t s) {
@@ -365,16 +346,11 @@ __global__ void __launch_bounds__(kThreads) csc_matvec_kernel(ColArgs a) {
       p2 += __shfl_xor_sync(0xffffffffu, p2, off);
     }
     if (ns > 1) {
-      int last = 0;
       if (lane == 0) {
         a.slot[2 * t] = p1;
         a.slot[2 * t + 1] = p2;
-        __threadfence();
-        last = atomicAdd(a.ticket + j, 1u) == (unsigned)(ns - 1);
       }
-      last = __shfl_sync(0xffffffffu, last, 0);
-      if (!last) continue;
-      __threadfence();
+      if (!last_warp(a.ticket + j, (unsigned)ns)) continue;
       p1 = p2 = 0.0;                                 // the slots of column j in segment order: lane-strided, then the tree
       for (long long u = lane; u < ns; u += 32) {
         p1 += __ldcg(a.slot + 2 * (s0 + u));
@@ -420,7 +396,6 @@ struct GramArgs {
 template <typename T>
 __global__ void __launch_bounds__(kThreads) gram_csr_kernel(GramArgs a) {
   extern __shared__ double s_row[];              // [warps][d]
-  __shared__ int s_last;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, W = blockDim.x >> 5;
   const int d = a.d;
   const long long* seg_off = a.plan + ST_N;
@@ -473,12 +448,7 @@ __global__ void __launch_bounds__(kThreads) gram_csr_kernel(GramArgs a) {
     }
     if (split) {
       const long long runs = (ns + GS - 1) / GS;
-      __threadfence();
-      __syncthreads();
-      if (tid == 0) s_last = atomicAdd(a.ticket + j, 1u) == (unsigned)(runs - 1);
-      __syncthreads();
-      if (s_last) {
-        __threadfence();
+      if (last_block(a.ticket + j, (unsigned)runs)) {
         const double* src = a.slot + (size_t)gseg_off[j] * d;
         double* g = a.gram + (size_t)j * d;
         for (int k = tid; k < d; k += blockDim.x) {
@@ -511,7 +481,7 @@ static bool val_dtype_ok(int t) { return t == BKM_F32 || t == BKM_F64; }
 
 extern "C" int bkm_glm_csr_workspace_bytes(int64_t n, size_t* out) {
   if (!out || n < 0) return BKM_EINVAL;
-  *out = row_ws(sms_or_default());
+  *out = row_ws(sm_count_or_default());
   return 0;
 }
 
@@ -529,7 +499,7 @@ extern "C" int bkm_glm_csr_pass_chunk(const int64_t* crow, const int64_t* col, c
   if (mode == GLM_NEWTON && (!hrow || (n > 0 && !w))) return BKM_EINVAL;
   if (!accumulate && n > 0 && !out) return BKM_EINVAL;
   if (!accumulate && n == 0) return 0;
-  const int sms = sms_or_default();
+  const int sms = sm_count_or_default();
   const int G = row_group(n, nnz);
   const int grid = row_grid(n, G, sms);
   cudaStream_t s = (cudaStream_t)stream;
@@ -544,10 +514,7 @@ extern "C" int bkm_glm_csr_pass_chunk(const int64_t* crow, const int64_t* col, c
   if (accumulate) {
     const size_t need = row_ws(sms);
     if (ws_bytes < need) return BKM_EWORKSPACE;
-    unsigned char* ws = reinterpret_cast<unsigned char*>(workspace);
-    a.part = reinterpret_cast<double*>(ws);
-    a.ticket = reinterpret_cast<unsigned int*>(ws + need - 256);
-    BKM_CUDA_TRY(cudaMemsetAsync(a.ticket, 0, 4, s));
+    BKM_CUDA_TRY(carve_partials(workspace, need, &a.part, &a.ticket, s));
   }
   if (val_dtype == BKM_F32) return launch_row<float>(a, G, grid, s);
   return launch_row<double>(a, G, grid, s);
@@ -593,7 +560,7 @@ extern "C" int bkm_csr_transpose_chunk(const int64_t* crow, const int64_t* col, 
   long long* gseg_off = seg_off + d + 1;
   int* seg_col = reinterpret_cast<int*>(gseg_off + d + 1);
   const long long* cr = reinterpret_cast<const long long*>(crow);
-  const int sms = sms_or_default();
+  const int sms = sm_count_or_default();
   BKM_CUDA_TRY(cudaMemsetAsync(status, 0, ST_N * 8, s));
   if (n > 0) {
     expand_kernel<<<grid_for(n, kWarps, 16 * sms), kThreads, 0, s>>>(cr, reinterpret_cast<const long long*>(col), n, d,
@@ -655,7 +622,7 @@ extern "C" int bkm_csc_matvec_chunk(const int64_t* colptr, const int32_t* rows, 
   a.ticket = reinterpret_cast<unsigned*>(ws + align_up((size_t)seg_cap(d, nnz) * 16, 256));
   a.first = (flags & BKM_FLAG_FIRST_CHUNK) ? 1 : 0;
   BKM_CUDA_TRY(cudaMemsetAsync(a.ticket, 0, (size_t)d * 4, s));
-  const int grid = grid_for(seg_cap(d, nnz), kWarps, 16 * sms_or_default());
+  const int grid = grid_for(seg_cap(d, nnz), kWarps, 16 * sm_count_or_default());
   if (val_dtype == BKM_F32) csc_matvec_kernel<float><<<grid, kThreads, 0, s>>>(a);
   else csc_matvec_kernel<double><<<grid, kThreads, 0, s>>>(a);
   BKM_CUDA_TRY(cudaGetLastError());
@@ -695,7 +662,7 @@ extern "C" int bkm_gram_weighted_csr_chunk(const int64_t* crow, const int64_t* c
   a.ticket = reinterpret_cast<unsigned*>(ws + align_up((size_t)n_slots * d * 8, 256));
   a.first = (flags & BKM_FLAG_FIRST_CHUNK) ? 1 : 0;
   BKM_CUDA_TRY(cudaMemsetAsync(a.ticket, 0, (size_t)d * 4, s));
-  const int sms = sms_or_default();
+  const int sms = sm_count_or_default();
   const int per_sm = (228 * 1024) / (W * d * 8 + 1024);
   const int grid = grid_for(seg_cap(d, nnz), 1, (per_sm < 1 ? 1 : per_sm) * sms);
   const size_t smem = (size_t)W * d * 8;

@@ -2,9 +2,8 @@
 // multi-rank merge are the per-column key tables of bkm_keys.cu.
 //
 //   bkm_impute_stats_chunk   per column, in float64 and in one read of X: the missing count, the NaN and inf counts and
-//                            sum (x - s) over the non-missing finite x.  Same geometry and fold as bkm_colstats_chunk:
-//                            threads add their rows in row order, row groups and then CTA partials are added in a fixed
-//                            order (a ticket counter elects the last CTA), so two calls give the same bits.
+//                            sum (x - s) over the non-missing finite x.  The layout and fold of column_reduce
+//                            (bkm_select.cuh), so two calls give the same bits.
 //   bkm_impute_chunk         one read of X, one write of the output: kept columns with missing elements replaced by
 //                            their statistic, then 0 / 1 indicator columns; NaN / inf counted on the way for validation.
 //                            The inverse writes the missing value where an indicator is 1.
@@ -30,22 +29,12 @@ struct IStatsArgs {
   int first;
 };
 
-static int istats_grid(long long n, int d, int sms) {
-  const int G = kThreads / col_block(d);
-  long long g = (n + 16LL * G - 1) / (16LL * G);
-  if (g > 4LL * sms) g = 4LL * sms;
-  if (g < 1) g = 1;
-  return (int)g;
-}
-
-static size_t istats_ws(long long n, int d, int sms) {
-  return align_up((size_t)istats_grid(n, d, sms) * IS_N * (size_t)d * 8, 256) + 256;
-}
-
+// column_reduce's layout and fold (bkm_select.cuh), written out: with this row loop passed to column_reduce, ptxas
+// gives the float64 kernel 70 registers instead of 54, so 3 CTAs per SM are resident instead of 4 and the kernel took
+// 28 % longer on 10M x 64 float64 rows (H100 80GB HBM3, 700 W).
 template <typename T>
 __global__ void __launch_bounds__(kThreads) impute_stats_kernel(IStatsArgs a) {
   __shared__ double s_fold[IS_N][kThreads];
-  __shared__ int s_last;
   const int tid = threadIdx.x;
   const int d = a.d;
   const int CB = col_block(d), G = kThreads / CB;
@@ -102,12 +91,7 @@ __global__ void __launch_bounds__(kThreads) impute_stats_kernel(IStatsArgs a) {
     }
   }
 
-  __threadfence();
-  __syncthreads();
-  if (tid == 0) s_last = atomicAdd(a.ticket, 1u) == gridDim.x - 1;
-  __syncthreads();
-  if (!s_last) return;
-  __threadfence();
+  if (!last_block(a.ticket, gridDim.x)) return;
   for (int e = tid; e < IS_N * d; e += kThreads) {
     double v = 0.0;
     for (unsigned c = 0; c < gridDim.x; ++c) v += __ldcg(a.part + (size_t)c * IS_N * d + e);
@@ -212,11 +196,7 @@ __global__ void __launch_bounds__(kThreads) impute_fill_kernel(FillArgs p) {
 template <typename T, typename C>
 static int launch_fill(const FillArgs& p, int sms, cudaStream_t s) {
   const int tasks = p.inverse ? p.d_out : p.n_keep + p.n_ind + p.n_check;
-  const int G = kThreads / col_block(tasks);
-  long long g = (p.n + 8LL * G - 1) / (8LL * G);
-  if (g > 8LL * sms) g = 8LL * sms;
-  if (g < 1) g = 1;
-  impute_fill_kernel<T, C><<<(unsigned)g, kThreads, 0, s>>>(p);
+  impute_fill_kernel<T, C><<<col_pass_grid(p.n, tasks, sms), kThreads, 0, s>>>(p);
   BKM_CUDA_TRY(cudaGetLastError());
   note_launch();
   return 0;
@@ -229,9 +209,7 @@ using namespace bkm;
 
 extern "C" int bkm_impute_stats_workspace_bytes(int64_t n, int d, size_t* out) {
   if (!out || n < 0 || d <= 0) return BKM_EINVAL;
-  int sms = 0;
-  if (sm_count(&sms) != 0 || sms <= 0) sms = kDefaultSMs;
-  *out = istats_ws(n, d, sms);
+  *out = partials_bytes(reduce_grid(n, kThreads / col_block(d), 4, sm_count_or_default()), IS_N * (size_t)d);
   return 0;
 }
 
@@ -244,16 +222,14 @@ extern "C" int bkm_impute_stats_chunk(const void* X, int64_t n, int d, int64_t l
   int sms = 0;
   const int rc = sm_count(&sms);
   if (rc) return rc;
-  if (ws_bytes < istats_ws(n, d, sms)) return BKM_EWORKSPACE;
+  const int grid = reduce_grid(n, kThreads / col_block(d), 4, sms);
+  const size_t need = partials_bytes(grid, IS_N * (size_t)d);
+  if (ws_bytes < need) return BKM_EWORKSPACE;
   cudaStream_t s = (cudaStream_t)stream;
   IStatsArgs a;
   a.X = X; a.n = n; a.d = d; a.ldx = ldx; a.miss.is_nan = miss_is_nan; a.miss.value = miss_value; a.shift = shift;
   a.acc = acc; a.first = (flags & BKM_FLAG_FIRST_CHUNK) ? 1 : 0;
-  unsigned char* ws = reinterpret_cast<unsigned char*>(workspace);
-  a.part = reinterpret_cast<double*>(ws);
-  a.ticket = reinterpret_cast<unsigned int*>(ws + istats_ws(n, d, sms) - 256);
-  BKM_CUDA_TRY(cudaMemsetAsync(a.ticket, 0, 4, s));
-  const int grid = istats_grid(n, d, sms);
+  BKM_CUDA_TRY(carve_partials(workspace, need, &a.part, &a.ticket, s));
   if (x_dtype == BKM_F32) impute_stats_kernel<float><<<grid, kThreads, 0, s>>>(a);
   else if (x_dtype == BKM_F64) impute_stats_kernel<double><<<grid, kThreads, 0, s>>>(a);
   else impute_stats_kernel<__nv_bfloat16><<<grid, kThreads, 0, s>>>(a);

@@ -4,11 +4,9 @@
 //                        EQ       one output column: [sum w [row of a == row of b] | sum w]
 //                        ERR      m output columns:  [sum (b - a)^2 | sum |b - a| | sum (a - s_j) | sum (a - s_j)^2]
 //                        LOGLOSS  one output column: [sum -w log(q[a] / sum_j q_j) | sum w], q = clip(p, eps, 1 - eps)
-//                      The geometry is the one of bkm_colstats_chunk: the threads split into G row groups of CB columns
-//                      (ERR: CB = min(m, 256) output columns, so that the CTA's loads are contiguous whatever m is;
-//                      EQ / LOGLOSS: CB = 1, a thread owns whole rows).  A thread adds its rows in row order, the row
-//                      groups are added in order, each CTA writes its partial to the workspace and the last CTA to finish
-//                      (a ticket counter) folds the partials in CTA order: same inputs, same bits, no float atomics.
+//                      A column_reduce pass (bkm_select.cuh), same inputs, same bits: ERR with CB = min(m, 256) output
+//                      columns, so that the CTA's loads are contiguous whatever m is; EQ / LOGLOSS with CB = 1, a thread
+//                      owns whole rows.
 //                      The operands' element types are run-time codes: the pass is bound by memory, and a uniform
 //                      switch per load costs nothing next to it, where a template over both types would be 49 kernels.
 #include "bkm_select.cuh"
@@ -60,44 +58,25 @@ static bool metric_dtype_ok(int dt) { return dt >= BKM_F32 && dt <= BKM_M_U8; }
 
 __host__ __device__ __forceinline__ int metric_cols(int m, int mode) { return mode == BKM_METRIC_ERR ? m : 1; }
 
+// at most 8 CTAs per SM
 static int metric_grid(long long n, int m, int mode, int sms) {
   const int cols = metric_cols(m, mode);
-  const int G = kThreads / (cols < kThreads ? cols : kThreads);
-  long long g = (n + 16LL * G - 1) / (16LL * G);     // at least 16 rows per thread
-  if (g > 8LL * sms) g = 8LL * sms;
-  return (int)(g < 1 ? 1 : g);
-}
-
-static size_t metric_ws(long long n, int m, int mode, int sms) {
-  return align_up((size_t)metric_grid(n, m, mode, sms) * kStats * (size_t)metric_cols(m, mode) * 8, 256) + 256;
+  return reduce_grid(n, kThreads / (cols < kThreads ? cols : kThreads), 8, sms);
 }
 
 // NaN stays NaN, as in np.clip
 __device__ __forceinline__ double clip(double p, double lo, double hi) { return p < lo ? lo : (p > hi ? hi : p); }
 
-__global__ void __launch_bounds__(kThreads) metric_kernel(MetricArgs a) {
-  __shared__ double s_fold[kStats][kThreads];
-  __shared__ int s_last;
-  const int tid = threadIdx.x;
-  const int m = a.m, mode = a.mode;
-  const int cols = metric_cols(m, mode);
-  const int CB = min(cols, kThreads), G = kThreads / CB;
-  const int bc = tid % CB, bg = tid / CB;
-  const long long per = (a.n + gridDim.x - 1) / gridDim.x;
-  const long long rb = (long long)blockIdx.x * per, re = min(a.n, rb + per);
-  double* part = a.part + (size_t)blockIdx.x * kStats * cols;
-  const bool both_int = is_int_code(a.a_dt) && is_int_code(a.b_dt);
-  const double hi = 1.0 - a.eps;
-
-#pragma unroll 1
-  for (int j0 = 0; j0 < cols; j0 += CB) {
-    const int j = j0 + bc;
-    const bool on = bg < G && j < cols;
-    double f[kStats] = {0.0, 0.0, 0.0, 0.0};
-    if (on && mode == BKM_METRIC_ERR) {
+struct MetricRows {
+  const MetricArgs& a;
+  bool both_int;
+  double hi;
+  __device__ __forceinline__ void operator()(double (&f)[kStats], int j, long long r0, long long re, int G) const {
+    const int m = a.m;
+    if (a.mode == BKM_METRIC_ERR) {
       const double s = a.shift ? a.shift[j] : 0.0;
 #pragma unroll 4
-      for (long long r = rb + bg; r < re; r += G) {
+      for (long long r = r0; r < re; r += G) {
         const double x = load_f64(a.a, a.a_dt, r * m + j), y = load_f64(a.b, a.b_dt, r * m + j);
         const double dl = y - x, t = x - s;
         f[0] = fma(dl, dl, f[0]);
@@ -105,9 +84,9 @@ __global__ void __launch_bounds__(kThreads) metric_kernel(MetricArgs a) {
         f[2] += t;
         f[3] = fma(t, t, f[3]);
       }
-    } else if (on && mode == BKM_METRIC_EQ) {
+    } else if (a.mode == BKM_METRIC_EQ) {
 #pragma unroll 2
-      for (long long r = rb + bg; r < re; r += G) {
+      for (long long r = r0; r < re; r += G) {
         bool eq = true;
         for (int q = 0; q < m; ++q) {
           const long long e = r * m + q;
@@ -118,9 +97,9 @@ __global__ void __launch_bounds__(kThreads) metric_kernel(MetricArgs a) {
         f[0] += eq ? wt : wt * 0.0;          // a NaN or infinite weight reaches the sum as numpy's w * [eq] does
         f[1] += wt;
       }
-    } else if (on) {
+    } else {
 #pragma unroll 2
-      for (long long r = rb + bg; r < re; r += G) {
+      for (long long r = r0; r < re; r += G) {
         const long long cls = load_i64(a.a, a.a_dt, r);
         double sum, pick;
         if (m == 1) {
@@ -141,41 +120,15 @@ __global__ void __launch_bounds__(kThreads) metric_kernel(MetricArgs a) {
         f[1] += wt;
       }
     }
-    // the row groups, in order
-    if (G > 1) {
-#pragma unroll
-      for (int k = 0; k < kStats; ++k) s_fold[k][tid] = f[k];
-      __syncthreads();
-      if (bg == 0 && on) {
-        for (int g = 1; g < G; ++g) {
-#pragma unroll
-          for (int k = 0; k < kStats; ++k) f[k] += s_fold[k][g * CB + bc];
-        }
-#pragma unroll
-        for (int k = 0; k < kStats; ++k) part[(size_t)k * cols + j] = f[k];
-      }
-      __syncthreads();
-    } else if (on) {
-#pragma unroll
-      for (int k = 0; k < kStats; ++k) part[(size_t)k * cols + j] = f[k];
-    }
   }
+};
 
-  __threadfence();
-  __syncthreads();
-  if (tid == 0) s_last = atomicAdd(a.ticket, 1u) == gridDim.x - 1;
-  __syncthreads();
-  if (!s_last) return;
-  __threadfence();
-
-  // ---- the last CTA: the CTA partials in CTA order ----
-  const int nout = (mode == BKM_METRIC_ERR ? kStats : 2) * cols;      // part rows [0, nout / cols) are the live ones
-  for (int e = tid; e < nout; e += kThreads) {
-    double v = 0.0;
-    for (unsigned c = 0; c < gridDim.x; ++c) v += __ldcg(a.part + (size_t)c * kStats * cols + e);
-    a.acc[e] = a.first ? v : a.acc[e] + v;
-  }
-  if (tid == 0) *a.ticket = 0u;
+// ERR writes its four rows, EQ and LOGLOSS their first two
+__global__ void __launch_bounds__(kThreads) metric_kernel(MetricArgs a) {
+  const int cols = metric_cols(a.m, a.mode);
+  const MetricRows rows{a, is_int_code(a.a_dt) && is_int_code(a.b_dt), 1.0 - a.eps};
+  const SumFold fold{a.acc, cols, a.mode == BKM_METRIC_ERR ? kStats : 2, a.first};
+  column_reduce<kStats>(rows, fold, a.n, cols, min(cols, kThreads), a.part, a.ticket);
 }
 
 }  // namespace
@@ -185,9 +138,7 @@ using namespace bkm;
 
 extern "C" int bkm_metric_workspace_bytes(int64_t n, int m, int mode, size_t* out) {
   if (!out || n < 0 || m <= 0 || mode < BKM_METRIC_EQ || mode > BKM_METRIC_LOGLOSS) return BKM_EINVAL;
-  int sms = 0;
-  if (sm_count(&sms) != 0 || sms <= 0) sms = kDefaultSMs;
-  *out = metric_ws(n, m, mode, sms);
+  *out = partials_bytes(metric_grid(n, m, mode, sm_count_or_default()), kStats * (size_t)metric_cols(m, mode));
   return 0;
 }
 
@@ -204,17 +155,16 @@ extern "C" int bkm_metric_chunk(const void* a, int a_dtype, const void* b, int b
   int sms = 0;
   const int rc = sm_count(&sms);
   if (rc) return rc;
-  if (ws_bytes < metric_ws(n, m, mode, sms)) return BKM_EWORKSPACE;
+  const int grid = metric_grid(n, m, mode, sms);
+  const size_t need = partials_bytes(grid, kStats * (size_t)metric_cols(m, mode));
+  if (ws_bytes < need) return BKM_EWORKSPACE;
   cudaStream_t s = (cudaStream_t)stream;
   MetricArgs g;
   g.a = a; g.b = b; g.a_dt = a_dtype; g.b_dt = b_dtype; g.w = mode == BKM_METRIC_ERR ? nullptr : w;
   g.n = n; g.m = m; g.mode = mode; g.shift = shift; g.eps = eps; g.acc = acc;
   g.first = (flags & BKM_FLAG_FIRST_CHUNK) ? 1 : 0;
-  unsigned char* ws = reinterpret_cast<unsigned char*>(workspace);
-  g.part = reinterpret_cast<double*>(ws);
-  g.ticket = reinterpret_cast<unsigned int*>(ws + metric_ws(n, m, mode, sms) - 256);
-  BKM_CUDA_TRY(cudaMemsetAsync(g.ticket, 0, 4, s));
-  metric_kernel<<<metric_grid(n, m, mode, sms), kThreads, 0, s>>>(g);
+  BKM_CUDA_TRY(carve_partials(workspace, need, &g.part, &g.ticket, s));
+  metric_kernel<<<grid, kThreads, 0, s>>>(g);
   BKM_CUDA_TRY(cudaGetLastError());
   note_launch();
   return 0;

@@ -474,15 +474,6 @@ __global__ void __launch_bounds__(JT, 4) jll_kernel(JllArgs a, JllSmem L) {
   }
 }
 
-static bool dtype_ok(int t) { return t == BKM_F32 || t == BKM_F64 || t == BKM_BF16; }
-
-static int sm_count(int* out) {
-  int dev = 0;
-  BKM_CUDA_TRY(cudaGetDevice(&dev));
-  BKM_CUDA_TRY(cudaDeviceGetAttribute(out, cudaDevAttrMultiProcessorCount, dev));
-  return 0;
-}
-
 template <typename T>
 static int launch_moments(const MomArgs& a, const MomGeom& G, cudaStream_t s) {
   BKM_CUDA_TRY(cudaFuncSetAttribute(moments_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)G.smem));
@@ -546,9 +537,7 @@ using namespace bkm;
 
 extern "C" int bkm_nb_workspace_bytes(int64_t n, int d, int K, size_t* out) {
   if (!out || n < 0 || d <= 0 || K <= 0) return BKM_EINVAL;
-  int sms = 0;
-  if (sm_count(&sms) != 0 || sms <= 0) sms = kDefaultSMs;
-  *out = mom_geom(n, d, K, sms).total;
+  *out = mom_geom(n, d, K, sm_count_or_default()).total;
   return 0;
 }
 

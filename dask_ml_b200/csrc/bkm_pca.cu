@@ -110,7 +110,6 @@ __global__ void __launch_bounds__(kThreads) gram_kernel(GramArgs a) {
   T* raw = reinterpret_cast<T*>(smem + 2 * GR * GP * 8);
   double* cred = reinterpret_cast<double*>(smem + 2 * GR * GP * 8 + 2 * 2 * GR * GB * sizeof(T));
   const uint32_t bar0 = smem_u32(cred + 4 * GB);
-  __shared__ int s_last;
 
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int d = a.d;
@@ -237,12 +236,7 @@ __global__ void __launch_bounds__(kThreads) gram_kernel(GramArgs a) {
     if (tid < GB)
       a.cpart[((size_t)bi * a.splits + split) * GB + tid] = ((cred[tid] + cred[GB + tid]) + cred[2 * GB + tid]) + cred[3 * GB + tid];
   }
-  __threadfence();
-  __syncthreads();
-  if (tid == 0) s_last = atomicAdd(&a.ticket[pair], 1u) == (unsigned)(a.splits - 1);
-  __syncthreads();
-  if (!s_last) return;
-  __threadfence();
+  if (!last_block(&a.ticket[pair], (unsigned)a.splits)) return;
 
   // ---- the last CTA of the tile: the splits in order, then the tile and its mirror ----
   const double* P0 = a.part + (size_t)pair * a.splits * tile_elems;
@@ -409,16 +403,6 @@ __global__ void __launch_bounds__(kThreads) project_kernel(ProjArgs a) {
   }
 }
 
-static bool dtype_ok(int t) { return t == BKM_F32 || t == BKM_F64 || t == BKM_BF16; }
-static size_t esize(int t) { return t == BKM_F64 ? 8 : (t == BKM_F32 ? 4 : 2); }
-
-static int sm_count(int* out) {
-  int dev = 0;
-  BKM_CUDA_TRY(cudaGetDevice(&dev));
-  BKM_CUDA_TRY(cudaDeviceGetAttribute(out, cudaDevAttrMultiProcessorCount, dev));
-  return 0;
-}
-
 template <typename T, bool WEIGHTED = false>
 static int launch_gram(const GramArgs& a, int pairs, int splits, cudaStream_t s) {
   const size_t sm = gram_smem_bytes<T>();
@@ -456,7 +440,7 @@ static int gram_run(const void* X, int64_t n, int d, int64_t ldx, int x_dtype, c
   cudaStream_t s = (cudaStream_t)stream;
   unsigned char* ws = reinterpret_cast<unsigned char*>(workspace);
   BKM_CUDA_TRY(cudaMemsetAsync(ws + G.off_ticket, 0, (size_t)G.pairs * 4, s));
-  const size_t es = esize(x_dtype);
+  const size_t es = elem_size(x_dtype);
   GramArgs a;
   a.X = X; a.n = n; a.d = d; a.ldx = ldx; a.shift = shift; a.colsum = colsum; a.gram = gram; a.w = w;
   a.part = reinterpret_cast<double*>(ws + G.off_part);
@@ -478,9 +462,7 @@ using namespace bkm;
 
 extern "C" int bkm_gram_workspace_bytes(int64_t n, int d, size_t* out) {
   if (!out || n < 0 || d <= 0) return BKM_EINVAL;
-  int sms = 0;
-  if (sm_count(&sms) != 0 || sms <= 0) sms = kDefaultSMs;
-  *out = gram_geom(n, d, sms).total;
+  *out = gram_geom(n, d, sm_count_or_default()).total;
   return 0;
 }
 

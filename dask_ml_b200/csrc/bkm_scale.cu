@@ -2,11 +2,8 @@
 // (sm_90a).
 //
 //   bkm_colstats_chunk     per column, in float64 and in one read of X: sum (x - s) and sum (x - s)^2 over the finite
-//                          x, min and max over the non-NaN x, and the counts of NaN, +inf and -inf.  The threads split
-//                          the columns into passes of CB columns and the CTA's rows into G interleaved row groups; each
-//                          thread adds its rows in row order, the row groups are added in order, each CTA writes its
-//                          partial to the workspace and the last CTA to finish (a ticket counter) folds the partials
-//                          in CTA order.  So two calls with the same inputs give the same bits, without float atomics.
+//                          x, min and max over the non-NaN x, and the counts of NaN, +inf and -inf.  A column_reduce
+//                          pass (bkm_select.cuh): two calls with the same inputs give the same bits.
 //   bkm_radix_hist_chunk   one round of an exact radix select: every value maps to an order-preserving unsigned key
 //                          (16 bits for bf16, 32 for fp32, 64 for fp64); for each (column, target) it counts the next
 //                          8-bit digit of the keys that carry the target's prefix.  Targets with equal prefixes share
@@ -43,118 +40,63 @@ struct StatsArgs {
   int first;
 };
 
-static int stats_grid(long long n, int d, int sms) {
-  const int G = kThreads / col_block(d);
-  long long g = (n + 16LL * G - 1) / (16LL * G);     // at least 16 rows per thread
-  if (g > 4LL * sms) g = 4LL * sms;
-  if (g < 1) g = 1;
-  return (int)g;
-}
-
-static size_t stats_ws(long long n, int d, int sms) {
-  return align_up((size_t)stats_grid(n, d, sms) * ST_N * (size_t)d * 8, 256) + 256;
-}
-
 template <typename T>
-__global__ void __launch_bounds__(kThreads) colstats_kernel(StatsArgs a) {
-  __shared__ double s_fold[ST_N][kThreads];
-  __shared__ int s_last;
-  const int tid = threadIdx.x;
-  const int d = a.d;
-  const int CB = col_block(d), G = kThreads / CB;
-  const int bc = tid % CB, bg = tid / CB;
-  const T* X = reinterpret_cast<const T*>(a.X);
-  const long long per = (a.n + gridDim.x - 1) / gridDim.x;
-  const long long rb = (long long)blockIdx.x * per, re = min(a.n, rb + per);
-  double* part = a.part + (size_t)blockIdx.x * ST_N * d;
-  constexpr int U = 8;
-
+struct StatsRows {
+  const StatsArgs& a;
+  __device__ __forceinline__ void operator()(double (&f)[ST_N], int j, long long r0, long long re, int G) const {
+    const T* X = reinterpret_cast<const T*>(a.X);
+    const double s = a.shift ? a.shift[j] : 0.0;
+    constexpr int U = 8;
 #pragma unroll 1
-  for (int j0 = 0; j0 < d; j0 += CB) {
-    const int j = j0 + bc;
-    const bool on = j < d;
-    const double s = (on && a.shift) ? a.shift[j] : 0.0;
-    double sum = 0.0, sq = 0.0, cn = 0.0, cp = 0.0, cm = 0.0, mn = CUDART_INF, mx = -CUDART_INF;
-    if (on) {
-#pragma unroll 1
-      for (long long r = rb + bg; r < re; r += (long long)G * U) {
-        T v[U];
+    for (long long r = r0; r < re; r += (long long)G * U) {
+      T v[U];
 #pragma unroll
-        for (int u = 0; u < U; ++u) {
-          const long long rr = r + (long long)u * G;
-          if (rr < re) v[u] = X[rr * a.ldx + j];
-        }
+      for (int u = 0; u < U; ++u) {
+        const long long rr = r + (long long)u * G;
+        if (rr < re) v[u] = X[rr * a.ldx + j];
+      }
 #pragma unroll
-        for (int u = 0; u < U; ++u) {
-          if (r + (long long)u * G < re) {
-            const double x = widen(v[u]);
-            if (x != x) {
-              cn += 1.0;
+      for (int u = 0; u < U; ++u) {
+        if (r + (long long)u * G < re) {
+          const double x = widen(v[u]);
+          if (x != x) {
+            f[ST_NAN] += 1.0;
+          } else {
+            f[ST_MIN] = fmin(f[ST_MIN], x);
+            f[ST_MAX] = fmax(f[ST_MAX], x);
+            if (isinf(x)) {
+              if (x > 0) f[ST_PINF] += 1.0; else f[ST_NINF] += 1.0;
             } else {
-              mn = fmin(mn, x);
-              mx = fmax(mx, x);
-              if (isinf(x)) {
-                if (x > 0) cp += 1.0; else cm += 1.0;
-              } else {
-                const double t = x - s;
-                sum += t;
-                sq = fma(t, t, sq);
-              }
+              const double t = x - s;
+              f[ST_SUM] += t;
+              f[ST_SQ] = fma(t, t, f[ST_SQ]);
             }
           }
         }
       }
     }
-    // the row groups, in order
-    const double mine[ST_N] = {sum, sq, cn, cp, cm, mn, mx};
-    if (G > 1) {
-#pragma unroll
-      for (int k = 0; k < ST_N; ++k) s_fold[k][tid] = mine[k];
-      __syncthreads();
-      if (bg == 0 && on) {
-        double f[ST_N];
-#pragma unroll
-        for (int k = 0; k < ST_N; ++k) f[k] = mine[k];
-        for (int g = 1; g < G; ++g) {
-#pragma unroll
-          for (int k = 0; k < ST_MIN; ++k) f[k] += s_fold[k][g * CB + bc];
-          f[ST_MIN] = fmin(f[ST_MIN], s_fold[ST_MIN][g * CB + bc]);
-          f[ST_MAX] = fmax(f[ST_MAX], s_fold[ST_MAX][g * CB + bc]);
-        }
-#pragma unroll
-        for (int k = 0; k < ST_N; ++k) part[(size_t)k * d + j] = f[k];
-      }
-      __syncthreads();
-    } else if (on) {
-#pragma unroll
-      for (int k = 0; k < ST_N; ++k) part[(size_t)k * d + j] = mine[k];
-    }
   }
+};
 
-  __threadfence();
-  __syncthreads();
-  if (tid == 0) s_last = atomicAdd(a.ticket, 1u) == gridDim.x - 1;
-  __syncthreads();
-  if (!s_last) return;
-  __threadfence();
-
-  // ---- the last CTA: the CTA partials in CTA order ----
-  for (int e = tid; e < ST_N * d; e += kThreads) {
-    const int k = e / d, j = e - k * d;
-    double v = k == ST_MIN ? CUDART_INF : (k == ST_MAX ? -CUDART_INF : 0.0);
-    for (unsigned c = 0; c < gridDim.x; ++c) {
-      const double p = __ldcg(a.part + (size_t)c * ST_N * d + e);
-      v = k == ST_MIN ? fmin(v, p) : (k == ST_MAX ? fmax(v, p) : v + p);
-    }
-    if (k < ST_MIN) {
-      double* dst = a.acc + (size_t)k * d + j;
-      *dst = a.first ? v : *dst + v;
-    } else {
-      double* dst = a.minmax + (size_t)(k - ST_MIN) * d + j;
-      *dst = a.first ? v : (k == ST_MIN ? fmin(*dst, v) : fmax(*dst, v));
-    }
+// sums for the first five statistics, min and max for the last two, which go to minmax
+struct StatsFold {
+  const StatsArgs& a;
+  static constexpr int live = ST_N;
+  __device__ __forceinline__ static double identity(int k) {
+    return k == ST_MIN ? CUDART_INF : (k == ST_MAX ? -CUDART_INF : 0.0);
   }
-  if (tid == 0) *a.ticket = 0u;
+  __device__ __forceinline__ static double combine(int k, double v, double p) {
+    return k == ST_MIN ? fmin(v, p) : (k == ST_MAX ? fmax(v, p) : v + p);
+  }
+  __device__ __forceinline__ void store(int k, int j, double v) const {
+    double* dst = k < ST_MIN ? a.acc + (size_t)k * a.d + j : a.minmax + (size_t)(k - ST_MIN) * a.d + j;
+    *dst = a.first ? v : combine(k, *dst, v);
+  }
+};
+
+template <typename T>
+__global__ void __launch_bounds__(kThreads) colstats_kernel(StatsArgs a) {
+  column_reduce<ST_N>(StatsRows<T>{a}, StatsFold{a}, a.n, a.d, col_block(a.d), a.part, a.ticket);
 }
 
 // ============================================ radix select ============================================
@@ -369,14 +311,6 @@ __global__ void __launch_bounds__(kThreads) affine_kernel(AffineArgs p) {
   }
 }
 
-static int affine_grid(long long n, int d, int sms) {
-  const int G = kThreads / col_block(d);
-  long long g = (n + 8LL * G - 1) / (8LL * G);
-  if (g > 8LL * sms) g = 8LL * sms;
-  if (g < 1) g = 1;
-  return (int)g;
-}
-
 template <typename T, typename C>
 static int launch_affine(const AffineArgs& p, int grid, cudaStream_t s) {
   affine_kernel<T, C><<<grid, kThreads, 0, s>>>(p);
@@ -409,9 +343,7 @@ using namespace bkm;
 
 extern "C" int bkm_colstats_workspace_bytes(int64_t n, int d, size_t* out) {
   if (!out || n < 0 || d <= 0) return BKM_EINVAL;
-  int sms = 0;
-  if (sm_count(&sms) != 0 || sms <= 0) sms = kDefaultSMs;
-  *out = stats_ws(n, d, sms);
+  *out = partials_bytes(reduce_grid(n, kThreads / col_block(d), 4, sm_count_or_default()), ST_N * (size_t)d);
   return 0;
 }
 
@@ -424,16 +356,14 @@ extern "C" int bkm_colstats_chunk(const void* X, int64_t n, int d, int64_t ldx, 
   int sms = 0;
   const int rc = sm_count(&sms);
   if (rc) return rc;
-  if (ws_bytes < stats_ws(n, d, sms)) return BKM_EWORKSPACE;
+  const int grid = reduce_grid(n, kThreads / col_block(d), 4, sms);
+  const size_t need = partials_bytes(grid, ST_N * (size_t)d);
+  if (ws_bytes < need) return BKM_EWORKSPACE;
   cudaStream_t s = (cudaStream_t)stream;
   StatsArgs a;
   a.X = X; a.n = n; a.d = d; a.ldx = ldx; a.shift = shift; a.acc = acc; a.minmax = minmax;
   a.first = (flags & BKM_FLAG_FIRST_CHUNK) ? 1 : 0;
-  unsigned char* ws = reinterpret_cast<unsigned char*>(workspace);
-  a.part = reinterpret_cast<double*>(ws);
-  a.ticket = reinterpret_cast<unsigned int*>(ws + stats_ws(n, d, sms) - 256);
-  BKM_CUDA_TRY(cudaMemsetAsync(a.ticket, 0, 4, s));
-  const int grid = stats_grid(n, d, sms);
+  BKM_CUDA_TRY(carve_partials(workspace, need, &a.part, &a.ticket, s));
   if (x_dtype == BKM_F32) colstats_kernel<float><<<grid, kThreads, 0, s>>>(a);
   else if (x_dtype == BKM_F64) colstats_kernel<double><<<grid, kThreads, 0, s>>>(a);
   else colstats_kernel<__nv_bfloat16><<<grid, kThreads, 0, s>>>(a);
@@ -502,7 +432,7 @@ extern "C" int bkm_affine_chunk(const void* X, int64_t n, int d, int64_t ldx, in
   if (rc) return rc;
   AffineArgs p;
   p.X = X; p.n = n; p.d = d; p.ldx = ldx; p.a = a; p.b = b; p.op1 = op1; p.op2 = op2; p.out = out; p.ldo = ld_out;
-  const int grid = affine_grid(n, d, sms);
+  const int grid = col_pass_grid(n, d, sms);
   cudaStream_t s = (cudaStream_t)stream;
   if (out_dtype == BKM_F32) {
     if (x_dtype == BKM_F32) return launch_affine<float, float>(p, grid, s);

@@ -1,7 +1,8 @@
 // bkm_select.cuh — pieces shared by the scaler passes (bkm_scale.cu), the QuantileTransformer passes
 // (bkm_quantile.cu), SimpleImputer (bkm_impute.cu), the encoders (bkm_encode.cu) and the per-column key tables
-// (bkm_keys.cu): the element helpers, the column-pass geometry, the missing-value test, the order-preserving keys of
-// the exact radix selection and the keys of the key tables.
+// (bkm_keys.cu) and the scoring metrics (bkm_metrics.cu): the element helpers, the column-pass geometry, the
+// deterministic column reduction, the missing-value test, the order-preserving keys of the exact radix selection and the
+// keys of the key tables.
 #pragma once
 #include "bkm_common.cuh"
 #include <cuda_bf16.h>
@@ -19,18 +20,101 @@ __device__ __forceinline__ double widen(__nv_bfloat16 v) { return (double)__bflo
 // kThreads), G = kThreads / CB interleaved row groups
 __host__ __device__ __forceinline__ int col_block(int d) { return min(kThreads, (d + 31) / 32 * 32); }
 
-static int sm_count(int* out) {
-  int dev = 0;
-  BKM_CUDA_TRY(cudaGetDevice(&dev));
-  BKM_CUDA_TRY(cudaDeviceGetAttribute(out, cudaDevAttrMultiProcessorCount, dev));
-  return 0;
+// Grid of the element passes (bkm_affine_chunk, bkm_impute_chunk) over `cols` columns: at least 8 rows per thread, at
+// most 8 CTAs per SM
+static int col_pass_grid(long long n, int cols, int sms) {
+  const int G = kThreads / col_block(cols);
+  long long g = (n + 8LL * G - 1) / (8LL * G);
+  if (g > 8LL * sms) g = 8LL * sms;
+  if (g < 1) g = 1;
+  return (int)g;
 }
 
-static bool dtype_ok(int t) { return t == BKM_F32 || t == BKM_F64 || t == BKM_BF16; }
+// Grid of a column_reduce pass with G row groups: at least 16 rows per thread, at most cap_per_sm CTAs per SM.  Its
+// workspace is partials_bytes(grid, N * cols).
+static int reduce_grid(long long n, int G, int cap_per_sm, int sms) {
+  long long g = (n + 16LL * G - 1) / (16LL * G);
+  if (g > (long long)cap_per_sm * sms) g = (long long)cap_per_sm * sms;
+  if (g < 1) g = 1;
+  return (int)g;
+}
+
+// The deterministic column reduction of the statistics passes (bkm_colstats_chunk, bkm_metric_chunk; written out in
+// bkm_impute_stats_chunk): N float64 statistics of each of `cols` columns over the n rows, with the same bits from two calls
+// with the same inputs and no float atomics.
+//   - The threads split into G = kThreads / CB interleaved row groups of CB columns.  The CTA takes a contiguous range
+//     of rows; for each column, a thread starts f[N] at Fold::identity and runs rows(f, j, first row, end, G), which
+//     adds its rows in row order.
+//   - The row groups are combined in order through shared memory, and each CTA writes its partial [N][cols] to `part`.
+//   - The last CTA to finish (last_block) combines the partials in CTA order and hands row k < fold.live of the
+//     result to fold.store(k, j, v).
+// Fold::combine is the fold rule: a sum, or a min / max.
+template <int N, typename Rows, typename Fold>
+__device__ __forceinline__ void column_reduce(const Rows& rows, const Fold& fold, long long n, int cols, int CB,
+                                              double* part, unsigned* ticket) {
+  __shared__ double s_fold[N][kThreads];
+  const int tid = threadIdx.x;
+  const int G = kThreads / CB;
+  const int bc = tid % CB, bg = tid / CB;
+  const long long per = (n + gridDim.x - 1) / gridDim.x;
+  const long long rb = (long long)blockIdx.x * per, re = min(n, rb + per);
+  double* mine = part + (size_t)blockIdx.x * N * cols;
+
+#pragma unroll 1
+  for (int j0 = 0; j0 < cols; j0 += CB) {
+    const int j = j0 + bc;
+    const bool on = bg < G && j < cols;
+    double f[N];
+#pragma unroll
+    for (int k = 0; k < N; ++k) f[k] = Fold::identity(k);
+    if (on) rows(f, j, rb + bg, re, G);
+    // the row groups, in order
+    if (G > 1) {
+#pragma unroll
+      for (int k = 0; k < N; ++k) s_fold[k][tid] = f[k];
+      __syncthreads();
+      if (bg == 0 && on) {
+        for (int g = 1; g < G; ++g) {
+#pragma unroll
+          for (int k = 0; k < N; ++k) f[k] = Fold::combine(k, f[k], s_fold[k][g * CB + bc]);
+        }
+#pragma unroll
+        for (int k = 0; k < N; ++k) mine[(size_t)k * cols + j] = f[k];
+      }
+      __syncthreads();
+    } else if (on) {
+#pragma unroll
+      for (int k = 0; k < N; ++k) mine[(size_t)k * cols + j] = f[k];
+    }
+  }
+
+  if (!last_block(ticket, gridDim.x)) return;
+  // ---- the last CTA: the CTA partials in CTA order ----
+  for (int e = tid; e < fold.live * cols; e += kThreads) {
+    const int k = e / cols, j = e - k * cols;
+    double v = Fold::identity(k);
+    for (unsigned c = 0; c < gridDim.x; ++c) v = Fold::combine(k, v, __ldcg(part + (size_t)c * N * cols + e));
+    fold.store(k, j, v);
+  }
+  if (tid == 0) *ticket = 0u;
+}
+
+// The fold rule of statistics that are all sums: row k of the result goes to acc[k][cols], written over on the first
+// chunk and added to after it.  Rows from `live` on are not written.
+struct SumFold {
+  double* acc;
+  int cols, live, first;
+  __device__ __forceinline__ static double identity(int) { return 0.0; }
+  __device__ __forceinline__ static double combine(int, double v, double p) { return v + p; }
+  __device__ __forceinline__ void store(int k, int j, double v) const {
+    double* dst = acc + (size_t)k * cols + j;
+    *dst = first ? v : *dst + v;
+  }
+};
+
 static bool enc_dtype_ok(int t) {
   return t == BKM_F32 || t == BKM_F64 || t == BKM_BF16 || t == BKM_M_I32 || t == BKM_M_I64 || t == BKM_M_U8;
 }
-static size_t elem_size(int t) { return t == BKM_F64 ? 8 : (t == BKM_F32 ? 4 : 2); }
 
 // Per (column, target) state of a radix selection, 32 bytes; the host reads `prefix` (the full key after the last
 // round) and `nvalid`.

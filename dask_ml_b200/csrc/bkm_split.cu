@@ -117,12 +117,7 @@ __global__ void __launch_bounds__(kThreads) gather_rows_kernel(GatherArgs a) {
 }
 
 static int grid_for(long long work_items, int per_thread) {
-  int dev = 0, sms = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess ||
-      cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) {
-    (void)cudaGetLastError();
-    sms = kDefaultSMs;
-  }
+  const int sms = sm_count_or_default();
   long long g = (work_items + (long long)kThreads * per_thread - 1) / ((long long)kThreads * per_thread);
   if (g > 16LL * sms) g = 16LL * sms;
   return (int)(g < 1 ? 1 : g);

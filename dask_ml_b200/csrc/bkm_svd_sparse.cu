@@ -196,13 +196,7 @@ __global__ void __launch_bounds__(kThreads) csc_panel_kernel(ColPanelArgs a) {
       }
     }
     if (ns > 1) {
-      __threadfence();
-      __syncwarp();
-      int last = 0;
-      if (lane == 0) last = atomicAdd(a.ticket + j, 1u) == (unsigned)(ns - 1);
-      last = __shfl_sync(0xffffffffu, last, 0);
-      if (!last) continue;
-      __threadfence();
+      if (!last_warp(a.ticket + j, (unsigned)ns)) continue;
       const double* src = a.slot + (size_t)(2 * (s0 - j)) * l;
       for (int cc = lane; cc < l; cc += 32) {
         double v = 0.0;
@@ -216,16 +210,6 @@ __global__ void __launch_bounds__(kThreads) csc_panel_kernel(ColPanelArgs a) {
 
 static size_t slots_bytes(long long nnz, int l) { return align_up((size_t)2 * (nnz / SEG + 1) * l * 8, 256); }
 static size_t col_panel_ws(int p, long long nnz, int l) { return slots_bytes(nnz, l) + align_up((size_t)p * 4, 256); }
-
-static int sm_count_or_default() {
-  int dev = 0, sms = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess ||
-      cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) {
-    (void)cudaGetLastError();
-    sms = kDefaultSMs;
-  }
-  return sms;
-}
 
 static int grid_for(long long work, int per_cta, long long cap) {
   long long g = (work + per_cta - 1) / per_cta;
