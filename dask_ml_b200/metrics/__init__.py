@@ -1,5 +1,5 @@
 """Distance operators on the KMeans path (dask_ml/metrics/pairwise.py:18-97), the kernel built on them (:131-139), and
-the scoring metrics (dask_ml/metrics/classification.py, regression.py)."""
+the scoring metrics (dask_ml/metrics/classification.py, regression.py) and their scorers (scorer.py)."""
 from .classification import accuracy_score, log_loss  # noqa: F401
 from .pairwise import (  # noqa: F401
     euclidean_distances,
@@ -9,3 +9,4 @@ from .pairwise import (  # noqa: F401
     rbf_kernel,
 )
 from .regression import mean_absolute_error, mean_squared_error, r2_score  # noqa: F401
+from .scorer import SCORERS, check_scoring, get_scorer  # noqa: F401

@@ -1,8 +1,8 @@
-"""ShuffleSplit and train_test_split with the dask_ml.model_selection API, executed block-wise on the device.
+"""ShuffleSplit, KFold and train_test_split with the dask_ml.model_selection API, executed block-wise on the device.
 
-Mirrors dask_ml/model_selection/_split.py:24-202 and :321-465 (reference @ 0310a90): every row block is permuted on its
-own and cut into a test part (positions [0, n_test) of the block's permutation) and a train part (the next n_train
-positions), so no row leaves its block, its device or its rank.  Per block of c rows
+Mirrors dask_ml/model_selection/_split.py:24-318 and :321-465 (reference @ 0310a90).  ShuffleSplit: every row block
+is permuted on its own and cut into a test part (positions [0, n_test) of the block's permutation) and a train part (the
+next n_train positions), so no row leaves its block, its device or its rank.  Per block of c rows
 
     seeds     check_random_state(random_state).randint(0, 2**32 - 1, size=n_blocks, dtype="u8")   (the reference's draw)
     sizes     scikit-learn's _validate_shuffle_split(c, test_size, train_size)
@@ -251,6 +251,139 @@ class ShuffleSplit(BaseCrossValidator):
         return self.n_splits
 
 
+def _rank_layout(chunks):
+    """(n, lo): the global number of rows, and the global position of this rank's first row (rank order, then block
+    order).  One ``allgather_obj`` with torch.distributed, none without."""
+    from ..engine import Comm
+
+    comm = Comm()
+    counts = comm.allgather_obj(int(sum(chunks)))
+    return int(sum(counts)), int(sum(counts[:comm.rank]))
+
+
+class KFold(BaseCrossValidator):
+    """K-Folds cross-validator over row blocks (API of dask_ml.model_selection.KFold).
+
+    The global rows, in rank order and then block order, are cut into ``n_splits`` consecutive windows (the first
+    ``n % n_splits`` one row longer); fold f tests window f and trains on the rest.  ``split`` yields
+    ``(train_idx, test_idx)``: int64 ChunkedArrays of row indices (rank-local, as ``ShuffleSplit``'s), made of index
+    pieces in the reference's order: per block of X, the train piece before the window, the test piece, the train
+    piece after it, each piece non-empty and on the device (or host) its block of X is on.  A rank none of whose
+    blocks meets a part holds one 0-row block there.
+
+    ``shuffle=True`` draws one seed per block once per ``split`` call (``ShuffleSplit``'s draw), so every fold sees
+    the same permutation of each block and the test parts partition the rows; positions [a, b) of a block hold
+    ``offset + pi_seed(p)`` for p in [a, b), the split permutation of DESIGN.md A26, one ``bkm_split_indices_chunk``
+    launch per piece of a device block.  Rows never leave their block.  ``random_state`` is ignored without
+    ``shuffle``, as in the reference.
+    """
+
+    def __init__(self, n_splits=5, shuffle=False, random_state=None):
+        if not isinstance(n_splits, numbers.Integral) or isinstance(n_splits, bool):
+            raise ValueError("The number of folds must be of Integral type. %r of type %s was passed."
+                             % (n_splits, type(n_splits)))
+        if n_splits < 2:
+            raise ValueError("k-fold cross-validation requires at least one train/test split by setting n_splits=2 "
+                             "or more, got n_splits={0}.".format(n_splits))
+        if not isinstance(shuffle, bool):
+            raise TypeError("shuffle must be True or False; got {0}".format(shuffle))
+        self.n_splits = int(n_splits)
+        self.shuffle = shuffle
+        self.random_state = random_state
+
+    def _windows(self, chunks):
+        """Per fold, (train, test): lists of (block, start, stop) positions within this rank's blocks."""
+        n, lo = _rank_layout(chunks)
+        if self.n_splits > n:
+            raise ValueError("Cannot have number of splits n_splits={0} greater than the number of samples: "
+                             "n_samples={1}.".format(self.n_splits, n))
+        sizes = np.full(self.n_splits, n // self.n_splits, dtype=np.int64)
+        sizes[: n % self.n_splits] += 1
+        stops = np.cumsum(sizes)
+        starts = stops - sizes
+        folds = []
+        for t0, t1 in zip(starts, stops):
+            train, test = [], []
+            start = lo
+            for i, c in enumerate(chunks):
+                stop = start + c
+                a, b = max(int(t0), start), min(int(t1), stop)
+                if min(a, stop) > start:
+                    train.append((i, 0, min(a, stop) - start))
+                if a < b:
+                    test.append((i, a - start, b - start))
+                if max(b, start) < stop:
+                    train.append((i, max(b, start) - start, c))
+                start = stop
+            folds.append((train, test))
+        return folds
+
+    def split(self, X, y=None, groups=None):
+        X = _as_blocks(X)
+        chunks = X.chunks[0]
+        folds = self._windows(chunks)
+        seeds = _block_seeds(self.random_state, len(chunks)) if self.shuffle else None
+        offsets = np.hstack([0, np.cumsum(chunks)])
+        for train, test in folds:
+            yield tuple(ChunkedArray(self._indices(X, part, seeds, offsets)) for part in (train, test))
+
+    def _indices(self, X, pieces, seeds, offsets):
+        out = []
+        for i, a, b in pieces:
+            blk, c, off = X.blocks[i], int(X.chunks[0][i]), int(offsets[i])
+            dev = _cuda_device(blk)
+            if dev is not None:
+                import torch
+
+                if seeds is None:
+                    out.append(torch.arange(off + a, off + b, dtype=torch.int64, device=dev))
+                else:
+                    out.append(_backend(dev).split_indices_chunk(int(seeds[i]), c, a, b - a, off))
+            elif seeds is None:
+                out.append(np.arange(off + a, off + b, dtype=np.int64))
+            else:
+                out.append(permutation_indices(seeds[i], c, np.arange(a, b)) + off)
+        return out or [_empty_like_rows(X.blocks[0], np.int64)]
+
+    def get_n_splits(self, X=None, y=None, groups=None):
+        return self.n_splits
+
+
+def _empty_like_rows(b, dtype=None):
+    """A 0-row block on the device (or host) of ``b``: of ``b``'s trailing shape and dtype, or 1-D of ``dtype``."""
+    if dtype is None:
+        return b[:0]
+    if _is_torch(b):
+        import torch
+
+        return torch.empty(0, dtype=torch.int64, device=b.device)
+    return np.empty(0, dtype=dtype)
+
+
+def _gather(b, ix, off, validate):
+    """Rows ``ix - off`` of block ``b``, where ``b`` is: the row-gather kernel for a device block, numpy on the host."""
+    n = int(b.shape[0])
+    dev = _cuda_device(b)
+    if dev is not None:
+        import torch
+
+        ix = ix if _is_torch(ix) else torch.as_tensor(np.ascontiguousarray(ix))
+        ix = ix.to(device=dev, dtype=torch.int64)
+        if validate and ix.numel():
+            lo, hi = (int(v) for v in torch.aminmax(ix))
+            if lo < off or hi >= off + n:
+                raise IndexError("index block holds rows outside its block [%d, %d)" % (off, off + n))
+        return _backend(dev).gather_rows_chunk(b, ix, off)
+    ix = ix.cpu().numpy() if _is_torch(ix) else np.asarray(ix)
+    if validate and ix.size and (ix.min() < off or ix.max() >= off + n):
+        raise IndexError("index block holds rows outside its block [%d, %d)" % (off, off + n))
+    if _is_torch(b):
+        import torch
+
+        return b[torch.as_tensor(ix - off)]
+    return np.asarray(b)[ix - off]
+
+
 def _blockwise_slice(arr, idx, validate=True):
     """Slice an array that is blockwise-aligned with idx: block i of the result is ``arr`` block i at the rows
     ``idx`` block i names (global indices, each within block i), on the device (or host) ``arr`` block i is on.
@@ -258,31 +391,47 @@ def _blockwise_slice(arr, idx, validate=True):
     Device blocks go through the row-gather kernel, whatever their dtype; host blocks through numpy.  ``validate``
     checks the index range (the kernel does not); ``train_test_split`` skips it for indices it has just generated."""
     offsets = np.hstack([0, np.cumsum(arr.chunks[0])[:-1]])
+    return ChunkedArray([_gather(b, ix, int(off), validate) for b, ix, off in zip(arr.blocks, idx.blocks, offsets)])
+
+
+def _take(arr, idx):
+    """``arr[idx]`` for index blocks that need not match ``arr``'s blocks: KFold's pieces, ShuffleSplit's parts, or the
+    one host array of indices a scikit-learn splitter returns.  Each index block is cut where its values cross a
+    boundary of ``arr``'s blocks (a binary search on the block offsets) and every cut is gathered from its one source
+    block as ``_blockwise_slice`` gathers, so the result has one block per cut, where its source block is.  A host
+    index block is grouped by source block first (stably, so sorted indices keep their order); a device index block
+    must lie inside one block of ``arr`` (IndexError otherwise), which KFold's and ShuffleSplit's do.  Index values
+    are rank-local, as the splitters give them."""
+    bounds = np.hstack([0, np.cumsum(arr.chunks[0])])
+    n = int(bounds[-1])
     out = []
-    for b, ix, off in zip(arr.blocks, idx.blocks, offsets):
-        off, n = int(off), int(b.shape[0])
-        dev = _cuda_device(b)
-        if dev is not None:
+    for ix in idx.blocks:
+        if _is_torch(ix) and ix.is_cuda:
+            if not ix.numel():
+                continue
             import torch
 
-            ix = ix if _is_torch(ix) else torch.as_tensor(np.ascontiguousarray(ix))
-            ix = ix.to(device=dev, dtype=torch.int64)
-            if validate and ix.numel():
-                lo, hi = (int(v) for v in torch.aminmax(ix))
-                if lo < off or hi >= off + n:
-                    raise IndexError("index block holds rows outside its block [%d, %d)" % (off, off + n))
-            out.append(_backend(dev).gather_rows_chunk(b, ix, off))
-        else:
-            ix = ix.cpu().numpy() if _is_torch(ix) else np.asarray(ix)
-            if validate and ix.size and (ix.min() < off or ix.max() >= off + n):
-                raise IndexError("index block holds rows outside its block [%d, %d)" % (off, off + n))
-            if _is_torch(b):
-                import torch
-
-                out.append(b[torch.as_tensor(ix - off)])
-            else:
-                out.append(np.asarray(b)[ix - off])
-    return ChunkedArray(out)
+            lo, hi = (int(v) for v in torch.aminmax(ix))
+            k = int(np.searchsorted(bounds, lo, side="right")) - 1
+            if lo < 0 or hi >= n or hi >= bounds[k + 1]:
+                raise IndexError("a device index block must name rows of one block of the array; it spans [%d, %d]"
+                                 % (lo, hi))
+            out.append(_gather(arr.blocks[k], ix, int(bounds[k]), validate=False))
+            continue
+        ix = np.asarray(ix.cpu().numpy() if _is_torch(ix) else ix)
+        if ix.dtype == bool:
+            ix = np.flatnonzero(ix)
+        ix = ix.astype(np.int64, copy=False)
+        if ix.size and (ix.min() < 0 or ix.max() >= n):
+            raise IndexError("index out of range for %d rows" % n)
+        which = np.searchsorted(bounds, ix, side="right") - 1
+        if np.any(which[1:] < which[:-1]):
+            order = np.argsort(which, kind="stable")
+            ix, which = ix[order], which[order]
+        cuts = np.flatnonzero(np.diff(which)) + 1
+        for part, k in zip(np.split(ix, cuts), which[np.hstack([0, cuts]).astype(np.int64)] if ix.size else []):
+            out.append(_gather(arr.blocks[int(k)], part, int(bounds[k]), validate=False))
+    return ChunkedArray(out or [_empty_like_rows(arr.blocks[0])])
 
 
 def train_test_split(*arrays, **options):
