@@ -106,6 +106,17 @@ SIGNATURES = {
     "bkm_csc_panel_workspace_bytes": (_int, [_int, _i64, _int, _szp]),
     "bkm_csc_panel_chunk": (_int, [_c_void_p, _c_void_p, _c_void_p, _int, _int, _i64, _c_void_p, _c_void_p, _int,
                                    _c_void_p, _c_void_p, ctypes.c_size_t, _int, _c_void_p]),
+    "bkm_sparse_pack_workspace_bytes": (_int, [_int, _int, _szp]),
+    "bkm_sparse_pack_centers": (_int, [_c_void_p, _int, _int, _c_void_p, _c_void_p, ctypes.c_size_t, _c_void_p]),
+    "bkm_csr_assign_workspace_bytes": (_int, [_i64, _int, _szp]),
+    "bkm_csr_assign_chunk": (_int, [_c_void_p, _c_void_p, _c_void_p, _int, _i64, _int, _i64, _c_void_p, _int, _int,
+                                    _c_void_p, _c_void_p, _int, _c_void_p, _c_void_p, _c_void_p, _i64, _int, _c_void_p,
+                                    ctypes.c_size_t, _int, _c_void_p, _c_void_p]),
+    "bkm_csc_label_sums_workspace_bytes": (_int, [_int, _i64, _int, _szp]),
+    "bkm_csc_label_sums_chunk": (_int, [_c_void_p, _c_void_p, _c_void_p, _int, _int, _i64, _c_void_p, _c_void_p, _int,
+                                        _c_void_p, _c_void_p, ctypes.c_size_t, _int, _c_void_p, _c_void_p]),
+    "bkm_sparse_finalize_step": (_int, [_c_void_p, _c_void_p, _c_void_p, _c_void_p, _int, _int, _c_void_p,
+                                        ctypes.c_size_t, _c_void_p]),
     "bkm_colstats_workspace_bytes": (_int, [_i64, _int, _szp]),
     "bkm_colstats_chunk": (_int, [_c_void_p, _i64, _int, _i64, _int, _c_void_p, _c_void_p, _c_void_p, _c_void_p,
                                   ctypes.c_size_t, _int, _c_void_p]),

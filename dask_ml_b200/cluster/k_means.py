@@ -12,11 +12,13 @@ import logging
 from numbers import Integral
 
 import numpy as np
+import scipy.sparse
 import torch
 from sklearn.base import BaseEstimator, TransformerMixin
 from sklearn.utils.validation import check_is_fitted
 
 from ..chunked import ChunkedArray, as_chunked, is_dask_array, is_dask_dataframe, _is_torch
+from .._sparse import _SparseData, _sparse_data
 from ..engine import Comm, CudaBackend, DeviceData, _NP_TO_TORCH
 from ..utils import _timed, _timer, check_array
 
@@ -52,9 +54,14 @@ def _block_np_dtype(b):
 
 
 def _to_device_data(X, backend=None, comm=None, check_finite=True):
-    """Validated array-like -> DeviceData (rows resident on the device)."""
-    if isinstance(X, DeviceData):
+    """Validated array-like -> DeviceData (rows resident on the device), or ``_SparseData`` for sparse X."""
+    if isinstance(X, (DeviceData, _SparseData)):
         return X
+    sp = _sparse_data(X)
+    if sp is not None:
+        if check_finite:
+            sp.check_finite()
+        return sp
     backend = backend or _get_backend()
     blocks = _to_blocks(X)
     from ..chunked import is_bf16_block
@@ -148,8 +155,12 @@ class KMeans(TransformerMixin, BaseEstimator):
             pass
         if is_dask_dataframe(X):
             raise TypeError("Cannot fit on dask.dataframe due to unknown partition lengths.")
-        if isinstance(X, DeviceData):
+        if isinstance(X, (DeviceData, _SparseData)):
             return X
+        sp = _sparse_data(X)                    # sparse CSR blocks (engine extension: the reference rejects them)
+        if sp is not None:
+            sp.check_finite()
+            return sp
         X = check_array(
             X,
             accept_dask_dataframe=False,
@@ -157,6 +168,11 @@ class KMeans(TransformerMixin, BaseEstimator):
             accept_sparse=False,
         )
         return _to_device_data(X)
+
+    def __sklearn_tags__(self):
+        tags = super().__sklearn_tags__()
+        tags.input_tags.sparse = True           # sparse CSR blocks run through the sparse passes
+        return tags
 
     def fit(self, X, y=None):
         X = self._check_array(X)
@@ -179,7 +195,7 @@ class KMeans(TransformerMixin, BaseEstimator):
         return self
 
     def _check_n_features(self, X):
-        d = X.d if isinstance(X, DeviceData) else X.shape[1]
+        d = X.d if isinstance(X, (DeviceData, _SparseData)) else X.shape[1]
         n_in = getattr(self, "n_features_in_", self.cluster_centers_.shape[1])
         if d != n_in:
             raise ValueError(
@@ -263,7 +279,7 @@ def k_init(
     weighted=False,
 ):
     """Choose the initial centres (k_means.py:291-369).  Returns np.ndarray (k, d)."""
-    n_features = X.d if isinstance(X, DeviceData) else X.shape[1]
+    n_features = X.d if isinstance(X, (DeviceData, _SparseData)) else X.shape[1]
     if isinstance(init, np.ndarray):
         K, P = init.shape
 
@@ -285,6 +301,8 @@ def k_init(
         raise ValueError("'init' must be one of {}, got {}".format(valid, init))
 
     X = _to_device_data(X, check_finite=False)
+    if weighted and isinstance(X, _SparseData):
+        raise NotImplementedError("weighted k-means|| is not implemented for sparse X")
     if isinstance(random_state, Integral) or random_state is None:
         random_state = _as_random_state(random_state, X.comm)
 
@@ -315,7 +333,8 @@ def init_random(X, n_clusters, random_state):
     """Centres = randomly chosen rows (k_means.py:387-393)."""
     logger.info("Initializing randomly")
     idx = sorted(random_state.randint(0, X.n_global, size=n_clusters))
-    return X.global_rows(idx)
+    rows = X.global_rows(idx)
+    return rows.toarray() if scipy.sparse.issparse(rows) else rows
 
 
 class _AssignPass(object):
@@ -350,6 +369,52 @@ class _AssignPass(object):
         return v
 
 
+class _SparseAssignPass(_AssignPass):
+    """``_AssignPass`` over sparse CSR blocks (``bkm_csr_assign_chunk``): the centres (dense, or the sparse candidate
+    rows of k-means||) are densified on the device into the sparse pack; the minimum is float64."""
+
+    def run(self, centers64, want_labels=False, want_min=False, squared=True):
+        be, X = self.be, self.X
+        C = _dense_centres(centers64, X.d, be)
+        k = int(C.shape[0])
+        pack = be.sparse_pack_centers(C)
+        acc = be.zeros((1,), torch.float64)
+        labels, mins = [], []
+        for blk in X.blocks:
+            n = int(blk[3])
+            lab = be.empty((n,), torch.int32) if want_labels else None
+            mn = be.empty((n,), torch.float64) if want_min else None
+            be.csr_assign_chunk(blk, X.d, pack, k, labels=lab, min_dist=mn, squared=squared, dist_sum=acc)
+            labels.append(lab)
+            mins.append(mn)
+        X.comm.allreduce_sum_(acc)
+        return labels, mins, acc
+
+
+def _dense_centres(C, d, be):
+    """(k, d) float64 device centres from an array or a host scipy CSR (densified on the device)."""
+    if not scipy.sparse.issparse(C):
+        return torch.as_tensor(np.ascontiguousarray(C, dtype=np.float64)).to(be.device)
+    C = scipy.sparse.csr_matrix(C)
+    out = be.zeros((C.shape[0], d), torch.float64)
+    rows = np.repeat(np.arange(C.shape[0], dtype=np.int64), np.diff(C.indptr))
+    if len(rows):
+        out[torch.as_tensor(rows).to(be.device), torch.as_tensor(C.indices.astype(np.int64)).to(be.device)] = \
+            torch.as_tensor(C.data.astype(np.float64)).to(be.device)
+    return out
+
+
+def _assign_pass(X):
+    return _SparseAssignPass(X) if isinstance(X, _SparseData) else _AssignPass(X)
+
+
+def _sweep_rows(X):
+    """Candidates per k-means|| sweep: 256 (the tensor path's limit); for sparse X also at most 32 MB of pack."""
+    if isinstance(X, _SparseData):
+        return int(max(1, min(256, (1 << 22) // max(1, X.d))))
+    return 256
+
+
 @_timed(_logger=logger)
 def init_scalable(X, n_clusters, random_state=None, max_iter=None, oversampling_factor=2, weighted=False):
     """k-means|| (Bahmani et al. 2012, Alg. 2) following k_means.py:396-463.
@@ -370,15 +435,15 @@ def init_scalable(X, n_clusters, random_state=None, max_iter=None, oversampling_
     rs = random_state if isinstance(random_state, np.random.RandomState) else _as_random_state(random_state, comm)
     c_idx = _scalable_candidates(X, rs, max_iter, oversampling_factor)
     sweep = _AssignPass(X)
-    # sorted, like the reference (k_means.py:432-435); fetched once, after the last round
+    # sorted, like the reference (k_means.py:432-435); fetched once, after the last round.  Sparse X: a CSR of the rows
     centers = X.global_rows(c_idx)
 
-    if len(centers) < n_clusters:
+    if centers.shape[0] < n_clusters:
         logger.warning("Found fewer than %d clusters in init.", n_clusters)
         # supplement with random rows (k_means.py:445-455).  The reference permutes all n row indices for this
         # (random_state.choice(arange(n), replace=False)): O(n) host work for a handful of rows.  Same distribution in
         # O(need): draw, de-duplicate, repeat.
-        need = n_clusters - len(centers)
+        need = n_clusters - centers.shape[0]
         n = int(X.n_global)
         chosen = set()
         while len(chosen) < need:
@@ -387,6 +452,8 @@ def init_scalable(X, n_clusters, random_state=None, max_iter=None, oversampling_
                     chosen.add(int(v))
         locs = sorted(chosen)
         extra = X.global_rows(locs)
+        if scipy.sparse.issparse(centers):
+            return np.vstack([centers.toarray(), extra.toarray()])
         return np.vstack([centers, extra])
     else:
         # Steps 7, 8 (k_means.py:457-463): reduce the candidates to n_clusters centres
@@ -405,7 +472,7 @@ def init_scalable(X, n_clusters, random_state=None, max_iter=None, oversampling_
 def _scalable_candidates(X, rs, max_iter, oversampling_factor):
     """Steps 1-6 of k-means|| (k_means.py:406-435): the sorted global row indices of the candidate centres."""
     be, comm = X.backend, X.comm
-    sweep = _AssignPass(X)
+    sweep = _assign_pass(X)
 
     # Step 1: first centre = global row 0 (k_means.py:406-408)
     idx = 0
@@ -432,7 +499,8 @@ def _scalable_candidates(X, rs, max_iter, oversampling_factor):
             seed = int(rs.randint(0, 2 ** 31 - 1)) | (int(rs.randint(0, 2 ** 31 - 1)) << 32)
             fresh = sorted(c_idx - swept)
             phi_t = be.zeros((1,), torch.float64)
-            blocks = [fresh[b0:b0 + 256] for b0 in range(0, len(fresh), 256)]
+            step = _sweep_rows(X)
+            blocks = [fresh[b0:b0 + step] for b0 in range(0, len(fresh), step)]
             for bi, blk in enumerate(blocks):
                 block = X.global_rows(blk).astype(np.float64)
                 _, mins_b, _ = sweep.run(block, want_min=True, squared=True)
@@ -481,25 +549,43 @@ def _reduce_candidates(cand, n_clusters, seed, be, weights=None, n_init=10, max_
     Distances go through ``bkm_assign_chunk`` / the fused Lloyd kernels; the D^2 sampling and, for the weighted
     variant only, the weighted centre update are a few vector operations on the (m,) / (m, d) candidate arrays."""
     from ..engine import Comm, DeviceData
+    from .._sparse import _csr_block
 
-    cand = np.ascontiguousarray(cand)
-    m, d = cand.shape
-    dt = torch.float64 if cand.dtype == np.float64 else torch.float32
-    Xc = DeviceData([be.to_device(cand, dt)], be, _LocalComm())
-    x = Xc.chunks[0]
+    sparse = scipy.sparse.issparse(cand)
+    if sparse:
+        # the candidates stay a CSR block and run through the sparse passes
+        cand = scipy.sparse.csr_matrix(cand)
+        m, d = cand.shape
+        Xc = _SparseData([_csr_block(cand, be.device)], d, be, _LocalComm())
+        c64 = cand.astype(np.float64)
+        var = np.asarray(c64.multiply(c64).mean(axis=0)).ravel() - np.asarray(c64.mean(axis=0)).ravel() ** 2
+        var_tol = float(np.mean(var) * tol)                                          # sklearn's _tolerance
+        sweep = _SparseAssignPass(Xc)
+
+        def dist_to(i):
+            return sweep.run(cand[i], want_min=True)[1][0]
+    else:
+        cand = np.ascontiguousarray(cand)
+        m, d = cand.shape
+        dt = torch.float64 if cand.dtype == np.float64 else torch.float32
+        Xc = DeviceData([be.to_device(cand, dt)], be, _LocalComm())
+        x = Xc.chunks[0]
+        var_tol = float(np.mean(np.var(cand.astype(np.float64), axis=0)) * tol)       # sklearn's _tolerance
     g = torch.Generator(device=be.device)
     g.manual_seed(int(seed) & 0x7FFFFFFFFFFFFFFF)
     w = None if weights is None else torch.as_tensor(np.asarray(weights, dtype=np.float64)).to(be.device).clamp_(min=0.0)
-    var_tol = float(np.mean(np.var(cand.astype(np.float64), axis=0)) * tol)       # sklearn's _tolerance
     best = None
     for _ in range(int(n_init)):
         # ---- k-means++ seeding (D^2 sampling) over the candidates
         first = int(torch.randint(0, m, (1,), generator=g, device=be.device).item()) if w is None else \
             int(torch.multinomial(w / w.sum(), 1, generator=g).item())
         chosen = [first]
-        closest = be.empty((m,), Xc.out_dtype)
-        c1 = x[first:first + 1].to(torch.float64)
-        be.assign_chunk(x, be.pack_centers(c1.contiguous(), dt), 1, None, closest, True, None)
+        if sparse:
+            closest = dist_to([first])
+        else:
+            closest = be.empty((m,), Xc.out_dtype)
+            c1 = x[first:first + 1].to(torch.float64)
+            be.assign_chunk(x, be.pack_centers(c1.contiguous(), dt), 1, None, closest, True, None)
         for _j in range(1, n_clusters):
             p = closest.to(torch.float64)
             if w is not None:
@@ -508,13 +594,20 @@ def _reduce_candidates(cand, n_clusters, seed, be, weights=None, n_init=10, max_
             nxt = int(torch.multinomial(p / tot, 1, generator=g).item()) if tot > 0 else \
                 int(torch.randint(0, m, (1,), generator=g, device=be.device).item())
             chosen.append(nxt)
-            newd = be.empty((m,), Xc.out_dtype)
-            be.assign_chunk(x, be.pack_centers(x[nxt:nxt + 1].to(torch.float64).contiguous(), dt), 1, None, newd, True, None)
+            if sparse:
+                newd = dist_to([nxt])
+            else:
+                newd = be.empty((m,), Xc.out_dtype)
+                be.assign_chunk(x, be.pack_centers(x[nxt:nxt + 1].to(torch.float64).contiguous(), dt), 1, None, newd,
+                                True, None)
             be.min_fold(closest, newd, None)
-        C0 = x[torch.as_tensor(chosen, device=be.device)].to(torch.float64).cpu().numpy()
+        if sparse:
+            C0 = cand[chosen].toarray().astype(np.float64)
+        else:
+            C0 = x[torch.as_tensor(chosen, device=be.device)].to(torch.float64).cpu().numpy()
         # ---- Lloyd on the candidates
         if w is None:
-            st = LloydState(Xc, C0)
+            st = _lloyd_state(Xc, C0)
             lloyd_loop(st, max_iter, var_tol)
             inertia = float(st.relabel(squared=True).item())
             C = st.C.cpu().numpy()
@@ -560,7 +653,7 @@ class _LocalComm(object):
 def evaluate_cost(X, centers):
     """phi_X(C) = sum_i min_j ||x_i - c_j||^2 (k_means.py:466-469); X is DeviceData."""
     X = _to_device_data(X, check_finite=False)
-    _, _, acc = _AssignPass(X).run(np.asarray(centers, dtype=np.float64), squared=True)
+    _, _, acc = _assign_pass(X).run(np.asarray(centers, dtype=np.float64), squared=True)
     return float(acc.item())
 
 
@@ -690,6 +783,106 @@ class LloydState(object):
         return acc
 
 
+class _SparseLloydState(object):
+    """``LloydState`` on sparse CSR blocks.  The centres live in a sparse pack (``bkm_sparse_pack_centers``): CT (d, k),
+    the transposed centres, then their squared norms; two packs, iteration i reads packs[cur] and writes the other.
+
+    One iteration on each rank: the assign pass (labels and counts) over every block, the label-sum pass
+    (sumsT (d, k) = X^T onehot(labels)) over every block's transpose, one all-reduce of ``[d*k sumsT | k counts |
+    inertia]``, then ``bkm_sparse_finalize_step`` (centre update + shift + stop test + the next pack).  Memory: the two
+    packs and the reduced buffer, 3 * 8 d k bytes.
+      * ``run(max_iter, tol)`` — the device-resident loop, as ``LloydState.run``.
+      * ``step()`` / ``accept()`` — one iteration with the shift left in ``shift`` (the CPU checker backend)."""
+
+    def __init__(self, X, centers):
+        be = X.backend
+        self.X, self.be = X, be
+        k, d = centers.shape
+        self.k, self.d = int(k), int(d)
+        c0 = torch.from_numpy(np.array(centers, dtype=np.float64, order="C", copy=True)).to(be.device)
+        self.packs = [be.sparse_pack_centers(c0), be.empty((d * k + k,), torch.float64)]
+        self.cur = 0
+        self.red = be.zeros((d * k + k + 1,), torch.float64)
+        self.sums = self.red[: d * k].view(d, k)
+        self.counts_f = self.red[d * k: d * k + k]
+        self.shift = be.zeros((1,), torch.float64)
+        self.labels = [be.empty((int(b[3]),), torch.int32) for b in X.blocks]
+        self.device_loop = hasattr(be, "sparse_finalize_step") and hasattr(be, "loop_state_new")
+        self.kernel_event_hook = None
+        self.sync_every = 8
+
+    @property
+    def C(self):
+        """The current centres, (k, d) float64 (a view of the pack's CT)."""
+        return self.packs[self.cur][: self.d * self.k].view(self.d, self.k).t()
+
+    def _sweep(self, pack, state=None):
+        """The two passes of one iteration into ``red`` (before the all-reduce)."""
+        be, X, k, d = self.be, self.X, self.k, self.d
+        work = [(b, c, lab) for b, c, lab in zip(X.blocks, X.transposes(), self.labels) if int(b[3]) > 0]
+        if not work:
+            self.red.zero_()                  # a rank without rows still takes part in the all-reduce
+        for i, (b, _c, lab) in enumerate(work):
+            be.csr_assign_chunk(b, d, pack, k, labels=lab, counts=self.counts_f, first=i == 0, loop_state=state)
+        for i, (_b, c, lab) in enumerate(work):
+            be.csc_label_sums_chunk(c, d, lab, k, self.sums, first=i == 0, loop_state=state)
+
+    def step(self):
+        self._sweep(self.packs[self.cur])
+        self.X.comm.allreduce_sum_(self.red)
+        self.be.sparse_finalize(self.red, self.packs[self.cur], self.packs[self.cur ^ 1], self.shift, self.k, self.d)
+
+    def accept(self):
+        self.cur ^= 1
+
+    def run(self, max_iter, tol):
+        """The device-resident loop.  Returns ``(shift, index of the last iteration, accepted)`` like ``lloyd_loop``."""
+        be, X, k, d = self.be, self.X, self.k, self.d
+        state, hist = be.loop_state_new(tol, max_iter)
+        base = self.cur
+        issued = 0
+        done = n_iter = 0
+        shift = None
+        logged = 0
+        while issued < max_iter and not done:
+            for _ in range(min(self.sync_every, max_iter - issued)):
+                p_in, p_out = self.packs[(base + issued) & 1], self.packs[(base + issued + 1) & 1]
+                ev = self.kernel_event_hook() if self.kernel_event_hook is not None else None
+                if ev is not None:
+                    ev[0].record()
+                self._sweep(p_in, state)
+                if ev is not None:
+                    ev[1].record()
+                X.comm.allreduce_sum_(self.red)
+                be.sparse_finalize_step(self.red, p_in, p_out, state, k, d)
+                issued += 1
+            done, n_iter, shift = be.loop_state_read(state)
+            _check_engine(be, shift, "the centre shift")
+            if logger.isEnabledFor(logging.INFO):
+                for v in hist[logged:n_iter].cpu().numpy().tolist():
+                    logger.info("Lloyd loop %2d. Shift: %0.4f", logged, v)
+                    logged += 1
+        if shift is None:
+            return None, -1, False
+        # converged in iteration n_iter - 1: its pack was NOT taken over (Q3) -> the pack it read is current
+        self.cur = (base + n_iter - 1) & 1 if done else (base + n_iter) & 1
+        self.shift.fill_(shift)
+        return shift, n_iter - 1, not done
+
+    def relabel(self, squared):
+        """E-step only against the current centres; returns the summed min distance tensor."""
+        be, X, k = self.be, self.X, self.k
+        acc = be.zeros((1,), torch.float64)
+        for b, lab in zip(X.blocks, self.labels):
+            be.csr_assign_chunk(b, X.d, self.packs[self.cur], k, labels=lab, squared=squared, dist_sum=acc)
+        X.comm.allreduce_sum_(acc)
+        return acc
+
+
+def _lloyd_state(X, centers):
+    return _SparseLloydState(X, centers) if isinstance(X, _SparseData) else LloydState(X, centers)
+
+
 def _check_engine(be, value, what):
     """A poisoned step (NaN shift / cost, see bkm_debug_abort_code) becomes an error."""
     if value == value and abs(value) != float("inf"):
@@ -753,7 +946,7 @@ def _kmeans_single_lloyd(
         max_iter=init_max_iter,
     )
     dt = X.np_dtype
-    st = LloydState(X, np.asarray(centers))
+    st = _lloyd_state(X, np.asarray(centers))
     shift, i, accepted = lloyd_loop(st, max_iter, tol)
 
     if shift is None:

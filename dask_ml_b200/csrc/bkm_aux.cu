@@ -255,14 +255,7 @@ finalize_step_kernel(const double* __restrict__ red, const double* __restrict__ 
   __syncthreads();
   if (tid == 0) last = atomicAdd(reinterpret_cast<unsigned int*>(&st->pad), 1u) == gridDim.x - 1;
   __syncthreads();
-  if (last && tid == 0) {
-    st->pad = 0;
-    st->shift = shift;
-    if (st->hist && st->n_iter < st->hist_cap) st->hist[st->n_iter] = shift;
-    st->n_iter += 1;
-    __threadfence();
-    if (converged) st->done = 1;
-  }
+  if (last && tid == 0) loop_commit(st, shift, converged);
 }
 
 __global__ void loop_reset_kernel(LoopState* st, double tol, double* hist, int hist_cap) {

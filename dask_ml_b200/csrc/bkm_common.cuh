@@ -302,6 +302,17 @@ struct LoopState {
   double* hist;      // nullable: shift of iteration i at hist[i] (i < hist_cap)
 };
 
+// The end of one iteration's step (bkm_finalize_step, bkm_sparse_finalize_step), by one thread after every CTA of the
+// step has read st->done and st->tol: record the shift, count the iteration, and stop the loop once it converged.
+__device__ __forceinline__ void loop_commit(LoopState* st, double shift, bool converged) {
+  st->pad = 0;
+  st->shift = shift;
+  if (st->hist && st->n_iter < st->hist_cap) st->hist[st->n_iter] = shift;
+  st->n_iter += 1;
+  __threadfence();
+  if (converged) st->done = 1;
+}
+
 // implemented in bkm_simt.cu
 int launch_simt(const ChunkArgs& a, bool mstep, int dtype, int sm_count, int* grid_out, cudaStream_t s);
 // implemented in bkm_tc.cu

@@ -21,15 +21,13 @@
 //                 finish (a ticket per column) adds them in segment order.
 #include "bkm_common.cuh"
 #include "bkm_csc_plan.cuh"
+#include "bkm_csr_rows.cuh"
 
 namespace bkm {
 namespace {
 
 constexpr int kThreads = 256;
 constexpr int kWarps = kThreads / 32;
-
-__device__ __forceinline__ double to_f64(float v) { return (double)v; }
-__device__ __forceinline__ double to_f64(double v) { return v; }
 
 // ---------------------------------------------------------------------------------------------------------------------
 // row panel
@@ -72,27 +70,8 @@ __global__ void __launch_bounds__(kThreads) csr_panel_kernel(RowPanelArgs a) {
     double acc[C];
 #pragma unroll
     for (int j = 0; j < C; ++j) acc[j] = 0.0;
-    const long long k0 = a.crow[i], k1 = a.crow[i + 1];
-#pragma unroll 1
-    for (long long e0 = k0; e0 < k1; e0 += 32) {
-      long long c = -1;
-      double v = 0.0;
-      if (e0 + lane < k1) {
-        c = a.col[e0 + lane];
-        v = to_f64(val[e0 + lane]);
-      }
-      const int m = (int)min(32LL, k1 - e0);
-#pragma unroll 4
-      for (int q = 0; q < m; ++q) {
-        const long long cq = __shfl_sync(0xffffffffu, c, q);
-        const double vq = __shfl_sync(0xffffffffu, v, q);
-        if ((unsigned long long)cq >= (unsigned long long)a.p) continue;      // uniform over the warp
-        const double* w = a.W + (size_t)cq * a.l + c0 + lane;
-#pragma unroll
-        for (int j = 0; j < C; ++j)
-          if (own[j]) acc[j] = fma(vq, __ldg(w + 32 * j), acc[j]);
-      }
-    }
+    double xn = 0.0;
+    csr_row_gather<T, C, false>(a.crow, a.col, val, i, a.p, a.W, a.l, c0, own, acc, xn);
     const long long grow = a.row_offset + i;
 #pragma unroll
     for (int j = 0; j < C; ++j) {
@@ -147,21 +126,16 @@ template <typename T, int C>
 __global__ void __launch_bounds__(kThreads) csc_panel_kernel(ColPanelArgs a) {
   constexpr int CW = 32 * C;
   const int lane = threadIdx.x & 31;
-  const long long* seg_off = a.plan + ST_N;
-  const int* seg_col = reinterpret_cast<const int*>(a.plan + ST_N + 2 * ((long long)a.p + 1));
   const long long T_ = a.plan[ST_SEGS];
   const T* vals = reinterpret_cast<const T*>(a.vals);
   const int l = a.l;
   const long long nw = ((long long)gridDim.x * kThreads) >> 5;
 #pragma unroll 1
   for (long long t = ((long long)blockIdx.x * kThreads + threadIdx.x) >> 5; t < T_; t += nw) {
-    const int j = seg_col[t];
-    const long long s0 = seg_off[j], ns = seg_off[j + 1] - s0;
-    const long long e0 = a.colptr[j] + (t - s0) * SEG;
-    const long long e1 = min(a.colptr[j + 1], e0 + SEG);
-    // the segments of a multi-segment column own slots 2 (s0 - j) + s: s0 - j is the number of segments beyond the
-    // first of every column before j, so these ranges do not overlap and stay below 2 (nnz / SEG + 1)
-    double* slot = a.slot + (size_t)(2 * (s0 - j) + (t - s0)) * l;
+    const SegSpan sp = seg_span(a.plan, a.colptr, a.p, t);
+    const int j = sp.j;
+    const long long ns = sp.ns, e0 = sp.e0, e1 = sp.e1;
+    double* slot = seg_slot(a.slot, sp, t, l);
 #pragma unroll 1
     for (int c0 = 0; c0 < l; c0 += CW) {
       const int lim = l - c0 - lane;                 // this lane's columns c0 + lane + 32 u with 32 u < lim
@@ -195,21 +169,10 @@ __global__ void __launch_bounds__(kThreads) csc_panel_kernel(ColPanelArgs a) {
         else a.out[(size_t)j * l + cc] = a.first ? acc[u] : a.out[(size_t)j * l + cc] + acc[u];
       }
     }
-    if (ns > 1) {
-      if (!last_warp(a.ticket + j, (unsigned)ns)) continue;
-      const double* src = a.slot + (size_t)(2 * (s0 - j)) * l;
-      for (int cc = lane; cc < l; cc += 32) {
-        double v = 0.0;
-        for (long long u = 0; u < ns; ++u) v += __ldcg(src + (size_t)u * l + cc);
-        a.out[(size_t)j * l + cc] = a.first ? v : a.out[(size_t)j * l + cc] + v;
-      }
-      if (lane == 0) a.ticket[j] = 0u;
-    }
+    if (ns > 1) seg_fold(sp, a.slot, a.ticket, a.out, l, a.first);
   }
 }
 
-static size_t slots_bytes(long long nnz, int l) { return align_up((size_t)2 * (nnz / SEG + 1) * l * 8, 256); }
-static size_t col_panel_ws(int p, long long nnz, int l) { return slots_bytes(nnz, l) + align_up((size_t)p * 4, 256); }
 
 static int grid_for(long long work, int per_cta, long long cap) {
   long long g = (work + per_cta - 1) / per_cta;
@@ -278,7 +241,7 @@ extern "C" int bkm_csr_panel_chunk(const int64_t* crow, const int64_t* col, cons
 
 extern "C" int bkm_csc_panel_workspace_bytes(int p, int64_t nnz, int l, size_t* out) {
   if (!out || p <= 0 || nnz < 0 || l <= 0) return BKM_EINVAL;
-  *out = col_panel_ws(p, nnz, l);
+  *out = seg_fold_ws(p, nnz, l);
   return 0;
 }
 
@@ -288,7 +251,7 @@ extern "C" int bkm_csc_panel_chunk(const int64_t* colptr, const int32_t* rows, c
   if (p <= 0 || nnz < 0 || l <= 0 || !colptr || !plan || !out || !workspace) return BKM_EINVAL;
   if (nnz > 0 && (!rows || !vals || !P)) return BKM_EINVAL;
   if (val_dtype != BKM_F32 && val_dtype != BKM_F64) return BKM_EDTYPE;
-  if (ws_bytes < col_panel_ws(p, nnz, l)) return BKM_EWORKSPACE;
+  if (ws_bytes < seg_fold_ws(p, nnz, l)) return BKM_EWORKSPACE;
   cudaStream_t s = (cudaStream_t)stream;
   unsigned char* ws = reinterpret_cast<unsigned char*>(workspace);
   ColPanelArgs a;
@@ -296,7 +259,7 @@ extern "C" int bkm_csc_panel_chunk(const int64_t* colptr, const int32_t* rows, c
   a.rows = rows; a.vals = vals; a.p = p; a.plan = reinterpret_cast<const long long*>(plan);
   a.P = P; a.l = l; a.out = out;
   a.slot = reinterpret_cast<double*>(ws);
-  a.ticket = reinterpret_cast<unsigned*>(ws + slots_bytes(nnz, l));
+  a.ticket = reinterpret_cast<unsigned*>(ws + seg_slots_bytes(nnz, l));
   a.first = (flags & BKM_FLAG_FIRST_CHUNK) ? 1 : 0;
   BKM_CUDA_TRY(cudaMemsetAsync(a.ticket, 0, (size_t)p * 4, s));
   const int sms = sm_count_or_default();

@@ -625,6 +625,72 @@ class CudaBackend(object):
                 self._ptr(P), l, self._ptr(out), self._ptr(ws), ws.numel(), flags, self._stream()),
                 "bkm_csc_panel_chunk")
 
+    # -- KMeans on sparse CSR blocks ---------------------------------------------------------
+    def sparse_pack_centers(self, C64, out=None):
+        """The sparse pack of the float64 centres C64 (k, p): one float64 buffer [CT (p, k) | cn (k)] with CT the
+        transposed centres and cn their squared norms (``out`` is reused when given)."""
+        k, p = C64.shape
+        if out is None:
+            out = torch.empty(p * k + k, dtype=torch.float64, device=self.device)
+        nb = ctypes.c_size_t(0)
+        _lib.check(self.lib.bkm_sparse_pack_workspace_bytes(int(k), int(p), ctypes.byref(nb)),
+                   "bkm_sparse_pack_workspace_bytes")
+        ws = self._scratch("sparse_pack", nb.value)
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.bkm_sparse_pack_centers(self._ptr(C64), int(k), int(p), self._ptr(out), self._ptr(ws),
+                                                        ws.numel(), self._stream()), "bkm_sparse_pack_centers")
+        return out
+
+    def csr_assign_chunk(self, blk, d, pack, k, labels=None, min_dist=None, squared=True, dist_sum=None, counts=None,
+                         out=None, mode=0, first=False, loop_state=None):
+        """The E-step of one CSR block against a sparse pack: mode 0 writes labels (int32), min_dist (float64, squared
+        or not) and adds to dist_sum (1,) / counts (k,) float64 (``first`` overwrites them); modes 1 / 2 write the
+        distances / squared distances into ``out`` (n, k) float32 / float64 with any row pitch."""
+        crow, col, val, n = blk
+        ws = None
+        if mode == 0 and (dist_sum is not None or counts is not None):
+            nb = ctypes.c_size_t(0)
+            _lib.check(self.lib.bkm_csr_assign_workspace_bytes(int(n), int(k), ctypes.byref(nb)),
+                       "bkm_csr_assign_workspace_bytes")
+            ws = self._scratch("csr_assign", nb.value)
+        flags = self.flags | (_lib.FLAG_FIRST_CHUNK if first else 0)
+        odt = _DT_CODE[out.dtype] if out is not None else _lib.BKM_F64
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.bkm_csr_assign_chunk(
+                self._ptr(crow), self._ptr(col), self._ptr(val), _DT_CODE[val.dtype], int(n), int(d), int(col.numel()),
+                self._ptr(pack), int(k), int(mode), self._ptr(labels), self._ptr(min_dist), int(bool(squared)),
+                self._ptr(dist_sum), self._ptr(counts), self._ptr(out), (out.stride(0) if n else k) if out is not None
+                else k, odt, self._ptr(ws), ws.numel() if ws is not None else 0, flags, self._ptr(loop_state),
+                self._stream()), "bkm_csr_assign_chunk")
+
+    def csc_label_sums_chunk(self, csc, d, labels, k, sumsT, first=False, loop_state=None):
+        """sumsT (d, k) (+)= X^T onehot(labels) over the transpose ``csc`` of one block, each (column, cluster) sum in
+        ascending row order.  ``first`` overwrites."""
+        colptr, rows, vals, plan = csc
+        nnz = int(rows.numel())
+        nb = ctypes.c_size_t(0)
+        _lib.check(self.lib.bkm_csc_label_sums_workspace_bytes(int(d), nnz, int(k), ctypes.byref(nb)),
+                   "bkm_csc_label_sums_workspace_bytes")
+        ws = self._scratch("csc_label_sums", nb.value)
+        flags = self.flags | (_lib.FLAG_FIRST_CHUNK if first else 0)
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.bkm_csc_label_sums_chunk(
+                self._ptr(colptr), self._ptr(rows), self._ptr(vals), _DT_CODE[vals.dtype], int(d), nnz, self._ptr(plan),
+                self._ptr(labels), int(k), self._ptr(sumsT), self._ptr(ws), ws.numel(), flags, self._ptr(loop_state),
+                self._stream()), "bkm_csc_label_sums_chunk")
+
+    def sparse_finalize_step(self, red, pack_in, pack_out, state, k, d):
+        """bkm_finalize_step on the transposed layout: red = [d*k sumsT | k counts | inertia] -> the shift, the stop
+        test and pack_out = the sparse pack of the new centres."""
+        nb = ctypes.c_size_t(0)
+        _lib.check(self.lib.bkm_sparse_pack_workspace_bytes(int(k), int(d), ctypes.byref(nb)),
+                   "bkm_sparse_pack_workspace_bytes")
+        ws = self._scratch("sparse_pack", nb.value)
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.bkm_sparse_finalize_step(self._ptr(red), self._ptr(pack_in), self._ptr(pack_out),
+                                                         self._ptr(state), int(k), int(d), self._ptr(ws), ws.numel(),
+                                                         self._stream()), "bkm_sparse_finalize_step")
+
     def colstats_chunk(self, x, shift, acc, minmax, first=False):
         """The scalers' statistics pass over one chunk, float64 on the device: acc (5, d) (+)= [sum (x - shift) |
         sum (x - shift)^2 over the finite x | NaN count | +inf count | -inf count] and minmax (2, d) = [min | max] over

@@ -1,6 +1,7 @@
 """GPU versions of the three distance operators the KMeans path uses
 (dask_ml/metrics/pairwise.py:18-52, 55-66, 69-97).  Only the euclidean metric exists on this
-path; every result is a device-resident ``ChunkedArray`` with the reference's dtypes."""
+path; every result is a device-resident ``ChunkedArray`` with the reference's dtypes.  ``pairwise_distances_argmin_min``
+and ``euclidean_distances`` also take sparse CSR X (any form ``KMeans`` takes) against a dense Y."""
 import numpy as np
 import torch
 
@@ -23,6 +24,26 @@ def _prep(X, Y):
     return X, be, pack, int(Y.shape[0])
 
 
+def _sparse_x(X):
+    """``_SparseData`` for sparse X, else None."""
+    from .._sparse import _SparseData, _sparse_data
+
+    return X if isinstance(X, _SparseData) else _sparse_data(X)
+
+
+def _sparse_prep(X, Y):
+    """Sparse X against dense Y: (X, backend, the sparse pack of Y, len(Y), Y's dtype)."""
+    Y = np.asarray(Y)
+    if Y.ndim != 2 or Y.shape[1] != X.d:
+        raise ValueError(
+            "Incompatible dimension for X and Y matrices: X.shape[1] == %d while Y.shape[1] == %d"
+            % (X.d, Y.shape[1] if Y.ndim == 2 else -1)
+        )
+    be = X.backend
+    C = torch.as_tensor(np.ascontiguousarray(Y, dtype=np.float64)).to(be.device)
+    return be, be.sparse_pack_centers(C), int(Y.shape[0]), Y.dtype
+
+
 def pairwise_distances_argmin_min(X, Y, axis=1, metric="euclidean", batch_size=None, metric_kwargs=None):
     """Per row of X: index of and distance to the nearest row of Y (pairwise.py:18-52).
 
@@ -36,6 +57,18 @@ def pairwise_distances_argmin_min(X, Y, axis=1, metric="euclidean", batch_size=N
     if axis != 1:
         raise NotImplementedError("axis must be 1")
     squared = bool((metric_kwargs or {}).get("squared", False)) or metric == "sqeuclidean"
+    Xs = _sparse_x(X)
+    if Xs is not None:
+        be, pack, k, _ = _sparse_prep(Xs, Y)
+        argmins, mins = [], []
+        for blk in Xs.blocks:
+            n = int(blk[3])
+            lab = be.empty((n,), torch.int32)
+            mn = be.empty((n,), torch.float64)
+            be.csr_assign_chunk(blk, Xs.d, pack, k, labels=lab, min_dist=mn, squared=squared)
+            argmins.append(lab.to(torch.int64))
+            mins.append(mn)
+        return ChunkedArray(argmins), ChunkedArray(mins)
     X, be, pack, k = _prep(X, Y)
     acc = be.zeros((1,), torch.float64)
     argmins, mins = [], []
@@ -97,6 +130,21 @@ def euclidean_distances(X, Y=None, Y_norm_squared=None, squared=False, X_norm_sq
     """
     from ..engine import DeviceData
 
+    Xs = _sparse_x(X)
+    if Xs is not None:
+        if X_norm_squared is not None or Y_norm_squared is not None:
+            raise NotImplementedError("X_norm_squared / Y_norm_squared are not supported for sparse X")
+        if Y is None:
+            raise NotImplementedError("sparse X needs a dense Y")
+        be, pack, k, ydt = _sparse_prep(Xs, Y)
+        # dtype of -2 * dot(X, Y.T) + XX + YY: float32 only when both are float32
+        odt = torch.float32 if Xs.dtype == torch.float32 and ydt == np.float32 else torch.float64
+        outs = []
+        for blk in Xs.blocks:
+            out = be.empty((int(blk[3]), k), odt)
+            be.csr_assign_chunk(blk, Xs.d, pack, k, out=out, mode=2 if squared else 1)
+            outs.append(out)
+        return ChunkedArray(outs)
     X = _as_device(X)
     if Y is None:
         Y = X.to_host()

@@ -30,6 +30,10 @@
  *   the same per-iteration terms on sparse CSR blocks, which the      bkm_glm_csr_pass_chunk, bkm_csr_transpose_chunk,
  *     reference cannot take (linear_model/utils.py:34-53 appends a    bkm_csc_matvec_chunk,
  *     dense ones column to every block)                               bkm_gram_weighted_csr_chunk
+ *   the Lloyd iterations, predict and transform of KMeans on sparse   bkm_csr_assign_chunk,
+ *     CSR blocks, which the reference rejects (k_means.py:168)          bkm_csc_label_sums_chunk,
+ *                                                                       bkm_sparse_pack_centers,
+ *                                                                       bkm_sparse_finalize_step
  *   da.linalg.svd_compressed's X.dot(omega), X.T.dot(q) and the        bkm_csr_panel_chunk, bkm_csc_panel_chunk
  *     projection of TruncatedSVD on sparse CSR blocks, which the
  *     reference densifies (decomposition/truncated_svd.py)
@@ -91,8 +95,10 @@ extern "C" {
  * 5 = bkm_glm_csr_workspace_bytes, bkm_glm_csr_pass_chunk, bkm_csr_transpose_workspace_bytes, bkm_csr_transpose_chunk,
  *     bkm_csc_matvec_workspace_bytes, bkm_csc_matvec_chunk, bkm_gram_weighted_csr_workspace_bytes,
  *     bkm_gram_weighted_csr_chunk
- * 6 = bkm_csr_panel_chunk, bkm_csc_panel_workspace_bytes, bkm_csc_panel_chunk */
-#define BKM_VERSION_MINOR 6
+ * 6 = bkm_csr_panel_chunk, bkm_csc_panel_workspace_bytes, bkm_csc_panel_chunk
+ * 7 = bkm_csr_assign_workspace_bytes, bkm_csr_assign_chunk, bkm_csc_label_sums_workspace_bytes,
+ *     bkm_csc_label_sums_chunk, bkm_sparse_pack_workspace_bytes, bkm_sparse_pack_centers, bkm_sparse_finalize_step */
+#define BKM_VERSION_MINOR 7
 
 /* element types of X */
 #define BKM_F32 0
@@ -353,6 +359,53 @@ int bkm_csc_panel_workspace_bytes(int p, int64_t nnz, int l, size_t* out);
 int bkm_csc_panel_chunk(const int64_t* colptr, const int32_t* rows, const void* vals, int val_dtype, int p,
                         int64_t nnz, const int64_t* plan, const double* P, int l, double* out, void* workspace,
                         size_t ws_bytes, int flags, void* stream);
+
+/* ---- KMeans on sparse CSR blocks: the E-step, the M-step sums and the centre update on transposed centres -----------
+ * The block is given as for the linear models above.  Values are widened to float64; every sum runs in a fixed order
+ * (no float atomics): two calls with the same inputs give the same bits.  The centres live in a SPARSE PACK of
+ * p k + k float64: CT [p][k] (the centres transposed, so that one entry of a row gathers k contiguous values), then
+ * cn [k] = ||c_j||^2.  Only bkm_sparse_pack_centers and bkm_sparse_finalize_step write packs, with the same kernel.
+ *   bkm_sparse_pack_centers   pack = the sparse pack of centres64 [k][p] float64.  cn_j sums c_jf^2 over f in a fixed
+ *                      order.  workspace: bkm_sparse_pack_workspace_bytes(k, p) bytes, any content.
+ *   bkm_csr_assign_chunk      d2_ij = max(||x_i||^2 - 2 x_i.c_j + cn_j, 0), ||x_i||^2 and x_i.c_j adding row i's
+ *                      entries in stored order by fma (column indices outside [0, p) are skipped).  Any k >= 1, one
+ *                      launch, no (n x k) intermediate.  mode:
+ *                        BKM_SPARSE_ARGMIN  labels [n] int32 = arg-min_j (ties to the lowest j), min_out [n] float64 =
+ *                          the minimum (d2, or its square root unless `squared`), dist_sum [1] float64 = the sum of
+ *                          min_out, counts [k] float64 = the rows per cluster; all nullable.  dist_sum and counts are
+ *                          OVERWRITTEN with BKM_FLAG_FIRST_CHUNK, else ACCUMULATED; they need the workspace
+ *                          (bkm_csr_assign_workspace_bytes(n, k) bytes, any content).  n = 0 still writes them.
+ *                        BKM_SPARSE_DIST / BKM_SPARSE_DIST2  out [n][ldo] (ldo >= k) = sqrt(d2) / d2 in out_dtype
+ *                          (BKM_F32 or BKM_F64).
+ *                      loop_state (nullable): a no-op once the loop of bkm_loop_reset is done.
+ *   bkm_csc_label_sums_chunk  sumsT [p][k] (+)= X^T onehot(labels) over the block's transpose and plan: entry (row, v)
+ *                      of column j adds v to sumsT[j][labels[row]] (labels outside [0, k) are skipped); each (j, c) sum
+ *                      runs in ascending row order, a column of more than 2048 entries in segments added in segment
+ *                      order.  OVERWRITTEN with BKM_FLAG_FIRST_CHUNK, else ACCUMULATED.  k <= 25600.  workspace:
+ *                      bkm_csc_label_sums_workspace_bytes(p, nnz, k) bytes, any content.  loop_state as above.
+ *   bkm_sparse_finalize_step  the contract of bkm_finalize_step on the transposed layout: reduced = [p k sumsT |
+ *                      k counts as float64 | inertia] of the iteration, C' = sumsT / max(counts, 1) (an empty cluster
+ *                      gets 0), shift = sum_j sum_f (CT_fj - C'_fj)^2 (f, then j, in a fixed order) -> the loop state
+ *                      and its history; pack_out (!= pack_in) = the sparse pack of C', written whether or not the
+ *                      iteration converged (the loop then keeps pack_in, Q3).  A no-op once the loop is done.
+ *                      workspace: bkm_sparse_pack_workspace_bytes(k, p) bytes. */
+#define BKM_SPARSE_ARGMIN 0
+#define BKM_SPARSE_DIST   1
+#define BKM_SPARSE_DIST2  2
+int bkm_sparse_pack_workspace_bytes(int k, int p, size_t* out);
+int bkm_sparse_pack_centers(const double* centers64, int k, int p, double* pack, void* workspace, size_t ws_bytes,
+                            void* stream);
+int bkm_csr_assign_workspace_bytes(int64_t n, int k, size_t* out);
+int bkm_csr_assign_chunk(const int64_t* crow, const int64_t* col, const void* val, int val_dtype, int64_t n, int p,
+                         int64_t nnz, const double* pack, int k, int mode, int32_t* labels, double* min_out,
+                         int squared, double* dist_sum, double* counts, void* out, int64_t ldo, int out_dtype,
+                         void* workspace, size_t ws_bytes, int flags, const void* loop_state, void* stream);
+int bkm_csc_label_sums_workspace_bytes(int p, int64_t nnz, int k, size_t* out);
+int bkm_csc_label_sums_chunk(const int64_t* colptr, const int32_t* rows, const void* vals, int val_dtype, int p,
+                             int64_t nnz, const int64_t* plan, const int32_t* labels, int k, double* sumsT,
+                             void* workspace, size_t ws_bytes, int flags, const void* loop_state, void* stream);
+int bkm_sparse_finalize_step(const double* reduced, const double* pack_in, double* pack_out, void* loop_state, int k,
+                             int p, void* workspace, size_t ws_bytes, void* stream);
 
 /* ---- StandardScaler / MinMaxScaler / RobustScaler: the fit passes and the transform pass over row chunks (replace
  * X.mean(0), X.var(0), X.min(0), X.max(0), da.percentile per column and the elementwise (X - m) / s of
