@@ -117,6 +117,13 @@ SIGNATURES = {
                                         _c_void_p, _c_void_p, ctypes.c_size_t, _int, _c_void_p, _c_void_p]),
     "bkm_sparse_finalize_step": (_int, [_c_void_p, _c_void_p, _c_void_p, _c_void_p, _int, _int, _c_void_p,
                                         ctypes.c_size_t, _c_void_p]),
+    "bkm_csr_kernel_colsum_workspace_bytes": (_int, [_i64, _int, _szp]),
+    "bkm_csr_kernel_colsum_chunk": (_int, [_c_void_p, _c_void_p, _c_void_p, _int, _i64, _int, _i64, _c_void_p, _int,
+                                           _dbl, _c_void_p, _c_void_p, ctypes.c_size_t, _int, _c_void_p]),
+    "bkm_csr_nystrom_embed_chunk": (_int, [_c_void_p, _c_void_p, _c_void_p, _int, _i64, _int, _i64, _c_void_p, _int,
+                                           _dbl, _c_void_p, _int, _c_void_p, _i64, _int, _int, _c_void_p]),
+    "bkm_sparse_minibatch_step": (_int, [_c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_void_p, _int, _int, _c_void_p,
+                                         ctypes.c_size_t, _c_void_p]),
     "bkm_colstats_workspace_bytes": (_int, [_i64, _int, _szp]),
     "bkm_colstats_chunk": (_int, [_c_void_p, _i64, _int, _i64, _int, _c_void_p, _c_void_p, _c_void_p, _c_void_p,
                                   ctypes.c_size_t, _int, _c_void_p]),

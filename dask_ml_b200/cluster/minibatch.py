@@ -10,11 +10,16 @@ float64 sums and counts), then ``bkm_minibatch_step`` (``_minibatch_update_dense
 and the next centre pack).  The host reads k weight sums and the batch inertia once per batch: the reassignment
 decision and the random draws of scikit-learn depend on them, and run on the host in numpy with the estimator's
 RandomState, so the RNG stream is scikit-learn's.
+
+Sparse CSR batches (any form ``KMeans`` takes) run scikit-learn's ``_minibatch_update_sparse`` the same way on the
+transposed centres: per block the CSR arg-min pass, the block's transpose and the label-indexed column sums, then
+``bkm_sparse_minibatch_step``.
 """
 import logging
 import warnings
 
 import numpy as np
+import scipy.sparse
 import torch
 from sklearn.base import _fit_context
 from sklearn.cluster import MiniBatchKMeans, kmeans_plusplus
@@ -22,6 +27,7 @@ from sklearn.utils import check_array as _sk_check_array
 from sklearn.utils import check_random_state
 from sklearn.utils.validation import _is_arraylike_not_scalar, check_is_fitted
 
+from .._sparse import _SparseData
 from ..chunked import ChunkedArray
 from ..engine import StreamedChunks, dist_info
 from . import k_means as _km
@@ -115,6 +121,97 @@ class _MiniBatchState(object):
         return v[: self.k].copy(), float(v[self.k])
 
 
+def _rows(x):
+    """Rows of a dense chunk or of a sparse (crow, col, val, n) block."""
+    return int(x[3]) if isinstance(x, tuple) else int(x.shape[0])
+
+
+class _SparseMiniBatchState(object):
+    """``_MiniBatchState`` for sparse CSR batches: two sparse packs (``bkm_sparse_pack_centers``: the centres transposed,
+    (d, k), then their squared norms) and two float64 weight-sum vectors, ping-pong pairs with ``[cur]`` current, and
+    the ``[d*k sumsT | k counts | inertia]`` buffer of one batch.  Memory: 3 * 8 d k bytes, as for sparse ``KMeans``.
+
+    Each block's transpose is built for its step and dropped after it; its canonical-CSR flag is added on the device
+    and read with the weight sums."""
+
+    def __init__(self, be, centers, weight_sums):
+        k, d = centers.shape
+        self.k, self.d = int(k), int(d)
+        c0 = torch.from_numpy(np.array(centers, dtype=np.float64, order="C", copy=True)).to(be.device)
+        w0 = torch.from_numpy(np.array(weight_sums, dtype=np.float64, copy=True)).to(be.device)
+        self.packs = [be.sparse_pack_centers(c0), be.empty((d * k + k,), torch.float64)]
+        self.Wb = [w0, be.empty((k,), torch.float64)]
+        self.cur = 0
+        self.red = be.zeros((d * k + k + 1,), torch.float64)
+        self.sums = self.red[: d * k].view(d, k)
+        self.counts = self.red[d * k: d * k + k]
+        self.inertia = self.red[d * k + k:]
+        self.bad = be.zeros((1,), torch.float64)
+        cuda = be.device.type == "cuda"
+        self.host = torch.empty((k + 2,), dtype=torch.float64, pin_memory=cuda)
+        self.read_done = None
+
+    @property
+    def C(self):
+        """The current centres, (k, d) float64 (a view of the current pack)."""
+        return self.packs[self.cur][: self.d * self.k].view(self.d, self.k).t()
+
+    @property
+    def W(self):
+        return self.Wb[self.cur]
+
+    def step(self, be, blocks, dtype=None):
+        """Enqueue one batch: per block with rows the assign pass (labels, counts, the batch inertia), the block's
+        transpose and the label sums; then the centre / weight-sum update and the next pack."""
+        k, d = self.k, self.d
+        pack = self.packs[self.cur]
+        self.bad.zero_()
+        first = True
+        for blk in blocks:
+            n = _rows(blk)
+            if n == 0:
+                continue
+            lab = be.empty((n,), torch.int32)
+            be.csr_assign_chunk(blk, d, pack, k, labels=lab, counts=self.counts, dist_sum=self.inertia, first=first)
+            csc = be.csr_transpose_chunk(blk, d)
+            self.bad += csc[3][0]
+            be.csc_label_sums_chunk(csc, d, lab, k, self.sums, first=first)
+            first = False
+        be.sparse_minibatch_step(self.red, pack, self.Wb[self.cur], self.packs[self.cur ^ 1], self.Wb[self.cur ^ 1], k, d)
+        self.cur ^= 1
+
+    def undo(self):
+        """Back to the state before the last step (its inputs are still in the other halves of the pairs)."""
+        self.cur ^= 1
+
+    def set_centres(self, be, C):
+        """Repack the current pack from the float64 centres C (k, d)."""
+        self.packs[self.cur] = be.sparse_pack_centers(C.contiguous(), out=self.packs[self.cur])
+
+    def start_read(self):
+        """Enqueue the copy of the weight sums, the batch inertia and the canonical-CSR flag to the host."""
+        self.host[: self.k].copy_(self.W, non_blocking=True)
+        self.host[self.k: self.k + 1].copy_(self.inertia, non_blocking=True)
+        self.host[self.k + 1:].copy_(self.bad, non_blocking=True)
+        if self.W.is_cuda:
+            self.read_done = torch.cuda.Event()
+            self.read_done.record(torch.cuda.current_stream(self.W.device))
+
+    def finish_read(self):
+        """(weight sums float64 (k,), batch inertia, non-canonical blocks)."""
+        if self.read_done is not None:
+            self.read_done.synchronize()
+            self.read_done = None
+        v = self.host.numpy()
+        return v[: self.k].copy(), float(v[self.k]), float(v[self.k + 1])
+
+
+def _new_state(be, X, centers, weight_sums):
+    if isinstance(X, _SparseData):
+        return _SparseMiniBatchState(be, centers, weight_sums)
+    return _MiniBatchState(be, centers, weight_sums, X.dtype)
+
+
 class PartialMiniBatchKMeans(MiniBatchKMeans):
     """Mini-batch k-means over the row blocks of X (API of dask_ml.cluster.PartialMiniBatchKMeans).
 
@@ -125,6 +222,10 @@ class PartialMiniBatchKMeans(MiniBatchKMeans):
     block is read once, so this is the estimator for data larger than device memory
     (``dask_ml_b200.engine.host_resident``).  Parameters, ``get_params``, ``clone`` and their validation are
     scikit-learn's ``MiniBatchKMeans``'s.
+
+    X may also be sparse (a ChunkedArray of torch CSR blocks, one torch CSR tensor or a scipy.sparse matrix): each
+    step then keeps the centres transposed in a sparse pack, 3 * 8 n_features n_clusters bytes of device memory.  Dense
+    and sparse batches may follow each other; they continue from the same float64 state.
 
     Differences from scikit-learn: centres and weight sums are kept in float64 on the device whatever the dtype of X
     (scikit-learn keeps float32 for float32 X, whose counters stop counting exactly above 2^24 rows per cluster);
@@ -197,7 +298,9 @@ class PartialMiniBatchKMeans(MiniBatchKMeans):
         X = self._check_array(X)
         order = list(range(len(X.chunk_rows)))
         check_random_state(None).shuffle(order)
-        if isinstance(X.chunks, StreamedChunks):
+        if isinstance(X, _SparseData):
+            blocks = (X.blocks[i] for i in order)
+        elif isinstance(X.chunks, StreamedChunks):
             blocks = X.chunks.iter_order(order)
         else:
             blocks = (X.chunks[i] for i in order)
@@ -218,8 +321,9 @@ class PartialMiniBatchKMeans(MiniBatchKMeans):
             raise NotImplementedError("sample_weight is not supported: the fused kernels add rows unweighted")
         _single_process()
         X = self._check_array(X)
-        reassign = self._step_begin(X, X.chunks, 0)
-        self._step_end(X, X.chunks, 0, reassign, self.compute_labels)
+        chunks = X.blocks if isinstance(X, _SparseData) else X.chunks
+        reassign = self._step_begin(X, chunks, 0)
+        self._step_end(X, chunks, 0, reassign, self.compute_labels)
         self._publish(X)
         return self
 
@@ -259,6 +363,16 @@ class PartialMiniBatchKMeans(MiniBatchKMeans):
             self._init_size = 3 * self.n_clusters
         self._init_size = min(self._init_size, n)
 
+    @staticmethod
+    def _host_rows(X, idx):
+        """Local rows of X on the host: numpy, or a scipy CSR for sparse X."""
+        return X._local_csr(idx) if isinstance(X, _SparseData) else X.local_rows(idx)
+
+    @staticmethod
+    def _dense_rows(X, idx):
+        """Local rows of X as a float64-able numpy array (sparse rows densified, as scikit-learn's ``toarray()``)."""
+        return X._local_csr(idx).toarray() if isinstance(X, _SparseData) else X.local_rows(idx)
+
     def _init_centroids_host(self, X, off, n):
         """``_BaseKMeans._init_centroids`` on ``init_size`` rows of the batch, gathered to the host."""
         rs = self._random_state
@@ -270,22 +384,24 @@ class PartialMiniBatchKMeans(MiniBatchKMeans):
         if self._init_size < n:
             idx = rs.randint(0, n, self._init_size)
         if isinstance(init, str) and init == "k-means++":
-            centers, _ = kmeans_plusplus(X.local_rows(off + idx), self.n_clusters, random_state=rs)
+            centers, _ = kmeans_plusplus(self._host_rows(X, off + idx), self.n_clusters, random_state=rs)
         elif isinstance(init, str) and init == "random":
             sw = np.ones(len(idx), dtype=X.np_dtype)
             seeds = rs.choice(len(idx), size=self.n_clusters, replace=False, p=sw / sw.sum())
-            centers = X.local_rows(off + idx[seeds])
+            centers = self._dense_rows(X, off + idx[seeds])
         elif _is_arraylike_not_scalar(init):
             centers = init
         else:
-            centers = init(X.local_rows(off + idx), self.n_clusters, random_state=rs)
+            centers = init(self._host_rows(X, off + idx), self.n_clusters, random_state=rs)
+            if scipy.sparse.issparse(centers):
+                centers = centers.toarray()
             centers = _sk_check_array(centers, dtype=X.np_dtype, copy=False, order="C")
             self._validate_center_shape(_Shape(n, X.d), centers)
         return centers
 
     @staticmethod
     def _batch_rows(X, chunks):
-        return int(sum(int(x.shape[0]) for x in chunks)) if isinstance(chunks, list) else X.n_local
+        return int(sum(_rows(x) for x in chunks)) if isinstance(chunks, list) else X.n_local
 
     def _step_begin(self, X, chunks, off):
         """First half of ``partial_fit`` on the batch made of the rows ``off, off + 1, ...`` of X that ``chunks``
@@ -309,10 +425,13 @@ class PartialMiniBatchKMeans(MiniBatchKMeans):
             self._counts = np.zeros(self.n_clusters, dtype=X.np_dtype)
             self._n_since_last_reassign = 0
             self.n_features_in_ = X.d
-            st = self._mb = _MiniBatchState(be, centers, self._counts, X.dtype)
+            st = self._mb = _new_state(be, X, centers, self._counts)
         elif st is None:                        # unpickled: the float64 state, or the published attributes
             centers, weight_sums = self.__dict__.pop("_mb_host", (self.cluster_centers_, self._counts))
-            st = self._mb = _MiniBatchState(be, centers, weight_sums, X.dtype)
+            st = self._mb = _new_state(be, X, centers, weight_sums)
+        elif isinstance(st, _SparseMiniBatchState) != isinstance(X, _SparseData):
+            # a sparse batch after a dense one, or the reverse: the same float64 state in the other layout
+            st = self._mb = _new_state(be, X, st.C.cpu().numpy(), st.W.cpu().numpy())
 
         random_reassign = self._random_reassign()
         st.step(be, chunks, X.dtype)
@@ -324,7 +443,15 @@ class PartialMiniBatchKMeans(MiniBatchKMeans):
         batch against the new centres."""
         be, st = X.backend, self._mb
         n = self._batch_rows(X, chunks)
-        w, batch_inertia = st.finish_read()
+        sparse = isinstance(st, _SparseMiniBatchState)
+        if sparse:
+            w, batch_inertia, bad = st.finish_read()
+            if bad != 0.0:
+                st.undo()
+                raise ValueError("Sparse input must be canonical CSR: the column indices of a block of the batch are "
+                                 "not strictly increasing within each row, or not in [0, %d)" % X.d)
+        else:
+            w, batch_inertia = st.finish_read()
         _km._check_engine(be, batch_inertia, "the batch inertia")
 
         # scikit-learn's _mini_batch_step after _minibatch_update_dense, on the weight sums in X's dtype
@@ -340,9 +467,16 @@ class PartialMiniBatchKMeans(MiniBatchKMeans):
                 if self.verbose:
                     print(f"[MiniBatchKMeans] Reassigning {n_reassigns} cluster centers.")
                 # streamed data: the rows come from the host copy of the batch, which stays valid
-                rows = torch.from_numpy(X.local_rows(off + new_centers)).to(device=st.C.device, dtype=torch.float64)
-                st.C[torch.as_tensor(np.where(to_reassign)[0], device=st.C.device)] = rows
-                st.pack = be.pack_centers(st.C, st.dtype, out=st.pack)
+                rows = torch.from_numpy(self._dense_rows(X, off + new_centers)).to(device=st.C.device,
+                                                                                    dtype=torch.float64)
+                where = torch.as_tensor(np.where(to_reassign)[0], device=st.C.device)
+                if sparse:
+                    C = st.C.contiguous()
+                    C[where] = rows
+                    st.set_centres(be, C)
+                else:
+                    st.C[where] = rows
+                    st.pack = be.pack_centers(st.C, st.dtype, out=st.pack)
             w[to_reassign] = np.min(w[~to_reassign])
             st.W.copy_(torch.from_numpy(w))
         self._counts = w.astype(X.np_dtype)
@@ -351,8 +485,11 @@ class PartialMiniBatchKMeans(MiniBatchKMeans):
             acc = be.zeros((1,), torch.float64)
             labels = []
             for x in chunks:
-                lab = be.empty((int(x.shape[0]),), torch.int32)
-                be.assign_chunk(x, st.pack, st.k, lab, None, True, acc)
+                lab = be.empty((_rows(x),), torch.int32)
+                if sparse:
+                    be.csr_assign_chunk(x, st.d, st.packs[st.cur], st.k, labels=lab, dist_sum=acc)
+                else:
+                    be.assign_chunk(x, st.pack, st.k, lab, None, True, acc)
                 labels.append(lab)
             self.labels_ = ChunkedArray(labels)
             self.inertia_ = float(acc.item())

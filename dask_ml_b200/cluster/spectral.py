@@ -13,16 +13,19 @@ embedding needs no (n, l) matrix at all:
 
 The same formula holds for keep rows and the other rows, so rows stay in input order (the reference's
 ``_slice_mostly_sorted`` reordering has nothing to undo).  For ``affinity='rbf'`` the two sums over X are two
-streaming passes of CUDA kernels (``bkm_kernel_colsum_chunk`` and ``bkm_nystrom_embed_chunk``); the rest is (l, l)
-host algebra in float64 and one ``KMeans.fit`` on the device-resident embedding.
+streaming passes of CUDA kernels (``bkm_kernel_colsum_chunk`` and ``bkm_nystrom_embed_chunk``; on sparse CSR blocks
+``bkm_csr_kernel_colsum_chunk`` and ``bkm_csr_nystrom_embed_chunk``); the rest is (l, l) host algebra in float64 and
+one ``KMeans.fit`` on the device-resident embedding.
 """
 import logging
 
 import numpy as np
+import scipy.sparse
 import torch
 from sklearn.base import BaseEstimator, ClusterMixin
 from sklearn.utils import check_random_state
 
+from .._sparse import _SparseData, _sparse_data
 from ..chunked import ChunkedArray, is_dask_dataframe
 from ..engine import DeviceData
 from ..utils import check_array
@@ -117,10 +120,19 @@ class SpectralClustering(BaseEstimator, ClusterMixin):
             pass
         if is_dask_dataframe(X):
             raise TypeError("Cannot fit on dask.dataframe due to unknown partition lengths.")
-        if isinstance(X, DeviceData):
+        if isinstance(X, (DeviceData, _SparseData)):
             return X
+        sp = _sparse_data(X)                    # sparse CSR blocks (engine extension: the reference rejects them)
+        if sp is not None:
+            sp.check_finite()
+            return sp
         X = check_array(X, accept_dask_dataframe=False, accept_unknown_chunks=False, accept_sparse=False)
         return _km._to_device_data(X)
+
+    def __sklearn_tags__(self):
+        tags = super().__sklearn_tags__()
+        tags.input_tags.sparse = True           # sparse CSR blocks run through the sparse Nystrom passes
+        return tags
 
     def fit(self, X, y=None):
         X = self._check_array(X)
@@ -178,6 +190,8 @@ class SpectralClustering(BaseEstimator, ClusterMixin):
         X_keep = X.global_rows(keep)
         if callable(metric):
             passes = _CallablePasses(X, X_keep, metric, params)
+        elif isinstance(X, _SparseData):
+            passes = _SparseRbfPasses(X, X_keep, self.gamma)
         else:
             passes = _RbfPasses(X, X_keep, self.gamma)
 
@@ -280,18 +294,68 @@ class _RbfPasses(object):
         return out
 
 
+class _SparseRbfPasses(object):
+    """``_RbfPasses`` on sparse CSR blocks: the keep rows (a host CSR) densified on the device into a sparse pack, which
+    takes 8 (p + 1) l bytes (839 MB at p = 2^20 features and l = 100); every distance and kernel value is float64.  The
+    embedding has the dtype of the values (float32 or float64)."""
+
+    def __init__(self, X, X_keep, gamma):
+        self.X, self.be = X, X.backend
+        self.l = int(X_keep.shape[0])
+        self.gamma = 1.0 / X.d if gamma is None else float(gamma)
+        self.keep = X_keep
+        self.pack = self.be.sparse_pack_centers(_km._dense_centres(X_keep, X.d, self.be))
+
+    def colsum(self):
+        be, X = self.be, self.X
+        c = be.zeros((self.l,), torch.float64)
+        for i, blk in enumerate(X.blocks):
+            be.csr_kernel_colsum(blk, X.d, self.pack, self.l, self.gamma, c, first=i == 0)
+        X.comm.allreduce_sum_(c)
+        return c.cpu().numpy()
+
+    def keep_block(self):
+        from sklearn.metrics.pairwise import rbf_kernel
+
+        return rbf_kernel(self.keep.astype(np.float64), gamma=self.gamma)
+
+    def embed(self, W):
+        be, X = self.be, self.X
+        k = int(W.shape[1])
+        dt = torch.float32 if X.dtype == torch.float32 else torch.float64
+        Wd = torch.as_tensor(np.ascontiguousarray(W, dtype=np.float64)).to(be.device)
+        out = []
+        for blk in X.blocks:
+            e = _embedding_buffer(be, int(blk[3]), k, dt)
+            if int(blk[3]):
+                be.csr_nystrom_embed(blk, X.d, self.pack, self.l, self.gamma, Wd, e)
+            out.append(e)
+        return out
+
+
+def _host_parts(X):
+    """(rows, host block) per block of X: numpy rows, or a scipy CSR for sparse X."""
+    if isinstance(X, _SparseData):
+        for crow, col, val, n in X.blocks:
+            yield int(n), scipy.sparse.csr_matrix((val.cpu().numpy(), col.cpu().numpy(), crow.cpu().numpy()),
+                                                  shape=(int(n), X.d))
+        return
+    for x in X.chunks:
+        yield int(x.shape[0]), (x.float() if x.dtype == torch.bfloat16 else x).cpu().numpy()
+
+
 class _CallablePasses(object):
-    """A user kernel ``metric(X_keep, Y=None, **params)``: evaluated per chunk, reduced in float64 torch."""
+    """A user kernel ``metric(X_keep, Y=None, **params)``: evaluated per chunk (numpy rows, or scipy CSR blocks for
+    sparse X), reduced in float64 torch."""
 
     def __init__(self, X, X_keep, metric, params):
         self.X, self.be = X, X.backend
         self.X_keep, self.metric, self.params = X_keep, metric, params
         self.l = int(X_keep.shape[0])
 
-    def _block(self, x):
-        """K(keep, x) as a float64 (l, m) tensor on the device."""
-        xh = x.float() if x.dtype == torch.bfloat16 else x
-        K = self.metric(self.X_keep, xh.cpu().numpy(), **self.params)
+    def _block(self, xh):
+        """K(keep, x) as a float64 (l, m) tensor on the device, for the host block ``xh``."""
+        K = self.metric(self.X_keep, xh, **self.params)
         if isinstance(K, ChunkedArray):
             K = [b if isinstance(b, torch.Tensor) else torch.as_tensor(np.asarray(b)) for b in K.blocks]
             K = torch.cat([b.to(self.be.device) for b in K], dim=0)
@@ -301,9 +365,9 @@ class _CallablePasses(object):
 
     def colsum(self):
         c = self.be.zeros((self.l,), torch.float64)
-        for x in self.X.chunks:
-            if int(x.shape[0]):
-                c += self._block(x).sum(1)
+        for m, xh in _host_parts(self.X):
+            if m:
+                c += self._block(xh).sum(1)
         self.X.comm.allreduce_sum_(c)
         return c.cpu().numpy()
 
@@ -319,11 +383,10 @@ class _CallablePasses(object):
         dt = torch.float64 if self.X.dtype == torch.float64 else torch.float32
         Wd = torch.as_tensor(np.ascontiguousarray(W)).to(self.be.device)
         out = []
-        for x in self.X.chunks:
-            m = int(x.shape[0])
+        for m, xh in _host_parts(self.X):
             e = _embedding_buffer(self.be, m, int(W.shape[1]), dt)
             if m:
-                v = self._block(x).T @ Wd
+                v = self._block(xh).T @ Wd
                 e.copy_(v / torch.sqrt((v * v).sum(1, keepdim=True)))
             out.append(e)
         return out

@@ -8,6 +8,12 @@
 //   bkm_csc_label_sums_chunk  sumsT (p x k) (+)= X^T onehot(labels) over the block's transpose
 //   bkm_sparse_finalize_step  bkm_finalize_step on the transposed layout: C' = sums / max(counts, 1), the shift, the stop
 //                             test, and the next iteration's sparse pack
+//   bkm_csr_kernel_colsum_chunk  colsum_j (+)= sum_i exp(-gamma d2_ij) against the sparse pack of the l keep rows: the
+//                             first Nystrom pass of SpectralClustering (the COLSUM epilogue of the assign kernel)
+//   bkm_csr_nystrom_embed_chunk  out_i = e_i / ||e_i||, e_i = sum_j exp(-gamma (d2_ij - m_i)) W_j, m_i = min_j d2_ij:
+//                             the second Nystrom pass (the EMBED epilogue of the assign kernel)
+//   bkm_sparse_minibatch_step bkm_minibatch_step on the transposed layout: scikit-learn's _minibatch_update_sparse on the
+//                             reduced [p k sumsT | k counts | inertia], the weight sums, and the next sparse pack
 //
 // Every value is widened to float64 from the block's dtype; every sum runs in a fixed order and no float atomics are
 // used, so two calls with the same inputs give the same bits.
@@ -21,6 +27,14 @@
 //                 accumulator in shared memory: entry (row, v) adds v to acc[labels[row]], the lane that owns
 //                 labels[row] mod 32 doing the add, so every (column, cluster) sum runs in row order.  Columns of several
 //                 segments use the segment-and-ticket fold of bkm_csc_plan.cuh.
+//   colsum        each warp adds exp(-gamma d2) of its rows, in row order, into a per-warp float64 row of shared
+//                 memory (a lane owns the keep rows c0 + lane + 32 j of each tile); the CTA adds its warps in warp order
+//                 into its partial row, and colsum_fold adds the CTA partials in CTA order.  At most 3200 keep rows per
+//                 launch (the shared rows of 8 warps in 200 KB): more are split into windows of keep rows.
+//   embed         per row, m_i first (one tile: from the tile's distances; several tiles: a first sweep over every
+//                 tile), then per tile the kernel values go through a per-warp row of shared memory and the lanes own
+//                 the outputs o = lane + 32 t, each adding the tile's keep rows in order by fma.  NaN where
+//                 gamma m_i > 745.13, the rule of bkm_nystrom_embed_chunk.
 //   pack / step   column_reduce (bkm_select.cuh) over the p rows of CT: each element of C' (from the centres or from the
 //                 reduced sums) is written to CT, and per cluster the CTA-ordered sums of (C - C')^2 and of C'^2 give the
 //                 shift terms and cn.  The step adds the k shift terms in cluster order.  One kernel writes every pack.
@@ -57,23 +71,117 @@ struct AssignArgs {
   double* counts;      // nullable, accumulated
   int first;
   const int* skip;     // nullable: LoopState::done
-  double* part;        // [grid] CTA partial distance sums
+  double* part;        // [grid] CTA partial distance sums (COLSUM: [grid][k] partial column sums)
   unsigned long long* cnt;  // [k] integer counts of this call, zero at launch
   unsigned* ticket;
+  double gamma;        // COLSUM / EMBED
+  int j0, jn;          // COLSUM: the keep rows [j0, j0 + jn) of this launch
+  const double* W;     // EMBED: [k][kw]
+  int kw;
 };
 
+// the epilogues of csr_assign_kernel: the E-step (arg-min or the full distance block), the Nystrom passes
+enum CsrEpi { CSR_EPI_ASSIGN = 0, CSR_EPI_COLSUM = 1, CSR_EPI_EMBED = 2 };
+constexpr int kColsumWindow = 3200;    // keep rows of one COLSUM launch: kWarps rows of float64 in 200 KB
+
+// One tile of row i: the lanes own the centres c0 + lane + 32 j below `hi` (own[j]); y[j] = d2 to each (CUDART_INF
+// where not owned).
 template <typename T, int C>
-__global__ void __launch_bounds__(kThreads) csr_assign_kernel(AssignArgs a) {
+__device__ __forceinline__ void csr_row_tile(const AssignArgs& a, const T* val, long long i, int c0, int hi,
+                                             bool (&own)[C], double (&y)[C]) {
+  const int lane = threadIdx.x & 31;
+  double acc[C];
+#pragma unroll
+  for (int j = 0; j < C; ++j) { own[j] = c0 + lane + 32 * j < hi; acc[j] = 0.0; }
+  double xn = 0.0;
+  csr_row_gather<T, C, true>(a.crow, a.col, val, i, a.p, a.CT, a.k, c0, own, acc, xn);
+#pragma unroll
+  for (int j = 0; j < C; ++j)
+    y[j] = own[j] ? fmax(fma(-2.0, acc[j], xn) + a.cn[c0 + lane + 32 * j], 0.0) : CUDART_INF;
+}
+
+// EMBED: row i of the embedding.  vw [32 C] and ew [kw] are the warp's rows of shared memory.
+template <typename T, int C>
+__device__ __forceinline__ void embed_row(const AssignArgs& a, const T* val, long long i, double* vw, double* ew) {
+  constexpr int CW = 32 * C;
+  const int lane = threadIdx.x & 31, l = a.k, kw = a.kw;
+  const bool one = l <= CW;
+  bool own[C];
+  double y[C];
+  double m = CUDART_INF;
+#pragma unroll 1
+  for (int c0 = 0; c0 < l; c0 += CW) {                  // one tile: its distances stay in y for the second sweep
+    csr_row_tile<T, C>(a, val, i, c0, l, own, y);
+#pragma unroll
+    for (int j = 0; j < C; ++j) m = fmin(m, y[j]);
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) m = fmin(m, __shfl_xor_sync(0xffffffffu, m, o));
+  for (int o = lane; o < kw; o += 32) ew[o] = 0.0;
+#pragma unroll 1
+  for (int c0 = 0; c0 < l; c0 += CW) {
+    if (!one) csr_row_tile<T, C>(a, val, i, c0, l, own, y);
+    __syncwarp();
+#pragma unroll
+    for (int j = 0; j < C; ++j)
+      if (own[j]) vw[lane + 32 * j] = exp(-a.gamma * (y[j] - m));
+    __syncwarp();
+    const int nb = min(CW, l - c0);
+    const double* w = a.W + (size_t)c0 * kw;
+    for (int o = lane; o < kw; o += 32) {
+      double e = ew[o];
+      for (int j = 0; j < nb; ++j) e = fma(vw[j], __ldg(w + (size_t)j * kw + o), e);
+      ew[o] = e;
+    }
+  }
+  double nrm = 0.0;
+  for (int o = lane; o < kw; o += 32) nrm = fma(ew[o], ew[o], nrm);
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) nrm += __shfl_xor_sync(0xffffffffu, nrm, o);
+  const double f = m * a.gamma > 745.13 ? CUDART_NAN : 1.0 / sqrt(nrm);
+  for (int o = lane; o < kw; o += 32) {
+    const double v = ew[o] * f;
+    if (a.out_dtype == BKM_F64) reinterpret_cast<double*>(a.out)[i * a.ldo + o] = v;
+    else reinterpret_cast<float*>(a.out)[i * a.ldo + o] = (float)v;
+  }
+}
+
+// The Nystrom epilogues ask for 3 CTAs per SM: without a minimum, ptxas holds them to 48 registers and spills.  The
+// E-step keeps its bounds (and registers).
+template <typename T, int C, int EPI = CSR_EPI_ASSIGN>
+__global__ void __launch_bounds__(kThreads, EPI == CSR_EPI_ASSIGN ? 0 : 3) csr_assign_kernel(AssignArgs a) {
   constexpr int CW = 32 * C;
   __shared__ double s_sum[kWarps];
+  extern __shared__ double s_dyn[];    // COLSUM: [kWarps][jn] column sums; EMBED: [kWarps][CW + kw] vw, ew
   if (a.skip && *a.skip) return;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const T* val = reinterpret_cast<const T*>(a.val);
   const bool argmin = a.mode == BKM_SPARSE_ARGMIN;
   double wsum = 0.0;
   const long long nw = (long long)gridDim.x * kWarps;
+  if constexpr (EPI == CSR_EPI_COLSUM) {
+    for (int j = lane; j < a.jn; j += 32) s_dyn[warp * a.jn + j] = 0.0;
+    __syncwarp();
+  }
 #pragma unroll 1
   for (long long i = (long long)blockIdx.x * kWarps + warp; i < a.n; i += nw) {
+    if constexpr (EPI == CSR_EPI_EMBED) {
+      double* vw = s_dyn + (size_t)warp * (CW + a.kw);
+      embed_row<T, C>(a, val, i, vw, vw + CW);
+      continue;
+    } else if constexpr (EPI == CSR_EPI_COLSUM) {
+      double* cs = s_dyn + (size_t)warp * a.jn - a.j0;
+#pragma unroll 1
+      for (int c0 = a.j0; c0 < a.j0 + a.jn; c0 += CW) {
+        bool own[C];
+        double y[C];
+        csr_row_tile<T, C>(a, val, i, c0, a.j0 + a.jn, own, y);
+#pragma unroll
+        for (int j = 0; j < C; ++j)
+          if (own[j]) cs[c0 + lane + 32 * j] += exp(-a.gamma * y[j]);
+      }
+      continue;
+    }
     double best = CUDART_INF;
     int bj = 0x7fffffff;
 #pragma unroll 1
@@ -114,6 +222,17 @@ __global__ void __launch_bounds__(kThreads) csr_assign_kernel(AssignArgs a) {
       if (a.counts) atomicAdd(a.cnt + bj, 1ull);
     }
   }
+  if constexpr (EPI == CSR_EPI_COLSUM) {
+    // ---- the CTA's partial: its warps in order ----
+    __syncthreads();
+    for (int j = tid; j < a.jn; j += kThreads) {
+      double v = 0.0;
+      for (int w = 0; w < kWarps; ++w) v += s_dyn[w * a.jn + j];
+      a.part[(size_t)blockIdx.x * a.k + a.j0 + j] = v;
+    }
+    return;
+  }
+  if constexpr (EPI != CSR_EPI_ASSIGN) return;
   if (!argmin || (!a.dist_sum && !a.counts)) return;
 
   // ---- the fold: warps in order, CTAs in order by the last CTA, which also publishes the counts ----
@@ -151,19 +270,37 @@ static size_t assign_ws(long long n, int k, int sms) {
   return align_up((size_t)assign_grid(n, sms) * 8, 256) + align_up((size_t)k * 8, 256) + 256;
 }
 
-template <typename T, int C>
+// dynamic shared memory of an epilogue launch
+template <int C, int EPI>
+static size_t assign_smem(const AssignArgs& a) {
+  if (EPI == CSR_EPI_COLSUM) return (size_t)kWarps * a.jn * 8;
+  if (EPI == CSR_EPI_EMBED) return (size_t)kWarps * (32 * C + a.kw) * 8;
+  return 0;
+}
+
+template <typename T, int C, int EPI>
 static int launch_assign(const AssignArgs& a, int grid, cudaStream_t s) {
-  csr_assign_kernel<T, C><<<grid, kThreads, 0, s>>>(a);
+  const size_t smem = assign_smem<C, EPI>(a);
+  if (smem > 200 * 1024) return BKM_EUNSUPPORTED;
+  if (smem > 48 * 1024)
+    BKM_CUDA_TRY(cudaFuncSetAttribute(csr_assign_kernel<T, C, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                      (int)smem));
+  csr_assign_kernel<T, C, EPI><<<grid, kThreads, smem, s>>>(a);
   BKM_CUDA_TRY(cudaGetLastError());
   note_launch();
   return 0;
 }
 
-template <typename T>
+template <typename T, int EPI = CSR_EPI_ASSIGN>
 static int assign(const AssignArgs& a, int grid, cudaStream_t s) {
-  if (a.k <= 32) return launch_assign<T, 1>(a, grid, s);
-  if (a.k <= 64) return launch_assign<T, 2>(a, grid, s);
-  return launch_assign<T, 4>(a, grid, s);
+  if (a.k <= 32) return launch_assign<T, 1, EPI>(a, grid, s);
+  if (a.k <= 64) return launch_assign<T, 2, EPI>(a, grid, s);
+  return launch_assign<T, 4, EPI>(a, grid, s);
+}
+
+template <int EPI>
+static int assign_dt(const AssignArgs& a, int val_dtype, int grid, cudaStream_t s) {
+  return val_dtype == BKM_F32 ? assign<float, EPI>(a, grid, s) : assign<double, EPI>(a, grid, s);
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -253,6 +390,26 @@ struct FromSums {
   }
 };
 
+// ... from the reduced buffer and the current pack and weight sums: scikit-learn's _minibatch_update_sparse,
+// C' = (C w + S) (1 / (w + n)) where n > 0, else C, with the explicit round-to-nearest intrinsics of
+// CentreFromMinibatch (bkm_aux.cu).  The element of row 0 of each cluster also writes w' = w + n.
+struct FromMinibatch {
+  const double* red;
+  const double* ct;    // the current CT [p][k]
+  const double* w_in;
+  double* w_out;
+  long long pk;
+  int k;
+  __device__ __forceinline__ double operator()(long long f, int j) const {
+    const double n = red[pk + j];
+    if (f == 0) w_out[j] = __dadd_rn(w_in[j], n);
+    const double c = ct[(size_t)f * k + j];
+    if (!(n > 0.0)) return c;
+    const double alpha = __ddiv_rn(1.0, __dadd_rn(w_in[j], n));
+    return __dmul_rn(__dadd_rn(__dmul_rn(c, w_in[j]), red[(size_t)f * k + j]), alpha);
+  }
+};
+
 template <typename Src>
 struct PackRows {
   Src src;
@@ -327,6 +484,8 @@ static int launch_pack(const Src& src, const double* ct_in, double* pack_out, in
 }
 
 }  // namespace
+
+int launch_colsum_fold(const double* part, int parts, int l, double* colsum, int first, cudaStream_t s);
 }  // namespace bkm
 
 using namespace bkm;
@@ -372,8 +531,66 @@ extern "C" int bkm_csr_assign_chunk(const int64_t* crow, const int64_t* col, con
     a.ticket = reinterpret_cast<unsigned*>(ws + o2);
     BKM_CUDA_TRY(cudaMemsetAsync(ws + o1, 0, o2 - o1 + 256, s));
   }
-  if (val_dtype == BKM_F32) return assign<float>(a, grid, s);
-  return assign<double>(a, grid, s);
+  return assign_dt<CSR_EPI_ASSIGN>(a, val_dtype, grid, s);
+}
+
+// AssignArgs of the Nystrom epilogues: the block against the sparse pack of the l keep rows
+static AssignArgs nystrom_args(const int64_t* crow, const int64_t* col, const void* val, int64_t n, int p,
+                               const double* pack, int l, double gamma) {
+  AssignArgs a = {};
+  a.crow = reinterpret_cast<const long long*>(crow);
+  a.col = reinterpret_cast<const long long*>(col);
+  a.val = val; a.n = n; a.p = p; a.CT = pack; a.cn = pack + (size_t)p * l; a.k = l;
+  a.gamma = gamma;
+  return a;
+}
+
+extern "C" int bkm_csr_kernel_colsum_workspace_bytes(int64_t n, int l, size_t* out) {
+  if (!out || n < 0 || l <= 0) return BKM_EINVAL;
+  *out = align_up((size_t)assign_grid(n, sm_count_or_default()) * l * 8, 256);
+  return 0;
+}
+
+extern "C" int bkm_csr_kernel_colsum_chunk(const int64_t* crow, const int64_t* col, const void* val, int val_dtype,
+                                           int64_t n, int p, int64_t nnz, const double* pack, int l, double gamma,
+                                           double* colsum, void* workspace, size_t ws_bytes, int flags, void* stream) {
+  if (n < 0 || p <= 0 || nnz < 0 || l <= 0 || !crow || !pack || !colsum) return BKM_EINVAL;
+  if (nnz > 0 && (!col || !val)) return BKM_EINVAL;
+  if (val_dtype != BKM_F32 && val_dtype != BKM_F64) return BKM_EDTYPE;
+  cudaStream_t s = (cudaStream_t)stream;
+  const int first = (flags & BKM_FLAG_FIRST_CHUNK) ? 1 : 0;
+  if (n == 0) {
+    if (first) BKM_CUDA_TRY(cudaMemsetAsync(colsum, 0, (size_t)l * sizeof(double), s));
+    return 0;
+  }
+  const int sms = sm_count_or_default();
+  const int grid = assign_grid(n, sms);
+  if (!workspace || ws_bytes < align_up((size_t)grid * l * 8, 256)) return BKM_EWORKSPACE;
+  AssignArgs a = nystrom_args(crow, col, val, n, p, pack, l, gamma);
+  a.part = reinterpret_cast<double*>(workspace);
+  for (int j0 = 0; j0 < l; j0 += kColsumWindow) {
+    a.j0 = j0;
+    a.jn = min(kColsumWindow, l - j0);
+    const int rc = assign_dt<CSR_EPI_COLSUM>(a, val_dtype, grid, s);
+    if (rc) return rc;
+  }
+  return launch_colsum_fold(a.part, grid, l, colsum, first, s);
+}
+
+extern "C" int bkm_csr_nystrom_embed_chunk(const int64_t* crow, const int64_t* col, const void* val, int val_dtype,
+                                           int64_t n, int p, int64_t nnz, const double* pack, int l, double gamma,
+                                           const double* W, int k, void* out, int64_t ldo, int out_dtype, int flags,
+                                           void* stream) {
+  (void)flags;
+  if (n < 0 || p <= 0 || nnz < 0 || l <= 0 || k <= 0 || ldo < k || !crow || !pack || !W) return BKM_EINVAL;
+  if (nnz > 0 && (!col || !val)) return BKM_EINVAL;
+  if (val_dtype != BKM_F32 && val_dtype != BKM_F64) return BKM_EDTYPE;
+  if (out_dtype != BKM_F32 && out_dtype != BKM_F64) return BKM_EDTYPE;
+  if (n == 0) return 0;
+  if (!out) return BKM_EINVAL;
+  AssignArgs a = nystrom_args(crow, col, val, n, p, pack, l, gamma);
+  a.W = W; a.kw = k; a.out = out; a.ldo = ldo; a.out_dtype = out_dtype;
+  return assign_dt<CSR_EPI_EMBED>(a, val_dtype, assign_grid(n, sm_count_or_default()), (cudaStream_t)stream);
 }
 
 extern "C" int bkm_csc_label_sums_workspace_bytes(int p, int64_t nnz, int k, size_t* out) {
@@ -443,4 +660,15 @@ extern "C" int bkm_sparse_finalize_step(const double* reduced, const double* pac
   if (ws_bytes < pack_ws(p, k, sm_count_or_default())) return BKM_EWORKSPACE;
   return launch_pack(FromSums{reduced, (long long)p * k, k}, pack_in, pack_out, p, k,
                      reinterpret_cast<LoopState*>(loop_state), workspace, ws_bytes, (cudaStream_t)stream);
+}
+
+extern "C" int bkm_sparse_minibatch_step(const double* reduced, const double* pack_in, const double* weights_in,
+                                         double* pack_out, double* weights_out, int k, int p, void* workspace,
+                                         size_t ws_bytes, void* stream) {
+  if (!reduced || !pack_in || !weights_in || !pack_out || !weights_out || !workspace || k <= 0 || p <= 0)
+    return BKM_EINVAL;
+  if (pack_in == pack_out || weights_in == weights_out) return BKM_EINVAL;
+  if (ws_bytes < pack_ws(p, k, sm_count_or_default())) return BKM_EWORKSPACE;
+  const FromMinibatch src{reduced, pack_in, weights_in, weights_out, (long long)p * k, k};
+  return launch_pack(src, nullptr, pack_out, p, k, nullptr, workspace, ws_bytes, (cudaStream_t)stream);
 }

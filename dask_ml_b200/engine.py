@@ -691,6 +691,47 @@ class CudaBackend(object):
                                                          self._ptr(state), int(k), int(d), self._ptr(ws), ws.numel(),
                                                          self._stream()), "bkm_sparse_finalize_step")
 
+    def sparse_minibatch_step(self, red, pack_in, w_in, pack_out, w_out, k, d):
+        """One mini-batch centre update on the transposed layout (scikit-learn's _minibatch_update_sparse, in float64):
+        red = [d*k sumsT | k counts | inertia] of the batch -> pack_out = the sparse pack of the new centres and
+        w_out = w_in + counts."""
+        nb = ctypes.c_size_t(0)
+        _lib.check(self.lib.bkm_sparse_pack_workspace_bytes(int(k), int(d), ctypes.byref(nb)),
+                   "bkm_sparse_pack_workspace_bytes")
+        ws = self._scratch("sparse_pack", nb.value)
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.bkm_sparse_minibatch_step(self._ptr(red), self._ptr(pack_in), self._ptr(w_in),
+                                                          self._ptr(pack_out), self._ptr(w_out), int(k), int(d),
+                                                          self._ptr(ws), ws.numel(), self._stream()),
+                       "bkm_sparse_minibatch_step")
+
+    def csr_kernel_colsum(self, blk, d, pack, l, gamma, colsum, first=False):
+        """colsum[j] (+)= sum_i exp(-gamma ||x_i - c_j||^2) over the rows of one CSR block against the sparse pack of the
+        l keep rows (float64 [l]); ``first`` overwrites.  The first Nystrom pass of SpectralClustering on sparse X."""
+        crow, col, val, n = blk
+        nb = ctypes.c_size_t(0)
+        _lib.check(self.lib.bkm_csr_kernel_colsum_workspace_bytes(int(n), int(l), ctypes.byref(nb)),
+                   "bkm_csr_kernel_colsum_workspace_bytes")
+        ws = self._scratch("csr_kernel_colsum", nb.value)
+        flags = self.flags | (_lib.FLAG_FIRST_CHUNK if first else 0)
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.bkm_csr_kernel_colsum_chunk(
+                self._ptr(crow), self._ptr(col), self._ptr(val), _DT_CODE[val.dtype], int(n), int(d), int(col.numel()),
+                self._ptr(pack), int(l), float(gamma), self._ptr(colsum), self._ptr(ws), ws.numel(), flags,
+                self._stream()), "bkm_csr_kernel_colsum_chunk")
+
+    def csr_nystrom_embed(self, blk, d, pack, l, gamma, W, out):
+        """out[i] = e_i / ||e_i||, e_i = sum_j exp(-gamma (||x_i - c_j||^2 - min_j ||x_i - c_j||^2)) W[j] over one CSR
+        block — the second Nystrom pass on sparse X.  ``W`` is (l, k) float64; ``out`` (n, k) float32 / float64 may have
+        a padded row pitch."""
+        crow, col, val, n = blk
+        k = int(W.shape[1])
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.bkm_csr_nystrom_embed_chunk(
+                self._ptr(crow), self._ptr(col), self._ptr(val), _DT_CODE[val.dtype], int(n), int(d), int(col.numel()),
+                self._ptr(pack), int(l), float(gamma), self._ptr(W), k, self._ptr(out), out.stride(0) if n else k,
+                _DT_CODE[out.dtype], self.flags, self._stream()), "bkm_csr_nystrom_embed_chunk")
+
     def colstats_chunk(self, x, shift, acc, minmax, first=False):
         """The scalers' statistics pass over one chunk, float64 on the device: acc (5, d) (+)= [sum (x - shift) |
         sum (x - shift)^2 over the finite x | NaN count | +inf count | -inf count] and minmax (2, d) = [min | max] over

@@ -1,7 +1,8 @@
 """GPU versions of the three distance operators the KMeans path uses
 (dask_ml/metrics/pairwise.py:18-52, 55-66, 69-97).  Only the euclidean metric exists on this
-path; every result is a device-resident ``ChunkedArray`` with the reference's dtypes.  ``pairwise_distances_argmin_min``
-and ``euclidean_distances`` also take sparse CSR X (any form ``KMeans`` takes) against a dense Y."""
+path; every result is a device-resident ``ChunkedArray`` with the reference's dtypes.  ``pairwise_distances_argmin_min``,
+``euclidean_distances``, ``rbf_kernel`` and ``pairwise_kernels(metric="rbf")`` also take sparse CSR X (any form
+``KMeans`` takes) against a dense Y."""
 import numpy as np
 import torch
 
@@ -217,7 +218,22 @@ def check_pairwise_arrays(X, Y, precomputed=False):
 
 def rbf_kernel(X, Y=None, gamma=None):
     """exp(-gamma * ||x - y||^2) (pairwise.py:131-139); ``gamma`` defaults to 1 / n_features.  One fused pass: the
-    distance kernel's epilogue applies the exponential (mode 2 of ``bkm_transform_chunk``)."""
+    distance kernel's epilogue applies the exponential (mode 2 of ``bkm_transform_chunk``).  Sparse X (against a dense
+    Y) takes the squared distances of ``bkm_csr_assign_chunk`` and exponentiates them in place, with the dtype rule of
+    ``euclidean_distances``."""
+    Xs = _sparse_x(X)
+    if Xs is not None:
+        if Y is None:
+            raise NotImplementedError("sparse X needs a dense Y")
+        be, pack, k, ydt = _sparse_prep(Xs, Y)
+        g = 1.0 / Xs.d if gamma is None else float(gamma)
+        odt = torch.float32 if Xs.dtype == torch.float32 and ydt == np.float32 else torch.float64
+        outs = []
+        for blk in Xs.blocks:
+            out = be.empty((int(blk[3]), k), odt)
+            be.csr_assign_chunk(blk, Xs.d, pack, k, out=out, mode=2)
+            outs.append(out.mul_(-g).exp_())
+        return ChunkedArray(outs)
     Xd = _as_device(X)
     if Y is None:
         Y = Xd.to_host()

@@ -34,6 +34,9 @@
  *     CSR blocks, which the reference rejects (k_means.py:168)          bkm_csc_label_sums_chunk,
  *                                                                       bkm_sparse_pack_centers,
  *                                                                       bkm_sparse_finalize_step
+ *   the mini-batch steps of PartialMiniBatchKMeans and the Nystrom      bkm_sparse_minibatch_step,
+ *     passes of SpectralClustering on sparse CSR blocks, which the      bkm_csr_kernel_colsum_chunk,
+ *     reference hands to scikit-learn / rejects                         bkm_csr_nystrom_embed_chunk
  *   da.linalg.svd_compressed's X.dot(omega), X.T.dot(q) and the        bkm_csr_panel_chunk, bkm_csc_panel_chunk
  *     projection of TruncatedSVD on sparse CSR blocks, which the
  *     reference densifies (decomposition/truncated_svd.py)
@@ -97,8 +100,10 @@ extern "C" {
  *     bkm_gram_weighted_csr_chunk
  * 6 = bkm_csr_panel_chunk, bkm_csc_panel_workspace_bytes, bkm_csc_panel_chunk
  * 7 = bkm_csr_assign_workspace_bytes, bkm_csr_assign_chunk, bkm_csc_label_sums_workspace_bytes,
- *     bkm_csc_label_sums_chunk, bkm_sparse_pack_workspace_bytes, bkm_sparse_pack_centers, bkm_sparse_finalize_step */
-#define BKM_VERSION_MINOR 7
+ *     bkm_csc_label_sums_chunk, bkm_sparse_pack_workspace_bytes, bkm_sparse_pack_centers, bkm_sparse_finalize_step
+ * 8 = bkm_csr_kernel_colsum_workspace_bytes, bkm_csr_kernel_colsum_chunk, bkm_csr_nystrom_embed_chunk,
+ *     bkm_sparse_minibatch_step */
+#define BKM_VERSION_MINOR 8
 
 /* element types of X */
 #define BKM_F32 0
@@ -406,6 +411,33 @@ int bkm_csc_label_sums_chunk(const int64_t* colptr, const int32_t* rows, const v
                              void* workspace, size_t ws_bytes, int flags, const void* loop_state, void* stream);
 int bkm_sparse_finalize_step(const double* reduced, const double* pack_in, double* pack_out, void* loop_state, int k,
                              int p, void* workspace, size_t ws_bytes, void* stream);
+
+/* ---- PartialMiniBatchKMeans and SpectralClustering on sparse CSR blocks: the same conventions (float64, fixed order, no
+ * float atomics, the same bits from two calls), over a sparse pack.
+ *   bkm_csr_kernel_colsum_chunk  the contract of bkm_kernel_colsum_chunk for one CSR block against the sparse pack of
+ *                      the l keep rows (bkm_sparse_pack_centers with k = l): colsum[j] (l, float64) = sum_i
+ *                      exp(-gamma y_ij), y_ij = max(||x_i||^2 - 2 x_i.c_j + ||c_j||^2, 0) as in bkm_csr_assign_chunk.
+ *                      Rows add in warp order, warps in CTA order, CTAs in CTA order.  OVERWRITTEN with
+ *                      BKM_FLAG_FIRST_CHUNK, else ACCUMULATED (n = 0 still overwrites).  workspace:
+ *                      bkm_csr_kernel_colsum_workspace_bytes(n, l) bytes, any content.
+ *   bkm_csr_nystrom_embed_chunk  the contract of bkm_nystrom_embed_chunk: out_i = e_i / ||e_i||, e_i = sum_j
+ *                      exp(-gamma (y_ij - m_i)) W_j, m_i = min_j y_ij, W [l][k] float64, out [n][ldo] (ldo >= k) in
+ *                      out_dtype (BKM_F32 or BKM_F64); NaN where gamma m_i > 745.13.  Any l; e_i adds j in ascending
+ *                      order by fma.  k <= 3000.
+ *   bkm_sparse_minibatch_step  scikit-learn's _minibatch_update_sparse on the transposed layout: reduced = [p k sumsT |
+ *                      k counts as float64 | inertia] of the batch, C' = (C w + S) (1 / (w + n)) where n > 0, else C
+ *                      (explicit round-to-nearest float64, as bkm_minibatch_step), w' = w + n; pack_out (!= pack_in)
+ *                      = the sparse pack of C', weights_out (!= weights_in) = w'.  workspace:
+ *                      bkm_sparse_pack_workspace_bytes(k, p) bytes. */
+int bkm_csr_kernel_colsum_workspace_bytes(int64_t n, int l, size_t* out);
+int bkm_csr_kernel_colsum_chunk(const int64_t* crow, const int64_t* col, const void* val, int val_dtype, int64_t n,
+                                int p, int64_t nnz, const double* pack, int l, double gamma, double* colsum,
+                                void* workspace, size_t ws_bytes, int flags, void* stream);
+int bkm_csr_nystrom_embed_chunk(const int64_t* crow, const int64_t* col, const void* val, int val_dtype, int64_t n,
+                                int p, int64_t nnz, const double* pack, int l, double gamma, const double* W, int k,
+                                void* out, int64_t ldo, int out_dtype, int flags, void* stream);
+int bkm_sparse_minibatch_step(const double* reduced, const double* pack_in, const double* weights_in, double* pack_out,
+                              double* weights_out, int k, int p, void* workspace, size_t ws_bytes, void* stream);
 
 /* ---- StandardScaler / MinMaxScaler / RobustScaler: the fit passes and the transform pass over row chunks (replace
  * X.mean(0), X.var(0), X.min(0), X.max(0), da.percentile per column and the elementwise (X - m) / s of
