@@ -41,6 +41,18 @@ _int = ctypes.c_int
 _dbl = ctypes.c_double
 _szp = ctypes.POINTER(ctypes.c_size_t)
 
+
+class SgdParams(ctypes.Structure):
+    """``bkm_sgd_params`` of include/bkm_b200.h."""
+
+    _fields_ = [("loss", ctypes.c_int), ("penalty", ctypes.c_int), ("learning_rate", ctypes.c_int),
+                ("fit_intercept", ctypes.c_int), ("epsilon", ctypes.c_double), ("alpha", ctypes.c_double),
+                ("l1_ratio", ctypes.c_double), ("eta0", ctypes.c_double), ("optimal_init", ctypes.c_double),
+                ("t0", ctypes.c_double), ("intercept_decay", ctypes.c_double), ("average", ctypes.c_double)]
+
+
+_sgdp = ctypes.POINTER(SgdParams)
+
 # name -> (restype, argtypes); mirrors include/bkm_b200.h one to one
 SIGNATURES = {
     "bkm_version": (_int, []),
@@ -124,6 +136,12 @@ SIGNATURES = {
                                            _dbl, _c_void_p, _int, _c_void_p, _i64, _int, _int, _c_void_p]),
     "bkm_sparse_minibatch_step": (_int, [_c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_void_p, _int, _int, _c_void_p,
                                          ctypes.c_size_t, _c_void_p]),
+    "bkm_sgd_order": (_int, [_i64, ctypes.c_uint32, _c_void_p]),
+    "bkm_sgd_block": (_int, [_c_void_p, _i64, _int, _i64, _int, _c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_void_p,
+                             _int, _sgdp, _c_void_p, _c_void_p, _c_void_p, _c_void_p, _c_void_p]),
+    "bkm_sgd_csr_block": (_int, [_c_void_p, _c_void_p, _c_void_p, _int, _i64, _int, _i64, _c_void_p, _c_void_p,
+                                 _c_void_p, _c_void_p, _c_void_p, _int, _sgdp, _c_void_p, _c_void_p, _c_void_p,
+                                 _c_void_p, _c_void_p]),
     "bkm_colstats_workspace_bytes": (_int, [_i64, _int, _szp]),
     "bkm_colstats_chunk": (_int, [_c_void_p, _i64, _int, _i64, _int, _c_void_p, _c_void_p, _c_void_p, _c_void_p,
                                   ctypes.c_size_t, _int, _c_void_p]),

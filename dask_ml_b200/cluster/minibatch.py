@@ -29,7 +29,7 @@ from sklearn.utils.validation import _is_arraylike_not_scalar, check_is_fitted
 
 from .._sparse import _SparseData
 from ..chunked import ChunkedArray
-from ..engine import StreamedChunks, dist_info
+from ..engine import StreamedChunks, single_process
 from . import k_means as _km
 from .k_means import KMeans
 
@@ -43,12 +43,7 @@ _partial_deprecation = (
 
 
 def _single_process():
-    """Blocks are visited one after another by one process.  Checked before anything that could be a collective, so
-    that every rank raises instead of waiting for the others."""
-    world = dist_info()[1]
-    if world > 1:
-        raise NotImplementedError("PartialMiniBatchKMeans steps through the blocks one after another in one process; "
-                                  "it does not run under torch.distributed (world size %d)" % world)
+    single_process("PartialMiniBatchKMeans")
 
 
 class _Shape(object):

@@ -44,6 +44,16 @@ def dist_info():
     return 0, 1
 
 
+def single_process(who):
+    """Raise NotImplementedError under torch.distributed with more than one rank, for the estimators that visit the
+    blocks one after another in one process.  Called before anything that could be a collective, so that every rank
+    raises instead of waiting for the others."""
+    world = dist_info()[1]
+    if world > 1:
+        raise NotImplementedError("%s steps through the blocks one after another in one process; it does not run "
+                                  "under torch.distributed (world size %d)" % (who, world))
+
+
 class Comm(object):
     """The path's only collective: sum all-reduce (plus tiny object gathers for the init)."""
 
@@ -731,6 +741,29 @@ class CudaBackend(object):
                 self._ptr(crow), self._ptr(col), self._ptr(val), _DT_CODE[val.dtype], int(n), int(d), int(col.numel()),
                 self._ptr(pack), int(l), float(gamma), self._ptr(W), k, self._ptr(out), out.stride(0) if n else k,
                 _DT_CODE[out.dtype], self.flags, self._stream()), "bkm_csr_nystrom_embed_chunk")
+
+    # -- the SGD family -----------------------------------------------------------------------
+    def sgd_block(self, x, order, y, sw, eta, cw, params, w, aw, q, st):
+        """One epoch of scikit-learn's ``_plain_sgd`` over the dense block ``x`` (n, d) for P = ``w.shape[0]`` problems:
+        ``order`` int32 (P, n), ``y`` float64 (P, n), ``sw`` float64 (n,) or None, ``eta`` float64 (n,) or None
+        ('invscaling'), ``cw`` float64 (P, 2), ``params`` an ``_lib.SgdParams``; updates w, aw, q (float64 (P, d)) and
+        st (float64 (P, 4): intercept, average intercept, non-finite flag)."""
+        n, d = x.shape
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.bkm_sgd_block(
+                self._ptr(x), int(n), int(d), x.stride(0) if n else d, _DT_CODE[x.dtype], self._ptr(order),
+                self._ptr(y), self._ptr(sw), self._ptr(eta), self._ptr(cw), int(w.shape[0]), ctypes.byref(params),
+                self._ptr(w), self._ptr(aw), self._ptr(q), self._ptr(st), self._stream()), "bkm_sgd_block")
+
+    def sgd_csr_block(self, blk, d, order, y, sw, eta, cw, params, w, aw, q, st):
+        """``sgd_block`` over one CSR block ``blk`` = (crow, col, val, n) of d columns."""
+        crow, col, val, n = blk
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.bkm_sgd_csr_block(
+                self._ptr(crow), self._ptr(col), self._ptr(val), _DT_CODE[val.dtype], int(n), int(d), int(col.numel()),
+                self._ptr(order), self._ptr(y), self._ptr(sw), self._ptr(eta), self._ptr(cw), int(w.shape[0]),
+                ctypes.byref(params), self._ptr(w), self._ptr(aw), self._ptr(q), self._ptr(st), self._stream()),
+                "bkm_sgd_csr_block")
 
     def colstats_chunk(self, x, shift, acc, minmax, first=False):
         """The scalers' statistics pass over one chunk, float64 on the device: acc (5, d) (+)= [sum (x - shift) |

@@ -66,6 +66,10 @@
  *   sklearn HashingVectorizer.transform per block of a 1-D dask array  bkm_text_tokens_chunk +
  *     of documents, feature_extraction/text.py:9-80 (tokenise, hash,     bkm_text_hash_chunk +
  *     sum duplicates, binary, normalize)                                 bkm_text_write_chunk
+ *   the SGDClassifier / SGDRegressor / Perceptron / PassiveAggressive  bkm_sgd_order (host) +
+ *     partial_fit of every block (_plain_sgd, one epoch), behind          bkm_sgd_block,
+ *     linear_model/{stochastic_gradient,perceptron,passive_aggressive}    bkm_sgd_csr_block
+ *     .py and _partial.py:39-100
  *
  * Conventions
  *   - extern "C", plain pointers and sizes only; no torch / C++ types.
@@ -102,8 +106,9 @@ extern "C" {
  * 7 = bkm_csr_assign_workspace_bytes, bkm_csr_assign_chunk, bkm_csc_label_sums_workspace_bytes,
  *     bkm_csc_label_sums_chunk, bkm_sparse_pack_workspace_bytes, bkm_sparse_pack_centers, bkm_sparse_finalize_step
  * 8 = bkm_csr_kernel_colsum_workspace_bytes, bkm_csr_kernel_colsum_chunk, bkm_csr_nystrom_embed_chunk,
- *     bkm_sparse_minibatch_step */
-#define BKM_VERSION_MINOR 8
+ *     bkm_sparse_minibatch_step
+ * 9 = bkm_sgd_order, bkm_sgd_block, bkm_sgd_csr_block */
+#define BKM_VERSION_MINOR 9
 
 /* element types of X */
 #define BKM_F32 0
@@ -802,6 +807,50 @@ int bkm_text_hash_chunk(const uint8_t* buf, int64_t n_bytes, const int64_t* tok_
                         size_t ws_bytes, void* stream);
 int bkm_text_write_chunk(const uint32_t* keys, const int64_t* pair_off, const int64_t* indptr, const double* scale,
                          int64_t n_docs, int binary, int64_t* indices, void* data, int out_dtype, void* stream);
+
+/* ---- one epoch of scikit-learn's _plain_sgd over one block, for P independent binary problems --------------------
+ *   bkm_sgd_order      HOST function, no CUDA: out_host[0..n) = the row order of SequentialDataset.shuffle(seed) (the
+ *                      Fisher-Yates shuffle driven by our_rand_r, sklearn/utils/_random.pxd), n <= 2^31 - 1.
+ *   bkm_sgd_block      rows of a dense block X (n, d), any row pitch ldx, float32 or float64.
+ *   bkm_sgd_csr_block  rows of a CSR block (crow int64 (n + 1), col int64 (nnz), val float32 / float64 (nnz)) of d
+ *                      columns; each row's entries are visited in stored order, as CSRDataset does.
+ * Problem p (0 <= p < P) visits the rows order[p*n + 0 .. n) (int32) with the labels y[p*n + row] (float64, in the
+ * block's row order) and sample_weight[row] (float64, NULL = 1) and updates, in float64:
+ *   w    (P, d)  the weights (WeightVector.w with wscale = 1 on entry and exit)
+ *   aw   (P, d)  the average weights, NULL without `average`
+ *   q    (P, d)  scratch of the L1 / elasticnet penalty (zeroed by the call), NULL otherwise
+ *   st   (P, 4)  [intercept | average intercept | non-finite flag | unused]: the flag is set to 1 when an intercept or
+ *                weight is not finite after the epoch (scikit-learn's under/overflow ValueError); w is then left
+ *                unscaled, as scikit-learn raises before reset_wscale.
+ *   cw   (P, 2)  [weight_pos | weight_neg] per problem.
+ * `eta` (n, float64) is the per-step learning rate of 'invscaling' (eta0 / pow(t, power_t), computed on the host),
+ * NULL otherwise.  Every product and sum is rounded on its own, in the order of _plain_sgd and WeightVector, except the
+ * fold of w into aw in reset_wscale, which is fused as the x86-64 BLAS daxpy fuses it; so everything but the exp of
+ * log_loss matches scikit-learn's float64 path bit for bit.  One launch; a CTA per
+ * problem.  w, aw and q stay in shared memory for the epoch when 8 d (1 + [aw] + [q]) bytes fit, in global memory
+ * otherwise. */
+#define BKM_SGD_HINGE 0                 /* threshold = epsilon (1 for hinge, 0 for perceptron) */
+#define BKM_SGD_LOG 1
+#define BKM_SGD_MODIFIED_HUBER 2
+#define BKM_SGD_SQUARED_HINGE 3         /* threshold = epsilon */
+#define BKM_SGD_SQUARED_ERROR 4
+#define BKM_SGD_HUBER 5
+#define BKM_SGD_EPS_INSENSITIVE 6
+#define BKM_SGD_SQ_EPS_INSENSITIVE 7
+typedef struct {
+  int loss, penalty, learning_rate, fit_intercept;   /* penalty 0 none, 1 l1, 2 l2, 3 elasticnet; learning_rate as
+                                                        _sgd_fast: 1 constant, 2 optimal, 3 invscaling, 4 adaptive,
+                                                        5 pa1, 6 pa2 */
+  double epsilon, alpha, l1_ratio, eta0, optimal_init, t0, intercept_decay, average;
+} bkm_sgd_params;
+int bkm_sgd_order(int64_t n, uint32_t seed, int32_t* out_host);
+int bkm_sgd_block(const void* X, int64_t n, int d, int64_t ldx, int x_dtype, const int32_t* order, const double* y,
+                  const double* sample_weight, const double* eta, const double* cw, int P,
+                  const bkm_sgd_params* params_host, double* w, double* aw, double* q, double* st, void* stream);
+int bkm_sgd_csr_block(const int64_t* crow, const int64_t* col, const void* val, int val_dtype, int64_t n, int d,
+                      int64_t nnz, const int32_t* order, const double* y, const double* sample_weight,
+                      const double* eta, const double* cw, int P, const bkm_sgd_params* params_host, double* w,
+                      double* aw, double* q, double* st, void* stream);
 
 /* ---- NaN/inf scan of a chunk (k_means.py:179-180): sets *flag (int32) nonzero -------- */
 int bkm_check_finite(const void* X, int64_t n, int d, int64_t ldx, int x_dtype,
