@@ -28,6 +28,10 @@ ENCODE_CSR = 2
 ENCODE_KEEP = 8
 TEXT_NORM = {None: 0, "l1": 1, "l2": 2}
 
+NB_JLL = 0
+NB_LOG_PROBA = 1
+NB_PROBA = 2
+
 FLAG_FORCE_SIMT = 1
 FLAG_FORCE_TC = 2
 FLAG_NO_RECHECK = 4
@@ -94,6 +98,15 @@ SIGNATURES = {
                                        _c_void_p, _c_void_p, ctypes.c_size_t, _int, _c_void_p]),
     "bkm_nb_jll_chunk": (_int, [_c_void_p, _i64, _int, _i64, _int, _c_void_p, _c_void_p, _c_void_p, _int, _c_void_p,
                                 _c_void_p, _i64, _int, _c_void_p, _int, _c_void_p]),
+    "bkm_class_counts_chunk": (_int, [_c_void_p, _i64, _int, _i64, _int, _c_void_p, _int, _c_void_p, _int, _dbl,
+                                      _c_void_p, _c_void_p, _c_void_p, ctypes.c_size_t, _int, _c_void_p]),
+    "bkm_csc_class_counts_chunk": (_int, [_c_void_p, _c_void_p, _c_void_p, _int, _int, _i64, _c_void_p, _c_void_p, _int,
+                                          _c_void_p, _int, _dbl, _c_void_p, _c_void_p, ctypes.c_size_t, _int,
+                                          _c_void_p]),
+    "bkm_nb_linear_jll_chunk": (_int, [_c_void_p, _i64, _int, _i64, _int, _int, _dbl, _c_void_p, _c_void_p, _int,
+                                       _c_void_p, _c_void_p, _i64, _int, _int, _c_void_p]),
+    "bkm_nb_csr_jll_chunk": (_int, [_c_void_p, _c_void_p, _c_void_p, _int, _i64, _int, _i64, _int, _dbl, _c_void_p,
+                                    _c_void_p, _int, _c_void_p, _c_void_p, _i64, _int, _int, _c_void_p]),
     "bkm_glm_workspace_bytes": (_int, [_i64, _int, _szp]),
     "bkm_glm_pass_chunk": (_int, [_c_void_p, _i64, _int, _i64, _int, _c_void_p, _c_void_p, _int, _int, _c_void_p,
                                   _c_void_p, _c_void_p, _c_void_p, _c_void_p, ctypes.c_size_t, _int, _c_void_p]),

@@ -198,3 +198,20 @@ def as_chunked(x):
         blocks = [np.asarray(b.compute()) for b in x.to_delayed().flatten().tolist()]
         return ChunkedArray(blocks)
     raise TypeError("not a chunked array: %r" % type(x))
+
+
+def _y_flat(y, who="GaussianNB.fit"):
+    """y (numpy, torch on any device, ChunkedArray or dask array, any chunking) -> one flat numpy array or tensor."""
+    if y is None:
+        raise ValueError("%s needs the labels y; got None" % who)
+    if isinstance(y, ChunkedArray):
+        blocks = y.blocks
+    elif is_dask_array(y):
+        blocks = as_chunked(y).blocks
+    else:
+        blocks = [y]
+    if all(_is_torch(b) for b in blocks):
+        flat = [b.detach().reshape(-1) for b in blocks]
+        return flat[0] if len(flat) == 1 else torch.cat([f.to(flat[0].device) for f in flat])
+    flat = [np.asarray(block_to_numpy(b) if _is_torch(b) else b).reshape(-1) for b in blocks]
+    return flat[0] if len(flat) == 1 else np.concatenate(flat)

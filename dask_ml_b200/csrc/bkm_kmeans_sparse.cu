@@ -14,6 +14,10 @@
 //                             the second Nystrom pass (the EMBED epilogue of the assign kernel)
 //   bkm_sparse_minibatch_step bkm_minibatch_step on the transposed layout: scikit-learn's _minibatch_update_sparse on the
 //                             reduced [p k sumsT | k counts | inertia], the weight sums, and the next sparse pack
+//   bkm_csc_class_counts_chunk  FC^T (p x K) (+)= X^T (w * onehot(labels)) with the entries optionally binarised (x > t):
+//                             the class counts of PartialMultinomialNB / PartialBernoulliNB (the label sums' kernel)
+//   bkm_nb_csr_jll_chunk      jll_ic = b_c + sum_j f(x_ij) W^T[j][c] and the arg-max / log-softmax epilogues of the
+//                             discrete naive Bayes models (the row body of bkm_csr_panel_chunk)
 //
 // Every value is widened to float64 from the block's dtype; every sum runs in a fixed order and no float atomics are
 // used, so two calls with the same inputs give the same bits.
@@ -35,9 +39,15 @@
 //                 tile), then per tile the kernel values go through a per-warp row of shared memory and the lanes own
 //                 the outputs o = lane + 32 t, each adding the tile's keep rows in order by fma.  NaN where
 //                 gamma m_i > 745.13, the rule of bkm_nystrom_embed_chunk.
+//   nb jll        one warp per row; its lanes walk the classes in tiles of 32 C and gather the W^T rows of the row's
+//                 entries (csr_row_gather, stored entries only).  Each lane keeps the first maximum / first NaN and a
+//                 running logsumexp of its classes; the warp folds them in a fixed butterfly order.  Raw jll goes out per
+//                 tile; normalised outputs are written from registers when K fits one tile, else rewritten by the
+//                 lanes that wrote them.
 //   pack / step   column_reduce (bkm_select.cuh) over the p rows of CT: each element of C' (from the centres or from the
 //                 reduced sums) is written to CT, and per cluster the CTA-ordered sums of (C - C')^2 and of C'^2 give the
 //                 shift terms and cn.  The step adds the k shift terms in cluster order.  One kernel writes every pack.
+#include <climits>
 #include <math_constants.h>
 #include "bkm_select.cuh"
 #include "bkm_csc_plan.cuh"
@@ -319,9 +329,13 @@ struct LabelSumArgs {
   unsigned* ticket;    // [p], zero
   int first;
   const int* skip;
+  const double* w;     // WB: the row weights [n], nullable
+  double thr;          // WB with bin: entries count as val > thr
+  int bin;
 };
 
-template <typename T>
+// WB (bkm_csc_class_counts_chunk): entry (row, v) adds f(v) w[row] in place of v
+template <typename T, bool WB = false>
 __global__ void __launch_bounds__(kThreads) csc_label_sums_kernel(LabelSumArgs a) {
   extern __shared__ double s_acc[];        // [warps][k]
   if (a.skip && *a.skip) return;
@@ -340,8 +354,16 @@ __global__ void __launch_bounds__(kThreads) csc_label_sums_kernel(LabelSumArgs a
       int lab = -1;
       double v = 0.0;
       if (eb + lane < sp.e1) {
-        lab = a.labels[a.rows[eb + lane]];
-        v = to_f64(vals[eb + lane]);
+        if (WB) {
+          const int r = a.rows[eb + lane];
+          lab = a.labels[r];
+          v = to_f64(vals[eb + lane]);
+          if (a.bin) v = v > a.thr ? 1.0 : 0.0;
+          if (a.w) v *= __ldg(a.w + r);
+        } else {
+          lab = a.labels[a.rows[eb + lane]];
+          v = to_f64(vals[eb + lane]);
+        }
       }
       const int m = (int)min(32LL, sp.e1 - eb);
 #pragma unroll 4
@@ -368,6 +390,137 @@ __global__ void __launch_bounds__(kThreads) csc_label_sums_kernel(LabelSumArgs a
 static int label_sums_warps(int k) {
   const long long w = (200LL * 1024) / ((long long)k * 8);
   return w > kWarps ? kWarps : (int)w;
+}
+
+template <typename T, bool WB>
+static int launch_label_sums(const LabelSumArgs& a, long long nnz, cudaStream_t s) {
+  const int warps = label_sums_warps(a.k);
+  const size_t smem = (size_t)warps * a.k * 8;
+  if (smem > 48 * 1024)
+    BKM_CUDA_TRY(cudaFuncSetAttribute(csc_label_sums_kernel<T, WB>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                      (int)smem));
+  const int grid = grid_for(seg_cap(a.p, nnz), warps, 16LL * sm_count_or_default());
+  csc_label_sums_kernel<T, WB><<<grid, warps * 32, smem, s>>>(a);
+  BKM_CUDA_TRY(cudaGetLastError());
+  note_launch();
+  return 0;
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// naive Bayes log-likelihood
+// ---------------------------------------------------------------------------------------------------------------------
+struct NbJllArgs {
+  const long long* crow;
+  const long long* col;
+  const void* val;
+  long long n;
+  int p;
+  const double* WT;    // [p][K]
+  const double* b;     // [K]
+  int K;
+  int bin;
+  double thr;
+  int32_t* labels;     // nullable
+  double* out;         // [n][ldo], nullable
+  long long ldo;
+  int out_mode;
+};
+
+template <typename T, int C, bool BIN>
+__global__ void __launch_bounds__(kThreads) csr_nb_jll_kernel(NbJllArgs a) {
+  constexpr int CW = 32 * C;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int K = a.K;
+  const bool one = K <= CW;
+  const bool norm = a.out && a.out_mode != BKM_NB_JLL;
+  const T* val = reinterpret_cast<const T*>(a.val);
+  const long long nw = (long long)gridDim.x * kWarps;
+#pragma unroll 1
+  for (long long i = (long long)blockIdx.x * kWarps + warp; i < a.n; i += nw) {
+    double best = -INFINITY, m = -INFINITY, ssum = 0.0;
+    int bi = INT_MAX, nani = INT_MAX;
+    double acc[C];
+    bool own[C];
+#pragma unroll 1
+    for (int c0 = 0; c0 < K; c0 += CW) {
+#pragma unroll
+      for (int j = 0; j < C; ++j) {
+        own[j] = c0 + lane + 32 * j < K;
+        acc[j] = 0.0;
+      }
+      double xn = 0.0;
+      csr_row_gather<T, C, false, BIN>(a.crow, a.col, val, i, a.p, a.WT, K, c0, own, acc, xn, a.thr);
+#pragma unroll
+      for (int j = 0; j < C; ++j) {
+        if (!own[j]) continue;
+        const int cc = c0 + lane + 32 * j;
+        const double v = acc[j] + __ldg(a.b + cc);
+        acc[j] = v;
+        if (isnan(v)) {
+          if (nani == INT_MAX) nani = cc;
+        } else {
+          if (bi == INT_MAX || v > best) { best = v; bi = cc; }
+          if (v > m) {
+            ssum = ssum * exp(m - v) + 1.0;
+            m = v;
+          } else if (v != -INFINITY) {
+            ssum += exp(v - m);
+          }
+        }
+        if (a.out && (!norm || !one)) a.out[i * a.ldo + cc] = v;
+      }
+    }
+    // ---- the warp's fold: first NaN, else the first maximum; the logsumexp terms by a fixed butterfly ----
+    nani = __reduce_min_sync(0xffffffffu, nani);
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1) {
+      const double ob = __shfl_xor_sync(0xffffffffu, best, off);
+      const int obi = __shfl_xor_sync(0xffffffffu, bi, off);
+      if (obi != INT_MAX && (bi == INT_MAX || ob > best || (ob == best && obi < bi))) { best = ob; bi = obi; }
+      const double om = __shfl_xor_sync(0xffffffffu, m, off);
+      const double os = __shfl_xor_sync(0xffffffffu, ssum, off);
+      const double M = fmax(m, om);
+      // rounded products: the two lanes of a pair get the same bits
+      if (M != -INFINITY)
+        ssum = __dadd_rn(m == -INFINITY ? 0.0 : __dmul_rn(ssum, exp(m - M)), om == -INFINITY ? 0.0 : __dmul_rn(os, exp(om - M)));
+      m = M;
+    }
+    if (a.labels && lane == 0) a.labels[i] = nani != INT_MAX ? nani : (bi == INT_MAX ? 0 : bi);
+    if (!norm) continue;
+    const double lse = (nani != INT_MAX || !(fabs(m) < INFINITY)) ? (double)NAN : log(ssum) + m;
+    const bool ex = a.out_mode == BKM_NB_PROBA;
+    if (one) {
+#pragma unroll
+      for (int j = 0; j < C; ++j) {
+        if (!own[j]) continue;
+        double o = acc[j] - lse;
+        if (ex) o = exp(o);
+        a.out[i * a.ldo + lane + 32 * j] = o;
+      }
+    } else {
+      for (int cc = lane; cc < K; cc += 32) {          // the lane that wrote each raw value rewrites it
+        double* q = a.out + i * a.ldo + cc;
+        double o = *q - lse;
+        if (ex) o = exp(o);
+        *q = o;
+      }
+    }
+  }
+}
+
+template <typename T, int C, bool BIN>
+static int launch_nb_jll(const NbJllArgs& a, int sms, cudaStream_t s) {
+  csr_nb_jll_kernel<T, C, BIN><<<assign_grid(a.n, sms), kThreads, 0, s>>>(a);
+  BKM_CUDA_TRY(cudaGetLastError());
+  note_launch();
+  return 0;
+}
+
+template <typename T, bool BIN>
+static int nb_jll(const NbJllArgs& a, int sms, cudaStream_t s) {
+  if (a.K <= 32) return launch_nb_jll<T, 1, BIN>(a, sms, s);
+  if (a.K <= 64) return launch_nb_jll<T, 2, BIN>(a, sms, s);
+  return launch_nb_jll<T, 4, BIN>(a, sms, s);
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -619,23 +772,57 @@ extern "C" int bkm_csc_label_sums_chunk(const int64_t* colptr, const int32_t* ro
   a.ticket = reinterpret_cast<unsigned*>(ws + seg_slots_bytes(nnz, k));
   a.first = (flags & BKM_FLAG_FIRST_CHUNK) ? 1 : 0;
   a.skip = loop_state ? &reinterpret_cast<const LoopState*>(loop_state)->done : nullptr;
+  a.w = nullptr; a.thr = 0.0; a.bin = 0;
   BKM_CUDA_TRY(cudaMemsetAsync(a.ticket, 0, (size_t)p * 4, s));
-  const size_t smem = (size_t)warps * k * 8;
-  if (val_dtype == BKM_F32) {
-    if (smem > 48 * 1024)
-      BKM_CUDA_TRY(cudaFuncSetAttribute(csc_label_sums_kernel<float>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                        (int)smem));
-  } else if (smem > 48 * 1024) {
-    BKM_CUDA_TRY(cudaFuncSetAttribute(csc_label_sums_kernel<double>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                      (int)smem));
-  }
+  if (val_dtype == BKM_F32) return launch_label_sums<float, false>(a, nnz, s);
+  return launch_label_sums<double, false>(a, nnz, s);
+}
+
+extern "C" int bkm_csc_class_counts_chunk(const int64_t* colptr, const int32_t* rows, const void* vals, int val_dtype,
+                                          int p, int64_t nnz, const int64_t* plan, const int32_t* labels, int k,
+                                          const double* w, int binarize, double threshold, double* fcT,
+                                          void* workspace, size_t ws_bytes, int flags, void* stream) {
+  if (p <= 0 || nnz < 0 || k <= 0 || !colptr || !plan || !fcT || !workspace) return BKM_EINVAL;
+  if (nnz > 0 && (!rows || !vals || !labels)) return BKM_EINVAL;
+  if (val_dtype != BKM_F32 && val_dtype != BKM_F64) return BKM_EDTYPE;
+  if (label_sums_warps(k) < 1) return BKM_EINVAL;
+  if (ws_bytes < seg_fold_ws(p, nnz, k)) return BKM_EWORKSPACE;
+  cudaStream_t s = (cudaStream_t)stream;
+  unsigned char* ws = reinterpret_cast<unsigned char*>(workspace);
+  LabelSumArgs a;
+  a.colptr = reinterpret_cast<const long long*>(colptr);
+  a.rows = rows; a.vals = vals; a.p = p; a.plan = reinterpret_cast<const long long*>(plan);
+  a.labels = labels; a.k = k; a.out = fcT;
+  a.slot = reinterpret_cast<double*>(ws);
+  a.ticket = reinterpret_cast<unsigned*>(ws + seg_slots_bytes(nnz, k));
+  a.first = (flags & BKM_FLAG_FIRST_CHUNK) ? 1 : 0;
+  a.skip = nullptr;
+  a.w = w; a.thr = threshold; a.bin = binarize ? 1 : 0;
+  BKM_CUDA_TRY(cudaMemsetAsync(a.ticket, 0, (size_t)p * 4, s));
+  if (val_dtype == BKM_F32) return launch_label_sums<float, true>(a, nnz, s);
+  return launch_label_sums<double, true>(a, nnz, s);
+}
+
+extern "C" int bkm_nb_csr_jll_chunk(const int64_t* crow, const int64_t* col, const void* val, int val_dtype, int64_t n,
+                                    int p, int64_t nnz, int binarize, double threshold, const double* WT,
+                                    const double* b, int K, int32_t* labels, double* out, int64_t ldo, int out_mode,
+                                    int flags, void* stream) {
+  (void)flags;
+  if (n < 0 || p <= 0 || nnz < 0 || K <= 0 || !crow || !WT || !b) return BKM_EINVAL;
+  if (nnz > 0 && (!col || !val)) return BKM_EINVAL;
+  if (val_dtype != BKM_F32 && val_dtype != BKM_F64) return BKM_EDTYPE;
+  if (out_mode != BKM_NB_JLL && out_mode != BKM_NB_LOG_PROBA && out_mode != BKM_NB_PROBA) return BKM_EINVAL;
+  if (out && ldo < K) return BKM_EINVAL;
+  if (n == 0 || (!labels && !out)) return 0;
+  NbJllArgs a;
+  a.crow = reinterpret_cast<const long long*>(crow);
+  a.col = reinterpret_cast<const long long*>(col);
+  a.val = val; a.n = n; a.p = p; a.WT = WT; a.b = b; a.K = K; a.bin = binarize ? 1 : 0; a.thr = threshold;
+  a.labels = labels; a.out = out; a.ldo = ldo; a.out_mode = out_mode;
   const int sms = sm_count_or_default();
-  const int grid = grid_for(seg_cap(p, nnz), warps, 16LL * sms);
-  if (val_dtype == BKM_F32) csc_label_sums_kernel<float><<<grid, warps * 32, smem, s>>>(a);
-  else csc_label_sums_kernel<double><<<grid, warps * 32, smem, s>>>(a);
-  BKM_CUDA_TRY(cudaGetLastError());
-  note_launch();
-  return 0;
+  cudaStream_t s = (cudaStream_t)stream;
+  if (val_dtype == BKM_F32) return a.bin ? nb_jll<float, true>(a, sms, s) : nb_jll<float, false>(a, sms, s);
+  return a.bin ? nb_jll<double, true>(a, sms, s) : nb_jll<double, false>(a, sms, s);
 }
 
 extern "C" int bkm_sparse_pack_workspace_bytes(int k, int p, size_t* out) {

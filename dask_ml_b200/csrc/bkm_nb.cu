@@ -5,6 +5,13 @@
 //   bkm_nb_jll_chunk         jll_ic = logc_c - 1/2 sum_j (x_ij - theta_cj)^2 w_cj, then per row either the arg-max
 //                            (labels) or jll - logsumexp(jll) (float64 log-probabilities, optionally exponentiated)
 //
+// and the dense passes of PartialMultinomialNB / PartialBernoulliNB:
+//
+//   bkm_class_counts_chunk   FC[c][j] (+)= sum_{i: y_i = c} w_i f(x_ij),  CC[c] (+)= sum_{i: y_i = c} w_i  (w_i = 1 without
+//                            weights; f the identity, or x > t when binarising): the moments kernel's mode 0
+//   bkm_nb_linear_jll_chunk  jll_ic = b_c + sum_j f(x_ij) W_cj in float64 on the fp64 tensor cores, then per row the
+//                            arg-max (labels) and / or jll, jll - logsumexp(jll) or its exp (float64, any row pitch)
+//
 // Moments.  A CTA owns one row split and one (class slice x feature slice) of the accumulators.  Its threads are
 // `groups` row groups of `fs` feature lanes; every group has its own float64 accumulator copy in shared memory, so the
 // lane of feature j in group g is the only writer of acc[g][c][j]: no atomics, and the order of its additions is the
@@ -22,7 +29,17 @@
 // depend on the blocking.  The sum is taken in direct form, fma((x - theta) w, x - theta, acc), never expanded.
 // fp32 rows whose best class is not ahead of every other class by more than the error bound E (DESIGN.md, A21) are
 // re-decided in float64 by the same thread, with the float64 path's exact arithmetic.
+//
+// Linear log-likelihood.  One CTA owns a 64-row tile and all K classes; it walks the classes in blocks of 16, 32 or 64
+// columns (chosen from K as bkm_project_chunk chooses them, so a small K pads no columns).  For each block the rows
+// and W are staged 32 features at a time, widened to float64 (f(x) applied) in shared memory, and multiplied with
+// DMMA.16x8x16 as in bkm_project_chunk: the products of fp32 and bf16 rows are exact, and 0 (-inf) stays NaN as in
+// numpy's BLAS product.  After each block, b is added and thread r folds row r's block into its running arg-max (the
+// first maximum, the first NaN, as np.argmax) and running logsumexp, in class order.  The raw block goes out at once;
+// normalised outputs are rewritten by the CTA after the tile's last block (directly from shared memory when K fits one
+// block).
 #include "bkm_common.cuh"
+#include "bkm_ptx.cuh"
 #include <cuda_bf16.h>
 
 namespace bkm {
@@ -86,9 +103,13 @@ struct MomArgs {
   double* cpart;
   int fs, groups, ks, nk;
   long long rows_per_split;
+  const double* w;          // COUNTS: the row weights [n], nullable
+  double thr;               // COUNTS with bin: f(x) = x > thr
+  int bin;
 };
 
-template <typename T>
+// COUNTS (bkm_class_counts_chunk): mode 0 with f(x) w_i in place of x and w_i in place of 1
+template <typename T, bool COUNTS = false>
 __global__ void __launch_bounds__(MT) moments_kernel(MomArgs a) {
   extern __shared__ __align__(16) unsigned char smem[];
   __shared__ int wcount[MT / 32];
@@ -140,6 +161,13 @@ __global__ void __launch_bounds__(MT) moments_kernel(MomArgs a) {
         const int2 e = mem[m];
         const double x = to_f64(X[(r0 + e.x) * a.ldx + f0 + f]);
         double v = x;
+        if (COUNTS) {
+          if (a.bin) v = x > a.thr ? 1.0 : 0.0;
+          const double wi = a.w ? __ldg(a.w + r0 + e.x) : 1.0;
+          A[e.y * FS] += v * wi;
+          if (counter && f == 0) C[e.y] += wi;
+          continue;
+        }
         if (a.mode != 0) {
           const double t = x - __ldg(a.theta + (size_t)(k0 + e.y) * a.d + f0 + f);
           v = t * t;
@@ -474,10 +502,11 @@ __global__ void __launch_bounds__(JT, 4) jll_kernel(JllArgs a, JllSmem L) {
   }
 }
 
-template <typename T>
+template <typename T, bool COUNTS = false>
 static int launch_moments(const MomArgs& a, const MomGeom& G, cudaStream_t s) {
-  BKM_CUDA_TRY(cudaFuncSetAttribute(moments_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)G.smem));
-  moments_kernel<T><<<dim3(G.splits, G.nk * G.nf), MT, G.smem, s>>>(a);
+  BKM_CUDA_TRY(cudaFuncSetAttribute(moments_kernel<T, COUNTS>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                    (int)G.smem));
+  moments_kernel<T, COUNTS><<<dim3(G.splits, G.nk * G.nf), MT, G.smem, s>>>(a);
   BKM_CUDA_TRY(cudaGetLastError());
   note_launch();
   return 0;
@@ -530,6 +559,224 @@ static int launch_jll_f64(const JllArgs& a, int sms, cudaStream_t s) {
   return launch_jll_fc<double, double, JC, true>(a, sms, s);
 }
 
+// ------------------------------------------------------------------------------------- linear log-likelihood
+constexpr int LT = 256;                       // threads
+constexpr int LR = 64;                        // rows per tile
+constexpr int LF = 32;                        // features per staged step
+constexpr int LP = LF + 4;                    // float64 operand pitch (as bkm_project_chunk's)
+
+struct LinArgs {
+  const void* X;
+  long long n;
+  int d;
+  long long ldx;
+  int bin;
+  double thr;
+  const double* W;          // [K][d]
+  const double* b;          // [K]
+  int K;
+  int32_t* labels;          // nullable
+  double* out;              // nullable
+  long long ldo;
+  int out_mode;             // BKM_NB_JLL, BKM_NB_LOG_PROBA, BKM_NB_PROBA
+};
+
+template <int NT>
+static size_t lin_smem() {
+  constexpr int CW = 2 * NT * 8;
+  return (size_t)(LR + CW) * LP * 8 + (size_t)LR * (CW + 1) * 8 + (size_t)LR * 8;
+}
+
+template <typename T, int NT>
+__global__ void __launch_bounds__(LT) linear_jll_kernel(LinArgs a) {
+  using namespace ptx;
+  constexpr int CW = 2 * NT * 8;                // classes per block
+  extern __shared__ __align__(16) unsigned char smem[];
+  double* Xs = reinterpret_cast<double*>(smem);           // [LR][LP]
+  double* Ws = Xs + LR * LP;                              // [CW][LP]
+  double* ob = Ws + CW * LP;                              // [LR][CW + 1]
+  double* lse_s = ob + LR * (CW + 1);                     // [LR]
+
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int g = lane >> 2, tq = lane & 3;
+  const int mb = warp & 3, nh = warp >> 2;
+  const int d = a.d, K = a.K;
+  const int nblk = (K + CW - 1) / CW;
+  const T* X = reinterpret_cast<const T*>(a.X);
+  const long long ntiles = (a.n + LR - 1) / LR;
+  const bool want_lab = a.labels != nullptr, want_out = a.out != nullptr;
+  const bool norm = want_out && a.out_mode != BKM_NB_JLL;
+
+#pragma unroll 1
+  for (long long tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+    const long long r0 = tile * LR;
+    const int rows = (int)min((long long)LR, a.n - r0);
+    // row tid's running arg-max and logsumexp (threads tid < rows)
+    double best = -INFINITY, m = -INFINITY, ssum = 0.0;
+    int bi = 0, nani = -1;
+    bool anynan = false;
+
+#pragma unroll 1
+    for (int blk = 0; blk < nblk; ++blk) {
+      const int c0 = blk * CW, kw = min(CW, K - c0);
+      double acc[NT][4];
+#pragma unroll
+      for (int nt = 0; nt < NT; ++nt)
+#pragma unroll
+        for (int q = 0; q < 4; ++q) acc[nt][q] = 0.0;
+#pragma unroll 1
+      for (int f0 = 0; f0 < d; f0 += LF) {
+        __syncthreads();                        // the previous step's MMAs (and block's epilogue) are done
+        const int f = tid & (LF - 1);
+        const bool fin = f0 + f < d;
+#pragma unroll 4
+        for (int e = tid; e < LR * LF; e += LT) {
+          const int r = e >> 5;
+          double v = 0.0;
+          if (r < rows && fin) {
+            v = to_f64(X[(r0 + r) * a.ldx + f0 + f]);
+            if (a.bin) v = v > a.thr ? 1.0 : 0.0;
+          }
+          Xs[r * LP + f] = v;
+        }
+        for (int e = tid; e < CW * LF; e += LT) {
+          const int c = e >> 5;
+          Ws[c * LP + f] = (c < kw && fin) ? a.W[(size_t)(c0 + c) * d + f0 + f] : 0.0;
+        }
+        __syncthreads();
+#pragma unroll
+        for (int ks = 0; ks < LF / 16; ++ks) {
+          const int k0 = ks * 16;
+          double af[8];
+#pragma unroll
+          for (int i = 0; i < 8; ++i) af[i] = Xs[(mb * 16 + g + 8 * (i & 1)) * LP + k0 + tq + 4 * (i >> 1)];
+#pragma unroll
+          for (int nt = 0; nt < NT; ++nt) {
+            double bf[4];
+#pragma unroll
+            for (int i = 0; i < 4; ++i) bf[i] = Ws[(nh * NT * 8 + nt * 8 + g) * LP + k0 + tq + 4 * i];
+            dmma16816(acc[nt], af, bf);
+          }
+        }
+      }
+      // ---- the block's jll into shared memory, then row tid's fold in class order ----
+#pragma unroll
+      for (int nt = 0; nt < NT; ++nt)
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+          const int r = mb * 16 + g + 8 * (q >> 1), c = nh * NT * 8 + nt * 8 + 2 * tq + (q & 1);
+          if (c < kw) ob[r * (CW + 1) + c] = acc[nt][q] + __ldg(a.b + c0 + c);
+        }
+      __syncthreads();
+      if (tid < rows && (want_lab || norm)) {
+#pragma unroll 1
+        for (int c = 0; c < kw; ++c) {
+          const double v = ob[tid * (CW + 1) + c];
+          if (isnan(v)) {
+            if (nani < 0) nani = c0 + c;
+            anynan = true;
+          } else {
+            if (v > best) { best = v; bi = c0 + c; }
+            if (norm) {
+              if (v > m) {
+                ssum = ssum * exp(m - v) + 1.0;
+                m = v;
+              } else if (v != -INFINITY) {
+                ssum += exp(v - m);
+              }
+            }
+          }
+        }
+      }
+      if (want_out && (!norm || nblk > 1)) {    // the raw block goes out now
+        for (int e = tid; e < rows * kw; e += LT) {
+          const int r = e / kw, c = e - r * kw;
+          a.out[(r0 + r) * a.ldo + c0 + c] = ob[r * (CW + 1) + c];
+        }
+      }
+    }
+
+    if (want_lab && tid < rows) a.labels[r0 + tid] = nani >= 0 ? nani : bi;
+    if (norm) {
+      // jll - (log sum exp(jll - max) + max), NaN throughout for a row with a NaN or without a finite maximum
+      if (tid < LR) lse_s[tid] = (anynan || !(fabs(m) < INFINITY)) ? (double)NAN : log(ssum) + m;
+      __syncthreads();
+      const bool ex = a.out_mode == BKM_NB_PROBA;
+      for (int e = tid; e < rows * K; e += LT) {
+        const int r = e / K, c = e - r * K;
+        double* p = a.out + (r0 + r) * a.ldo + c;
+        double o = (nblk == 1 ? ob[r * (CW + 1) + c] : *p) - lse_s[r];
+        if (ex) o = exp(o);
+        *p = o;
+      }
+    }
+  }
+}
+
+template <typename T, int NT>
+static int launch_linear_nt(const LinArgs& a, int sms, cudaStream_t s) {
+  const size_t sm = lin_smem<NT>();
+  auto kern = linear_jll_kernel<T, NT>;
+  BKM_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
+  int per_sm = 0;
+  BKM_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, LT, sm));
+  if (per_sm < 1) per_sm = 1;
+  const long long ntiles = (a.n + LR - 1) / LR;
+  long long gx = (long long)per_sm * sms;
+  if (gx > ntiles) gx = ntiles;
+  kern<<<(unsigned)gx, LT, sm, s>>>(a);
+  BKM_CUDA_TRY(cudaGetLastError());
+  note_launch();
+  return 0;
+}
+
+template <typename T>
+static int launch_linear(const LinArgs& a, int sms, cudaStream_t s) {
+  if (a.K <= 16) return launch_linear_nt<T, 1>(a, sms, s);
+  if (a.K <= 32) return launch_linear_nt<T, 2>(a, sms, s);
+  return launch_linear_nt<T, 4>(a, sms, s);
+}
+
+static int moments_run(const void* X, int64_t n, int d, int64_t ldx, int x_dtype, const int32_t* cls, int K, int mode,
+                       const double* theta, bool counts_pass, const double* w, int bin, double thr, double* sums,
+                       double* counts, void* workspace, size_t ws_bytes, int flags, void* stream) {
+  int sms = 0;
+  const int rc = sm_count(&sms);
+  if (rc) return rc;
+  const MomGeom G = mom_geom(n, d, K, sms);
+  if (ws_bytes < G.total) return BKM_EWORKSPACE;
+  cudaStream_t s = (cudaStream_t)stream;
+  unsigned char* ws = reinterpret_cast<unsigned char*>(workspace);
+  MomArgs a;
+  a.X = X; a.n = n; a.d = d; a.ldx = ldx; a.cls = cls; a.K = K; a.mode = mode; a.theta = theta;
+  a.part = reinterpret_cast<double*>(ws + G.off_part);
+  a.cpart = reinterpret_cast<double*>(ws + G.off_cpart);
+  a.fs = G.fs; a.groups = G.groups; a.ks = G.ks; a.nk = G.nk; a.rows_per_split = G.rows_per_split;
+  a.w = w; a.thr = thr; a.bin = bin ? 1 : 0;
+  if (G.splits > 0) {
+    int r = 0;
+    if (counts_pass) {
+      if (x_dtype == BKM_F32) r = launch_moments<float, true>(a, G, s);
+      else if (x_dtype == BKM_F64) r = launch_moments<double, true>(a, G, s);
+      else r = launch_moments<__nv_bfloat16, true>(a, G, s);
+    } else {
+      if (x_dtype == BKM_F32) r = launch_moments<float>(a, G, s);
+      else if (x_dtype == BKM_F64) r = launch_moments<double>(a, G, s);
+      else r = launch_moments<__nv_bfloat16>(a, G, s);
+    }
+    if (r) return r;
+  }
+  const long long total = (long long)K * d + (mode == 0 ? K : 0);
+  long long blocks = (total + 255) / 256;
+  if (blocks > 4LL * sms) blocks = 4LL * sms;
+  moments_fold_kernel<<<(unsigned)blocks, 256, 0, s>>>(a.part, a.cpart, G.splits, K, d, mode, sums,
+                                                       mode == 0 ? counts : nullptr,
+                                                       (flags & BKM_FLAG_FIRST_CHUNK) ? 1 : 0);
+  BKM_CUDA_TRY(cudaGetLastError());
+  note_launch();
+  return 0;
+}
+
 }  // namespace
 }  // namespace bkm
 
@@ -548,34 +795,18 @@ extern "C" int bkm_class_moments_chunk(const void* X, int64_t n, int d, int64_t 
   if (n > 0 && (!X || !cls)) return BKM_EINVAL;
   if (mode == 0 ? !counts : (mode != 1 || !theta)) return BKM_EINVAL;
   if (!dtype_ok(x_dtype)) return BKM_EDTYPE;
-  int sms = 0;
-  const int rc = sm_count(&sms);
-  if (rc) return rc;
-  const MomGeom G = mom_geom(n, d, K, sms);
-  if (ws_bytes < G.total) return BKM_EWORKSPACE;
-  cudaStream_t s = (cudaStream_t)stream;
-  unsigned char* ws = reinterpret_cast<unsigned char*>(workspace);
-  MomArgs a;
-  a.X = X; a.n = n; a.d = d; a.ldx = ldx; a.cls = cls; a.K = K; a.mode = mode; a.theta = theta;
-  a.part = reinterpret_cast<double*>(ws + G.off_part);
-  a.cpart = reinterpret_cast<double*>(ws + G.off_cpart);
-  a.fs = G.fs; a.groups = G.groups; a.ks = G.ks; a.nk = G.nk; a.rows_per_split = G.rows_per_split;
-  if (G.splits > 0) {
-    int r = 0;
-    if (x_dtype == BKM_F32) r = launch_moments<float>(a, G, s);
-    else if (x_dtype == BKM_F64) r = launch_moments<double>(a, G, s);
-    else r = launch_moments<__nv_bfloat16>(a, G, s);
-    if (r) return r;
-  }
-  const long long total = (long long)K * d + (mode == 0 ? K : 0);
-  long long blocks = (total + 255) / 256;
-  if (blocks > 4LL * sms) blocks = 4LL * sms;
-  moments_fold_kernel<<<(unsigned)blocks, 256, 0, s>>>(a.part, a.cpart, G.splits, K, d, mode, sums,
-                                                       mode == 0 ? counts : nullptr,
-                                                       (flags & BKM_FLAG_FIRST_CHUNK) ? 1 : 0);
-  BKM_CUDA_TRY(cudaGetLastError());
-  note_launch();
-  return 0;
+  return moments_run(X, n, d, ldx, x_dtype, cls, K, mode, theta, false, nullptr, 0, 0.0, sums, counts, workspace,
+                     ws_bytes, flags, stream);
+}
+
+extern "C" int bkm_class_counts_chunk(const void* X, int64_t n, int d, int64_t ldx, int x_dtype, const int32_t* cls,
+                                      int K, const double* w, int binarize, double threshold, double* fc, double* cc,
+                                      void* workspace, size_t ws_bytes, int flags, void* stream) {
+  if (n < 0 || d <= 0 || K <= 0 || ldx < d || !fc || !cc || !workspace) return BKM_EINVAL;
+  if (n > 0 && (!X || !cls)) return BKM_EINVAL;
+  if (!dtype_ok(x_dtype)) return BKM_EDTYPE;
+  return moments_run(X, n, d, ldx, x_dtype, cls, K, 0, nullptr, true, w, binarize, threshold, fc, cc, workspace,
+                     ws_bytes, flags, stream);
 }
 
 extern "C" int bkm_nb_jll_chunk(const void* X, int64_t n, int d, int64_t ldx, int x_dtype, const double* theta,
@@ -598,4 +829,26 @@ extern "C" int bkm_nb_jll_chunk(const void* X, int64_t n, int d, int64_t ldx, in
   if (x_dtype == BKM_F32) return launch_jll_f32<float>(a, sms, s);
   if (x_dtype == BKM_BF16) return launch_jll_f32<__nv_bfloat16>(a, sms, s);
   return launch_jll_f64(a, sms, s);
+}
+
+extern "C" int bkm_nb_linear_jll_chunk(const void* X, int64_t n, int d, int64_t ldx, int x_dtype, int binarize,
+                                       double threshold, const double* W, const double* b, int K, int32_t* labels,
+                                       double* out, int64_t ldo, int out_mode, int flags, void* stream) {
+  (void)flags;
+  if (n < 0 || d <= 0 || K <= 0 || ldx < d || !W || !b) return BKM_EINVAL;
+  if (out_mode != BKM_NB_JLL && out_mode != BKM_NB_LOG_PROBA && out_mode != BKM_NB_PROBA) return BKM_EINVAL;
+  if (!dtype_ok(x_dtype)) return BKM_EDTYPE;
+  if (n == 0) return 0;
+  if (!X || (!labels && !out)) return BKM_EINVAL;
+  if (out && ldo < K) return BKM_EINVAL;
+  int sms = 0;
+  const int rc = sm_count(&sms);
+  if (rc) return rc;
+  LinArgs a;
+  a.X = X; a.n = n; a.d = d; a.ldx = ldx; a.bin = binarize ? 1 : 0; a.thr = threshold; a.W = W; a.b = b; a.K = K;
+  a.labels = labels; a.out = out; a.ldo = ldo; a.out_mode = out_mode;
+  cudaStream_t s = (cudaStream_t)stream;
+  if (x_dtype == BKM_F32) return launch_linear<float>(a, sms, s);
+  if (x_dtype == BKM_F64) return launch_linear<double>(a, sms, s);
+  return launch_linear<__nv_bfloat16>(a, sms, s);
 }

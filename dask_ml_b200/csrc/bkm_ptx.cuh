@@ -1,4 +1,5 @@
-// bkm_ptx.cuh — inline-PTX wrappers shared by the CUDA-core kernels (bkm_stream.cu, bkm_rowpass.cu, bkm_p2p.cu).
+// bkm_ptx.cuh — inline-PTX wrappers shared by the CUDA-core kernels (bkm_stream.cu, bkm_rowpass.cu, bkm_p2p.cu) and the
+// float64 tensor-core passes (bkm_pca.cu, bkm_nb.cu).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -77,6 +78,16 @@ __device__ __forceinline__ float fset_le(float a, float b) {
   float r;
   asm("set.le.f32.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b));
   return r;
+}
+
+// D = A B + D, A 16x16 (row), B 16x8 (col), float64.  Fragments (g = lane / 4, t = lane % 4):
+//   a[i] = A[g + 8 (i & 1)][t + 4 (i >> 1)],  b[i] = B[t + 4 i][g],  c = {(g, 2t), (g, 2t+1), (g+8, 2t), (g+8, 2t+1)}
+__device__ __forceinline__ void dmma16816(double (&c)[4], const double (&a)[8], const double (&b)[4]) {
+  asm("mma.sync.aligned.m16n8k16.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5,%6,%7,%8,%9,%10,%11}, "
+      "{%12,%13,%14,%15}, {%0,%1,%2,%3};"
+      : "+d"(c[0]), "+d"(c[1]), "+d"(c[2]), "+d"(c[3])
+      : "d"(a[0]), "d"(a[1]), "d"(a[2]), "d"(a[3]), "d"(a[4]), "d"(a[5]), "d"(a[6]), "d"(a[7]),
+        "d"(b[0]), "d"(b[1]), "d"(b[2]), "d"(b[3]));
 }
 
 }  // namespace ptx

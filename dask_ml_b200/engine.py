@@ -499,6 +499,64 @@ class CudaBackend(object):
                 (out.stride(0) if n else K) if out is not None else K, int(bool(exp_out)), self._ptr(n_deferred),
                 self.flags, self._stream()), "bkm_nb_jll_chunk")
 
+    def class_counts_chunk(self, x, cls, K, fc, cc, w=None, binarize=None, first=False):
+        """The count pass of the discrete naive Bayes models over one chunk, by int32 class index ``cls`` (indices
+        outside [0, K) are skipped): fc (K, d) (+)= per-class sums of w_i f(x_i) and cc (K,) (+)= per-class sums of w_i,
+        float64 on the device, ``w`` float64 (n,) or None (ones), f(x) = x, or x > ``binarize`` when it is not None.
+        ``first`` overwrites."""
+        n, d = x.shape
+        nb = ctypes.c_size_t(0)
+        _lib.check(self.lib.bkm_nb_workspace_bytes(int(n), int(d), int(K), ctypes.byref(nb)), "bkm_nb_workspace_bytes")
+        ws = self._scratch("nb", nb.value)
+        flags = self.flags | (_lib.FLAG_FIRST_CHUNK if first else 0)
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.bkm_class_counts_chunk(
+                self._ptr(x), n, d, x.stride(0) if n else d, _DT_CODE[x.dtype], self._ptr(cls), int(K), self._ptr(w),
+                int(binarize is not None), float(binarize or 0.0), self._ptr(fc), self._ptr(cc), self._ptr(ws),
+                ws.numel(), flags, self._stream()), "bkm_class_counts_chunk")
+
+    def csc_class_counts_chunk(self, csc, d, labels, K, fcT, w=None, binarize=None, first=False):
+        """``class_counts_chunk``'s feature sums over the transpose ``csc`` of one CSR block, transposed: fcT (d, K)
+        (+)= per-class sums of w_i f(x_ij), each in ascending row order; an entry not above ``binarize`` adds nothing.
+        ``first`` overwrites."""
+        colptr, rows, vals, plan = csc
+        nnz = int(rows.numel())
+        nb = ctypes.c_size_t(0)
+        _lib.check(self.lib.bkm_csc_label_sums_workspace_bytes(int(d), nnz, int(K), ctypes.byref(nb)),
+                   "bkm_csc_label_sums_workspace_bytes")
+        ws = self._scratch("csc_label_sums", nb.value)
+        flags = self.flags | (_lib.FLAG_FIRST_CHUNK if first else 0)
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.bkm_csc_class_counts_chunk(
+                self._ptr(colptr), self._ptr(rows), self._ptr(vals), _DT_CODE[vals.dtype], int(d), nnz, self._ptr(plan),
+                self._ptr(labels), int(K), self._ptr(w), int(binarize is not None), float(binarize or 0.0),
+                self._ptr(fcT), self._ptr(ws), ws.numel(), flags, self._stream()), "bkm_csc_class_counts_chunk")
+
+    def nb_linear_jll_chunk(self, x, W, b, labels=None, out=None, out_mode=0, binarize=None):
+        """The predict pass of the discrete naive Bayes models over one chunk: jll = f(x) W^T + b (``W`` float64 (K, d),
+        ``b`` float64 (K,) on the device; f as in ``class_counts_chunk``), into ``labels`` (int32 (n,)) its arg-max and /
+        or ``out`` (float64 (n, K), any row pitch) jll (``out_mode`` 0), its log-softmax (1) or softmax (2)."""
+        n, d = x.shape
+        K = int(W.shape[0])
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.bkm_nb_linear_jll_chunk(
+                self._ptr(x), n, d, x.stride(0) if n else d, _DT_CODE[x.dtype], int(binarize is not None),
+                float(binarize or 0.0), self._ptr(W), self._ptr(b), K, self._ptr(labels), self._ptr(out),
+                (out.stride(0) if n else K) if out is not None else K, int(out_mode), self.flags, self._stream()),
+                "bkm_nb_linear_jll_chunk")
+
+    def nb_csr_jll_chunk(self, blk, d, WT, b, labels=None, out=None, out_mode=0, binarize=None):
+        """``nb_linear_jll_chunk`` on one CSR block of d columns over its stored entries, ``WT`` float64 (d, K)
+        row-major."""
+        crow, col, val, n = blk
+        K = int(WT.shape[1])
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.bkm_nb_csr_jll_chunk(
+                self._ptr(crow), self._ptr(col), self._ptr(val), _DT_CODE[val.dtype], int(n), int(d), int(col.numel()),
+                int(binarize is not None), float(binarize or 0.0), self._ptr(WT), self._ptr(b), K, self._ptr(labels),
+                self._ptr(out), (out.stride(0) if n else K) if out is not None else K, int(out_mode), self.flags,
+                self._stream()), "bkm_nb_csr_jll_chunk")
+
     def glm_pass_chunk(self, x, y, beta, family, mode, grad=None, hrow=None, w=None, out=None, first=False):
         """The fused pass of the linear models over one chunk (float64 arithmetic): eta = x . beta[:d] + beta[d] with
         ``family`` 0 logistic, 1 normal, 2 poisson.  ``mode`` 0: grad (d + 2,) (+)= [sum r x | sum r | loss];

@@ -70,6 +70,10 @@
  *     partial_fit of every block (_plain_sgd, one epoch), behind          bkm_sgd_block,
  *     linear_model/{stochastic_gradient,perceptron,passive_aggressive}    bkm_sgd_csr_block
  *     .py and _partial.py:39-100
+ *   the MultinomialNB / BernoulliNB partial_fit counts (Y^T X) and       bkm_class_counts_chunk,
+ *     the safe_sparse_dot(X, W^T) + b of their predict methods, behind    bkm_csc_class_counts_chunk,
+ *     PartialMultinomialNB / PartialBernoulliNB (naive_bayes.py:125-134   bkm_nb_linear_jll_chunk,
+ *     and _partial.py)                                                    bkm_nb_csr_jll_chunk
  *
  * Conventions
  *   - extern "C", plain pointers and sizes only; no torch / C++ types.
@@ -107,8 +111,9 @@ extern "C" {
  *     bkm_csc_label_sums_chunk, bkm_sparse_pack_workspace_bytes, bkm_sparse_pack_centers, bkm_sparse_finalize_step
  * 8 = bkm_csr_kernel_colsum_workspace_bytes, bkm_csr_kernel_colsum_chunk, bkm_csr_nystrom_embed_chunk,
  *     bkm_sparse_minibatch_step
- * 9 = bkm_sgd_order, bkm_sgd_block, bkm_sgd_csr_block */
-#define BKM_VERSION_MINOR 9
+ * 9 = bkm_sgd_order, bkm_sgd_block, bkm_sgd_csr_block
+ * 10 = bkm_class_counts_chunk, bkm_csc_class_counts_chunk, bkm_nb_linear_jll_chunk, bkm_nb_csr_jll_chunk */
+#define BKM_VERSION_MINOR 10
 
 /* element types of X */
 #define BKM_F32 0
@@ -278,6 +283,41 @@ int bkm_class_moments_chunk(const void* X, int64_t n, int d, int64_t ldx, int x_
 int bkm_nb_jll_chunk(const void* X, int64_t n, int d, int64_t ldx, int x_dtype, const double* theta,
                      const double* inv_sigma, const double* logc, int K, int32_t* labels, double* out, int64_t ldo,
                      int exp_out, int* n_deferred, int flags, void* stream);
+
+/* ---- PartialMultinomialNB / PartialBernoulliNB: the count pass of partial_fit and the predict pass, on dense row
+ * chunks and on CSR blocks (replace scikit-learn's safe_sparse_dot(Y^T, X) in _count and safe_sparse_dot(X, W^T) + b in
+ * _joint_log_likelihood) -------------------------------------------------------------------------------------------
+ * f(x) is x, or 1.0 where x > threshold and 0.0 elsewhere when `binarize` is nonzero (scikit-learn's binarize; for CSR
+ * blocks an entry that is not above the threshold is dropped, as scipy drops the zeros binarize makes).
+ *   bkm_class_counts_chunk      fc [K][d] (+)= sum_{i: cls_i = c} w_i f(x_ij),  cc [K] (+)= sum_{i: cls_i = c} w_i, w [n]
+ *                               float64 (nullable: w_i = 1).  cls, the order of the sums, OVERWRITE / ACCUMULATE and the
+ *                               workspace (bkm_nb_workspace_bytes) are those of bkm_class_moments_chunk mode 0.
+ *   bkm_csc_class_counts_chunk  fcT [p][K] (+)= the same sums over the transpose of one CSR block (bkm_csr_transpose_chunk),
+ *                               each (feature, class) sum in ascending row order; labels [n] int32 class indices (outside
+ *                               [0, K) skipped).  Workspace: bkm_csc_label_sums_workspace_bytes(p, nnz, K) bytes.
+ *   bkm_nb_linear_jll_chunk     jll_ic = b_c + sum_j f(x_ij) W_cj  (W [K][d], b [K] float64), float64 products on the fp64
+ *                               tensor cores (0 * -inf = NaN, as BLAS).  Any d, any row pitch ldx >= d.
+ *   bkm_nb_csr_jll_chunk        the same for one CSR block over the stored entries only, WT [p][K] float64 row-major.
+ *   Both: labels [n] int32 (nullable) = the arg-max over c (the first maximum; the first NaN class if any, as np.argmax);
+ *   out [n][ldo] float64 (nullable) = jll (BKM_NB_JLL), jll - (log sum_c exp(jll - max) + max) (BKM_NB_LOG_PROBA) or its
+ *   exp (BKM_NB_PROBA); a normalised row with a NaN jll or no finite maximum is NaN throughout.  The sums run in a fixed
+ *   order: two calls with the same inputs give the same bits. */
+#define BKM_NB_JLL        0
+#define BKM_NB_LOG_PROBA  1
+#define BKM_NB_PROBA      2
+int bkm_class_counts_chunk(const void* X, int64_t n, int d, int64_t ldx, int x_dtype, const int32_t* cls, int K,
+                           const double* w, int binarize, double threshold, double* fc, double* cc, void* workspace,
+                           size_t ws_bytes, int flags, void* stream);
+int bkm_csc_class_counts_chunk(const int64_t* colptr, const int32_t* rows, const void* vals, int val_dtype, int p,
+                               int64_t nnz, const int64_t* plan, const int32_t* labels, int K, const double* w,
+                               int binarize, double threshold, double* fcT, void* workspace, size_t ws_bytes, int flags,
+                               void* stream);
+int bkm_nb_linear_jll_chunk(const void* X, int64_t n, int d, int64_t ldx, int x_dtype, int binarize, double threshold,
+                            const double* W, const double* b, int K, int32_t* labels, double* out, int64_t ldo,
+                            int out_mode, int flags, void* stream);
+int bkm_nb_csr_jll_chunk(const int64_t* crow, const int64_t* col, const void* val, int val_dtype, int64_t n, int p,
+                         int64_t nnz, int binarize, double threshold, const double* WT, const double* b, int K,
+                         int32_t* labels, double* out, int64_t ldo, int out_mode, int flags, void* stream);
 
 /* ---- LogisticRegression / LinearRegression / PoissonRegression: the per-iteration passes of the solvers (replace
  * dask_glm's X.dot(beta) and the family's loglike / gradient / hessian, linear_model/glm.py) ------------------------
