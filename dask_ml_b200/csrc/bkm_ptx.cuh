@@ -56,6 +56,12 @@ __device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t
                ::"r"(dst), "l"(src), "r"(bytes), "r"(bar) : "memory");
 }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+// 2-D tensor-map (TMA) copy of the box at element coordinates (c0, c1) -> shared, completion on an mbarrier; `tmap` is
+// the generic address of a __grid_constant__ CUtensorMap parameter
+__device__ __forceinline__ void tma_load_2d(uint32_t dst, const void* tmap, int c0, int c1, uint32_t bar) {
+  asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
+               ::"r"(dst), "l"(tmap), "r"(c0), "r"(c1), "r"(bar) : "memory");
+}
 
 // packed fp32 pairs: two fused multiply-adds on the halves of a 64-bit register pair (sm_90 has no paired FFMA, so this
 // is two FFMA; keeping the pair form lets the callers load / store operands as 64-bit pairs)

@@ -12,8 +12,10 @@
 // re-decided in float64 (as are rows whose scaled entries leave fp16's range).  The M-step (_centers_dense,
 // dask_ml/cluster/k_means.py:572-582) is fused: rows are added into shared-memory per-CTA sums, X is read from HBM once.
 //
-// CTA = 2 warpgroups (1 CTA per SM).  Each warpgroup owns alternate 64-row tiles of the CTA and runs, per tile:
-//   cp.async of the NEXT tile into its second stage (fp32 rows, zero-filled beyond n and d);
+// CTA = 2 warpgroups (1 CTA per SM).  The CTA's tiles stream through a ring of S shared-memory slots filled by TMA
+// (local tile lt -> slot lt % S, one "full" mbarrier per slot; fp32 rows in 32-column SWIZZLE_128B boxes, zero-filled
+// beyond n and d by the copy engine).  Each warpgroup owns alternate 64-row tiles of the CTA (lt % 2) and runs, per tile:
+//   the wait for the tile's slot;
 //   the fp16 (hi, lo) A fragments of s X built in registers (and ||s x||^2);
 //   3 KS wgmma.m64nNk16 (KS = ceil(d/16), a template parameter so that they issue back to back) with B
 //   (= -2 s C as fp16 hi / lo, SWIZZLE_128B K-major) resident in shared memory; N = 256 runs as two column halves in
@@ -21,7 +23,8 @@
 //   the arg-min epilogue from the register accumulators in two passes (the row minimum, then the count and index
 //   of the columns within the near-tie bound of it), the first pass over the first column half while the tensor
 //   cores compute the second;
-//   the winning distance in direct form (x - c)^2 in fp32, and the M-step.
+//   the winning distance in direct form (x - c)^2 in fp32, and the M-step;
+//   after the warpgroup's last read of the slot, the load of tile lt + S into it (no separate producer).
 // The M-step adds the tile's rows in row order into the CTA's sums; the two warpgroups take turns (named barriers),
 // so every cluster's sum is formed in one fixed order and the sums are bit-reproducible.  Each sums element has one
 // owning thread (feature f, label parity q); before its turn a warp lists the tile's rows of its parity, so that the
@@ -30,19 +33,30 @@
 // overlap the other's epilogue / M-step.
 #include "bkm_common.cuh"
 #include "bkm_wgmma.cuh"
+#include <cuda.h>
+#include <cudaTypedefs.h>
 #include <cuda_fp16.h>
 #include <math_constants.h>
 
 namespace bkm {
 
 static const int TBM = 64;           // rows per warpgroup tile (wgmma M)
-static const int XP = 72;            // fp32 row pitch of a staged X tile (16-byte multiple; rows 8 banks apart)
 static const int TC_THREADS = 256;   // two warpgroups
+// X ring: a slot holds one 64 x 64 fp32 tile as two TMA boxes of 32 columns (box b: columns 32b .. 32b + 31, 64 rows of
+// 128 bytes, SWIZZLE_128B: 16-byte chunk q of row r sits at chunk q ^ (r & 7)), so that a warp's reads of 8 rows x one
+// chunk, or of one row x 32 columns, hit 32 different banks
+static const uint32_t XBOX_BYTES = TBM * 128u;
+static const uint32_t XSLOT_BYTES = 2u * XBOX_BYTES;
+static const int TC_MAX_STAGES = 8;
+// two slots per warpgroup: the tile being worked on and the next one.  Every supported shape (d <= 64, k <= 256) leaves
+// room for at least 4 (the M-step variants at N = 256: 5)
+static const int TC_MIN_STAGES = 4;
 
 struct TcCfg {
   int KS;        // MMA K-steps of 16 (ceil(d/16))
   int NP;        // padded centre count (multiple of 16, <= 256)
-  uint32_t off_bhi, off_blo, off_x, off_sum, off_cn, off_cnt, off_lab, off_dp, off_red, off_cls, total;
+  int S;         // slots of the X ring
+  uint32_t off_bhi, off_blo, off_sum, off_cn, off_cnt, off_lab, off_dp, off_cls, off_bar, off_ring, total;
 };
 
 // Epilogue of tc_chunk_kernel (all four share the MMAs, the tile pipeline and the A-fragment build):
@@ -75,12 +89,19 @@ __device__ unsigned int g_tc_dbg[64];
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void bar_sync(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
 __device__ __forceinline__ void bar_arrive(int id, int n) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(n) : "memory"); }
-// M-step class-list entry of row `row` of a tile with label `c`: the byte offset of sums row c (bits 0-16) and of the
-// staged X row (bits 17-31).  Rows of the sums are 64 floats, so a thread adds 4 f to the first.
+// byte offset of X element (row r, feature f) in a ring slot
+__device__ __forceinline__ uint32_t xsw(int r, int f) {
+  return (uint32_t)((f >> 5) * XBOX_BYTES + r * 128 + ((((f >> 2) & 7) ^ (r & 7)) << 4) + (f & 3) * 4);
+}
+// M-step class-list entry of row `row` of a tile with label `c`: the byte offset of sums row c (bits 0-16) and the row's
+// part of its slot offset, 128 row | (row & 7) << 4 (bits 17-31).  Rows of the sums are 64 floats, so a thread adds 4 f to
+// the first; to the second it applies its feature's swizzle, ^ ((f >> 2) & 7) << 4, and adds its box and (f & 3) * 4.
 static const int CLS_ROW_SHIFT = 17;
 static const uint32_t CLS_SUM_MASK = (1u << CLS_ROW_SHIFT) - 1u;
-static_assert((256 + 1) * 64 * 4 <= (int)CLS_SUM_MASK && (TBM - 1) * XP * 4 < (1 << (32 - CLS_ROW_SHIFT)), "class-list entry fields");
-__device__ __forceinline__ uint32_t cls_entry(int c, int row) { return ((uint32_t)(row * XP * 4) << CLS_ROW_SHIFT) | (uint32_t)(c * 64 * 4); }
+static_assert((256 + 1) * 64 * 4 <= (int)CLS_SUM_MASK && ((TBM - 1) * 128 | 0x70) < (1 << (32 - CLS_ROW_SHIFT)), "class-list entry fields");
+__device__ __forceinline__ uint32_t cls_entry(int c, int row) {
+  return ((uint32_t)(row * 128 | (row & 7) << 4) << CLS_ROW_SHIFT) | (uint32_t)(c * 64 * 4);
+}
 __device__ __forceinline__ uint32_t pack_half2(float lo, float hi) {
   const __half2 h = __floats2half2_rn(lo, hi);          // low half = lower column
   return *reinterpret_cast<const uint32_t*>(&h);
@@ -91,7 +112,7 @@ __device__ __forceinline__ uint32_t pack_half2(float lo, float hi) {
 // of the Nystrom embedding (dask_ml/cluster/spectral.py:237-282).  Same MMAs, no M-step.
 template <int N, int KS, bool MSTEP, bool WANT_DIST, int EPI>
 __global__ void __launch_bounds__(TC_THREADS, 1)
-tc_chunk_kernel(ChunkArgs a, typename TcCfgOf<EPI>::type cfg) {
+tc_chunk_kernel(ChunkArgs a, typename TcCfgOf<EPI>::type cfg, const __grid_constant__ CUtensorMap xmap) {
   constexpr bool XFORM = EPI == EPI_XFORM;
   if (a.skip && *a.skip) return;                            // converged loop: no-op iteration
 
@@ -108,7 +129,7 @@ tc_chunk_kernel(ChunkArgs a, typename TcCfgOf<EPI>::type cfg) {
   float* sum_s = reinterpret_cast<float*>(smem + cfg.off_sum);        // [N + 2][64] (rows N, N + 1: M-step list padding)
   int* lab_s = reinterpret_cast<int*>(smem + cfg.off_lab) + wgi * TBM;        // label of each row of the tile, -1: none
   float* dp_s = reinterpret_cast<float*>(smem + cfg.off_dp) + wgi * 2 * TBM;  // [2][TBM] halves of the direct distances
-  double* red_s = reinterpret_cast<double*>(smem + cfg.off_red);
+  double* red_s = reinterpret_cast<double*>(smem + cfg.off_ring);    // teardown only: the ring is drained by then
   const PackHeader* hdr = reinterpret_cast<const PackHeader*>(a.pack);
   const float sc = hdr->scale;
   const float inv_s = 1.0f / sc;                             // exact: s is a power of two, s and 1/s are normal
@@ -143,29 +164,26 @@ tc_chunk_kernel(ChunkArgs a, typename TcCfgOf<EPI>::type cfg) {
     }
     wg::fence_proxy_async();                                 // generic-proxy stores -> visible to wgmma
   }
-  __syncthreads();
-
   const long long ntiles = (a.n + TBM - 1) / TBM;
   const long long my_tiles = blockIdx.x < ntiles ? (ntiles - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;
   const long long npairs = (my_tiles + 1) / 2;               // warpgroup w takes the CTA's tiles 2p + w
-  const float* X = reinterpret_cast<const float*>(a.X);
-  const uint32_t stage_bytes = TBM * XP * 4;
-  const uint32_t xs_u32 = sbase + cfg.off_x + (uint32_t)wgi * 2u * stage_bytes;
-  const float* xs_f = reinterpret_cast<const float*>(smem + cfg.off_x) + wgi * 2 * TBM * XP;
-  constexpr int nq = KS * 4;                                 // 16-byte chunks per staged row
-  auto load_tile = [&](long long p, int stage) {
-    const long long lt = 2 * p + wgi;
-    if (lt < my_tiles) {
-      const long long row0 = (blockIdx.x + lt * gridDim.x) * TBM;
-      for (int i = t; i < TBM * nq; i += 128) {
-        const int r = i / nq, col = (i - r * nq) * 4;
-        const long long row = row0 + r;
-        const int bytes = (row < a.n && col < d) ? min(16, (d - col) * 4) : 0;
-        wg::cp16(xs_u32 + (uint32_t)stage * stage_bytes + (uint32_t)(r * XP + col) * 4u, bytes ? X + row * a.ldx + col : X, bytes);
-      }
-    }
-    wg::cp_commit();
+  const int S = cfg.S;
+  const uint32_t bar0 = sbase + cfg.off_bar, ring0 = sbase + cfg.off_ring;
+  // tile lt -> slot lt % S: its ceil(d / 32) boxes, completion counted in bytes on the slot's mbarrier
+  auto load_tile = [&](long long lt, int slot) {
+    const uint32_t bar = bar0 + 8u * (uint32_t)slot, dst = ring0 + (uint32_t)slot * XSLOT_BYTES;
+    const int row0 = (int)((blockIdx.x + lt * gridDim.x) * TBM);
+    constexpr int nbox = (KS + 1) / 2;
+    ptx::mbar_expect_tx(bar, nbox * XBOX_BYTES);
+#pragma unroll
+    for (int b = 0; b < nbox; ++b) ptx::tma_load_2d(dst + b * XBOX_BYTES, &xmap, 32 * b, row0, bar);
   };
+  if (tid == 0) {
+    for (int i = 0; i < S; ++i) ptx::mbar_init(bar0 + 8u * i, 1);
+    ptx::mbar_fence_init();
+    for (int lt = 0; lt < S && lt < my_tiles; ++lt) load_tile(lt, lt);
+  }
+  __syncthreads();
 
   const int g = lane >> 2, c2 = (lane & 3) * 2;
   const int rA = wq * 16 + g;                                // this thread's accumulator rows: rA, rA + 8
@@ -174,17 +192,20 @@ tc_chunk_kernel(ChunkArgs a, typename TcCfgOf<EPI>::type cfg) {
   double dsum = 0.0;
   double cs0 = 0.0, cs1 = 0.0;                               // COLSUM: this warpgroup's sums of columns t, t + 128
 
-  load_tile(0, 0);
+  int slot = wgi;                                            // lt % S and the parity (lt / S) & 1 of the slot's fill
+  uint32_t fill = 0;
 #pragma unroll 1
   for (long long p = 0; p < npairs; ++p) {
-    const int stage = (int)(p & 1);
-    load_tile(p + 1, stage ^ 1);
-    wg::cp_wait1();
-    wg::wg_sync(1 + wgi);                                    // tile p is in shared memory (every thread's copies)
     const long long lt = 2 * p + wgi;
     const bool has = lt < my_tiles;
     const long long row0 = (blockIdx.x + lt * gridDim.x) * TBM;
-    const float* xs = xs_f + stage * TBM * XP;
+    unsigned char* xs = smem + cfg.off_ring + (uint32_t)slot * XSLOT_BYTES;
+    // The previous fill of this slot (tile lt - S) must have landed before this wait starts: if it has not, the
+    // barrier is still in that phase, and the parity of tile lt's phase, which is also that of tile lt - 2S's, reads as
+    // complete.  With S even, tile lt - S is this warpgroup's own earlier tile.  With S odd (the M-step variants only,
+    // see place_ring) it is the other warpgroup's, and the turn order covers it: this warpgroup's previous turn (tile
+    // lt - 2) waited for the other's turn of tile lt - 3 >= lt - S + 2, which came after its wait for tile lt - S.
+    if (has) ptx::mbar_wait(bar0 + 8u * (uint32_t)slot, fill);
     if (has) {
       // ---- s X -> fp16 (hi, lo) A fragments, ||s x||^2 of rows rA / rA + 8 ----
       uint32_t ahi[4][4], alo[4][4];
@@ -195,7 +216,7 @@ tc_chunk_kernel(ChunkArgs a, typename TcCfgOf<EPI>::type cfg) {
         for (int h = 0; h < 4; ++h) {
           ahi[s][h] = 0u; alo[s][h] = 0u;
           if (s < KS) {
-            const float2 v = *reinterpret_cast<const float2*>(xs + (rA + (h & 1) * 8) * XP + s * 16 + c2 + (h >> 1) * 8);
+            const float2 v = *reinterpret_cast<const float2*>(xs + xsw(rA + (h & 1) * 8, s * 16 + c2 + (h >> 1) * 8));
             const float e0 = v.x * sc, e1 = v.y * sc;
             const __half2 hh = __floats2half2_rn(e0, e1);
             const float2 hf = __half22float2(hh);
@@ -282,10 +303,9 @@ tc_chunk_kernel(ChunkArgs a, typename TcCfgOf<EPI>::type cfg) {
           }
         }
         // e = v . W in groups of 8 outputs: per thread over its columns, then the quad's 4 partial sums (the same
-        // value lands in all 4 lanes); lane q of the quad stages outputs 2q, 2q + 1 of the group in the tile's X stage
-        // (rows of this warp only: their A fragments are built and consumed)
+        // value lands in all 4 lanes); lane q of the quad stages outputs 2q, 2q + 1 of the group in the tile's X
+        // slot (rows of this warp only: their A fragments are built and consumed)
         const float* w_s = reinterpret_cast<const float*>(smem + cfg.off_w);
-        float* est = reinterpret_cast<float*>(smem + cfg.off_x) + (wgi * 2 + stage) * TBM * XP;
         const int q = lane & 3;
         float n0 = 0.f, n1 = 0.f;
         __syncwarp();
@@ -316,8 +336,8 @@ tc_chunk_kernel(ChunkArgs a, typename TcCfgOf<EPI>::type cfg) {
                           : q == 2 ? make_float2(e0[4], e0[5]) : make_float2(e0[6], e0[7]);
           const float2 p1 = q == 0 ? make_float2(e1[0], e1[1]) : q == 1 ? make_float2(e1[2], e1[3])
                           : q == 2 ? make_float2(e1[4], e1[5]) : make_float2(e1[6], e1[7]);
-          *reinterpret_cast<float2*>(est + rA * XP + o0 + 2 * q) = p0;
-          *reinterpret_cast<float2*>(est + (rA + 8) * XP + o0 + 2 * q) = p1;
+          *reinterpret_cast<float2*>(xs + xsw(rA, o0 + 2 * q)) = p0;
+          *reinterpret_cast<float2*>(xs + xsw(rA + 8, o0 + 2 * q)) = p1;
         }
         // per-row factor 1 / ||e||; NaN where gamma * m (unscaled, float64) is beyond the float64 reference's underflow
         if (q == 0) {
@@ -331,8 +351,9 @@ tc_chunk_kernel(ChunkArgs a, typename TcCfgOf<EPI>::type cfg) {
         for (int e = lane; e < 16 * kw; e += 32) {
           const int rr = e / kw, o = e - rr * kw, r = wq * 16 + rr;
           const long long row = row0 + r;
-          if (row < a.n) __stcs(a.xf_out + row * a.xf_ld + o, est[r * XP + o] * dp_s[r]);
+          if (row < a.n) __stcs(a.xf_out + row * a.xf_ld + o, *reinterpret_cast<const float*>(xs + xsw(r, o)) * dp_s[r]);
         }
+        ptx::fence_proxy_async();                            // these generic writes before the slot's next TMA fill
       } else if constexpr (EPI == EPI_XFORM) {
         wg::wait_all();
         wg::pin(acc);
@@ -432,8 +453,8 @@ tc_chunk_kernel(ChunkArgs a, typename TcCfgOf<EPI>::type cfg) {
 #pragma unroll 8
           for (int i = 0; i < 32; i += 2) {
             const int f0 = hh * 32 + ((i + r) & 31), f1 = hh * 32 + ((i + 1 + r) & 31);
-            if (f0 < d) { const float e = fmaf(sc, xs[r * XP + f0], -(sc * cr[f0])); s0 = fmaf(e, e, s0); }
-            if (f1 < d) { const float e = fmaf(sc, xs[r * XP + f1], -(sc * cr[f1])); s1 = fmaf(e, e, s1); }
+            if (f0 < d) { const float e = fmaf(sc, *reinterpret_cast<const float*>(xs + xsw(r, f0)), -(sc * cr[f0])); s0 = fmaf(e, e, s0); }
+            if (f1 < d) { const float e = fmaf(sc, *reinterpret_cast<const float*>(xs + xsw(r, f1)), -(sc * cr[f1])); s1 = fmaf(e, e, s1); }
           }
         }
         dp_s[hh * TBM + r] = s0 + s1;
@@ -485,9 +506,9 @@ tc_chunk_kernel(ChunkArgs a, typename TcCfgOf<EPI>::type cfg) {
         // repeated label, a row continues from the running sum of that label's earlier row.  So every element receives
         // its rows in tile order, then row order, one rounded addition each
         if (f < d) {
-          const uint32_t fo = (uint32_t)f * 4u;
+          const uint32_t fo = (uint32_t)f * 4u, fx = (uint32_t)((f >> 2) & 7) << 4;
           unsigned char* sum_b = reinterpret_cast<unsigned char*>(sum_s);
-          const unsigned char* xs_b = reinterpret_cast<const unsigned char*>(xs) + fo;
+          const unsigned char* xs_b = xs + (f >> 5) * XBOX_BYTES + (f & 3) * 4;
           const uint4* cl4 = reinterpret_cast<const uint4*>(cls);
           uint4 ea = cl4[0], eb = cl4[1];
 #pragma unroll 1
@@ -497,7 +518,7 @@ tc_chunk_kernel(ChunkArgs a, typename TcCfgOf<EPI>::type cfg) {
 #pragma unroll
             for (int j = 0; j < 8; ++j) {
               v[j] = *reinterpret_cast<const float*>(sum_b + ((e[j] & CLS_SUM_MASK) | fo));
-              x[j] = *reinterpret_cast<const float*>(xs_b + (e[j] >> CLS_ROW_SHIFT));
+              x[j] = *reinterpret_cast<const float*>(xs_b + ((e[j] >> CLS_ROW_SHIFT) ^ fx));
             }
             if (8 * (b + 1) < ncls) { ea = cl4[2 * b + 2]; eb = cl4[2 * b + 3]; }
             if ((rep >> (8 * b)) & 0xffu) {
@@ -523,7 +544,13 @@ tc_chunk_kernel(ChunkArgs a, typename TcCfgOf<EPI>::type cfg) {
         else if (p + 1 < npairs) bar_arrive(4 + 2 * wq, 64);
       }
     }
-    wg::wg_sync(1 + wgi);                                    // the stage and lab_s may be refilled
+    wg::wg_sync(1 + wgi);                                    // the slot and lab_s may be refilled
+    if (t == 0 && lt + S < my_tiles) {
+      ptx::fence_proxy_async();                              // the warpgroup's accesses to the slot before the async-proxy fill
+      load_tile(lt + S, slot);
+    }
+    slot += 2;
+    if (slot >= S) { slot -= S; fill ^= 1u; }
   }
 
   // ---------------- teardown: per-CTA partials ----------------
@@ -682,49 +709,84 @@ void tc_abort_reset() {
 }
 
 bool tc_supported(int d, int k, int dtype) {
-  // any d <= 64: columns beyond d are zero-filled when a tile is staged; what the staging copies do need is a
+  // any d <= 64: columns beyond d are zero-filled when a tile is staged; what the TMA copies do need is a
   // 16-byte row pitch and base (launch_tc returns BKM_EALIGN otherwise and the caller falls back to the CUDA-core
   // kernel), which the host side provides by uploading row chunks with a padded pitch (engine.CudaBackend.to_device)
   return dtype == BKM_F32 && d >= 1 && d <= 64 && k >= 1 && k <= 256;
 }
 
-static bool make_cfg(int d, int k, bool mstep, TcCfg* c) {
+// The arrays of every variant; returns the end of the last one
+static uint32_t layout_common(int d, int k, bool mstep, TcCfg* c) {
   c->KS = (d + 15) / 16;
   c->NP = (k + 15) / 16 * 16;
   const uint32_t N = (uint32_t)wg::mma_n(c->NP);
   uint32_t o = 0;
   c->off_bhi = o; o += N * 128u;                    // fp16 B tiles: N rows x 64 halves (one 128-byte swizzle atom)
   c->off_blo = o; o += N * 128u;
-  c->off_x = o; o += 2u * 2u * TBM * XP * 4u;       // 2 warpgroups x 2 stages of fp32 X tiles
   c->off_sum = o; if (mstep) o += (N + 2u) * 64u * 4u;   // per-CTA sums [N][64] + 2 spare rows
   c->off_cn = o; o += N * 4u;
   c->off_cnt = o; o += N * 4u;
   c->off_lab = o; o += 2u * TBM * 4u;
   c->off_dp = o; o += 2u * 2u * TBM * 4u;
-  c->off_red = o; o += TC_THREADS * 8u;
   c->off_cls = o; if (mstep) o += TC_THREADS / 32u * TBM * 4u;   // per-warp class lists of the M-step
-  c->total = o;
-  return o <= 227u * 1024u;
+  return o;
+}
+// The X ring fills what is left of the 227 KB from offset o: S = as many 16 KB slots as fit (at most TC_MAX_STAGES).
+// Without the M-step turns nothing orders the two warpgroups, so S is rounded down to even there: each slot is then
+// filled and read by one warpgroup only (see the wait in tc_chunk_kernel)
+static bool place_ring(TcCfg* c, uint32_t o, bool mstep) {
+  const uint32_t cap = 227u * 1024u;
+  c->off_bar = o; o += TC_MAX_STAGES * 8u;           // one "full" mbarrier per slot
+  o = (o + 1023u) & ~1023u;                          // the swizzle pattern repeats every 1024 bytes
+  c->off_ring = o;
+  c->S = o < cap ? (int)min((uint32_t)TC_MAX_STAGES, (cap - o) / XSLOT_BYTES) : 0;
+  if (!mstep) c->S &= ~1;
+  c->total = o + (uint32_t)c->S * XSLOT_BYTES;
+  static_assert(TC_THREADS * 8u <= XSLOT_BYTES, "the teardown's reduction array lives in the first slot");
+  return c->S >= TC_MIN_STAGES;
 }
 
+static bool make_cfg(int d, int k, bool mstep, TcCfg* c) { return place_ring(c, layout_common(d, k, mstep, c), mstep); }
+
 static bool make_cfg_nys(int d, int k, int epi, int kw, TcCfgNys* c) {
-  make_cfg(d, k, false, c);
-  const uint32_t N = (uint32_t)wg::mma_n(c->NP);
-  uint32_t o = c->total;
+  const uint32_t N = (uint32_t)wg::mma_n((k + 15) / 16 * 16);
+  uint32_t o = layout_common(d, k, false, c);
   c->off_cs = o; if (epi == EPI_COLSUM) o += 2u * 4u * N * 4u;     // per-warp column sums of a tile
   c->kw = kw;
   c->wp = (kw + 7) / 8 * 8 + 4;                     // 4 mod 8 floats: the quad's 4 W rows of a float4 load hit 4 bank groups
   c->w = nullptr;
   c->off_w = o; if (epi == EPI_EMBED) o += N * (uint32_t)c->wp * 4u;   // (every offset above is a multiple of 16)
-  c->total = o;
-  return o <= 227u * 1024u;
+  return place_ring(c, o, false);
+}
+
+// Tensor map of the chunk for the ring's TMA fills: fp32 (d, n) with row pitch ldx, boxes of 32 columns x 64 rows,
+// SWIZZLE_128B; the copy engine zero-fills what lies beyond d or n.  The encoder is the driver's, reached through the
+// runtime (the library links cudart statically and no driver library).
+static int encode_x_map(const ChunkArgs& a, CUtensorMap* m) {
+  static PFN_cuTensorMapEncodeTiled_v12000 encode = nullptr;
+  if (!encode) {
+    void* fn = nullptr;
+    cudaDriverEntryPointQueryResult q;
+    BKM_CUDA_TRY(cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &q));
+    if (q != cudaDriverEntryPointSuccess || !fn) return BKM_EUNSUPPORTED;
+    encode = reinterpret_cast<PFN_cuTensorMapEncodeTiled_v12000>(fn);
+  }
+  const cuuint64_t dims[2] = {(cuuint64_t)a.d, (cuuint64_t)(a.n > 0 ? a.n : 1)};
+  const cuuint64_t strides[1] = {(cuuint64_t)a.ldx * 4u};
+  const cuuint32_t box[2] = {32u, (cuuint32_t)TBM}, estr[2] = {1u, 1u};
+  const CUresult r = encode(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<void*>(a.X), dims, strides, box, estr,
+                            CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                            CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  return r == CUDA_SUCCESS ? 0 : BKM_EUNSUPPORTED;
 }
 
 template <int N, int KS, bool M, bool W, int XF>
 static int launch_variant(const ChunkArgs& a, const typename TcCfgOf<XF>::type& cfg, int grid, cudaStream_t s) {
+  CUtensorMap xmap;
+  if (const int rc = encode_x_map(a, &xmap)) return rc;
   auto kern = tc_chunk_kernel<N, KS, M, W, XF>;
   BKM_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cfg.total));
-  kern<<<grid, TC_THREADS, cfg.total, s>>>(a, cfg);
+  kern<<<grid, TC_THREADS, cfg.total, s>>>(a, cfg, xmap);
   return 0;
 }
 template <int N, bool M, bool W, int XF>
