@@ -1,23 +1,27 @@
-// bkm_stream.cu — bandwidth-class fused E+M chunk kernel for tiny k*d (fp32, d <= 16, k <= 32): BASELINE config C4
+// bkm_stream.cu — bandwidth-class fused E+M chunk kernels for tiny k*d (fp32, d <= 16, k <= 32): BASELINE config C4
 // (120M x 13, k = 20; benchmarks/kmeans_airline.py shape) and the small plumbing shapes.
+// Two kernels (launch_stream picks one): stream2_chunk_kernel, two rows per thread, serves k <= 24 at a row pitch of
+// at most 32 floats (C4); stream_chunk_kernel, one row per thread, serves k = 25..32 and pitches of 33..64 floats.
 //
-// The shape is HBM-bound (52..64 B per row, 2*d*k = 520 flops): the kernel is organised around the row stream.
-//   * every WARP owns a private ring of SNSTG stages of 32 rows and keeps it full with 1-D bulk async copies
+// The shape is HBM-bound (52..64 B per row, 2*d*k = 520 flops): both kernels are organised around the row stream.
+//   * every WARP owns a private ring of bulk-copied row tiles and keeps it full with 1-D bulk async copies
 //     (cp.async.bulk global -> shared, completion on a per-stage mbarrier, issued by lane 0): no CTA-wide barrier in
 //     the main loop, HBM requests stay in flight while the warp computes;
-//   * E-step (sklearn pairwise_distances_argmin_min per chunk, dask_ml/metrics/pairwise.py:35-38): thread = row, the row
-//     in registers, centres in shared memory as PAIRS {-2 c_2p, -2 c_2p+1} per feature so that one 64-bit load feeds
-//     two distances (ptx::ffma2: two FFMA on sm_90); all k distances stay in registers, the arg-min and the near-tie test are
-//     decoded from one FSET+FFMA per distance (same scheme as the tensor-path epilogue);
 //   * rows whose best/second margin is inside the fp32 rounding bound are re-decided by the SAME thread in float64
 //     against the float64 centres (rare: the warp diverges for them only);
+//   * the arg-min and the near-tie test are decoded from one FSET+FFMA per distance (same scheme as the tensor-path
+//     epilogue); partial sums are combined in a fixed order -> reduce_partials (float64, CTA order).
+// One row per thread (below): SNSTG stages of 32 rows per warp.
+//   * E-step (sklearn pairwise_distances_argmin_min per chunk, dask_ml/metrics/pairwise.py:35-38): thread = row, the row
+//     in registers, centres in shared memory as PAIRS {-2 c_2p, -2 c_2p+1} per feature so that one 64-bit load feeds
+//     two distances (ptx::ffma2: two FFMA on sm_90); all k distances stay in registers;
 //   * M-step (_centers_dense, dask_ml/cluster/k_means.py:572-582): lane j owns cluster j and adds the rows of its
 //     warp's tile that carry label j into register-resident sums (k ballots per tile, no atomics, fixed order);
-//     per-warp sums are folded in warp order into the CTA's partial at the end -> reduce_partials (float64, CTA order).
+//     per-warp sums are folded in warp order into the CTA's partial at the end.
+// Two rows per thread: see the section further down.
 #include "bkm_common.cuh"
 #include "bkm_ptx.cuh"
 #include <math_constants.h>
-#include <stdlib.h>
 
 namespace bkm {
 
@@ -766,7 +770,7 @@ static int launch_stream_d(const ChunkArgs& a, bool mstep, int sm_count, int* gr
 int launch_stream(const ChunkArgs& a, bool mstep, int sm_count, int* grid_out, cudaStream_t s) {
   if (!stream_supported(a.d, a.k, BKM_F32)) return BKM_EUNSUPPORTED;
   if ((reinterpret_cast<uintptr_t>(a.X) & 15) || a.ldx > 64) return BKM_EALIGN;
-  if (a.k <= 24 && a.ldx <= 32 && !getenv("BKM_STREAM_V1")) {        // two rows per thread
+  if (a.k <= 24 && a.ldx <= 32) {        // two rows per thread
     if (a.d <= 4) return launch_stream2_d<2>(a, mstep, sm_count, grid_out, s);
     if (a.d <= 8) return launch_stream2_d<4>(a, mstep, sm_count, grid_out, s);
     if (a.d <= 12) return launch_stream2_d<6>(a, mstep, sm_count, grid_out, s);

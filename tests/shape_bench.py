@@ -25,6 +25,12 @@ SHAPES = {
     "C2": ("C2 10M x 64 f32 k=256", 10_000_000, 64, 256, torch.float32, 0),
     "C2simt": ("C2 on the generic CUDA-core kernel (FORCE_SIMT) 2M x 64 f32 k=256", 2_000_000, 64, 256, torch.float32, 1),
     "C4simt": ("C4 on the generic CUDA-core kernel (FORCE_SIMT)", 15_000_000, 13, 20, torch.float32, 1),
+    # family 2 with k = 25..32, which runs on the one-row-per-thread streaming kernel (k <= 24: two rows per thread)
+    "F2d15k32": ("family 2, 15M x 15 f32 k=32", 15_000_000, 15, 32, torch.float32, 0),
+    "F2d16k28": ("family 2, 15M x 16 f32 k=28", 15_000_000, 16, 28, torch.float32, 0),
+    "F2d12k32": ("family 2, 15M x 12 f32 k=32", 15_000_000, 12, 32, torch.float32, 0),
+    "F2d8k32": ("family 2, 15M x 8 f32 k=32", 15_000_000, 8, 32, torch.float32, 0),
+    "F2d4k30": ("family 2, 15M x 4 f32 k=30", 15_000_000, 4, 30, torch.float32, 0),
 }
 args = [a for a in sys.argv[1:] if not a.startswith("--")]
 steps = 10

@@ -335,13 +335,16 @@ def test_tcgen05_odd_feature_counts(be, oracle, n, d, k):
 # ------------------------------------------------------------------------------------------ streaming kernel (family 2)
 @pytest.mark.parametrize("n", [1, 31, 32, 33, 255, 256, 257, 4097, 148 * 8 * 32 * 3 + 5, 1_000_003])
 @pytest.mark.parametrize("d,k,pitch", [(13, 20, 13), (13, 20, 16), (13, 20, 14), (16, 31, 16), (1, 2, 1), (3, 5, 3),
-                                       (7, 1, 7), (9, 31, 12), (5, 8, 24)])
+                                       (7, 1, 7), (9, 31, 12), (5, 8, 24), (16, 28, 16), (14, 32, 14), (4, 30, 4),
+                                       (5, 8, 40)])
 def test_stream_kernel_tails(be, n, d, k, pitch):
     """Family 2 (bkm_stream.cu): every tail of the per-warp ring (fewer tiles than warps, a partial last tile, rows with
-    and without a padded pitch), all entry points, against the float64 arg-min evaluated on the device."""
+    and without a padded pitch), all entry points, against the float64 arg-min evaluated on the device.  Every call runs
+    on a streaming kernel, none on the generic fallback."""
     import torch
 
     assert be.kernel_family(d, k, torch.float32) == 2
+    fallbacks = int(be.lib.bkm_debug_fallback_count())
     g = torch.Generator(device=be.device).manual_seed(n * 31 + d * 7 + k)
     cent = torch.empty((max(2, k // 2), d), device=be.device).uniform_(-10, 10, generator=g)
     Xc = cent[torch.randint(0, cent.shape[0], (n,), device=be.device, generator=g)] + \
@@ -391,6 +394,7 @@ def test_stream_kernel_tails(be, n, d, k, pitch):
     torch.cuda.synchronize()
     assert torch.equal(lab3, labels) and torch.equal(counts2, counts)
     assert torch.equal(sums2, sums)            # bit-reproducible: fixed CTA / warp order
+    assert int(be.lib.bkm_debug_fallback_count()) == fallbacks
 
 
 def test_stream_kernel_matches_generic_kernel(be):
