@@ -248,6 +248,7 @@ int bkm_transform_chunk(const void* X, int64_t n, int d, int64_t ldx, int x_dtyp
                         const void* pack, int k, void* out, int64_t ld_out, int mode, double gamma, int flags,
                         void* stream) {
   if (n < 0 || d <= 0 || k <= 0 || ldx < d || !pack || ld_out < k || mode < 0 || mode > 2) return BKM_EINVAL;
+  if (n > 0x7fffffffLL) return BKM_EUNSUPPORTED;      // TMA row coordinates of the tensor path are 32-bit
   if (x_dtype != BKM_F32 && x_dtype != BKM_F64) return BKM_EDTYPE;
   if (n == 0) return 0;
   if (!X || !out) return BKM_EINVAL;
@@ -265,6 +266,7 @@ int bkm_transform_chunk(const void* X, int64_t n, int d, int64_t ldx, int x_dtyp
     rc = launch_tc_transform(a, sm, (cudaStream_t)stream);
     if (rc != BKM_EALIGN && rc != BKM_EUNSUPPORTED) return rc;
     if (flags & BKM_FLAG_FORCE_TC) return rc;
+    if (rc == BKM_EALIGN) g_fallbacks.fetch_add(1, std::memory_order_relaxed);
   } else if (flags & BKM_FLAG_FORCE_TC) return BKM_EUNSUPPORTED;
   return launch_transform(X, n, d, ldx, x_dtype, pack, k, out, ld_out, mode, gamma, sm, (cudaStream_t)stream);
 }
@@ -285,6 +287,7 @@ int bkm_kernel_colsum_chunk(const void* X, int64_t n, int d, int64_t ldx, int x_
                             double gamma, double* colsum, void* workspace, size_t workspace_bytes, int flags,
                             void* stream) {
   if (n < 0 || d <= 0 || l <= 0 || ldx < d || !pack || !colsum || !workspace) return BKM_EINVAL;
+  if (n > 0x7fffffffLL) return BKM_EUNSUPPORTED;      // TMA row coordinates of the tensor path are 32-bit
   if (x_dtype != BKM_F32 && x_dtype != BKM_F64) return BKM_EDTYPE;
   if (n > 0 && !X) return BKM_EINVAL;
   cudaStream_t s = (cudaStream_t)stream;
@@ -310,6 +313,7 @@ int bkm_kernel_colsum_chunk(const void* X, int64_t n, int d, int64_t ldx, int x_
     rc = launch_tc_colsum(nystrom_args(X, n, d, ldx, pack, l, gamma), part, part_bytes, sm, &parts, s);
     if (rc != 0 && (flags & BKM_FLAG_FORCE_TC)) return rc;
     if (rc != 0 && rc != BKM_EALIGN) return rc;
+    if (rc == BKM_EALIGN) g_fallbacks.fetch_add(1, std::memory_order_relaxed);
   } else if (flags & BKM_FLAG_FORCE_TC) return BKM_EUNSUPPORTED;
   if (rc != 0) {
     rc = launch_nystrom(X, n, d, ldx, x_dtype, pack, l, gamma, 0, nullptr, 0, nullptr, 0, part, part_bytes, sm, &parts, s);
@@ -321,6 +325,7 @@ int bkm_kernel_colsum_chunk(const void* X, int64_t n, int d, int64_t ldx, int x_
 int bkm_nystrom_embed_chunk(const void* X, int64_t n, int d, int64_t ldx, int x_dtype, const void* pack, int l,
                             double gamma, const void* W, int k, void* out, int64_t ld_out, int flags, void* stream) {
   if (n < 0 || d <= 0 || l <= 0 || k <= 0 || ldx < d || ld_out < k || !pack || !W) return BKM_EINVAL;
+  if (n > 0x7fffffffLL) return BKM_EUNSUPPORTED;      // TMA row coordinates of the tensor path are 32-bit
   if (x_dtype != BKM_F32 && x_dtype != BKM_F64) return BKM_EDTYPE;
   if (n == 0) return 0;
   if (!X || !out) return BKM_EINVAL;
@@ -333,6 +338,7 @@ int bkm_nystrom_embed_chunk(const void* X, int64_t n, int d, int64_t ldx, int x_
     a.xf_out = (float*)out; a.xf_ld = ld_out;
     rc = launch_tc_embed(a, (const float*)W, k, sm, s);
     if (rc != BKM_EALIGN || (flags & BKM_FLAG_FORCE_TC)) return rc;
+    g_fallbacks.fetch_add(1, std::memory_order_relaxed);
   } else if (flags & BKM_FLAG_FORCE_TC) return BKM_EUNSUPPORTED;
   int parts = 0;
   return launch_nystrom(X, n, d, ldx, x_dtype, pack, l, gamma, 1, W, k, out, ld_out, nullptr, 0, sm, &parts, s);

@@ -877,3 +877,21 @@ int launch_tc_embed(const ChunkArgs& a, const float* W, int kw, int sm_count, cu
 }
 
 }  // namespace bkm
+
+// The variant of tc_chunk_kernel a call would run, from the same configuration functions the launches use
+extern "C" int bkm_debug_tc_layout(int d, int k, int epi, int mstep, int kw, int* out4) {
+  using namespace bkm;
+  if (!out4 || epi < EPI_ARGMIN || epi > EPI_EMBED || (mstep && epi != EPI_ARGMIN)) return BKM_EINVAL;
+  if (!tc_supported(d, k, BKM_F32)) return BKM_EUNSUPPORTED;
+  TcCfgNys c;
+  bool ok;
+  if (epi == EPI_ARGMIN || epi == EPI_XFORM) ok = make_cfg(d, k, mstep != 0, &c);
+  else if (epi == EPI_COLSUM) ok = make_cfg_nys(d, k, EPI_COLSUM, 0, &c);
+  else ok = kw >= 1 && kw <= TC_EMBED_MAXK && make_cfg_nys(d, k, EPI_EMBED, kw, &c);
+  if (!ok) return BKM_EUNSUPPORTED;
+  out4[0] = c.KS;
+  out4[1] = wg::mma_n(c.NP);
+  out4[2] = c.S;
+  out4[3] = (int)c.total;
+  return 0;
+}

@@ -423,6 +423,7 @@ class CudaBackend(object):
                 self._ptr(x), n, d, x.stride(0) if n else d, _DT_CODE[x.dtype], self._ptr(pack), k,
                 self._ptr(out), out.stride(0) if n else k, int(mode), float(gamma), self.flags, self._stream()),
                 "bkm_transform_chunk")
+        self._note_fallback(x)
 
     def kernel_colsum(self, x, pack, l, gamma, colsum, first=False):
         """colsum[j] (+)= sum_i exp(-gamma ||x_i - c_j||^2) over the rows of the chunk (float64 [l]); ``first`` overwrites.
@@ -434,6 +435,7 @@ class CudaBackend(object):
             _lib.check(self.lib.bkm_kernel_colsum_chunk(
                 self._ptr(x), n, d, x.stride(0) if n else d, _DT_CODE[x.dtype], self._ptr(pack), int(l), float(gamma),
                 self._ptr(colsum), self._ptr(ws), ws.numel(), flags, self._stream()), "bkm_kernel_colsum_chunk")
+        self._note_fallback(x)
 
     def gram_chunk(self, x, shift, colsum, gram, first=False):
         """colsum (+)= sum_i (x_i - shift) and gram (+)= sum_i (x_i - shift)(x_i - shift)^T over the rows of the chunk
@@ -1131,6 +1133,7 @@ class CudaBackend(object):
                 self._ptr(x), n, d, x.stride(0) if n else d, _DT_CODE[x.dtype], self._ptr(pack), int(l), float(gamma),
                 self._ptr(W), k, self._ptr(out), out.stride(0) if n else k, self.flags, self._stream()),
                 "bkm_nystrom_embed_chunk")
+        self._note_fallback(x)
 
     def finalize(self, sums, counts, C_old, C_new, shift):
         k, d = C_old.shape

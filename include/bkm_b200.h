@@ -112,8 +112,9 @@ extern "C" {
  * 8 = bkm_csr_kernel_colsum_workspace_bytes, bkm_csr_kernel_colsum_chunk, bkm_csr_nystrom_embed_chunk,
  *     bkm_sparse_minibatch_step
  * 9 = bkm_sgd_order, bkm_sgd_block, bkm_sgd_csr_block
- * 10 = bkm_class_counts_chunk, bkm_csc_class_counts_chunk, bkm_nb_linear_jll_chunk, bkm_nb_csr_jll_chunk */
-#define BKM_VERSION_MINOR 10
+ * 10 = bkm_class_counts_chunk, bkm_csc_class_counts_chunk, bkm_nb_linear_jll_chunk, bkm_nb_csr_jll_chunk
+ * 11 = bkm_debug_tc_layout */
+#define BKM_VERSION_MINOR 11
 
 /* element types of X */
 #define BKM_F32 0
@@ -915,9 +916,9 @@ int bkm_allreduce_p2p(double* buf, int64_t n, void* const* mailboxes_dev, int ra
 
 /* Number of kernel launches this library has enqueued since load (for bench accounting). */
 int64_t bkm_launch_count(void);
-/* Number of chunk calls whose shape belongs to the tensor-core / streaming family but whose rows were not 16-byte aligned
- * (base or pitch), so that the generic CUDA-core kernel ran instead: correct, several times slower.  The Python host
- * warns once when this moves. */
+/* Number of chunk calls (bkm_lloyd_chunk, bkm_assign_chunk, bkm_transform_chunk and the two Nystrom passes) whose shape
+ * belongs to the tensor-core / streaming family but whose rows were not 16-byte aligned (base or pitch), so that a
+ * CUDA-core kernel ran instead: correct, several times slower.  The Python host warns once when this moves. */
 int64_t bkm_debug_fallback_count(void);
 
 /* Debug: nonzero once a pipeline wait inside a tensor-core kernel has timed out (the kernel then drains
@@ -932,6 +933,11 @@ void bkm_debug_reset(void);
 int bkm_debug_deferred_rows(const void* workspace, int64_t n, int d, int k, int x_dtype, int* count_host);
 /* Pipeline timeline of the tensor-core kernel: not recorded by the sm_90a kernels; returns 0 (kept for ABI stability) */
 int bkm_debug_trace(long long* out_host, int n);
+/* The variant of the fp32 tensor-core chunk kernel (d <= 64, k <= 256) that a call would run, from the configuration
+ * its launch uses: out4 = {KS (K-steps of 16 features), N (MMA width), S (slots of its X ring), dynamic shared-memory
+ * bytes}.  epi: 0 = arg-min (Lloyd / assign; mstep = 1 for the Lloyd call), 1 = transform, 2 = Nystrom column sums,
+ * 3 = Nystrom embedding with kw outputs (1..64).  Host only, no device call; BKM_EUNSUPPORTED where no variant runs. */
+int bkm_debug_tc_layout(int d, int k, int epi, int mstep, int kw, int* out4);
 
 #ifdef __cplusplus
 }

@@ -1,5 +1,25 @@
 """Helpers shared by the parity tests."""
+import ctypes
+
 import numpy as np
+
+TC_ARGMIN, TC_XFORM, TC_COLSUM, TC_EMBED = 0, 1, 2, 3      # the epilogues of the fp32 tensor-core kernel (bkm_tc.cu)
+
+
+def tc_layout(lib, d, k, epi, mstep=0, kw=0):
+    """(KS, N, S, shared-memory bytes) of the fp32 tensor-core kernel variant that runs a (d, k) call of epilogue
+    ``epi``: S slots of its X ring, each refilled once the tile it holds is done."""
+    out = (ctypes.c_int * 4)()
+    rc = lib.bkm_debug_tc_layout(int(d), int(k), int(epi), int(mstep), int(kw), out)
+    assert rc == 0, rc
+    return tuple(out)
+
+
+def sm_count(lib, device=0):
+    """The device's SM count: the tensor-core kernel's grid (one CTA per SM, tiles dealt round-robin)."""
+    v = ctypes.c_int(0)
+    assert lib.bkm_device_info(int(device), ctypes.byref(v), None, None) == 0
+    return int(v.value)
 
 
 def d2_f64(X, C):

@@ -2,7 +2,7 @@
 import numpy as np
 import pytest
 
-from _util import assert_labels_match
+from _util import TC_ARGMIN, assert_labels_match, sm_count, tc_layout
 
 pytestmark = pytest.mark.gpu
 
@@ -201,15 +201,20 @@ def _exact_labels_f64(x, C):
     return out, second
 
 
-# Pipeline stress of the tensor-core kernels: row counts that leave every kind of tail (fewer tiles than SMs, one
-# tile more on some SMs, a partial last tile), both kernel variants (pure Lloyd = lane-owns-cluster M-step with
-# the whole-tile M ring; with distances = quarter-tile ring), one and two accumulator units.
-@pytest.mark.parametrize("n", [1, 127, 128, 129, 148 * 128 - 1, 148 * 128 * 3 + 77, 200_000, 1_000_003])
+# Pipeline stress of the tensor-core kernel: row counts that leave every kind of tail (fewer tiles than SMs, a partial
+# last tile, three passes of every CTA's X ring and one more tile on two CTAs, the second partial; G SMs, 64-row tiles,
+# S ring slots), the Lloyd variants with and without distances, N = 16, 128 and 256 (N = 256: an odd ring of 5).
+TAIL_ROWS = {"64G-1": lambda G, S: 64 * G - 1, "64G*3S+77": lambda G, S: 64 * G * 3 * S + 77}
+
+
+@pytest.mark.parametrize("n", [1, 127, 128, 129, "64G-1", "64G*3S+77", 200_000, 1_000_003])
 @pytest.mark.parametrize("d,k", [(64, 256), (64, 100), (32, 130), (8, 16)])
 @pytest.mark.parametrize("want_dist", [False, True])
-def test_tcgen05_pipeline_tails(be, n, d, k, want_dist):
+def test_pipeline_tails(be, n, d, k, want_dist):
     import torch
 
+    if n in TAIL_ROWS:
+        n = TAIL_ROWS[n](sm_count(be.lib, be.device.index or 0), tc_layout(be.lib, d, k, TC_ARGMIN, mstep=1)[2])
     be.flags = 2          # FORCE_TC: also the shapes the dispatcher would leave to the CUDA cores (k d < 512)
     g = torch.Generator(device=be.device).manual_seed(n + d + k)
     cent = torch.empty((max(2, k // 2), d), device=be.device).uniform_(-10, 10, generator=g)
