@@ -248,3 +248,10 @@ def check(rc, what):
     if rc != 0:
         msg = load().bkm_error_string(rc)
         raise RuntimeError("%s failed: %s (code %d)" % (what, msg.decode() if msg else "?", rc))
+
+
+def call(name, *args):
+    """Call the entry point ``name``; raise with its name and the library's message on a non-zero status."""
+    rc = getattr(_lib or load(), name)(*args)
+    if rc:
+        check(rc, name)

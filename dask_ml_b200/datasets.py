@@ -88,12 +88,9 @@ def make_blobs(n_samples=100, n_features=2, centers=None, cluster_std=1.0, cente
             ys.append(yb.astype(np.int64))
         return ChunkedArray(Xs), ChunkedArray(ys)
 
-    import ctypes
-
     import torch
 
-    from . import _lib
-    from .engine import CudaBackend, _DT_CODE
+    from .engine import CudaBackend
 
     be = CudaBackend(torch.device(device) if not isinstance(device, torch.device) else device)
     tdt = torch.float64 if dtype is None else {np.dtype("float32"): torch.float32, np.dtype("float64"): torch.float64}[np.dtype(dtype)]
@@ -102,16 +99,12 @@ def make_blobs(n_samples=100, n_features=2, centers=None, cluster_std=1.0, cente
     Cd = torch.as_tensor(centers).to(be.device)
     Sd = torch.as_tensor(std).to(be.device)
     Xs, ys = [], []
-    with torch.cuda.device(be.device):
-        for i, m in enumerate(sizes):
-            Xb = torch.empty((m, int(n_features)), dtype=tdt, device=be.device)
-            yb = torch.empty((m,), dtype=torch.int64, device=be.device)
-            _lib.check(be.lib.bkm_make_blobs_chunk(
-                ctypes.c_void_p(Xb.data_ptr()), ctypes.c_void_p(yb.data_ptr()), m, int(n_features), int(n_features),
-                _DT_CODE[tdt], ctypes.c_void_p(Cd.data_ptr()), ctypes.c_void_p(Sd.data_ptr()), k, i,
-                ctypes.c_void_p(torch.cuda.current_stream(be.device).cuda_stream)), "bkm_make_blobs_chunk")
-            Xs.append(Xb)
-            ys.append(yb)
+    for i, m in enumerate(sizes):
+        Xb = torch.empty((m, int(n_features)), dtype=tdt, device=be.device)
+        yb = torch.empty((m,), dtype=torch.int64, device=be.device)
+        be.make_blobs_chunk(Xb, yb, Cd, Sd, i)
+        Xs.append(Xb)
+        ys.append(yb)
     return ChunkedArray(Xs), ChunkedArray(ys)
 
 
@@ -352,33 +345,25 @@ def _generate(sizes, d, dtype, family, info, key, device, n_targets=1, bias=0.0,
             ys.append(_response_host(Xb, family, info, key, row0, n_targets, bias, noise))
             row0 += m
     else:
-        import ctypes
-
         import torch
 
-        from . import _lib
-        from .engine import CudaBackend, _DT_CODE
+        from .engine import CudaBackend
 
         be = CudaBackend(torch.device(device) if not isinstance(device, torch.device) else device)
         tdt = torch.float32 if dt == np.dtype(np.float32) else torch.float64
         ydt = torch.float64 if family == _NORMAL else torch.int64
         Xs, ys, row0 = [], [], 0
-        with torch.cuda.device(be.device):
-            info_d = torch.as_tensor(np.ascontiguousarray(info, dtype=np.float64)).to(be.device)
-            flag = torch.zeros(1, dtype=torch.int32, device=be.device)
-            stream = ctypes.c_void_p(torch.cuda.current_stream(be.device).cuda_stream)
-            for m in sizes:
-                Xb = torch.empty((m, d), dtype=tdt, device=be.device)
-                yb = torch.empty((m, n_targets) if family == _NORMAL else (m,), dtype=ydt, device=be.device)
-                _lib.check(be.lib.bkm_make_glm_chunk(
-                    ctypes.c_void_p(Xb.data_ptr()), ctypes.c_void_p(yb.data_ptr()), m, d, d, _DT_CODE[tdt], row0,
-                    family, ctypes.c_void_p(info_d.data_ptr()), int(info.shape[0]), n_targets, float(bias),
-                    float(noise), key, ctypes.c_void_p(flag.data_ptr()), stream), "bkm_make_glm_chunk")
-                Xs.append(Xb)
-                ys.append(yb)
-                row0 += m
-            if family == _POISSON and int(flag.item()):
-                raise ValueError("lam value too large")
+        info_d = torch.as_tensor(np.ascontiguousarray(info, dtype=np.float64)).to(be.device)
+        flag = torch.zeros(1, dtype=torch.int32, device=be.device)
+        for m in sizes:
+            Xb = torch.empty((m, d), dtype=tdt, device=be.device)
+            yb = torch.empty((m, n_targets) if family == _NORMAL else (m,), dtype=ydt, device=be.device)
+            be.make_glm_chunk(Xb, yb, row0, family, info_d, n_targets, bias, noise, key, flag)
+            Xs.append(Xb)
+            ys.append(yb)
+            row0 += m
+        if family == _POISSON and int(flag.item()):
+            raise ValueError("lam value too large")
     if family == _NORMAL and n_targets == 1:
         ys = [yb.reshape(-1) for yb in ys]
     return ChunkedArray(Xs), ChunkedArray(ys)
@@ -393,20 +378,13 @@ def _normal_panel(key, m, d, device):
     device = torch.device(device)
     if device.type != "cuda":
         return torch.from_numpy(_x_block(key, 0, m, d, np.float64))
-    import ctypes
-
-    from . import _lib
     from .engine import CudaBackend
 
     be = CudaBackend(device)
     X = torch.empty((m, d), dtype=torch.float64, device=device)
     y = torch.empty((m,), dtype=torch.int64, device=device)       # the (unused) logistic response of the same call
     if m:
-        with torch.cuda.device(device):
-            _lib.check(be.lib.bkm_make_glm_chunk(
-                ctypes.c_void_p(X.data_ptr()), ctypes.c_void_p(y.data_ptr()), m, d, d, _lib.BKM_F64, 0, _LOGISTIC,
-                None, 0, 1, 0.0, 0.0, key, None, ctypes.c_void_p(torch.cuda.current_stream(device).cuda_stream)),
-                "bkm_make_glm_chunk")
+        be.make_glm_chunk(X, y, 0, _LOGISTIC, None, 1, 0.0, 0.0, key)
     return X
 
 

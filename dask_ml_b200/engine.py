@@ -115,10 +115,10 @@ class _P2PAllReduce(object):
             try:
                 with torch.cuda.device(device):
                     nb = ctypes.c_size_t(0)
-                    _lib.check(self.lib.bkm_p2p_mailbox_bytes(self.world, self.max_elems, ctypes.byref(nb)), "bkm_p2p_mailbox_bytes")
-                    _lib.check(self.lib.bkm_p2p_alloc(nb, ctypes.byref(self.box)), "bkm_p2p_alloc")
+                    _lib.call("bkm_p2p_mailbox_bytes", self.world, self.max_elems, ctypes.byref(nb))
+                    _lib.call("bkm_p2p_alloc", nb, ctypes.byref(self.box))
                     buf = ctypes.create_string_buffer(64)
-                    _lib.check(self.lib.bkm_p2p_export(self.box, buf), "bkm_p2p_export")
+                    _lib.call("bkm_p2p_export", self.box, buf)
                     handle = bytes(buf.raw)
             except Exception:
                 handle = None
@@ -133,7 +133,7 @@ class _P2PAllReduce(object):
                             ptrs.append(int(self.box.value))
                         else:
                             pp = ctypes.c_void_p(0)
-                            _lib.check(self.lib.bkm_p2p_import(ctypes.create_string_buffer(h, 64), ctypes.byref(pp)), "bkm_p2p_import")
+                            _lib.call("bkm_p2p_import", ctypes.create_string_buffer(h, 64), ctypes.byref(pp))
                             self.peers.append(pp)
                             ptrs.append(int(pp.value))
             except Exception:
@@ -148,10 +148,10 @@ class _P2PAllReduce(object):
     def allreduce_(self, t):
         self.seq += 1
         with torch.cuda.device(self.device):
-            _lib.check(self.lib.bkm_allreduce_p2p(
-                ctypes.c_void_p(t.data_ptr()), t.numel(), ctypes.c_void_p(self.table.data_ptr()), self.rank, self.world,
-                self.max_elems, ctypes.c_uint(self.seq & 0xFFFFFFFF),
-                ctypes.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)), "bkm_allreduce_p2p")
+            _lib.call("bkm_allreduce_p2p", ctypes.c_void_p(t.data_ptr()), t.numel(),
+                      ctypes.c_void_p(self.table.data_ptr()), self.rank, self.world, self.max_elems,
+                      ctypes.c_uint(self.seq & 0xFFFFFFFF),
+                      ctypes.c_void_p(torch.cuda.current_stream(self.device).cuda_stream))
 
     def close(self):
         try:
@@ -204,23 +204,69 @@ class CudaBackend(object):
         self._ws = {}
 
     # -- helpers -------------------------------------------------------------------------
+    # Pointers go to the library as plain addresses (None for NULL): the prototypes' c_void_p argtypes convert them,
+    # and a c_void_p object per argument would only add to the host cost of every call.
     def _stream(self):
-        return ctypes.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
+        return torch.cuda.current_stream(self.device).cuda_stream
 
     @staticmethod
     def _ptr(t):
-        return ctypes.c_void_p(t.data_ptr()) if t is not None else ctypes.c_void_p(0)
+        return t.data_ptr() if t is not None else None
+
+    def _call(self, name, *args):
+        """Run the library entry point ``name`` on this backend's device, with the current stream as last argument."""
+        with torch.cuda.device(self.device):
+            _lib.call(name, *args, self._stream())
+
+    @staticmethod
+    def _query(name, *args, outs=1):
+        """The size in bytes a ``*_bytes`` entry point writes through its last argument (a tuple of the ``outs`` sizes
+        of an entry point with several)."""
+        if outs == 1:
+            nb = ctypes.c_size_t(0)
+            _lib.call(name, *args, ctypes.byref(nb))
+            return nb.value
+        nbs = [ctypes.c_size_t(0) for _ in range(outs)]
+        _lib.call(name, *args, *[ctypes.byref(nb) for nb in nbs])
+        return tuple(nb.value for nb in nbs)
+
+    def _rows(self, x, codes=_DT_CODE):
+        """(pointer, n, d, row pitch, element type) of a dense (n, d) block."""
+        n, d = x.shape
+        return x.data_ptr(), n, d, x.stride(0) if n else d, codes[x.dtype]
+
+    def _csr(self, blk, d):
+        """(crow, col, val, value type, n, d, nnz) of a CSR block ``blk`` = (crow, col, val, n) of d columns."""
+        crow, col, val, n = blk
+        return self._ptr(crow), self._ptr(col), self._ptr(val), _DT_CODE[val.dtype], int(n), int(d), int(col.numel())
+
+    def _csc(self, csc, d):
+        """(colptr, rows, vals, value type, d, nnz, plan) of the transpose ``csc`` = (colptr, rows, vals, plan)."""
+        colptr, rows, vals, plan = csc
+        return (self._ptr(colptr), self._ptr(rows), self._ptr(vals), _DT_CODE[vals.dtype], int(d), int(rows.numel()),
+                self._ptr(plan))
+
+    @staticmethod
+    def _ld(out, n, width):
+        """Row pitch of an optional (n, width) output: its stride, or ``width`` when it is absent or has no rows."""
+        return (out.stride(0) if n else width) if out is not None else width
+
+    def _ws_args(self, ws):
+        """(pointer, bytes) of a workspace; (NULL, 0) for a mode that needs none."""
+        return (ws.data_ptr(), ws.numel()) if ws is not None else (None, 0)
+
+    def _first(self, first):
+        """The flag word of a pass that overwrites its accumulators on the ``first`` chunk."""
+        return self.flags | _lib.FLAG_FIRST_CHUNK if first else self.flags
 
     def _workspace(self, n, d, k, dtype):
         """Scratch for one chunk call (per-CTA partials + the deferred-row list, 4 bytes per row)."""
         # one grow-only buffer for every shape: the layout inside it is recomputed by the library per call, and
         # k-means|| changes k every round (a buffer per k would allocate ~100 MB per round and keep them all)
         ws = self._ws.get("buf")
-        nbytes = ctypes.c_size_t(0)
-        _lib.check(self.lib.bkm_workspace_bytes(int(n), d, k, _DT_CODE[dtype], ctypes.byref(nbytes)),
-                   "bkm_workspace_bytes")
-        if ws is None or ws.numel() < nbytes.value:
-            ws = torch.empty(int(nbytes.value * 1.25) + (1 << 20), dtype=torch.uint8, device=self.device)
+        nbytes = self._query("bkm_workspace_bytes", int(n), d, k, _DT_CODE[dtype])
+        if ws is None or ws.numel() < nbytes:
+            ws = torch.empty(int(nbytes * 1.25) + (1 << 20), dtype=torch.uint8, device=self.device)
             ws[:8192].zero_()        # the persistent header (balance table of the M-step row pass) starts out empty
             self._ws["buf"] = ws
         return ws
@@ -232,6 +278,10 @@ class CudaBackend(object):
             ws = torch.empty(max(int(nbytes), 256), dtype=torch.uint8, device=self.device)
             self._ws[key] = ws
         return ws
+
+    def _scratch_for(self, key, sizer, *args):
+        """``_scratch(key)`` of the size the entry point ``sizer`` reports for ``args``."""
+        return self._scratch(key, self._query(sizer, *args))
 
     def kernel_family(self, d, k, dtype):
         return self.lib.bkm_kernel_family(d, k, _DT_CODE[dtype], self.flags)
@@ -268,8 +318,7 @@ class CudaBackend(object):
         if ws is None:
             return None
         c = ctypes.c_int(0)
-        _lib.check(self.lib.bkm_debug_deferred_rows(self._ptr(ws), int(n), d, k, _DT_CODE[dtype], ctypes.byref(c)),
-                   "bkm_debug_deferred_rows")
+        _lib.call("bkm_debug_deferred_rows", self._ptr(ws), int(n), d, k, _DT_CODE[dtype], ctypes.byref(c))
         return int(c.value)
 
     # -- data ----------------------------------------------------------------------------
@@ -317,23 +366,17 @@ class CudaBackend(object):
     # -- kernels -------------------------------------------------------------------------
     def check_finite(self, chunks):
         flag = torch.zeros(1, dtype=torch.int32, device=self.device)
-        with torch.cuda.device(self.device):
-            for x in chunks:
-                n, d = x.shape
-                _lib.check(self.lib.bkm_check_finite(self._ptr(x), n, d, x.stride(0), _DT_CODE[x.dtype],
-                                                     self._ptr(flag), self._stream()), "bkm_check_finite")
+        for x in chunks:
+            n, d = x.shape
+            self._call("bkm_check_finite", self._ptr(x), n, d, x.stride(0), _DT_CODE[x.dtype], self._ptr(flag))
         return flag
 
     def pack_centers(self, C64, dtype, out=None):
         k, d = C64.shape
-        nbytes = ctypes.c_size_t(0)
-        _lib.check(self.lib.bkm_centers_pack_bytes(k, d, _DT_CODE[dtype], ctypes.byref(nbytes)),
-                   "bkm_centers_pack_bytes")
-        if out is None or out.numel() < nbytes.value:
-            out = torch.empty(nbytes.value, dtype=torch.uint8, device=self.device)
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.bkm_pack_centers(self._ptr(C64), k, d, _DT_CODE[dtype], self._ptr(out),
-                                                 out.numel(), self._stream()), "bkm_pack_centers")
+        nbytes = self._query("bkm_centers_pack_bytes", k, d, _DT_CODE[dtype])
+        if out is None or out.numel() < nbytes:
+            out = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
+        self._call("bkm_pack_centers", self._ptr(C64), k, d, _DT_CODE[dtype], self._ptr(out), out.numel())
         return out
 
     def lloyd_chunk(self, x, pack, k, labels, min_d2, sums, counts, inertia, first=False, loop_state=None):
@@ -342,29 +385,20 @@ class CudaBackend(object):
         the call a no-op once the device-side loop has converged."""
         n, d = x.shape
         ws = self._workspace(n, d, k, x.dtype)
-        flags = self.flags
-        if first:
-            flags |= _lib.FLAG_FIRST_CHUNK
+        flags = self._first(first)
         if counts is not None and counts.dtype == torch.float64:
             flags |= _lib.FLAG_COUNTS_F64
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.bkm_lloyd_chunk(
-                self._ptr(x), n, d, x.stride(0) if n else d, _DT_CODE[x.dtype], self._ptr(pack), k,
-                self._ptr(labels), self._ptr(min_d2), self._ptr(sums), self._ptr(counts),
-                self._ptr(inertia), self._ptr(ws), ws.numel(), flags, self._ptr(loop_state), self._stream()),
-                "bkm_lloyd_chunk")
+        self._call("bkm_lloyd_chunk", *self._rows(x), self._ptr(pack), k, self._ptr(labels), self._ptr(min_d2),
+                   self._ptr(sums), self._ptr(counts), self._ptr(inertia), *self._ws_args(ws), flags,
+                   self._ptr(loop_state))
         self._note_fallback(x)
 
     # -- device-resident Lloyd loop ------------------------------------------------------
     def loop_state_new(self, tol, max_iter):
         """(state bytes, shift history) for one Lloyd loop, reset on the device."""
-        nb = ctypes.c_size_t(0)
-        _lib.check(self.lib.bkm_loop_state_bytes(ctypes.byref(nb)), "bkm_loop_state_bytes")
-        state = torch.zeros(int(nb.value), dtype=torch.uint8, device=self.device)
+        state = torch.zeros(int(self._query("bkm_loop_state_bytes")), dtype=torch.uint8, device=self.device)
         hist = torch.zeros(max(1, int(max_iter)), dtype=torch.float64, device=self.device)
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.bkm_loop_reset(self._ptr(state), float(tol), self._ptr(hist), int(hist.numel()),
-                                               self._stream()), "bkm_loop_reset")
+        self._call("bkm_loop_reset", self._ptr(state), float(tol), self._ptr(hist), int(hist.numel()))
         return state, hist
 
     def loop_state_read(self, state):
@@ -376,53 +410,38 @@ class CudaBackend(object):
 
     def finalize_step(self, red, c_in, c_out, state, pack, dtype):
         k, d = c_in.shape
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.bkm_finalize_step(self._ptr(red), self._ptr(c_in), self._ptr(c_out), self._ptr(state),
-                                                  k, d, _DT_CODE[dtype], self._ptr(pack), pack.numel(), self._stream()),
-                       "bkm_finalize_step")
+        self._call("bkm_finalize_step", self._ptr(red), self._ptr(c_in), self._ptr(c_out), self._ptr(state), k, d,
+                   _DT_CODE[dtype], self._ptr(pack), pack.numel())
 
     def minibatch_step(self, red, c_in, w_in, c_out, w_out, pack, dtype):
         """One mini-batch centre update from ``red = [k*d sums | k counts | inertia]`` of the batch: c_out, w_out and the
         pack of c_out (scikit-learn's _minibatch_update_dense, in float64)."""
         k, d = c_in.shape
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.bkm_minibatch_step(self._ptr(red), self._ptr(c_in), self._ptr(w_in), self._ptr(c_out),
-                                                   self._ptr(w_out), k, d, _DT_CODE[dtype], self._ptr(pack), pack.numel(),
-                                                   self._stream()), "bkm_minibatch_step")
+        self._call("bkm_minibatch_step", self._ptr(red), self._ptr(c_in), self._ptr(w_in), self._ptr(c_out),
+                   self._ptr(w_out), k, d, _DT_CODE[dtype], self._ptr(pack), pack.numel())
 
     def assign_chunk(self, x, pack, k, labels, min_dist, squared, dist_sum):
         n, d = x.shape
         ws = self._workspace(n, d, k, x.dtype)
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.bkm_assign_chunk(
-                self._ptr(x), n, d, x.stride(0) if n else d, _DT_CODE[x.dtype], self._ptr(pack), k,
-                self._ptr(labels), self._ptr(min_dist), int(bool(squared)), self._ptr(dist_sum),
-                self._ptr(ws), ws.numel(), self.flags, self._stream()), "bkm_assign_chunk")
+        self._call("bkm_assign_chunk", *self._rows(x), self._ptr(pack), k, self._ptr(labels), self._ptr(min_dist),
+                   int(bool(squared)), self._ptr(dist_sum), *self._ws_args(ws), self.flags)
         self._note_fallback(x)
 
     def sample_chunk(self, min_d2, ell_over_phi, seed, row_offset, picked, n_picked):
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.bkm_sample_chunk(
-                self._ptr(min_d2), min_d2.numel(), _DT_CODE[min_d2.dtype], float(ell_over_phi),
-                int(seed) & 0xFFFFFFFFFFFFFFFF, int(row_offset), self._ptr(picked), picked.numel(),
-                self._ptr(n_picked), self._stream()), "bkm_sample_chunk")
+        self._call("bkm_sample_chunk", self._ptr(min_d2), min_d2.numel(), _DT_CODE[min_d2.dtype], float(ell_over_phi),
+                   int(seed) & 0xFFFFFFFFFFFFFFFF, int(row_offset), self._ptr(picked), picked.numel(),
+                   self._ptr(n_picked))
 
     def min_fold(self, run_min, new_min, phi_acc):
         """run_min = min(run_min, new_min) (new_min may be None) and phi_acc += sum(run_min): one kernel."""
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.bkm_min_fold_chunk(self._ptr(run_min), self._ptr(new_min), run_min.numel(),
-                                                   _DT_CODE[run_min.dtype], self._ptr(phi_acc), self._stream()),
-                       "bkm_min_fold_chunk")
+        self._call("bkm_min_fold_chunk", self._ptr(run_min), self._ptr(new_min), run_min.numel(),
+                   _DT_CODE[run_min.dtype], self._ptr(phi_acc))
 
     def transform_chunk(self, x, pack, k, out, mode=0, gamma=0.0):
         """(n, k) block of distances (mode 0), squared distances (1) or exp(-gamma d^2) (2) into ``out`` — which may be a
         column block of a wider matrix (row pitch = out.stride(0))."""
-        n, d = x.shape
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.bkm_transform_chunk(
-                self._ptr(x), n, d, x.stride(0) if n else d, _DT_CODE[x.dtype], self._ptr(pack), k,
-                self._ptr(out), out.stride(0) if n else k, int(mode), float(gamma), self.flags, self._stream()),
-                "bkm_transform_chunk")
+        self._call("bkm_transform_chunk", *self._rows(x), self._ptr(pack), k, self._ptr(out),
+                   self._ld(out, x.shape[0], k), int(mode), float(gamma), self.flags)
         self._note_fallback(x)
 
     def kernel_colsum(self, x, pack, l, gamma, colsum, first=False):
@@ -430,38 +449,26 @@ class CudaBackend(object):
         The first pass of the Nystrom embedding (SpectralClustering)."""
         n, d = x.shape
         ws = self._workspace(n, d, l, x.dtype)
-        flags = self.flags | (_lib.FLAG_FIRST_CHUNK if first else 0)
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.bkm_kernel_colsum_chunk(
-                self._ptr(x), n, d, x.stride(0) if n else d, _DT_CODE[x.dtype], self._ptr(pack), int(l), float(gamma),
-                self._ptr(colsum), self._ptr(ws), ws.numel(), flags, self._stream()), "bkm_kernel_colsum_chunk")
+        self._call("bkm_kernel_colsum_chunk", *self._rows(x), self._ptr(pack), int(l), float(gamma), self._ptr(colsum),
+                   *self._ws_args(ws), self._first(first))
         self._note_fallback(x)
 
     def gram_chunk(self, x, shift, colsum, gram, first=False):
         """colsum (+)= sum_i (x_i - shift) and gram (+)= sum_i (x_i - shift)(x_i - shift)^T over the rows of the chunk
         (float64 [d] and [d, d] on the device); ``first`` overwrites.  The fit pass of PCA / TruncatedSVD."""
         n, d = x.shape
-        nb = ctypes.c_size_t(0)
-        _lib.check(self.lib.bkm_gram_workspace_bytes(int(n), int(d), ctypes.byref(nb)), "bkm_gram_workspace_bytes")
-        ws = self._scratch("gram", nb.value)
-        flags = self.flags | (_lib.FLAG_FIRST_CHUNK if first else 0)
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.bkm_gram_chunk(
-                self._ptr(x), n, d, x.stride(0) if n else d, _DT_CODE[x.dtype], self._ptr(shift), self._ptr(colsum),
-                self._ptr(gram), self._ptr(ws), ws.numel(), flags, self._stream()), "bkm_gram_chunk")
+        ws = self._scratch_for("gram", "bkm_gram_workspace_bytes", int(n), int(d))
+        self._call("bkm_gram_chunk", *self._rows(x), self._ptr(shift), self._ptr(colsum), self._ptr(gram),
+                   *self._ws_args(ws), self._first(first))
 
     def project_chunk(self, x, shift, W, out=None, colmax=None, row_offset=0):
         """out = (x - shift) W^T (``W`` float64 (k, d), ``shift`` float64 (d,) or None, ``out`` (n, k) float32 / float64
         with any row pitch, or None) and, into ``colmax`` (float64 (k, 4) records, see ``colmax_new``), per column
         the largest |out_ij| with its lowest global row ``row_offset + i`` and its signed value."""
-        n, d = x.shape
         k = int(W.shape[0])
         odt = _DT_CODE[out.dtype] if out is not None else _lib.BKM_F64
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.bkm_project_chunk(
-                self._ptr(x), n, d, x.stride(0) if n else d, _DT_CODE[x.dtype], self._ptr(shift), self._ptr(W), k,
-                self._ptr(out), (out.stride(0) if n else k) if out is not None else k, odt, self._ptr(colmax),
-                int(row_offset), self.flags, self._stream()), "bkm_project_chunk")
+        self._call("bkm_project_chunk", *self._rows(x), self._ptr(shift), self._ptr(W), k, self._ptr(out),
+                   self._ld(out, x.shape[0], k), odt, self._ptr(colmax), int(row_offset), self.flags)
 
     def colmax_new(self, k):
         """k empty arg-max records {absmax = -1, row = -1, value = 0, lock = 0} for ``project_chunk``."""
@@ -476,30 +483,20 @@ class CudaBackend(object):
         ``theta`` (float64 (K, d)), sums (+)= per-class sums of (x - theta_c)^2.  float64 on the device; ``first``
         overwrites."""
         n, d = x.shape
-        nb = ctypes.c_size_t(0)
-        _lib.check(self.lib.bkm_nb_workspace_bytes(int(n), int(d), int(K), ctypes.byref(nb)), "bkm_nb_workspace_bytes")
-        ws = self._scratch("nb", nb.value)
-        flags = self.flags | (_lib.FLAG_FIRST_CHUNK if first else 0)
+        ws = self._scratch_for("nb", "bkm_nb_workspace_bytes", int(n), int(d), int(K))
         mode = 0 if theta is None else 1
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.bkm_class_moments_chunk(
-                self._ptr(x), n, d, x.stride(0) if n else d, _DT_CODE[x.dtype], self._ptr(cls), int(K), mode,
-                self._ptr(theta), self._ptr(sums), self._ptr(counts), self._ptr(ws), ws.numel(), flags,
-                self._stream()), "bkm_class_moments_chunk")
+        self._call("bkm_class_moments_chunk", *self._rows(x), self._ptr(cls), int(K), mode, self._ptr(theta),
+                   self._ptr(sums), self._ptr(counts), *self._ws_args(ws), self._first(first))
 
     def nb_jll_chunk(self, x, theta, inv_sigma, logc, labels=None, out=None, exp_out=False, n_deferred=None):
         """GaussianNB's predict pass over one chunk: ``labels`` (int32 (n,)) the arg-max of the joint log-likelihood
         and / or ``out`` (float64 (n, K), any row pitch) its log-softmax, exponentiated with ``exp_out``.  ``theta``,
         ``inv_sigma`` float64 (K, d), ``logc`` float64 (K,) on the device; ``n_deferred`` (int32 (1,)) counts the fp32
         rows re-decided in float64."""
-        n, d = x.shape
         K = int(theta.shape[0])
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.bkm_nb_jll_chunk(
-                self._ptr(x), n, d, x.stride(0) if n else d, _DT_CODE[x.dtype], self._ptr(theta), self._ptr(inv_sigma),
-                self._ptr(logc), K, self._ptr(labels), self._ptr(out),
-                (out.stride(0) if n else K) if out is not None else K, int(bool(exp_out)), self._ptr(n_deferred),
-                self.flags, self._stream()), "bkm_nb_jll_chunk")
+        self._call("bkm_nb_jll_chunk", *self._rows(x), self._ptr(theta), self._ptr(inv_sigma), self._ptr(logc), K,
+                   self._ptr(labels), self._ptr(out), self._ld(out, x.shape[0], K), int(bool(exp_out)),
+                   self._ptr(n_deferred), self.flags)
 
     def class_counts_chunk(self, x, cls, K, fc, cc, w=None, binarize=None, first=False):
         """The count pass of the discrete naive Bayes models over one chunk, by int32 class index ``cls`` (indices
@@ -507,57 +504,37 @@ class CudaBackend(object):
         float64 on the device, ``w`` float64 (n,) or None (ones), f(x) = x, or x > ``binarize`` when it is not None.
         ``first`` overwrites."""
         n, d = x.shape
-        nb = ctypes.c_size_t(0)
-        _lib.check(self.lib.bkm_nb_workspace_bytes(int(n), int(d), int(K), ctypes.byref(nb)), "bkm_nb_workspace_bytes")
-        ws = self._scratch("nb", nb.value)
-        flags = self.flags | (_lib.FLAG_FIRST_CHUNK if first else 0)
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.bkm_class_counts_chunk(
-                self._ptr(x), n, d, x.stride(0) if n else d, _DT_CODE[x.dtype], self._ptr(cls), int(K), self._ptr(w),
-                int(binarize is not None), float(binarize or 0.0), self._ptr(fc), self._ptr(cc), self._ptr(ws),
-                ws.numel(), flags, self._stream()), "bkm_class_counts_chunk")
+        ws = self._scratch_for("nb", "bkm_nb_workspace_bytes", int(n), int(d), int(K))
+        self._call("bkm_class_counts_chunk", *self._rows(x), self._ptr(cls), int(K), self._ptr(w),
+                   int(binarize is not None), float(binarize or 0.0), self._ptr(fc), self._ptr(cc), *self._ws_args(ws),
+                   self._first(first))
 
     def csc_class_counts_chunk(self, csc, d, labels, K, fcT, w=None, binarize=None, first=False):
         """``class_counts_chunk``'s feature sums over the transpose ``csc`` of one CSR block, transposed: fcT (d, K)
         (+)= per-class sums of w_i f(x_ij), each in ascending row order; an entry not above ``binarize`` adds nothing.
         ``first`` overwrites."""
-        colptr, rows, vals, plan = csc
-        nnz = int(rows.numel())
-        nb = ctypes.c_size_t(0)
-        _lib.check(self.lib.bkm_csc_label_sums_workspace_bytes(int(d), nnz, int(K), ctypes.byref(nb)),
-                   "bkm_csc_label_sums_workspace_bytes")
-        ws = self._scratch("csc_label_sums", nb.value)
-        flags = self.flags | (_lib.FLAG_FIRST_CHUNK if first else 0)
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.bkm_csc_class_counts_chunk(
-                self._ptr(colptr), self._ptr(rows), self._ptr(vals), _DT_CODE[vals.dtype], int(d), nnz, self._ptr(plan),
-                self._ptr(labels), int(K), self._ptr(w), int(binarize is not None), float(binarize or 0.0),
-                self._ptr(fcT), self._ptr(ws), ws.numel(), flags, self._stream()), "bkm_csc_class_counts_chunk")
+        ws = self._scratch_for("csc_label_sums", "bkm_csc_label_sums_workspace_bytes", int(d), int(csc[1].numel()),
+                               int(K))
+        self._call("bkm_csc_class_counts_chunk", *self._csc(csc, d), self._ptr(labels), int(K), self._ptr(w),
+                   int(binarize is not None), float(binarize or 0.0), self._ptr(fcT), *self._ws_args(ws),
+                   self._first(first))
 
     def nb_linear_jll_chunk(self, x, W, b, labels=None, out=None, out_mode=0, binarize=None):
         """The predict pass of the discrete naive Bayes models over one chunk: jll = f(x) W^T + b (``W`` float64 (K, d),
         ``b`` float64 (K,) on the device; f as in ``class_counts_chunk``), into ``labels`` (int32 (n,)) its arg-max and /
         or ``out`` (float64 (n, K), any row pitch) jll (``out_mode`` 0), its log-softmax (1) or softmax (2)."""
-        n, d = x.shape
         K = int(W.shape[0])
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.bkm_nb_linear_jll_chunk(
-                self._ptr(x), n, d, x.stride(0) if n else d, _DT_CODE[x.dtype], int(binarize is not None),
-                float(binarize or 0.0), self._ptr(W), self._ptr(b), K, self._ptr(labels), self._ptr(out),
-                (out.stride(0) if n else K) if out is not None else K, int(out_mode), self.flags, self._stream()),
-                "bkm_nb_linear_jll_chunk")
+        self._call("bkm_nb_linear_jll_chunk", *self._rows(x), int(binarize is not None), float(binarize or 0.0),
+                   self._ptr(W), self._ptr(b), K, self._ptr(labels), self._ptr(out), self._ld(out, x.shape[0], K),
+                   int(out_mode), self.flags)
 
     def nb_csr_jll_chunk(self, blk, d, WT, b, labels=None, out=None, out_mode=0, binarize=None):
         """``nb_linear_jll_chunk`` on one CSR block of d columns over its stored entries, ``WT`` float64 (d, K)
         row-major."""
-        crow, col, val, n = blk
         K = int(WT.shape[1])
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.bkm_nb_csr_jll_chunk(
-                self._ptr(crow), self._ptr(col), self._ptr(val), _DT_CODE[val.dtype], int(n), int(d), int(col.numel()),
-                int(binarize is not None), float(binarize or 0.0), self._ptr(WT), self._ptr(b), K, self._ptr(labels),
-                self._ptr(out), (out.stride(0) if n else K) if out is not None else K, int(out_mode), self.flags,
-                self._stream()), "bkm_nb_csr_jll_chunk")
+        self._call("bkm_nb_csr_jll_chunk", *self._csr(blk, d), int(binarize is not None), float(binarize or 0.0),
+                   self._ptr(WT), self._ptr(b), K, self._ptr(labels), self._ptr(out), self._ld(out, blk[3], K),
+                   int(out_mode), self.flags)
 
     def glm_pass_chunk(self, x, y, beta, family, mode, grad=None, hrow=None, w=None, out=None, first=False):
         """The fused pass of the linear models over one chunk (float64 arithmetic): eta = x . beta[:d] + beta[d] with
@@ -566,49 +543,28 @@ class CudaBackend(object):
         3: out (n,) uint8 = mu > 0.5.  ``y`` float64 (n,) (modes 0 and 1), ``beta`` float64 (d + 1,) on the device;
         ``first`` overwrites."""
         n, d = x.shape
-        ws = None
-        if mode in (0, 1):
-            nb = ctypes.c_size_t(0)
-            _lib.check(self.lib.bkm_glm_workspace_bytes(int(n), int(d), ctypes.byref(nb)), "bkm_glm_workspace_bytes")
-            ws = self._scratch("glm", nb.value)
-        flags = self.flags | (_lib.FLAG_FIRST_CHUNK if first else 0)
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.bkm_glm_pass_chunk(
-                self._ptr(x), n, d, x.stride(0) if n else d, _DT_CODE[x.dtype], self._ptr(y), self._ptr(beta),
-                int(family), int(mode), self._ptr(grad), self._ptr(hrow), self._ptr(w), self._ptr(out), self._ptr(ws),
-                ws.numel() if ws is not None else 0, flags, self._stream()), "bkm_glm_pass_chunk")
+        ws = self._scratch_for("glm", "bkm_glm_workspace_bytes", int(n), int(d)) if mode in (0, 1) else None
+        self._call("bkm_glm_pass_chunk", *self._rows(x), self._ptr(y), self._ptr(beta), int(family), int(mode),
+                   self._ptr(grad), self._ptr(hrow), self._ptr(w), self._ptr(out), *self._ws_args(ws),
+                   self._first(first))
 
     def gram_weighted_chunk(self, x, w, gram, first=False):
         """gram (+)= sum_i w_i x_i x_i^T over the rows of the chunk (``w`` float64 (n,), ``gram`` float64 (d, d) on the
         device): the Hessian block of a Newton step.  ``first`` overwrites."""
         n, d = x.shape
-        nb = ctypes.c_size_t(0)
-        _lib.check(self.lib.bkm_gram_workspace_bytes(int(n), int(d), ctypes.byref(nb)), "bkm_gram_workspace_bytes")
-        ws = self._scratch("gram", nb.value)
-        flags = self.flags | (_lib.FLAG_FIRST_CHUNK if first else 0)
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.bkm_gram_weighted_chunk(
-                self._ptr(x), n, d, x.stride(0) if n else d, _DT_CODE[x.dtype], self._ptr(w), self._ptr(gram),
-                self._ptr(ws), ws.numel(), flags, self._stream()), "bkm_gram_weighted_chunk")
+        ws = self._scratch_for("gram", "bkm_gram_workspace_bytes", int(n), int(d))
+        self._call("bkm_gram_weighted_chunk", *self._rows(x), self._ptr(w), self._ptr(gram), *self._ws_args(ws),
+                   self._first(first))
 
     def glm_csr_pass_chunk(self, blk, d, y, beta, family, mode, r=None, w=None, grad=None, hrow=None, out=None,
                            first=False):
         """``glm_pass_chunk`` on one CSR block ``blk`` = (crow int64 (n + 1,), col int64 (nnz,), val float32 / float64
         (nnz,), n) of d columns.  Modes 0 and 1 write r (n,) (and w (n,)) float64 for ``csc_matvec_chunk`` and set
         grad[d:d + 2] = [sum r | loss] (and hrow[d] = sum w); modes 2 and 3 write ``out`` as the dense pass does."""
-        crow, col, val, n = blk
-        ws = None
-        if mode in (0, 1):
-            nb = ctypes.c_size_t(0)
-            _lib.check(self.lib.bkm_glm_csr_workspace_bytes(int(n), ctypes.byref(nb)), "bkm_glm_csr_workspace_bytes")
-            ws = self._scratch("glm_csr", nb.value)
-        flags = self.flags | (_lib.FLAG_FIRST_CHUNK if first else 0)
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.bkm_glm_csr_pass_chunk(
-                self._ptr(crow), self._ptr(col), self._ptr(val), _DT_CODE[val.dtype], int(n), int(d), int(col.numel()),
-                self._ptr(y), self._ptr(beta), int(family), int(mode), self._ptr(r), self._ptr(w), self._ptr(grad),
-                self._ptr(hrow), self._ptr(out), self._ptr(ws), ws.numel() if ws is not None else 0, flags,
-                self._stream()), "bkm_glm_csr_pass_chunk")
+        ws = self._scratch_for("glm_csr", "bkm_glm_csr_workspace_bytes", int(blk[3])) if mode in (0, 1) else None
+        self._call("bkm_glm_csr_pass_chunk", *self._csr(blk, d), self._ptr(y), self._ptr(beta), int(family), int(mode),
+                   self._ptr(r), self._ptr(w), self._ptr(grad), self._ptr(hrow), self._ptr(out), *self._ws_args(ws),
+                   self._first(first))
 
     def csr_transpose_chunk(self, blk, d):
         """The CSC of one CSR block: (colptr int64 (d + 1,), rows int32 (nnz,) ascending within each column, vals
@@ -616,84 +572,49 @@ class CudaBackend(object):
         column] (include/bkm_b200.h)."""
         crow, col, val, n = blk
         nnz = int(col.numel())
-        wb, pb = ctypes.c_size_t(0), ctypes.c_size_t(0)
-        _lib.check(self.lib.bkm_csr_transpose_workspace_bytes(int(n), int(d), nnz, ctypes.byref(wb), ctypes.byref(pb)),
-                   "bkm_csr_transpose_workspace_bytes")
-        ws = self._scratch("csr_transpose", wb.value)
+        wb, pb = self._query("bkm_csr_transpose_workspace_bytes", int(n), int(d), nnz, outs=2)
+        ws = self._scratch("csr_transpose", wb)
         colptr = torch.empty(int(d) + 1, dtype=torch.int64, device=self.device)
         rows = torch.empty(nnz, dtype=torch.int32, device=self.device)
         vals = torch.empty(nnz, dtype=val.dtype, device=self.device)
-        plan = torch.empty((pb.value + 7) // 8, dtype=torch.int64, device=self.device)
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.bkm_csr_transpose_chunk(
-                self._ptr(crow), self._ptr(col), self._ptr(val), _DT_CODE[val.dtype], int(n), int(d), nnz,
-                self._ptr(colptr), self._ptr(rows), self._ptr(vals), self._ptr(plan), plan.numel() * 8, self._ptr(ws),
-                ws.numel(), self._stream()), "bkm_csr_transpose_chunk")
+        plan = torch.empty((pb + 7) // 8, dtype=torch.int64, device=self.device)
+        self._call("bkm_csr_transpose_chunk", *self._csr(blk, d), self._ptr(colptr), self._ptr(rows), self._ptr(vals),
+                   self._ptr(plan), plan.numel() * 8, *self._ws_args(ws))
         return colptr, rows, vals, plan
 
     def csc_matvec_chunk(self, csc, d, v1, out1, v2=None, out2=None, first=False):
         """out1[:d] (+)= X^T v1 (and out2[:d] (+)= X^T v2) over the transpose ``csc`` of one block, each column's
         entries added in ascending row order.  ``first`` overwrites."""
-        colptr, rows, vals, plan = csc
-        nnz = int(rows.numel())
-        nb = ctypes.c_size_t(0)
-        _lib.check(self.lib.bkm_csc_matvec_workspace_bytes(int(d), nnz, ctypes.byref(nb)),
-                   "bkm_csc_matvec_workspace_bytes")
-        ws = self._scratch("csc_matvec", nb.value)
-        flags = self.flags | (_lib.FLAG_FIRST_CHUNK if first else 0)
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.bkm_csc_matvec_chunk(
-                self._ptr(colptr), self._ptr(rows), self._ptr(vals), _DT_CODE[vals.dtype], int(d), nnz, self._ptr(plan),
-                self._ptr(v1), self._ptr(v2), self._ptr(out1), self._ptr(out2), self._ptr(ws), ws.numel(), flags,
-                self._stream()), "bkm_csc_matvec_chunk")
+        ws = self._scratch_for("csc_matvec", "bkm_csc_matvec_workspace_bytes", int(d), int(csc[1].numel()))
+        self._call("bkm_csc_matvec_chunk", *self._csc(csc, d), self._ptr(v1), self._ptr(v2), self._ptr(out1),
+                   self._ptr(out2), *self._ws_args(ws), self._first(first))
 
     def gram_weighted_csr_chunk(self, blk, csc, d, w, gram, n_slots, first=False):
         """gram (d, d) (+)= sum_i w_i x_i x_i^T over one CSR block and its transpose; ``n_slots`` = plan[2] of the
         transpose (read once per fit).  ``first`` overwrites."""
-        crow, col, val, n = blk
         colptr, rows, vals, plan = csc
-        nb = ctypes.c_size_t(0)
-        _lib.check(self.lib.bkm_gram_weighted_csr_workspace_bytes(int(d), int(n_slots), ctypes.byref(nb)),
-                   "bkm_gram_weighted_csr_workspace_bytes")
-        ws = self._scratch("gram_csr", nb.value)
-        flags = self.flags | (_lib.FLAG_FIRST_CHUNK if first else 0)
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.bkm_gram_weighted_csr_chunk(
-                self._ptr(crow), self._ptr(col), self._ptr(val), _DT_CODE[val.dtype], int(n), int(d),
-                int(col.numel()), self._ptr(colptr), self._ptr(rows), self._ptr(vals), self._ptr(plan), int(n_slots),
-                self._ptr(w), self._ptr(gram), self._ptr(ws), ws.numel(), flags, self._stream()),
-                "bkm_gram_weighted_csr_chunk")
+        ws = self._scratch_for("gram_csr", "bkm_gram_weighted_csr_workspace_bytes", int(d), int(n_slots))
+        self._call("bkm_gram_weighted_csr_chunk", *self._csr(blk, d), self._ptr(colptr), self._ptr(rows),
+                   self._ptr(vals), self._ptr(plan), int(n_slots), self._ptr(w), self._ptr(gram), *self._ws_args(ws),
+                   self._first(first))
 
     def csr_panel_chunk(self, blk, d, W, out=None, colmax=None, row_offset=0):
         """out = X W over one CSR block ``blk`` of d columns (``W`` float64 (d, l) row-major, ``out`` (n, l) float32 /
         float64 with any row pitch, or None), each element adding its row's entries in column order, and, into
         ``colmax`` (``colmax_new(l)`` records), per column the largest |out_ij| with its lowest global row
         ``row_offset + i`` and its signed value."""
-        crow, col, val, n = blk
         l = int(W.shape[1])
         odt = _DT_CODE[out.dtype] if out is not None else _lib.BKM_F64
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.bkm_csr_panel_chunk(
-                self._ptr(crow), self._ptr(col), self._ptr(val), _DT_CODE[val.dtype], int(n), int(d), int(col.numel()),
-                self._ptr(W), l, self._ptr(out), (out.stride(0) if n else l) if out is not None else l, odt,
-                self._ptr(colmax), int(row_offset), self._stream()), "bkm_csr_panel_chunk")
+        self._call("bkm_csr_panel_chunk", *self._csr(blk, d), self._ptr(W), l, self._ptr(out), self._ld(out, blk[3], l),
+                   odt, self._ptr(colmax), int(row_offset))
 
     def csc_panel_chunk(self, csc, d, P, out, first=False):
         """out (d, l) (+)= X^T P over the transpose ``csc`` of one block (``P`` float64 (n, l) row-major, ``out`` float64
         (d, l) contiguous), each column's entries added in ascending row order.  ``first`` overwrites."""
-        colptr, rows, vals, plan = csc
-        nnz = int(rows.numel())
         l = int(out.shape[1])
-        nb = ctypes.c_size_t(0)
-        _lib.check(self.lib.bkm_csc_panel_workspace_bytes(int(d), nnz, l, ctypes.byref(nb)),
-                   "bkm_csc_panel_workspace_bytes")
-        ws = self._scratch("csc_panel", nb.value)
-        flags = self.flags | (_lib.FLAG_FIRST_CHUNK if first else 0)
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.bkm_csc_panel_chunk(
-                self._ptr(colptr), self._ptr(rows), self._ptr(vals), _DT_CODE[vals.dtype], int(d), nnz, self._ptr(plan),
-                self._ptr(P), l, self._ptr(out), self._ptr(ws), ws.numel(), flags, self._stream()),
-                "bkm_csc_panel_chunk")
+        ws = self._scratch_for("csc_panel", "bkm_csc_panel_workspace_bytes", int(d), int(csc[1].numel()), l)
+        self._call("bkm_csc_panel_chunk", *self._csc(csc, d), self._ptr(P), l, self._ptr(out), *self._ws_args(ws),
+                   self._first(first))
 
     # -- KMeans on sparse CSR blocks ---------------------------------------------------------
     def sparse_pack_centers(self, C64, out=None):
@@ -702,13 +623,8 @@ class CudaBackend(object):
         k, p = C64.shape
         if out is None:
             out = torch.empty(p * k + k, dtype=torch.float64, device=self.device)
-        nb = ctypes.c_size_t(0)
-        _lib.check(self.lib.bkm_sparse_pack_workspace_bytes(int(k), int(p), ctypes.byref(nb)),
-                   "bkm_sparse_pack_workspace_bytes")
-        ws = self._scratch("sparse_pack", nb.value)
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.bkm_sparse_pack_centers(self._ptr(C64), int(k), int(p), self._ptr(out), self._ptr(ws),
-                                                        ws.numel(), self._stream()), "bkm_sparse_pack_centers")
+        ws = self._scratch_for("sparse_pack", "bkm_sparse_pack_workspace_bytes", int(k), int(p))
+        self._call("bkm_sparse_pack_centers", self._ptr(C64), int(k), int(p), self._ptr(out), *self._ws_args(ws))
         return out
 
     def csr_assign_chunk(self, blk, d, pack, k, labels=None, min_dist=None, squared=True, dist_sum=None, counts=None,
@@ -716,91 +632,52 @@ class CudaBackend(object):
         """The E-step of one CSR block against a sparse pack: mode 0 writes labels (int32), min_dist (float64, squared
         or not) and adds to dist_sum (1,) / counts (k,) float64 (``first`` overwrites them); modes 1 / 2 write the
         distances / squared distances into ``out`` (n, k) float32 / float64 with any row pitch."""
-        crow, col, val, n = blk
+        n = blk[3]
         ws = None
         if mode == 0 and (dist_sum is not None or counts is not None):
-            nb = ctypes.c_size_t(0)
-            _lib.check(self.lib.bkm_csr_assign_workspace_bytes(int(n), int(k), ctypes.byref(nb)),
-                       "bkm_csr_assign_workspace_bytes")
-            ws = self._scratch("csr_assign", nb.value)
-        flags = self.flags | (_lib.FLAG_FIRST_CHUNK if first else 0)
+            ws = self._scratch_for("csr_assign", "bkm_csr_assign_workspace_bytes", int(n), int(k))
         odt = _DT_CODE[out.dtype] if out is not None else _lib.BKM_F64
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.bkm_csr_assign_chunk(
-                self._ptr(crow), self._ptr(col), self._ptr(val), _DT_CODE[val.dtype], int(n), int(d), int(col.numel()),
-                self._ptr(pack), int(k), int(mode), self._ptr(labels), self._ptr(min_dist), int(bool(squared)),
-                self._ptr(dist_sum), self._ptr(counts), self._ptr(out), (out.stride(0) if n else k) if out is not None
-                else k, odt, self._ptr(ws), ws.numel() if ws is not None else 0, flags, self._ptr(loop_state),
-                self._stream()), "bkm_csr_assign_chunk")
+        self._call("bkm_csr_assign_chunk", *self._csr(blk, d), self._ptr(pack), int(k), int(mode), self._ptr(labels),
+                   self._ptr(min_dist), int(bool(squared)), self._ptr(dist_sum), self._ptr(counts), self._ptr(out),
+                   self._ld(out, n, k), odt, *self._ws_args(ws), self._first(first), self._ptr(loop_state))
 
     def csc_label_sums_chunk(self, csc, d, labels, k, sumsT, first=False, loop_state=None):
         """sumsT (d, k) (+)= X^T onehot(labels) over the transpose ``csc`` of one block, each (column, cluster) sum in
         ascending row order.  ``first`` overwrites."""
-        colptr, rows, vals, plan = csc
-        nnz = int(rows.numel())
-        nb = ctypes.c_size_t(0)
-        _lib.check(self.lib.bkm_csc_label_sums_workspace_bytes(int(d), nnz, int(k), ctypes.byref(nb)),
-                   "bkm_csc_label_sums_workspace_bytes")
-        ws = self._scratch("csc_label_sums", nb.value)
-        flags = self.flags | (_lib.FLAG_FIRST_CHUNK if first else 0)
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.bkm_csc_label_sums_chunk(
-                self._ptr(colptr), self._ptr(rows), self._ptr(vals), _DT_CODE[vals.dtype], int(d), nnz, self._ptr(plan),
-                self._ptr(labels), int(k), self._ptr(sumsT), self._ptr(ws), ws.numel(), flags, self._ptr(loop_state),
-                self._stream()), "bkm_csc_label_sums_chunk")
+        ws = self._scratch_for("csc_label_sums", "bkm_csc_label_sums_workspace_bytes", int(d), int(csc[1].numel()),
+                               int(k))
+        self._call("bkm_csc_label_sums_chunk", *self._csc(csc, d), self._ptr(labels), int(k), self._ptr(sumsT),
+                   *self._ws_args(ws), self._first(first), self._ptr(loop_state))
 
     def sparse_finalize_step(self, red, pack_in, pack_out, state, k, d):
         """bkm_finalize_step on the transposed layout: red = [d*k sumsT | k counts | inertia] -> the shift, the stop
         test and pack_out = the sparse pack of the new centres."""
-        nb = ctypes.c_size_t(0)
-        _lib.check(self.lib.bkm_sparse_pack_workspace_bytes(int(k), int(d), ctypes.byref(nb)),
-                   "bkm_sparse_pack_workspace_bytes")
-        ws = self._scratch("sparse_pack", nb.value)
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.bkm_sparse_finalize_step(self._ptr(red), self._ptr(pack_in), self._ptr(pack_out),
-                                                         self._ptr(state), int(k), int(d), self._ptr(ws), ws.numel(),
-                                                         self._stream()), "bkm_sparse_finalize_step")
+        ws = self._scratch_for("sparse_pack", "bkm_sparse_pack_workspace_bytes", int(k), int(d))
+        self._call("bkm_sparse_finalize_step", self._ptr(red), self._ptr(pack_in), self._ptr(pack_out),
+                   self._ptr(state), int(k), int(d), *self._ws_args(ws))
 
     def sparse_minibatch_step(self, red, pack_in, w_in, pack_out, w_out, k, d):
         """One mini-batch centre update on the transposed layout (scikit-learn's _minibatch_update_sparse, in float64):
         red = [d*k sumsT | k counts | inertia] of the batch -> pack_out = the sparse pack of the new centres and
         w_out = w_in + counts."""
-        nb = ctypes.c_size_t(0)
-        _lib.check(self.lib.bkm_sparse_pack_workspace_bytes(int(k), int(d), ctypes.byref(nb)),
-                   "bkm_sparse_pack_workspace_bytes")
-        ws = self._scratch("sparse_pack", nb.value)
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.bkm_sparse_minibatch_step(self._ptr(red), self._ptr(pack_in), self._ptr(w_in),
-                                                          self._ptr(pack_out), self._ptr(w_out), int(k), int(d),
-                                                          self._ptr(ws), ws.numel(), self._stream()),
-                       "bkm_sparse_minibatch_step")
+        ws = self._scratch_for("sparse_pack", "bkm_sparse_pack_workspace_bytes", int(k), int(d))
+        self._call("bkm_sparse_minibatch_step", self._ptr(red), self._ptr(pack_in), self._ptr(w_in),
+                   self._ptr(pack_out), self._ptr(w_out), int(k), int(d), *self._ws_args(ws))
 
     def csr_kernel_colsum(self, blk, d, pack, l, gamma, colsum, first=False):
         """colsum[j] (+)= sum_i exp(-gamma ||x_i - c_j||^2) over the rows of one CSR block against the sparse pack of the
         l keep rows (float64 [l]); ``first`` overwrites.  The first Nystrom pass of SpectralClustering on sparse X."""
-        crow, col, val, n = blk
-        nb = ctypes.c_size_t(0)
-        _lib.check(self.lib.bkm_csr_kernel_colsum_workspace_bytes(int(n), int(l), ctypes.byref(nb)),
-                   "bkm_csr_kernel_colsum_workspace_bytes")
-        ws = self._scratch("csr_kernel_colsum", nb.value)
-        flags = self.flags | (_lib.FLAG_FIRST_CHUNK if first else 0)
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.bkm_csr_kernel_colsum_chunk(
-                self._ptr(crow), self._ptr(col), self._ptr(val), _DT_CODE[val.dtype], int(n), int(d), int(col.numel()),
-                self._ptr(pack), int(l), float(gamma), self._ptr(colsum), self._ptr(ws), ws.numel(), flags,
-                self._stream()), "bkm_csr_kernel_colsum_chunk")
+        ws = self._scratch_for("csr_kernel_colsum", "bkm_csr_kernel_colsum_workspace_bytes", int(blk[3]), int(l))
+        self._call("bkm_csr_kernel_colsum_chunk", *self._csr(blk, d), self._ptr(pack), int(l), float(gamma),
+                   self._ptr(colsum), *self._ws_args(ws), self._first(first))
 
     def csr_nystrom_embed(self, blk, d, pack, l, gamma, W, out):
         """out[i] = e_i / ||e_i||, e_i = sum_j exp(-gamma (||x_i - c_j||^2 - min_j ||x_i - c_j||^2)) W[j] over one CSR
         block — the second Nystrom pass on sparse X.  ``W`` is (l, k) float64; ``out`` (n, k) float32 / float64 may have
         a padded row pitch."""
-        crow, col, val, n = blk
         k = int(W.shape[1])
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.bkm_csr_nystrom_embed_chunk(
-                self._ptr(crow), self._ptr(col), self._ptr(val), _DT_CODE[val.dtype], int(n), int(d), int(col.numel()),
-                self._ptr(pack), int(l), float(gamma), self._ptr(W), k, self._ptr(out), out.stride(0) if n else k,
-                _DT_CODE[out.dtype], self.flags, self._stream()), "bkm_csr_nystrom_embed_chunk")
+        self._call("bkm_csr_nystrom_embed_chunk", *self._csr(blk, d), self._ptr(pack), int(l), float(gamma),
+                   self._ptr(W), k, self._ptr(out), self._ld(out, blk[3], k), _DT_CODE[out.dtype], self.flags)
 
     # -- the SGD family -----------------------------------------------------------------------
     def sgd_block(self, x, order, y, sw, eta, cw, params, w, aw, q, st):
@@ -808,134 +685,88 @@ class CudaBackend(object):
         ``order`` int32 (P, n), ``y`` float64 (P, n), ``sw`` float64 (n,) or None, ``eta`` float64 (n,) or None
         ('invscaling'), ``cw`` float64 (P, 2), ``params`` an ``_lib.SgdParams``; updates w, aw, q (float64 (P, d)) and
         st (float64 (P, 4): intercept, average intercept, non-finite flag)."""
-        n, d = x.shape
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.bkm_sgd_block(
-                self._ptr(x), int(n), int(d), x.stride(0) if n else d, _DT_CODE[x.dtype], self._ptr(order),
-                self._ptr(y), self._ptr(sw), self._ptr(eta), self._ptr(cw), int(w.shape[0]), ctypes.byref(params),
-                self._ptr(w), self._ptr(aw), self._ptr(q), self._ptr(st), self._stream()), "bkm_sgd_block")
+        self._call("bkm_sgd_block", *self._rows(x), self._ptr(order), self._ptr(y), self._ptr(sw), self._ptr(eta),
+                   self._ptr(cw), int(w.shape[0]), ctypes.byref(params), self._ptr(w), self._ptr(aw), self._ptr(q),
+                   self._ptr(st))
 
     def sgd_csr_block(self, blk, d, order, y, sw, eta, cw, params, w, aw, q, st):
         """``sgd_block`` over one CSR block ``blk`` = (crow, col, val, n) of d columns."""
-        crow, col, val, n = blk
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.bkm_sgd_csr_block(
-                self._ptr(crow), self._ptr(col), self._ptr(val), _DT_CODE[val.dtype], int(n), int(d), int(col.numel()),
-                self._ptr(order), self._ptr(y), self._ptr(sw), self._ptr(eta), self._ptr(cw), int(w.shape[0]),
-                ctypes.byref(params), self._ptr(w), self._ptr(aw), self._ptr(q), self._ptr(st), self._stream()),
-                "bkm_sgd_csr_block")
+        self._call("bkm_sgd_csr_block", *self._csr(blk, d), self._ptr(order), self._ptr(y), self._ptr(sw),
+                   self._ptr(eta), self._ptr(cw), int(w.shape[0]), ctypes.byref(params), self._ptr(w), self._ptr(aw),
+                   self._ptr(q), self._ptr(st))
 
     def colstats_chunk(self, x, shift, acc, minmax, first=False):
         """The scalers' statistics pass over one chunk, float64 on the device: acc (5, d) (+)= [sum (x - shift) |
         sum (x - shift)^2 over the finite x | NaN count | +inf count | -inf count] and minmax (2, d) = [min | max] over
         the non-NaN x, folded.  ``shift`` float64 (d,) or None; ``first`` overwrites."""
         n, d = x.shape
-        nb = ctypes.c_size_t(0)
-        _lib.check(self.lib.bkm_colstats_workspace_bytes(int(n), int(d), ctypes.byref(nb)),
-                   "bkm_colstats_workspace_bytes")
-        ws = self._scratch("colstats", nb.value)
-        flags = self.flags | (_lib.FLAG_FIRST_CHUNK if first else 0)
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.bkm_colstats_chunk(
-                self._ptr(x), n, d, x.stride(0) if n else d, _DT_CODE[x.dtype], self._ptr(shift), self._ptr(acc),
-                self._ptr(minmax), self._ptr(ws), ws.numel(), flags, self._stream()), "bkm_colstats_chunk")
+        ws = self._scratch_for("colstats", "bkm_colstats_workspace_bytes", int(n), int(d))
+        self._call("bkm_colstats_chunk", *self._rows(x), self._ptr(shift), self._ptr(acc), self._ptr(minmax),
+                   *self._ws_args(ws), self._first(first))
 
     def radix_state_new(self, d, T):
         """Device state of one radix selection of T order statistics in each of d columns (``radix_select_step``)."""
-        nb = ctypes.c_size_t(0)
-        _lib.check(self.lib.bkm_radix_state_bytes(int(d), int(T), ctypes.byref(nb)), "bkm_radix_state_bytes")
-        return torch.zeros(int(nb.value), dtype=torch.uint8, device=self.device)
+        return torch.zeros(self._query("bkm_radix_state_bytes", int(d), int(T)), dtype=torch.uint8, device=self.device)
 
     def radix_hist_chunk(self, x, state, T, rnd, hist, first=False):
         """hist (d, T, 256) float64 (+)= the round-``rnd`` digit counts of the chunk's keys under each target's prefix;
         ``first`` zeroes hist first."""
-        n, d = x.shape
-        flags = self.flags | (_lib.FLAG_FIRST_CHUNK if first else 0)
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.bkm_radix_hist_chunk(
-                self._ptr(x), n, d, x.stride(0) if n else d, _DT_CODE[x.dtype], self._ptr(state), int(T), int(rnd),
-                self._ptr(hist), flags, self._stream()), "bkm_radix_hist_chunk")
+        self._call("bkm_radix_hist_chunk", *self._rows(x), self._ptr(state), int(T), int(rnd), self._ptr(hist),
+                   self._first(first))
 
     def radix_select_step(self, hist, state, d, T, rnd, dtype, q):
         """Extend each target's key prefix by the digit that holds its rank (after the round's all-reduce of hist);
         ``q`` the T / 2 quantiles in [0, 1]."""
         qh = (ctypes.c_double * len(q))(*[float(v) for v in q])
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.bkm_radix_select_step(self._ptr(hist), self._ptr(state), int(d), int(T), int(rnd),
-                                                      _DT_CODE[dtype], ctypes.cast(qh, ctypes.c_void_p),
-                                                      self._stream()), "bkm_radix_select_step")
+        self._call("bkm_radix_select_step", self._ptr(hist), self._ptr(state), int(d), int(T), int(rnd),
+                   _DT_CODE[dtype], ctypes.cast(qh, ctypes.c_void_p))
 
     def quantile_state_new(self, d, n_q):
         """Device state of one selection of the 2 ``n_q`` QuantileTransformer order statistics in each of d columns
         (``quantile_select_step``); column j's record starts at byte j * (16 + 80 n_q)."""
-        nb = ctypes.c_size_t(0)
-        _lib.check(self.lib.bkm_quantile_state_bytes(int(d), int(n_q), ctypes.byref(nb)), "bkm_quantile_state_bytes")
-        return torch.zeros(int(nb.value), dtype=torch.uint8, device=self.device)
+        nb = self._query("bkm_quantile_state_bytes", int(d), int(n_q))
+        return torch.zeros(nb, dtype=torch.uint8, device=self.device)
 
     def quantile_hist_chunk(self, x, state, n_q, rnd, hist, first=False):
         """hist (d, min(2 n_q, 256^rnd), 256) float64 (+)= the round-``rnd`` digit counts of the chunk's keys under each
         live prefix; ``first`` zeroes hist first."""
-        n, d = x.shape
-        flags = self.flags | (_lib.FLAG_FIRST_CHUNK if first else 0)
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.bkm_quantile_hist_chunk(
-                self._ptr(x), n, d, x.stride(0) if n else d, _DT_CODE[x.dtype], self._ptr(state), int(n_q), int(rnd),
-                self._ptr(hist), flags, self._stream()), "bkm_quantile_hist_chunk")
+        self._call("bkm_quantile_hist_chunk", *self._rows(x), self._ptr(state), int(n_q), int(rnd), self._ptr(hist),
+                   self._first(first))
 
     def quantile_select_step(self, hist, state, d, n_q, rnd, dtype, qf):
         """Extend each distinct rank's key prefix by one digit and build the next live list (after the round's
         all-reduce of hist); ``qf`` float64 (n_q,) ascending quantiles in [0, 1] on the device."""
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.bkm_quantile_select_step(self._ptr(hist), self._ptr(state), int(d), int(n_q), int(rnd),
-                                                         _DT_CODE[dtype], self._ptr(qf), self._stream()),
-                       "bkm_quantile_select_step")
+        self._call("bkm_quantile_select_step", self._ptr(hist), self._ptr(state), int(d), int(n_q), int(rnd),
+                   _DT_CODE[dtype], self._ptr(qf))
 
     def quantile_transform_chunk(self, x, qT, ref, inverse, distribution, clip_lo, clip_hi, out):
         """QuantileTransformer's per-element pass: ``qT`` float64 (d, n_q) quantiles per column, ``ref`` float64
         (n_q,), ``distribution`` 0 uniform / 1 normal; ``out`` float64 (n, d), any row pitch."""
         n, d = x.shape
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.bkm_quantile_transform_chunk(
-                self._ptr(x), n, d, x.stride(0) if n else d, _DT_CODE[x.dtype], self._ptr(qT), self._ptr(ref),
-                int(ref.shape[0]), int(bool(inverse)), int(distribution), float(clip_lo), float(clip_hi),
-                self._ptr(out), out.stride(0) if n else d, self._stream()), "bkm_quantile_transform_chunk")
+        self._call("bkm_quantile_transform_chunk", *self._rows(x), self._ptr(qT), self._ptr(ref), int(ref.shape[0]),
+                   int(bool(inverse)), int(distribution), float(clip_lo), float(clip_hi), self._ptr(out),
+                   self._ld(out, n, d))
 
     def impute_stats_chunk(self, x, miss_is_nan, miss, shift, acc, first=False):
         """SimpleImputer's statistics pass over one chunk, float64 on the device: acc (4, d) (+)= [missing count | NaN
         count | inf count | sum (x - shift) over the non-missing finite x].  ``miss`` a value of X's dtype (ignored
         with ``miss_is_nan``); ``shift`` float64 (d,) or None; ``first`` overwrites."""
         n, d = x.shape
-        nb = ctypes.c_size_t(0)
-        _lib.check(self.lib.bkm_impute_stats_workspace_bytes(int(n), int(d), ctypes.byref(nb)),
-                   "bkm_impute_stats_workspace_bytes")
-        ws = self._scratch("impute_stats", nb.value)
-        flags = self.flags | (_lib.FLAG_FIRST_CHUNK if first else 0)
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.bkm_impute_stats_chunk(
-                self._ptr(x), n, d, x.stride(0) if n else d, _DT_CODE[x.dtype], int(bool(miss_is_nan)), float(miss),
-                self._ptr(shift), self._ptr(acc), self._ptr(ws), ws.numel(), flags, self._stream()),
-                "bkm_impute_stats_chunk")
+        ws = self._scratch_for("impute_stats", "bkm_impute_stats_workspace_bytes", int(n), int(d))
+        self._call("bkm_impute_stats_chunk", *self._rows(x), int(bool(miss_is_nan)), float(miss), self._ptr(shift),
+                   self._ptr(acc), *self._ws_args(ws), self._first(first))
 
     def quantile_hist_masked_chunk(self, x, miss, state, n_q, rnd, hist, first=False):
         """``quantile_hist_chunk`` with the elements equal to ``miss`` (a number, not NaN) skipped as well."""
-        n, d = x.shape
-        flags = self.flags | (_lib.FLAG_FIRST_CHUNK if first else 0)
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.bkm_quantile_hist_masked_chunk(
-                self._ptr(x), n, d, x.stride(0) if n else d, _DT_CODE[x.dtype], float(miss), self._ptr(state),
-                int(n_q), int(rnd), self._ptr(hist), flags, self._stream()), "bkm_quantile_hist_masked_chunk")
+        self._call("bkm_quantile_hist_masked_chunk", *self._rows(x), float(miss), self._ptr(state), int(n_q), int(rnd),
+                   self._ptr(hist), self._first(first))
 
     def mode_count_chunk(self, x, miss_is_nan, miss, keys, counts, off, total, first=False):
         """Count the distinct non-missing values of each column of ``x`` (a group of g columns) into the hash tables
         ``keys`` / ``counts`` (uint64 as int64 (total,)), column j owning slots [off[j], off[j + 1]) (``off`` int64
         (g + 1,) on the device); ``first`` resets the tables."""
-        n, g = x.shape
-        flags = self.flags | (_lib.FLAG_FIRST_CHUNK if first else 0)
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.bkm_mode_count_chunk(
-                self._ptr(x), n, g, x.stride(0) if n else g, _DT_CODE[x.dtype], int(bool(miss_is_nan)), float(miss),
-                self._ptr(keys), self._ptr(counts), self._ptr(off), int(total), flags, self._stream()),
-                "bkm_mode_count_chunk")
+        self._call("bkm_mode_count_chunk", *self._rows(x), int(bool(miss_is_nan)), float(miss), self._ptr(keys),
+                   self._ptr(counts), self._ptr(off), int(total), self._first(first))
 
     def mode_best(self, keys, counts, off, g, total):
         """(best_key int64 (g,) holding uint64 keys, best_count float64 (g,), distinct float64 (g,)) on the device: per
@@ -943,55 +774,38 @@ class CudaBackend(object):
         key = torch.empty(g, dtype=torch.int64, device=self.device)
         cnt = torch.empty(g, dtype=torch.float64, device=self.device)
         nd = torch.empty(g, dtype=torch.float64, device=self.device)
-        nb = ctypes.c_size_t(0)
-        _lib.check(self.lib.bkm_mode_best_workspace_bytes(int(g), int(total), ctypes.byref(nb)),
-                   "bkm_mode_best_workspace_bytes")
-        ws = self._scratch("mode_best", nb.value)
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.bkm_mode_best(self._ptr(keys), self._ptr(counts), self._ptr(off), int(g), int(total),
-                                              self._ptr(key), self._ptr(cnt), self._ptr(nd), self._ptr(ws), ws.numel(),
-                                              self._stream()), "bkm_mode_best")
+        ws = self._scratch_for("mode_best", "bkm_mode_best_workspace_bytes", int(g), int(total))
+        self._call("bkm_mode_best", self._ptr(keys), self._ptr(counts), self._ptr(off), int(g), int(total),
+                   self._ptr(key), self._ptr(cnt), self._ptr(nd), *self._ws_args(ws))
         return key, cnt, nd
 
     def mode_compact(self, keys, counts, off, g, entries):
         """The occupied slots of the tables as rows {column, key >> 32, key & 0xffffffff, count} of ``entries``
         (float64 (m, 4), m at least the number of occupied slots)."""
         cursor = torch.empty(1, dtype=torch.int64, device=self.device)
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.bkm_mode_compact(self._ptr(keys), self._ptr(counts), self._ptr(off), int(g),
-                                                 self._ptr(entries), self._ptr(cursor), self._stream()),
-                       "bkm_mode_compact")
+        self._call("bkm_mode_compact", self._ptr(keys), self._ptr(counts), self._ptr(off), int(g), self._ptr(entries),
+                   self._ptr(cursor))
 
     def mode_merge(self, entries, keys, counts, off, g, total):
         """Reset the tables and add every row of ``entries`` (float64 (m, 4)) with a non-zero count."""
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.bkm_mode_merge(self._ptr(entries), int(entries.shape[0]), self._ptr(keys),
-                                               self._ptr(counts), self._ptr(off), int(g), int(total), self._stream()),
-                       "bkm_mode_merge")
+        self._call("bkm_mode_merge", self._ptr(entries), int(entries.shape[0]), self._ptr(keys), self._ptr(counts),
+                   self._ptr(off), int(g), int(total))
 
     def impute_chunk(self, x, miss_is_nan, miss, stats, cols, n_keep, n_ind, n_check, inverse, out, invalid=None):
         """SimpleImputer's fill pass (or its inverse) over one chunk into ``out`` (any row pitch, X's dtype; float32
         for bf16 rows): see include/bkm_b200.h.  ``stats`` float64 (d,), ``cols`` int32 on the device; ``invalid``
         float64 (2,) (+)= the NaN and inf counts of the elements read."""
-        n, d = x.shape
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.bkm_impute_chunk(
-                self._ptr(x), n, d, x.stride(0) if n else d, _DT_CODE[x.dtype], int(bool(miss_is_nan)), float(miss),
-                self._ptr(stats), self._ptr(cols), int(n_keep), int(n_ind), int(n_check), int(bool(inverse)),
-                self._ptr(out), out.stride(0) if n else int(out.shape[1]), _DT_CODE[out.dtype], self._ptr(invalid),
-                self._stream()), "bkm_impute_chunk")
+        self._call("bkm_impute_chunk", *self._rows(x), int(bool(miss_is_nan)), float(miss), self._ptr(stats),
+                   self._ptr(cols), int(n_keep), int(n_ind), int(n_check), int(bool(inverse)), self._ptr(out),
+                   self._ld(out, x.shape[0], int(out.shape[1])), _DT_CODE[out.dtype], self._ptr(invalid))
 
     def distinct_chunk(self, x, keys, counts, off, total, state, first=False):
         """Record the distinct keys of each column of ``x`` (a group of g columns, any element type of
         ``ENCODE_DTYPES``) in the tables ``keys`` / ``counts`` (uint64 as int64 (total,)), column j owning slots
         [off[j], off[j + 1]); ``state`` int64 (2, g) on the device (+)= [occupied slots | status bits: 1 overflow,
         2 holds INT64_MAX]; ``first`` resets tables and state."""
-        n, g = x.shape
-        flags = self.flags | (_lib.FLAG_FIRST_CHUNK if first else 0)
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.bkm_distinct_chunk(
-                self._ptr(x), n, g, x.stride(0) if n else g, _ENC_CODE[x.dtype], self._ptr(keys), self._ptr(counts),
-                self._ptr(off), int(total), self._ptr(state), flags, self._stream()), "bkm_distinct_chunk")
+        self._call("bkm_distinct_chunk", *self._rows(x, _ENC_CODE), self._ptr(keys), self._ptr(counts), self._ptr(off),
+                   int(total), self._ptr(state), self._first(first))
 
     def encode_chunk(self, x, cat_keys, cat_off, n_cats, layout, out, unknown, indices=None):
         """One read of ``x`` (n, d): codes, a dense one-hot block or the CSR indices / data of every element, by its
@@ -1002,27 +816,15 @@ class CudaBackend(object):
             ld = int(n_cats)
         else:
             ld = out.stride(0) if layout == _lib.ENCODE_CODES and n else d
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.bkm_encode_chunk(
-                self._ptr(x), n, d, x.stride(0) if n else d, _ENC_CODE[x.dtype], self._ptr(cat_keys),
-                self._ptr(cat_off), int(n_cats), int(layout), self._ptr(out), ld, _ENC_CODE[out.dtype],
-                self._ptr(indices), self._ptr(unknown), self._stream()), "bkm_encode_chunk")
+        self._call("bkm_encode_chunk", *self._rows(x, _ENC_CODE), self._ptr(cat_keys), self._ptr(cat_off), int(n_cats),
+                   int(layout), self._ptr(out), ld, _ENC_CODE[out.dtype], self._ptr(indices), self._ptr(unknown))
 
     def decode_chunk(self, codes, cat_vals, cat_off, out, unknown):
         """out (n, d) = cat_vals[cat_off[j] + codes[:, j]] (``codes`` int32 / int64 (n, d), ``cat_vals`` any dtype of
         1, 2, 4 or 8 bytes, ``out`` of the same dtype); codes outside [0, K_j) add to ``unknown``."""
         n, d = codes.shape
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.bkm_decode_chunk(
-                self._ptr(codes), n, d, codes.stride(0) if n else d, _ENC_CODE[codes.dtype], self._ptr(cat_vals),
-                self._ptr(cat_off), cat_vals.element_size(), self._ptr(out), out.stride(0) if n else d,
-                self._ptr(unknown), self._stream()), "bkm_decode_chunk")
-
-    def _text_workspace(self, n_bytes, n_docs, n_pairs):
-        nb = ctypes.c_size_t(0)
-        _lib.check(self.lib.bkm_text_workspace_bytes(int(n_bytes), int(n_docs), int(n_pairs), ctypes.byref(nb)),
-                   "bkm_text_workspace_bytes")
-        return self._scratch("text", nb.value)
+        self._call("bkm_decode_chunk", *self._rows(codes, _ENC_CODE), self._ptr(cat_vals), self._ptr(cat_off),
+                   cat_vals.element_size(), self._ptr(out), self._ld(out, n, d), self._ptr(unknown))
 
     def text_tokens_chunk(self, buf, doc_off, min_n, max_n, tok_start, tok_off, pair_off, totals):
         """HashingVectorizer's token pass over the documents packed in ``buf`` (uint8, each document ending in a byte
@@ -1030,12 +832,10 @@ class CudaBackend(object):
         len(buf) // 3 + 1,) the tokens' byte positions, ``tok_off`` / ``pair_off`` int64 (n + 1,) each document's first
         token and first n-gram of length in [min_n, max_n]; ``totals`` int64 (3,) [0:2] = the token and n-gram counts."""
         nb, n = int(buf.numel()), int(doc_off.numel()) - 1
-        ws = self._text_workspace(nb, n, 0)
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.bkm_text_tokens_chunk(
-                self._ptr(buf), nb, self._ptr(doc_off), n, int(min_n), int(max_n), self._ptr(tok_start),
-                int(tok_start.numel()), self._ptr(tok_off), self._ptr(pair_off), self._ptr(totals), self._ptr(ws),
-                ws.numel(), self._stream()), "bkm_text_tokens_chunk")
+        ws = self._scratch_for("text", "bkm_text_workspace_bytes", nb, n, 0)
+        self._call("bkm_text_tokens_chunk", self._ptr(buf), nb, self._ptr(doc_off), n, int(min_n), int(max_n),
+                   self._ptr(tok_start), int(tok_start.numel()), self._ptr(tok_off), self._ptr(pair_off),
+                   self._ptr(totals), *self._ws_args(ws))
 
     def text_hash_chunk(self, buf, tok_start, tok_off, pair_off, n_tokens, n_pairs, min_n, max_n, lowercase,
                         n_features, alternate_sign, binary, norm, dtype, keys, indptr, scale, totals):
@@ -1044,40 +844,32 @@ class CudaBackend(object):
         of the output in ``dtype`` (torch float32 / float64) with ``norm`` None / 'l1' / 'l2'; totals[2] = stored
         entries."""
         nb, n = int(buf.numel()), int(pair_off.numel()) - 1
-        ws = self._text_workspace(nb, n, n_pairs)
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.bkm_text_hash_chunk(
-                self._ptr(buf), nb, self._ptr(tok_start), self._ptr(tok_off), self._ptr(pair_off), n, int(n_tokens),
-                int(n_pairs), int(min_n), int(max_n), int(bool(lowercase)), int(n_features), int(bool(alternate_sign)),
-                int(bool(binary)), _lib.TEXT_NORM[norm], _DT_CODE[dtype], self._ptr(keys), self._ptr(indptr),
-                self._ptr(scale), self._ptr(totals), self._ptr(ws), ws.numel(), self._stream()), "bkm_text_hash_chunk")
+        ws = self._scratch_for("text", "bkm_text_workspace_bytes", nb, n, int(n_pairs))
+        self._call("bkm_text_hash_chunk", self._ptr(buf), nb, self._ptr(tok_start), self._ptr(tok_off),
+                   self._ptr(pair_off), n, int(n_tokens), int(n_pairs), int(min_n), int(max_n), int(bool(lowercase)),
+                   int(n_features), int(bool(alternate_sign)), int(bool(binary)), _lib.TEXT_NORM[norm],
+                   _DT_CODE[dtype], self._ptr(keys), self._ptr(indptr), self._ptr(scale), self._ptr(totals),
+                   *self._ws_args(ws))
 
     def text_write_chunk(self, keys, pair_off, indptr, scale, binary, indices, data):
         """Write the CSR ``indices`` int64 and ``data`` (float32 / float64) of every stored entry."""
         n = int(pair_off.numel()) - 1
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.bkm_text_write_chunk(
-                self._ptr(keys), self._ptr(pair_off), self._ptr(indptr), self._ptr(scale), n, int(bool(binary)),
-                self._ptr(indices), self._ptr(data), _DT_CODE[data.dtype], self._stream()), "bkm_text_write_chunk")
+        self._call("bkm_text_write_chunk", self._ptr(keys), self._ptr(pair_off), self._ptr(indptr), self._ptr(scale),
+                   n, int(bool(binary)), self._ptr(indices), self._ptr(data), _DT_CODE[data.dtype])
 
     def affine_chunk(self, x, a, b, op1, op2, out):
         """out = op2(op1(x, a), b) per element (op1: 0 none, 1 subtract a, 2 multiply by a; op2: 0 none, 1 divide by b,
         2 add b), each step rounded once in out's dtype.  ``a``, ``b`` float64 (d,) or None; ``out`` (n, d) float32 /
         float64, any row pitch."""
         n, d = x.shape
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.bkm_affine_chunk(
-                self._ptr(x), n, d, x.stride(0) if n else d, _DT_CODE[x.dtype], self._ptr(a), self._ptr(b), int(op1),
-                int(op2), self._ptr(out), out.stride(0) if n else d, _DT_CODE[out.dtype], self._stream()),
-                "bkm_affine_chunk")
+        self._call("bkm_affine_chunk", *self._rows(x), self._ptr(a), self._ptr(b), int(op1), int(op2), self._ptr(out),
+                   self._ld(out, n, d), _DT_CODE[out.dtype])
 
     def split_indices_chunk(self, seed, c, start, count, offset):
         """int64 (count,) on the device: ``offset + pi_seed(start + i)``, the split permutation of a block of ``c`` rows
         (include/bkm_b200.h) at positions [start, start + count)."""
         out = torch.empty(int(count), dtype=torch.int64, device=self.device)
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.bkm_split_indices_chunk(int(seed), int(c), int(start), int(count), int(offset),
-                                                        self._ptr(out), self._stream()), "bkm_split_indices_chunk")
+        self._call("bkm_split_indices_chunk", int(seed), int(c), int(start), int(count), int(offset), self._ptr(out))
         return out
 
     def gather_rows_chunk(self, src, idx, idx_offset=0):
@@ -1098,10 +890,8 @@ class CudaBackend(object):
         if n == 0:
             raise IndexError("cannot gather rows of an empty block")
         ld_src = src.stride(0) * esz if (src.dim() == 2 and n > 1) else row_bytes
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.bkm_gather_rows_chunk(self._ptr(src), n, row_bytes, ld_src, self._ptr(idx),
-                                                      int(idx_offset), count, self._ptr(out), row_bytes,
-                                                      self._stream()), "bkm_gather_rows_chunk")
+        self._call("bkm_gather_rows_chunk", self._ptr(src), n, row_bytes, ld_src, self._ptr(idx), int(idx_offset),
+                   count, self._ptr(out), row_bytes)
         return out
 
     def metric_chunk(self, a, b, mode, acc, w=None, shift=None, eps=0.0, first=False):
@@ -1112,35 +902,44 @@ class CudaBackend(object):
         ``b`` (n,) or (n, K) probabilities clipped to [eps, 1 - eps] and renormalised.  ``first`` overwrites acc."""
         n = int(b.shape[0])
         m = int(b.shape[1]) if b.dim() == 2 else 1
-        nb = ctypes.c_size_t(0)
-        _lib.check(self.lib.bkm_metric_workspace_bytes(n, m, int(mode), ctypes.byref(nb)),
-                   "bkm_metric_workspace_bytes")
-        ws = self._scratch("metric", nb.value)
-        flags = _lib.FLAG_FIRST_CHUNK if first else 0
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.bkm_metric_chunk(
-                self._ptr(a), _METRIC_CODE[a.dtype], self._ptr(b), _METRIC_CODE[b.dtype], self._ptr(w), n, m, int(mode),
-                self._ptr(shift), float(eps), self._ptr(acc), self._ptr(ws), ws.numel(), flags, self._stream()),
-                "bkm_metric_chunk")
+        ws = self._scratch_for("metric", "bkm_metric_workspace_bytes", n, m, int(mode))
+        flags = _lib.FLAG_FIRST_CHUNK if first else 0        # bkm_metric_chunk reads no other flag; not self.flags
+        self._call("bkm_metric_chunk", self._ptr(a), _METRIC_CODE[a.dtype], self._ptr(b), _METRIC_CODE[b.dtype],
+                   self._ptr(w), n, m, int(mode), self._ptr(shift), float(eps), self._ptr(acc), *self._ws_args(ws),
+                   flags)
 
     def nystrom_embed(self, x, pack, l, gamma, W, out):
         """out[i] = e_i / ||e_i||, e_i = sum_j exp(-gamma (||x_i - c_j||^2 - min_j ||x_i - c_j||^2)) W[j] — the second
         pass of the Nystrom embedding.  ``W`` is (l, k) in the dtype of x; ``out`` (n, k) may have a padded row pitch."""
-        n, d = x.shape
         k = int(W.shape[1])
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.bkm_nystrom_embed_chunk(
-                self._ptr(x), n, d, x.stride(0) if n else d, _DT_CODE[x.dtype], self._ptr(pack), int(l), float(gamma),
-                self._ptr(W), k, self._ptr(out), out.stride(0) if n else k, self.flags, self._stream()),
-                "bkm_nystrom_embed_chunk")
+        self._call("bkm_nystrom_embed_chunk", *self._rows(x), self._ptr(pack), int(l), float(gamma), self._ptr(W), k,
+                   self._ptr(out), self._ld(out, x.shape[0], k), self.flags)
         self._note_fallback(x)
 
     def finalize(self, sums, counts, C_old, C_new, shift):
         k, d = C_old.shape
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.bkm_finalize(self._ptr(sums), self._ptr(counts), self._ptr(C_old),
-                                             self._ptr(C_new), self._ptr(shift), k, d, self._stream()),
-                       "bkm_finalize")
+        self._call("bkm_finalize", self._ptr(sums), self._ptr(counts), self._ptr(C_old), self._ptr(C_new),
+                   self._ptr(shift), k, d)
+
+    # -- dataset generators -------------------------------------------------------------
+    def make_blobs_chunk(self, X, y, centers, std, seed):
+        """One block of ``datasets.make_blobs``: X (m, d) float32 / float64 rows centers[y_i] + std[y_i] N(0, I) and
+        y (m,) int64 their centre, from the block's ``seed`` (``centers`` float64 (k, d), ``std`` float64 (k,) on the
+        device)."""
+        m, d = X.shape
+        self._call("bkm_make_blobs_chunk", self._ptr(X), self._ptr(y), m, d, d, _DT_CODE[X.dtype], self._ptr(centers),
+                   self._ptr(std), int(centers.shape[0]), int(seed))
+
+    def make_glm_chunk(self, X, y, row0, family, info, n_targets, bias, noise, key, flag=None):
+        """One block of the stream of make_classification / make_regression / make_counts (include/bkm_b200.h): X
+        (m, d) float32 / float64 from global row ``row0`` under ``key`` and its response y of ``family``, ``info``
+        float64 (n_info, 1 + n_targets) on the device or None; ``flag`` int32 (1,) ORs in 1 for a rejected poisson
+        rate."""
+        m, d = X.shape
+        n_info = int(info.shape[0]) if info is not None else 0
+        self._call("bkm_make_glm_chunk", self._ptr(X), self._ptr(y), m, d, d, _DT_CODE[X.dtype], int(row0),
+                   int(family), self._ptr(info), n_info, int(n_targets), float(bias), float(noise), int(key),
+                   self._ptr(flag))
 
 
 def _host_unregister(tensors):

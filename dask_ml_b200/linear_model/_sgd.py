@@ -148,7 +148,7 @@ class _PartialSGDMixin(_PartialMixin):
         out = np.empty((len(seeds), n), dtype=np.int32)
         for p, seed in enumerate(seeds):
             if self.shuffle:
-                _lib.check(_lib.load().bkm_sgd_order(n, int(seed), out[p].ctypes.data), "bkm_sgd_order")
+                _lib.call("bkm_sgd_order", n, int(seed), out[p].ctypes.data)
             else:
                 out[p] = np.arange(n, dtype=np.int32)
         return out
