@@ -37,6 +37,7 @@ FLAG_FORCE_TC = 2
 FLAG_NO_RECHECK = 4
 FLAG_FIRST_CHUNK = 8
 FLAG_COUNTS_F64 = 16
+FLAG_FULL_PROBE = 32
 
 _c_void_p = ctypes.c_void_p
 _i64 = ctypes.c_int64

@@ -10,7 +10,9 @@
 //                            power of two >= 2 x the values it can receive: it never fills.
 //   bkm_distinct_chunk       per column, every distinct key (count 1).  Tables start small: a column whose occupancy
 //                            passes half its capacity, or whose probe chain passes kMaxProbe, is flagged and the host
-//                            grows it and runs the group again.  Before it probes global memory, the leader looks the
+//                            grows it and runs the group again.  With BKM_FLAG_FULL_PROBE the bound is the capacity: a
+//                            table sized so that it can never pass half full then never overflows: a chain longer than
+//                            kMaxProbe is walked, not grown away.  Before it probes global memory, the leader looks the
 //                            key up in a per-CTA, per-column direct-mapped cache of keys already in the table (shared
 //                            memory): a column of few distinct values costs about one global lookup per value per CTA.
 //                            INT64_MAX, whose key is kEmpty, is carried as a per-column flag.
@@ -73,6 +75,7 @@ struct ScanArgs {
   const long long* off;            // [g + 1]
   unsigned long long* occupied;    // !COUNT: [g]
   unsigned long long* status;      // !COUNT: [g]
+  int full_probe;                  // !COUNT: probe bound the capacity instead of min(capacity, kMaxProbe)
 };
 
 // COUNT: add each non-missing, non-NaN value's multiplicity to its key's count.  !COUNT: record each key (count 1),
@@ -140,7 +143,8 @@ __global__ void __launch_bounds__(kThreads) key_scan_kernel(ScanArgs a) {
           volatile unsigned long long* slot = s_cache + c * FS + (int)((mix64(key) >> 40) & (FS - 1));
           if (*slot == key) continue;
           bool claimed = false;
-          const long long h = probe<true>(a.keys + o, cap, cap < kMaxProbe ? cap : kMaxProbe, key, &claimed);
+          const long long h = probe<true>(a.keys + o, cap, a.full_probe || cap < kMaxProbe ? cap : kMaxProbe, key,
+                                            &claimed);
           if (h < 0) {
             atomicOr(a.status + j, (unsigned long long)ST_OVERFLOW);
             continue;
@@ -359,6 +363,7 @@ extern "C" int bkm_distinct_chunk(const void* X, int64_t n, int g, int64_t ldx, 
   ScanArgs a = {};
   a.X = X; a.n = n; a.g = g; a.ldx = ldx; a.keys = keys; a.counts = counts;
   a.off = reinterpret_cast<const long long*>(slot_off); a.occupied = state; a.status = state + g;
+  a.full_probe = (flags & BKM_FLAG_FULL_PROBE) ? 1 : 0;
   switch (x_dtype) {
     case BKM_F32: return launch_key_scan<float, false>(a, sms, s);
     case BKM_F64: return launch_key_scan<double, false>(a, sms, s);

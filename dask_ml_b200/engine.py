@@ -799,13 +799,15 @@ class CudaBackend(object):
                    self._ptr(cols), int(n_keep), int(n_ind), int(n_check), int(bool(inverse)), self._ptr(out),
                    self._ld(out, x.shape[0], int(out.shape[1])), _DT_CODE[out.dtype], self._ptr(invalid))
 
-    def distinct_chunk(self, x, keys, counts, off, total, state, first=False):
+    def distinct_chunk(self, x, keys, counts, off, total, state, first=False, full_probe=False):
         """Record the distinct keys of each column of ``x`` (a group of g columns, any element type of
         ``ENCODE_DTYPES``) in the tables ``keys`` / ``counts`` (uint64 as int64 (total,)), column j owning slots
         [off[j], off[j + 1]); ``state`` int64 (2, g) on the device (+)= [occupied slots | status bits: 1 overflow,
-        2 holds INT64_MAX]; ``first`` resets tables and state."""
+        2 holds INT64_MAX]; ``first`` resets tables and state; ``full_probe`` bounds a probe by the capacity, not by
+        1024 slots."""
+        flags = self._first(first) | (_lib.FLAG_FULL_PROBE if full_probe else 0)
         self._call("bkm_distinct_chunk", *self._rows(x, _ENC_CODE), self._ptr(keys), self._ptr(counts), self._ptr(off),
-                   int(total), self._ptr(state), self._first(first))
+                   int(total), self._ptr(state), flags)
 
     def encode_chunk(self, x, cat_keys, cat_off, n_cats, layout, out, unknown, indices=None):
         """One read of ``x`` (n, d): codes, a dense one-hot block or the CSR indices / data of every element, by its

@@ -3,7 +3,8 @@ the encoding passes (DESIGN.md, "The passes of the encoders"):
 
     fit (bkm_distinct_chunk, one read of X per column group and growth step): every distinct value's order-preserving
                     key in a per-column hash table that starts at INITIAL_SLOTS slots; a column whose table passes half
-                    full is grown (x8, capped by its key space and rows) and its group runs again.  The occupied keys are
+                    full is grown (x8, capped by its key space and rows) and its group runs again; one whose table is
+                    at that cap runs again with probes bounded by the capacity.  The occupied keys are
                     compacted (bkm_mode_compact) and sorted per column in torch.  With several ranks the tables are
                     gathered by the sum all-reduce and merged (bkm_mode_merge), as SimpleImputer's mode does
     transform (bkm_encode_chunk, one read of X): codes, the dense one-hot matrix or the CSR indices, by binary search
@@ -159,18 +160,29 @@ def _group_keys(X, j0, j1):
     """Every distinct key of columns [j0, j1) over every rank: (column within the group, key) int64 device tensors,
     unsorted."""
     be, comm, g = X.backend, X.comm, j1 - j0
-    limit = _keytables.capacity(max(1, X.n_local), X.dtype)         # a table that cannot overflow
+    limit = _keytables.capacity(max(1, X.n_local), X.dtype)         # a table that is never more than half full
     caps = np.full(g, min(INITIAL_SLOTS, limit), dtype=np.int64)
+    full = False
     while True:
         keys, counts, off, total = _keytables.alloc(be, caps)
         state = be.zeros((2, g), torch.int64)
+        # full_probe is passed only when set: a backend without it still runs every group that does not need it
+        probe = {"full_probe": True} if full else {}
         for i, x in enumerate(X.chunks):
-            be.distinct_chunk(x[:, j0:j1], keys, counts, off, total, state, first=i == 0)
+            be.distinct_chunk(x[:, j0:j1], keys, counts, off, total, state, first=i == 0, **probe)
         st = state.cpu().numpy()
         over = (st[1] & 1) != 0
         if not over.any():
             break
-        caps[over] = np.where(caps[over] < limit, np.minimum(caps[over] * GROWTH, limit), caps[over] * 2)
+        # a table at its limit overflows only by a probe chain past 1024 slots, which a larger table need not
+        # shorten (keys may share any number of low hash bits): the group runs again with probes bounded by the
+        # capacity, which such a table never fills
+        at_limit = over & (caps >= limit)
+        if full and at_limit.any():
+            raise RuntimeError("a key table at its limit overflowed under a full probe")
+        full = full or bool(at_limit.any())
+        grow = over & ~at_limit
+        caps[grow] = np.minimum(caps[grow] * GROWTH, limit)
     occupied, marker = st[0], (st[1] & 2) != 0
     if comm.world > 1:
         (keys, counts, off, total), (_, _, nd), marker = _keytables.merge_ranks(

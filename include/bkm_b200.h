@@ -113,8 +113,9 @@ extern "C" {
  *     bkm_sparse_minibatch_step
  * 9 = bkm_sgd_order, bkm_sgd_block, bkm_sgd_csr_block
  * 10 = bkm_class_counts_chunk, bkm_csc_class_counts_chunk, bkm_nb_linear_jll_chunk, bkm_nb_csr_jll_chunk
- * 11 = bkm_debug_tc_layout */
-#define BKM_VERSION_MINOR 11
+ * 11 = bkm_debug_tc_layout
+ * 12 = BKM_FLAG_FULL_PROBE of bkm_distinct_chunk */
+#define BKM_VERSION_MINOR 12
 
 /* element types of X */
 #define BKM_F32 0
@@ -137,6 +138,7 @@ extern "C" {
                                      instead of accumulating: saves the memsets of the step */
 #define BKM_FLAG_COUNTS_F64  16   /* bkm_lloyd_chunk: `counts` points to float64 (so that sums | counts | inertia are ONE
                                      float64 buffer for the per-iteration all-reduce) */
+#define BKM_FLAG_FULL_PROBE  32   /* bkm_distinct_chunk: probe up to the table's capacity, not up to 1024 slots */
 
 int bkm_version(void);
 const char* bkm_error_string(int code);
@@ -781,8 +783,9 @@ int bkm_impute_chunk(const void* X, int64_t n, int d, int64_t ldx, int x_dtype, 
  *                        state [2][g] uint64: [occupied slots | status bits]; status 1 = OVERFLOW (the occupancy passed
  *                        half the capacity or a probe chain passed 1024 slots: the column's table is incomplete, grow it
  *                        and run the group again), 2 = MARKER (the column holds the key ~0, i.e. INT64_MAX, which the
- *                        tables cannot store).  With BKM_FLAG_FIRST_CHUNK the tables and state are reset first, else
- *                        ACCUMULATED.
+ *                        tables cannot store).  With BKM_FLAG_FULL_PROBE the probe bound is the capacity instead of 1024
+ *                        slots: a table that can never pass half full then never overflows.  With BKM_FLAG_FIRST_CHUNK
+ *                        the tables and state are reset first, else ACCUMULATED.
  *   bkm_encode_chunk     cat_keys [n_cats] uint64: column j's sorted keys at [cat_off[j], cat_off[j + 1]) (cat_off [d + 1]
  *                        int64, device).  The code of x[i, j] is the position of its key in its column's list.
  *                        layout CODES: out [n][ld_out >= d] int64 codes (-1 for an unknown key; out_dtype ignored).

@@ -329,6 +329,7 @@ def _drive(rec, be):
     dstate = t("dstate", (2, g), i64)
     s("distinct/first", be.distinct_chunk, xi, keys, kcounts, off, total, dstate, first=True)
     s("distinct/next", be.distinct_chunk, x[:, :g], keys, kcounts, off, total, dstate)
+    s("distinct/full", be.distinct_chunk, x[:, :g], keys, kcounts, off, total, dstate, full_probe=True)
     cat_keys, cat_off, unknown = t("cat_keys", 8, i64), t("cat_off", 3, i64), t("unknown", 1 + 2 + 2 * 8, i64)
     codes = t("codes", (n, 4), i32)
     s("encode/codes", be.encode_chunk, xi, cat_keys, cat_off, 7, _lib.ENCODE_CODES, codes[:, :2], unknown)
