@@ -134,6 +134,19 @@ class _SparseData(object):
         return self._csc
 
 
+# The label-sum pass over a block's transpose (bkm_csc_label_sums_chunk, bkm_csc_class_counts_chunk) keeps one k-wide
+# float64 accumulator per warp in 200 KB of shared memory, so it takes at most this many clusters or classes.
+MAX_LABEL_SUM_CLASSES = 25600
+
+
+def check_label_sum_classes(k, what):
+    """ValueError at intake when sparse X would need the label-sum pass for more than MAX_LABEL_SUM_CLASSES values of
+    ``what`` ("clusters" or "classes")."""
+    if int(k) > MAX_LABEL_SUM_CLASSES:
+        raise ValueError("Sparse input supports at most %d %s, got %d: the label-sum pass keeps a float64 sum for "
+                         "each of them in shared memory" % (MAX_LABEL_SUM_CLASSES, what, int(k)))
+
+
 def _sparse_values(v):
     """float32 / float64 values as they are; integer and bool values widened once to float64."""
     if v.dtype in (torch.float32, torch.float64):

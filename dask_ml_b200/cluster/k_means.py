@@ -18,7 +18,7 @@ from sklearn.base import BaseEstimator, TransformerMixin
 from sklearn.utils.validation import check_is_fitted
 
 from ..chunked import ChunkedArray, as_chunked, is_dask_array, is_dask_dataframe, _is_torch
-from .._sparse import _SparseData, _sparse_data
+from .._sparse import _SparseData, _sparse_data, check_label_sum_classes
 from ..engine import Comm, CudaBackend, DeviceData, _NP_TO_TORCH
 from ..utils import _timed, _timer, check_array
 
@@ -937,6 +937,8 @@ def _kmeans_single_lloyd(
 ):
     """Lloyd iterations with the reference's exact control flow (k_means.py:499-569)."""
     X = _to_device_data(X)
+    if isinstance(X, _SparseData):
+        check_label_sum_classes(n_clusters, "clusters")
     centers = k_init(
         X,
         n_clusters,

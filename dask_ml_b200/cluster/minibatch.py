@@ -27,7 +27,7 @@ from sklearn.utils import check_array as _sk_check_array
 from sklearn.utils import check_random_state
 from sklearn.utils.validation import _is_arraylike_not_scalar, check_is_fitted
 
-from .._sparse import _SparseData
+from .._sparse import _SparseData, check_label_sum_classes
 from ..chunked import ChunkedArray
 from ..engine import StreamedChunks, single_process
 from . import k_means as _km
@@ -411,6 +411,8 @@ class PartialMiniBatchKMeans(MiniBatchKMeans):
                              % (X.d, type(self).__name__))
         if has_centers:
             self._check_n_features(X)
+        elif isinstance(X, _SparseData):
+            check_label_sum_classes(self.n_clusters, "clusters")
         self._random_state = getattr(self, "_random_state", check_random_state(self.random_state))
         self.n_steps_ = getattr(self, "n_steps_", 0)
 

@@ -49,7 +49,7 @@ from sklearn.utils.validation import _check_sample_weight, check_is_fitted
 
 from . import _lib
 from ._partial import _PartialMixin, _accuracy, _block_data, _copy_partial_doc
-from ._sparse import _SparseData
+from ._sparse import _SparseData, check_label_sum_classes
 from .chunked import ChunkedArray, _is_torch, _y_flat, block_to_numpy
 from .decomposition.pca import _device_data
 from .engine import single_process as _single_process
@@ -328,6 +328,8 @@ class _PartialDiscreteNBMixin(_PartialMixin):
         b = self._batch(X, y)
         thr = self._threshold(b.np_dtype, b.sparse)
         self._check_features(b, first_call)
+        if b.sparse and (classes is not None or not first_call):
+            check_label_sum_classes(len(np.unique(classes)) if classes is not None else len(self.classes_), "classes")
         be = b.backend
         if _check_partial_fit_first_call(self, classes):
             self._nb = _CountState(be, len(classes), b.d)
