@@ -27,10 +27,10 @@
 //   after the warpgroup's last read of the slot, the load of tile lt + S into it (no separate producer).
 // The M-step adds the tile's rows in row order into the CTA's sums; the two warpgroups take turns (named barriers),
 // so every cluster's sum is formed in one fixed order and the sums are bit-reproducible.  Each sums element has one
-// owning thread (feature f, label parity q); before its turn a warp lists the tile's rows of its parity, so that the
-// turn touches only owned rows, and marks the batches of 8 rows in which a label repeats (only those forward running
-// sums).  The turn order is kept per warp pair: warp w of each warpgroup owns the same elements.  One warpgroup's MMAs
-// overlap the other's epilogue / M-step.
+// owning thread (feature pair f2, label class q = c % 4, warp q of its warpgroup); before its turn a warp lists the
+// tile's rows of its class, so that the turn touches only owned rows, and marks the batches of 8 rows in which a label
+// repeats (only those forward running sums).  The turn order is kept per warp pair: warp w of each warpgroup owns the
+// same elements.  One warpgroup's MMAs overlap the other's epilogue / M-step.
 #include "bkm_common.cuh"
 #include "bkm_wgmma.cuh"
 #include <cuda.h>
@@ -94,11 +94,12 @@ __device__ __forceinline__ uint32_t xsw(int r, int f) {
   return (uint32_t)((f >> 5) * XBOX_BYTES + r * 128 + ((((f >> 2) & 7) ^ (r & 7)) << 4) + (f & 3) * 4);
 }
 // M-step class-list entry of row `row` of a tile with label `c`: the byte offset of sums row c (bits 0-16) and the row's
-// part of its slot offset, 128 row | (row & 7) << 4 (bits 17-31).  Rows of the sums are 64 floats, so a thread adds 4 f to
-// the first; to the second it applies its feature's swizzle, ^ ((f >> 2) & 7) << 4, and adds its box and (f & 3) * 4.
+// part of its slot offset, 128 row | (row & 7) << 4 (bits 17-31).  Rows of the sums are 64 floats, so a thread adds 8 f2
+// (its feature pair 2 f2, 2 f2 + 1) to the first; to the second it applies the pair's swizzle, ^ ((f2 >> 1) & 7) << 4,
+// and adds its box (f2 >> 4) and (f2 & 1) * 8.
 static const int CLS_ROW_SHIFT = 17;
 static const uint32_t CLS_SUM_MASK = (1u << CLS_ROW_SHIFT) - 1u;
-static_assert((256 + 1) * 64 * 4 <= (int)CLS_SUM_MASK && ((TBM - 1) * 128 | 0x70) < (1 << (32 - CLS_ROW_SHIFT)), "class-list entry fields");
+static_assert((256 - 1) * 64 * 4 <= (int)CLS_SUM_MASK && ((TBM - 1) * 128 | 0x70) < (1 << (32 - CLS_ROW_SHIFT)), "class-list entry fields");
 __device__ __forceinline__ uint32_t cls_entry(int c, int row) {
   return ((uint32_t)(row * 128 | (row & 7) << 4) << CLS_ROW_SHIFT) | (uint32_t)(c * 64 * 4);
 }
@@ -126,7 +127,7 @@ tc_chunk_kernel(ChunkArgs a, typename TcCfgOf<EPI>::type cfg, const __grid_const
   const int d = a.d, k = a.k;
   float* cn_s = reinterpret_cast<float*>(smem + cfg.off_cn);          // [N] s^2 ||c||^2 (padded columns: 3e38)
   int* cnt_s = reinterpret_cast<int*>(smem + cfg.off_cnt);            // [N]
-  float* sum_s = reinterpret_cast<float*>(smem + cfg.off_sum);        // [N + 2][64] (rows N, N + 1: M-step list padding)
+  float* sum_s = reinterpret_cast<float*>(smem + cfg.off_sum);        // [N][64]
   int* lab_s = reinterpret_cast<int*>(smem + cfg.off_lab) + wgi * TBM;        // label of each row of the tile, -1: none
   float* dp_s = reinterpret_cast<float*>(smem + cfg.off_dp) + wgi * 2 * TBM;  // [2][TBM] halves of the direct distances
   double* red_s = reinterpret_cast<double*>(smem + cfg.off_ring);    // teardown only: the ring is drained by then
@@ -153,7 +154,7 @@ tc_chunk_kernel(ChunkArgs a, typename TcCfgOf<EPI>::type cfg, const __grid_const
       cnt_s[j] = 0;
     }
     if (MSTEP)
-      for (int i = tid; i < (N + 2) * 64; i += TC_THREADS) sum_s[i] = 0.f;
+      for (int i = tid; i < N * 64; i += TC_THREADS) sum_s[i] = 0.f;
     if constexpr (EPI == EPI_EMBED) {
       // W rows j < k (keep rows), outputs o < kw; zero elsewhere
       float* w_s = reinterpret_cast<float*>(smem + cfg.off_w);
@@ -467,23 +468,23 @@ tc_chunk_kernel(ChunkArgs a, typename TcCfgOf<EPI>::type cfg, const __grid_const
         }
       }
       if (MSTEP) {
-        // thread (feature f, parity q) owns sums[c][f] of the clusters c with c % 2 == q (q is warp-uniform).  Before
-        // its turn each warp lists the tile's rows of its class in row order, as byte offsets (cls_entry), and pads the
-        // list to a multiple of 8 with the warp's spare sums row N + q (never read back); deferred rows are left out.
-        // Then it marks the list positions whose label repeats an earlier one of the same batch of 8
-        const int f = t & 63, q = t >> 6;
+        // thread (feature pair f2, class q) owns sums[c][2 f2] and sums[c][2 f2 + 1] of the clusters c with c % 4 == q,
+        // where q is the warp's index in its warpgroup: a warp covers all 64 features of one class, in 64-bit accesses.
+        // Before its turn each warp lists the tile's rows of its class in row order, as byte offsets (cls_entry);
+        // deferred rows are left out.  Then it marks the list positions whose label repeats an earlier one of the same
+        // batch of 8
+        const int f2 = lane, q = wq;
         uint32_t* cls = reinterpret_cast<uint32_t*>(smem + cfg.off_cls) + (tid >> 5) * TBM;
         int ncls = 0;
         uint64_t rep = 0;                                    // bit i: list position i repeats a label of its batch
         if (has) {
           const int la = lab_s[lane], lb = lab_s[32 + lane];
-          const unsigned ma = __ballot_sync(0xffffffffu, la >= 0 && (la & 1) == q);
-          const unsigned mb = __ballot_sync(0xffffffffu, lb >= 0 && (lb & 1) == q);
+          const unsigned ma = __ballot_sync(0xffffffffu, la >= 0 && (la & 3) == q);
+          const unsigned mb = __ballot_sync(0xffffffffu, lb >= 0 && (lb & 3) == q);
           const unsigned lt = (1u << lane) - 1u;
           if ((ma >> lane) & 1u) cls[__popc(ma & lt)] = cls_entry(la, lane);
           if ((mb >> lane) & 1u) cls[__popc(ma) + __popc(mb & lt)] = cls_entry(lb, 32 + lane);
           ncls = __popc(ma) + __popc(mb);
-          if (lane < ((-ncls) & 7)) cls[ncls + lane] = cls_entry(N + q, 0);
           __syncwarp();
           for (int h = 0; h < 2 && 32 * h < ncls; ++h) {
             const int pos = 32 * h + lane;
@@ -504,21 +505,28 @@ tc_chunk_kernel(ChunkArgs a, typename TcCfgOf<EPI>::type cfg, const __grid_const
         else if (p > 0) bar_sync(4 + 2 * wq, 64);
         // the rows of the list go in 8 at a time: the batch's sums are read before any is written; in a batch with a
         // repeated label, a row continues from the running sum of that label's earlier row.  So every element receives
-        // its rows in tile order, then row order, one rounded addition each
-        if (f < d) {
-          const uint32_t fo = (uint32_t)f * 4u, fx = (uint32_t)((f >> 2) & 7) << 4;
+        // its rows in tile order, then row order, one rounded addition each.  The positions of the last batch beyond
+        // the list are not accessed (the list is not padded: a padding row would cost shared-memory traffic like a
+        // real one).  A pair that straddles d also adds the zero-filled column d into its second element, which the
+        // teardown never reads
+        if (2 * f2 < d) {
+          const uint32_t fo = (uint32_t)f2 * 8u, fx = (uint32_t)((f2 >> 1) & 7) << 4;
           unsigned char* sum_b = reinterpret_cast<unsigned char*>(sum_s);
-          const unsigned char* xs_b = xs + (f >> 5) * XBOX_BYTES + (f & 3) * 4;
+          const unsigned char* xs_b = xs + (f2 >> 4) * XBOX_BYTES + (f2 & 1) * 8;
           const uint4* cl4 = reinterpret_cast<const uint4*>(cls);
           uint4 ea = cl4[0], eb = cl4[1];
 #pragma unroll 1
           for (int b = 0; 8 * b < ncls; ++b) {
             const uint32_t e[8] = {ea.x, ea.y, ea.z, ea.w, eb.x, eb.y, eb.z, eb.w};
-            float v[8], x[8];
+            const int nb = ncls - 8 * b;                     // list rows in this batch (warp-uniform)
+            float2 v[8], x[8];
 #pragma unroll
             for (int j = 0; j < 8; ++j) {
-              v[j] = *reinterpret_cast<const float*>(sum_b + ((e[j] & CLS_SUM_MASK) | fo));
-              x[j] = *reinterpret_cast<const float*>(xs_b + ((e[j] >> CLS_ROW_SHIFT) ^ fx));
+              v[j] = x[j] = make_float2(0.f, 0.f);
+              if (j < nb) {
+                v[j] = *reinterpret_cast<const float2*>(sum_b + ((e[j] & CLS_SUM_MASK) | fo));
+                x[j] = *reinterpret_cast<const float2*>(xs_b + ((e[j] >> CLS_ROW_SHIFT) ^ fx));
+              }
             }
             if (8 * (b + 1) < ncls) { ea = cl4[2 * b + 2]; eb = cl4[2 * b + 3]; }
             if ((rep >> (8 * b)) & 0xffu) {
@@ -527,15 +535,16 @@ tc_chunk_kernel(ChunkArgs a, typename TcCfgOf<EPI>::type cfg, const __grid_const
 #pragma unroll
                 for (int i = 0; i < j; ++i)
                   if (((e[i] ^ e[j]) & CLS_SUM_MASK) == 0u) v[j] = v[i];
-                v[j] += x[j];
+                v[j].x += x[j].x; v[j].y += x[j].y;
               }
             } else {
 #pragma unroll
-              for (int j = 0; j < 8; ++j) v[j] += x[j];
+              for (int j = 0; j < 8; ++j) { v[j].x += x[j].x; v[j].y += x[j].y; }
             }
             // a repeated label: the last store is the full sum
 #pragma unroll
-            for (int j = 0; j < 8; ++j) *reinterpret_cast<float*>(sum_b + ((e[j] & CLS_SUM_MASK) | fo)) = v[j];
+            for (int j = 0; j < 8; ++j)
+              if (j < nb) *reinterpret_cast<float2*>(sum_b + ((e[j] & CLS_SUM_MASK) | fo)) = v[j];
           }
         }
         // bar.arrive -> bar.sync orders these shared-memory writes before the next turn's accesses (PTX memory model:
@@ -723,7 +732,7 @@ static uint32_t layout_common(int d, int k, bool mstep, TcCfg* c) {
   uint32_t o = 0;
   c->off_bhi = o; o += N * 128u;                    // fp16 B tiles: N rows x 64 halves (one 128-byte swizzle atom)
   c->off_blo = o; o += N * 128u;
-  c->off_sum = o; if (mstep) o += (N + 2u) * 64u * 4u;   // per-CTA sums [N][64] + 2 spare rows
+  c->off_sum = o; if (mstep) o += N * 64u * 4u;          // per-CTA sums [N][64]
   c->off_cn = o; o += N * 4u;
   c->off_cnt = o; o += N * 4u;
   c->off_lab = o; o += 2u * TBM * 4u;
