@@ -48,7 +48,7 @@ __global__ void __launch_bounds__(kThreads) impute_stats_kernel(IStatsArgs a) {
 #pragma unroll 1
   for (int j0 = 0; j0 < d; j0 += CB) {
     const int j = j0 + bc;
-    const bool on = j < d;
+    const bool on = bg < G && j < d;
     const double s = (on && a.shift) ? a.shift[j] : 0.0;
     double f[IS_N] = {0.0, 0.0, 0.0, 0.0};
     if (on) {
@@ -140,7 +140,7 @@ __global__ void __launch_bounds__(kThreads) impute_fill_kernel(FillArgs p) {
 #pragma unroll 1
   for (int o0 = 0; o0 < tasks; o0 += CB) {
     const int o = o0 + bc;
-    if (o >= tasks) continue;
+    if (bg >= G || o >= tasks) continue;     // the spare threads would count row group 0's rows in invalid again
     int src, kind;                 // kind 0: filled column, 1: indicator, 2: validation only, 3: inverse
     int isrc = -1;
     C fill = (C)0;

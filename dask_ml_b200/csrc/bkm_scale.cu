@@ -284,7 +284,7 @@ __global__ void __launch_bounds__(kThreads) affine_kernel(AffineArgs p) {
 #pragma unroll 1
   for (int j0 = 0; j0 < d; j0 += CB) {
     const int j = j0 + bc;
-    if (j >= d) continue;
+    if (bg >= G || j >= d) continue;         // the 256 mod CB spare threads: their rows belong to row group 0
     const C a = p.op1 != OP1_NONE ? (C)p.a[j] : (C)0;
     const C b = p.op2 != OP2_NONE ? (C)p.b[j] : (C)0;
 #pragma unroll 1
