@@ -595,8 +595,9 @@ int launch_sample(const void* d2, long long n, int dtype, double eop, uint64_t s
 // ---------------------------------------------------------------------------------------
 // transform: out[i][j] = sqrt(max(||x_i||^2 - 2 x_i.c_j + ||c_j||^2, 0))   (pairwise.py:79-97)
 // computed in the dtype of X like the reference does.  Output-bandwidth bound: each CTA stages
-// 64 rows, every thread produces (row, 4 centres) micro-tiles, results go out through smem so
-// the global stores are coalesced along k.
+// a tile of TR rows (64, fewer for wide rows) and their norms in smem; the threads walk the tile's
+// (row, centre) pairs with the centre fastest and store each result directly, so consecutive
+// threads write consecutive outputs of a row.
 // ---------------------------------------------------------------------------------------
 template <typename T>
 __global__ void __launch_bounds__(256)
