@@ -12,25 +12,28 @@
 // re-decided in float64 (as are rows whose scaled entries leave fp16's range).  The M-step (_centers_dense,
 // dask_ml/cluster/k_means.py:572-582) is fused: rows are added into shared-memory per-CTA sums, X is read from HBM once.
 //
-// CTA = 2 warpgroups (1 CTA per SM).  The CTA's tiles stream through a ring of S shared-memory slots filled by TMA
-// (local tile lt -> slot lt % S, one "full" mbarrier per slot; fp32 rows in 32-column SWIZZLE_128B boxes, zero-filled
-// beyond n and d by the copy engine).  Each warpgroup owns alternate 64-row tiles of the CTA (lt % 2) and runs, per tile:
+// CTA = NWG warpgroups (1 CTA per SM): 3 in the M-step variants, 2 in the others (tc_warpgroups).  The CTA's tiles
+// stream through a ring of S shared-memory slots filled by TMA (local tile lt -> slot lt % S, one "full" mbarrier per
+// slot; fp32 rows in 32-column SWIZZLE_128B boxes, zero-filled beyond n and d by the copy engine).  Warpgroup w owns
+// the CTA's tiles lt with lt % NWG == w and runs, per tile:
 //   the wait for the tile's slot;
 //   the fp16 (hi, lo) A fragments of s X built in registers (and ||s x||^2);
 //   3 KS wgmma.m64nNk16 (KS = ceil(d/16), a template parameter so that they issue back to back) with B
-//   (= -2 s C as fp16 hi / lo, SWIZZLE_128B K-major) resident in shared memory; N = 256 runs as two column halves in
-//   two commit groups;
+//   (= -2 s C as fp16 hi / lo, SWIZZLE_128B K-major) resident in shared memory; N = 256 runs as two column halves of
+//   128;
 //   the arg-min epilogue from the register accumulators in two passes (the row minimum, then the count and index
-//   of the columns within the near-tie bound of it), the first pass over the first column half while the tensor
-//   cores compute the second;
+//   of the columns within the near-tie bound of it), one column half at a time: half 1's MMAs reuse half 0's
+//   accumulator registers once its passes are done (wg::near_tie_cols), so a thread keeps 64 of them, not 128;
 //   the winning distance in direct form (x - c)^2 in fp32, and the M-step;
 //   after the warpgroup's last read of the slot, the load of tile lt + S into it (no separate producer).
-// The M-step adds the tile's rows in row order into the CTA's sums; the two warpgroups take turns (named barriers),
-// so every cluster's sum is formed in one fixed order and the sums are bit-reproducible.  Each sums element has one
-// owning thread (feature pair f2, label class q = c % 4, warp q of its warpgroup); before its turn a warp lists the
-// tile's rows of its class, so that the turn touches only owned rows, and marks the batches of 8 rows in which a label
-// repeats (only those forward running sums).  The turn order is kept per warp pair: warp w of each warpgroup owns the
-// same elements.  One warpgroup's MMAs overlap the other's epilogue / M-step.
+// The M-step adds the tile's rows in row order into the CTA's sums; the warpgroups take turns in tile order (named
+// barriers), so every cluster's sum is formed in one fixed order and the sums are bit-reproducible.  Each sums element
+// has one owning thread (feature pair f2, label class q = c % 4, warp q of its warpgroup); before its turn a warp lists
+// the tile's rows of its class, so that the turn touches only owned rows, and marks the batches of 8 rows in which a
+// label repeats (only those forward running sums).  The turn order is kept per warp triple: warp w of each warpgroup
+// owns the same elements.  One warpgroup's MMAs overlap the others' epilogues / M-steps; the third warpgroup of the
+// M-step variants gives each scheduler a third warp to issue from while the others wait on shared memory, barriers
+// or the tensor cores.
 #include "bkm_common.cuh"
 #include "bkm_wgmma.cuh"
 #include <cuda.h>
@@ -41,15 +44,20 @@
 namespace bkm {
 
 static const int TBM = 64;           // rows per warpgroup tile (wgmma M)
-static const int TC_THREADS = 256;   // two warpgroups
+// Warpgroups of a CTA.  The M-step variants run three: at 384 threads a thread has 168 registers, which the arg-min by
+// column halves leaves enough.  The others keep two: without the turn order, a slot has one reader only when S is a
+// multiple of the warpgroup count (see place_ring), and their S = 8 is not a multiple of 3.
+__host__ __device__ constexpr int tc_warpgroups(bool mstep) { return mstep ? 3 : 2; }
+static const int TC_MAX_THREADS = 128 * tc_warpgroups(true);
 // X ring: a slot holds one 64 x 64 fp32 tile as two TMA boxes of 32 columns (box b: columns 32b .. 32b + 31, 64 rows of
 // 128 bytes, SWIZZLE_128B: 16-byte chunk q of row r sits at chunk q ^ (r & 7)), so that a warp's reads of 8 rows x one
 // chunk, or of one row x 32 columns, hit 32 different banks
 static const uint32_t XBOX_BYTES = TBM * 128u;
 static const uint32_t XSLOT_BYTES = 2u * XBOX_BYTES;
 static const int TC_MAX_STAGES = 8;
-// two slots per warpgroup: the tile being worked on and the next one.  Every supported shape (d <= 64, k <= 256) leaves
-// room for at least 4 (the M-step variants at N = 256: 5)
+// two slots per warpgroup of the two-warpgroup variants (the tile being worked on and the next one); more slots than
+// warpgroups for the three of the M-step variants (the slot-reuse argument at the wait in tc_chunk_kernel).  Every
+// supported shape (d <= 64, k <= 256) leaves room for at least 4 (the M-step variants at N = 256: 5)
 static const int TC_MIN_STAGES = 4;
 
 struct TcCfg {
@@ -112,13 +120,13 @@ __device__ __forceinline__ uint32_t pack_half2(float lo, float hi) {
 // (euclidean_distances, dask_ml/metrics/pairwise.py:69-97; rbf_kernel :131-139); COLSUM and EMBED are the two passes
 // of the Nystrom embedding (dask_ml/cluster/spectral.py:237-282).  Same MMAs, no M-step.
 template <int N, int KS, bool MSTEP, bool WANT_DIST, int EPI>
-__global__ void __launch_bounds__(TC_THREADS, 1)
+__global__ void __launch_bounds__(128 * tc_warpgroups(MSTEP), 1)
 tc_chunk_kernel(ChunkArgs a, typename TcCfgOf<EPI>::type cfg, const __grid_constant__ CUtensorMap xmap) {
-  constexpr bool XFORM = EPI == EPI_XFORM;
   if (a.skip && *a.skip) return;                            // converged loop: no-op iteration
 
   extern __shared__ __align__(1024) unsigned char smem[];
   constexpr bool HAS_M = MSTEP || WANT_DIST;
+  constexpr int NWG = tc_warpgroups(MSTEP), TC_THREADS = 128 * NWG;
   // N = 256: two MMA column halves of 128 (the second half's B rows start 128 x 128 bytes = 16 whole swizzle atoms on)
   constexpr int NH = N == 256 ? 2 : 1, NC = N / NH;
   const int tid = threadIdx.x, lane = tid & 31, wgi = tid >> 7, t = tid & 127, wq = t >> 5;
@@ -167,7 +175,7 @@ tc_chunk_kernel(ChunkArgs a, typename TcCfgOf<EPI>::type cfg, const __grid_const
   }
   const long long ntiles = (a.n + TBM - 1) / TBM;
   const long long my_tiles = blockIdx.x < ntiles ? (ntiles - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;
-  const long long npairs = (my_tiles + 1) / 2;               // warpgroup w takes the CTA's tiles 2p + w
+  const long long nrounds = (my_tiles + NWG - 1) / NWG;      // warpgroup w takes the CTA's tiles NWG p + w
   const int S = cfg.S;
   const uint32_t bar0 = sbase + cfg.off_bar, ring0 = sbase + cfg.off_ring;
   // tile lt -> slot lt % S: its ceil(d / 32) boxes, completion counted in bytes on the slot's mbarrier
@@ -196,16 +204,17 @@ tc_chunk_kernel(ChunkArgs a, typename TcCfgOf<EPI>::type cfg, const __grid_const
   int slot = wgi;                                            // lt % S and the parity (lt / S) & 1 of the slot's fill
   uint32_t fill = 0;
 #pragma unroll 1
-  for (long long p = 0; p < npairs; ++p) {
-    const long long lt = 2 * p + wgi;
+  for (long long p = 0; p < nrounds; ++p) {
+    const long long lt = NWG * p + wgi;
     const bool has = lt < my_tiles;
     const long long row0 = (blockIdx.x + lt * gridDim.x) * TBM;
     unsigned char* xs = smem + cfg.off_ring + (uint32_t)slot * XSLOT_BYTES;
     // The previous fill of this slot (tile lt - S) must have landed before this wait starts: if it has not, the
     // barrier is still in that phase, and the parity of tile lt's phase, which is also that of tile lt - 2S's, reads as
-    // complete.  With S even, tile lt - S is this warpgroup's own earlier tile.  With S odd (the M-step variants only,
-    // see place_ring) it is the other warpgroup's, and the turn order covers it: this warpgroup's previous turn (tile
-    // lt - 2) waited for the other's turn of tile lt - 3 >= lt - S + 2, which came after its wait for tile lt - S.
+    // complete.  Without the M-step (two warpgroups, S even, see place_ring) tile lt - S is this warpgroup's own
+    // earlier tile.  With it (three warpgroups, any S >= 4) the turn order covers it: this warpgroup's previous turn
+    // (tile lt - 3) came after the turns of tiles lt - 4, lt - 5, ..., lt - S, and the turn of tile lt - S came after
+    // its warpgroup's wait for that tile.
     if (has) ptx::mbar_wait(bar0 + 8u * (uint32_t)slot, fill);
     if (has) {
       // ---- s X -> fp16 (hi, lo) A fragments, ||s x||^2 of rows rA / rA + 8 ----
@@ -231,15 +240,8 @@ tc_chunk_kernel(ChunkArgs a, typename TcCfgOf<EPI>::type cfg, const __grid_const
       xn0 += __shfl_xor_sync(0xffffffffu, xn0, 1); xn0 += __shfl_xor_sync(0xffffffffu, xn0, 2);
       xn1 += __shfl_xor_sync(0xffffffffu, xn1, 1); xn1 += __shfl_xor_sync(0xffffffffu, xn1, 2);
 
-      // ---- acc = Xhi.Bhi + Xhi.Blo + Xlo.Bhi, column half by column half (NH commit groups of NC columns; the
-      //      accumulator fragment of columns [h NC, (h + 1) NC) is acc[h NC / 2 ...]) ----
-      float acc[N / 2];
-#pragma unroll
-      for (int i = 0; i < N / 2; ++i) acc[i] = 0.f;
-      wg::fence();
-#pragma unroll
-      for (int hf = 0; hf < NH; ++hf) {
-        float(&ah)[NC / 2] = *reinterpret_cast<float(*)[NC / 2]>(acc + hf * (NC / 2));
+      // ---- acc = Xhi.Bhi + Xhi.Blo + Xlo.Bhi of columns [hf NC, (hf + 1) NC) into ah, one commit group ----
+      auto mma_half = [&](float(&ah)[NC / 2], int hf) {
         const uint64_t bh = dbh + (uint64_t)(hf * NC * 128 / 16), bl = dbl + (uint64_t)(hf * NC * 128 / 16);
 #pragma unroll
         for (int s = 0; s < KS; ++s) wg::Mma<NC>::rs_f16(ah, ahi[s], bh + (uint64_t)(2 * s), s > 0);
@@ -248,6 +250,17 @@ tc_chunk_kernel(ChunkArgs a, typename TcCfgOf<EPI>::type cfg, const __grid_const
 #pragma unroll
         for (int s = 0; s < KS; ++s) wg::Mma<NC>::rs_f16(ah, alo[s], bh + (uint64_t)(2 * s), 1);
         wg::commit();
+      };
+      // the whole tile's accumulators (the epilogues other than the arg-min): the accumulator fragment of columns
+      // [hf NC, (hf + 1) NC) is acc[hf NC / 2 ...]
+      constexpr int NACC = EPI == EPI_ARGMIN ? NC : N;
+      float acc[NACC / 2];
+#pragma unroll
+      for (int i = 0; i < NACC / 2; ++i) acc[i] = 0.f;
+      if constexpr (EPI != EPI_ARGMIN) {
+        wg::fence();
+#pragma unroll
+        for (int hf = 0; hf < NH; ++hf) mma_half(*reinterpret_cast<float(*)[NC / 2]>(acc + hf * (NC / 2)), hf);
       }
 
       if constexpr (EPI == EPI_COLSUM) {
@@ -388,28 +401,19 @@ tc_chunk_kernel(ChunkArgs a, typename TcCfgOf<EPI>::type cfg, const __grid_const
         else store_block([&](float y) { return __expf(-gs * y); });
       } else {
         static_assert(EPI == EPI_ARGMIN, "epilogue");
-        // ---- arg-min, near-tie test (bound = tau (||s x||^2 + max ||s c||^2)) ----
-        // pass 1: the values in place and the row minimum m, over the first column half while the second computes
-        float m[2] = {CUDART_INF_F, CUDART_INF_F};
-        if constexpr (NH == 2) {
-          float(&a0)[NC / 2] = *reinterpret_cast<float(*)[NC / 2]>(acc);
-          float(&a1)[NC / 2] = *reinterpret_cast<float(*)[NC / 2]>(acc + NC / 2);
-          wg::wait_1();                                      // first column half done, second still running
-          wg::pin(a0);
-          wg::min_cols<NC>(a0, cn_s, 0, lane, m);
-          wg::wait_all();
-          wg::pin(a1);
-          wg::min_cols<NC>(a1, cn_s, NC, lane, m);
-        } else {
+        // ---- arg-min, near-tie test (bound = tau (||s x||^2 + max ||s c||^2)), one column half at a time: the row
+        //      minimum m of the half, then the count and index sum of its columns with value <= thr = m + bound over
+        //      the columns so far (tau >= 0; xn >= 0 or NaN) ----
+        float m[2] = {CUDART_INF_F, CUDART_INF_F}, thr[2], hits[2] = {0.f, 0.f};
+        const float xb[2] = {xn0 + cnmax, xn1 + cnmax};
+#pragma unroll
+        for (int hf = 0; hf < NH; ++hf) {
+          wg::fence();                                       // the registers of the previous half were written
+          mma_half(acc, hf);
           wg::wait_all();
           wg::pin(acc);
-          wg::min_cols<N>(acc, cn_s, 0, lane, m);
+          wg::near_tie_cols<NC>(acc, cn_s, hf * NC, lane, a.tau, xb, m, thr, hits);
         }
-        wg::min_quad_merge(m);
-        // pass 2: count and index sum of the columns with value <= thr = m + bound (tau >= 0; xn >= 0 or NaN)
-        const float thr[2] = {m[0] + a.tau * (xn0 + cnmax), m[1] + a.tau * (xn1 + cnmax)};
-        float hits[2];
-        wg::hit_cols<N>(acc, thr, hits);
         wg::hit_quad_merge(hits, lane);
         if ((lane & 3) == 0) {
 #pragma unroll
@@ -498,11 +502,14 @@ tc_chunk_kernel(ChunkArgs a, typename TcCfgOf<EPI>::type cfg, const __grid_const
             rep |= (uint64_t)__ballot_sync(0xffffffffu, r && pos < ncls) << (32 * h);
           }
         }
-        // turn order of the CTA's M-steps: warpgroup 0 tile p, warpgroup 1 tile p, warpgroup 0 tile p + 1, ...; only
-        // warp w of the other warpgroup owns the same sums elements, so the order is kept per warp pair (named barriers
-        // 3 + 2w: warpgroup 0 -> 1, 4 + 2w: warpgroup 1 -> 0)
-        if (wgi == 1) bar_sync(3 + 2 * wq, 64);
-        else if (p > 0) bar_sync(4 + 2 * wq, 64);
+        // turn order of the CTA's M-steps: the tile order lt = 0, 1, 2, ... (warpgroup 0 round p, warpgroup 1 round p,
+        // ..., warpgroup 0 round p + 1, ...; a round past the CTA's last tile takes its turn with an empty list).  Only
+        // warp w of the other warpgroups owns the same sums elements, so the order is kept per warp triple: named
+        // barrier 1 + NWG + NWG w + i hands warp w's turn from warpgroup i to warpgroup i + 1 mod NWG (ids 4 .. 15;
+        // 1 .. 3 are the warpgroups' own).  A barrier is not reused before its previous use completes: warpgroup i
+        // arrives at it again only after its own next turn, which waited on the whole cycle.
+        static_assert(1 + NWG + NWG * 4 <= 16, "named barriers");
+        if (lt > 0) bar_sync(1 + NWG + NWG * wq + (wgi + NWG - 1) % NWG, 64);
         // the rows of the list go in 8 at a time: the batch's sums are read before any is written; in a batch with a
         // repeated label, a row continues from the running sum of that label's earlier row.  So every element receives
         // its rows in tile order, then row order, one rounded addition each.  The positions of the last batch beyond
@@ -549,8 +556,7 @@ tc_chunk_kernel(ChunkArgs a, typename TcCfgOf<EPI>::type cfg, const __grid_const
         }
         // bar.arrive -> bar.sync orders these shared-memory writes before the next turn's accesses (PTX memory model:
         // the arrive synchronizes with the sync on the same barrier)
-        if (wgi == 0) bar_arrive(3 + 2 * wq, 64);
-        else if (p + 1 < npairs) bar_arrive(4 + 2 * wq, 64);
+        if (lt + 1 < NWG * nrounds) bar_arrive(1 + NWG + NWG * wq + wgi, 64);
       }
     }
     wg::wg_sync(1 + wgi);                                    // the slot and lab_s may be refilled
@@ -558,7 +564,7 @@ tc_chunk_kernel(ChunkArgs a, typename TcCfgOf<EPI>::type cfg, const __grid_const
       ptx::fence_proxy_async();                              // the warpgroup's accesses to the slot before the async-proxy fill
       load_tile(lt + S, slot);
     }
-    slot += 2;
+    slot += NWG;                                             // NWG < S: at most one wrap
     if (slot >= S) { slot -= S; fill ^= 1u; }
   }
 
@@ -735,14 +741,16 @@ static uint32_t layout_common(int d, int k, bool mstep, TcCfg* c) {
   c->off_sum = o; if (mstep) o += N * 64u * 4u;          // per-CTA sums [N][64]
   c->off_cn = o; o += N * 4u;
   c->off_cnt = o; o += N * 4u;
-  c->off_lab = o; o += 2u * TBM * 4u;
-  c->off_dp = o; o += 2u * 2u * TBM * 4u;
-  c->off_cls = o; if (mstep) o += TC_THREADS / 32u * TBM * 4u;   // per-warp class lists of the M-step
+  const uint32_t nwg = (uint32_t)tc_warpgroups(mstep);
+  c->off_lab = o; o += nwg * TBM * 4u;              // per warpgroup: the labels of its tile
+  c->off_dp = o; o += nwg * 2u * TBM * 4u;          // per warpgroup: halves of the direct distances
+  c->off_cls = o; if (mstep) o += nwg * 4u * TBM * 4u;   // per-warp class lists of the M-step
   return o;
 }
 // The X ring fills what is left of the 227 KB from offset o: S = as many 16 KB slots as fit (at most TC_MAX_STAGES).
 // Without the M-step turns nothing orders the two warpgroups, so S is rounded down to even there: each slot is then
-// filled and read by one warpgroup only (see the wait in tc_chunk_kernel)
+// filled and read by one warpgroup only.  The M-step variants' three warpgroups are ordered by their turns, which
+// covers any S >= 4 (see the wait in tc_chunk_kernel)
 static bool place_ring(TcCfg* c, uint32_t o, bool mstep) {
   const uint32_t cap = 227u * 1024u;
   c->off_bar = o; o += TC_MAX_STAGES * 8u;           // one "full" mbarrier per slot
@@ -751,7 +759,7 @@ static bool place_ring(TcCfg* c, uint32_t o, bool mstep) {
   c->S = o < cap ? (int)min((uint32_t)TC_MAX_STAGES, (cap - o) / XSLOT_BYTES) : 0;
   if (!mstep) c->S &= ~1;
   c->total = o + (uint32_t)c->S * XSLOT_BYTES;
-  static_assert(TC_THREADS * 8u <= XSLOT_BYTES, "the teardown's reduction array lives in the first slot");
+  static_assert(TC_MAX_THREADS * 8u <= XSLOT_BYTES, "the teardown's reduction array lives in the first slot");
   return c->S >= TC_MIN_STAGES;
 }
 
@@ -795,7 +803,7 @@ static int launch_variant(const ChunkArgs& a, const typename TcCfgOf<XF>::type& 
   if (const int rc = encode_x_map(a, &xmap)) return rc;
   auto kern = tc_chunk_kernel<N, KS, M, W, XF>;
   BKM_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cfg.total));
-  kern<<<grid, TC_THREADS, cfg.total, s>>>(a, cfg, xmap);
+  kern<<<grid, 128 * tc_warpgroups(M), cfg.total, s>>>(a, cfg, xmap);
   return 0;
 }
 template <int N, bool M, bool W, int XF>

@@ -210,20 +210,50 @@ __device__ __forceinline__ void min_quad_merge(float (&m)[2]) {
     m[h] = fminf(m[h], __shfl_xor_sync(0xffffffffu, m[h], 2));
   }
 }
-// Pass 2 over the values of all N columns (formed by min_cols) of the thread's two rows: hits[h] = the sum over the
-// columns j with value <= t[h] of 1 + j / 1024, without the lane's column offset 2 (lane % 4) in j, which
-// hit_quad_merge adds: each column then costs one FSET (0 for NaN) and one FFMA with an immediate.  Every partial sum
-// is a multiple of 2^-10 below 2^9, so it is exact in any order.  Two chains per row.
+// Pass 2 over the values of columns j0 .. j0 + N - 1 (formed by min_cols) of the thread's two rows: hits[h] = the sum
+// over those columns j with value <= t[h] of 1 + j / 1024, without the lane's column offset 2 (lane % 4) in j, which
+// hit_quad_merge adds: each column then costs one FSET (0 for NaN) and one FFMA with an immediate (j0 is a constant of
+// the unrolled caller).  Every partial sum is a multiple of 2^-10 below 2^9, so it is exact in any order.  Two chains
+// per row.
 template <int N>
-__device__ __forceinline__ void hit_cols(const float (&d)[N / 2], const float (&t)[2], float (&hits)[2]) {
+__device__ __forceinline__ void hit_cols(const float (&d)[N / 2], int j0, const float (&t)[2], float (&hits)[2]) {
   float c[2][2] = {{0.f, 0.f}, {0.f, 0.f}};         // [row][column parity]
 #pragma unroll
   for (int i = 0; i < N / 8; ++i)
 #pragma unroll
     for (int e = 0; e < 4; ++e)
-      c[e >> 1][e & 1] = fmaf(ptx::fset_le(d[4 * i + e], t[e >> 1]), 1.f + (float)(8 * i + (e & 1)) * 0.0009765625f, c[e >> 1][e & 1]);
+      c[e >> 1][e & 1] = fmaf(ptx::fset_le(d[4 * i + e], t[e >> 1]), 1.f + (float)(j0 + 8 * i + (e & 1)) * 0.0009765625f, c[e >> 1][e & 1]);
 #pragma unroll
   for (int h = 0; h < 2; ++h) hits[h] = c[h][0] + c[h][1];
+}
+// Both passes over one group of N columns (starting at j0) of a row whose columns are visited a group at a time, so
+// that only one group's accumulators are live.  Before the first group m = +inf and hits = 0; after the last, m is the
+// row minimum, thr = fma(tau, xb, m) (the near-tie bound tau xb does not depend on m) and hits is what hit_cols would
+// count at thr over all the columns, or, for a row with two or more columns <= thr, some value >= 2 per quad.  At each
+// group the running minimum mn = min(m, group minimum) gives thr; the earlier groups' hits were counted at the thr of
+// their own running minimum m >= mn:
+//   m == mn: thr is unchanged and they are exact;
+//   m > thr: every earlier column is > thr, so they are dropped (0 hits);
+//   mn < m <= thr: the earlier column at m and this group's column at mn are both <= thr: a near-tie either way, and the
+//   earlier hits, which include the column at m (m <= fma(tau, xb, m), tau xb >= 0), keep the total >= 2.
+// NaN values are skipped, and a NaN or infinite thr leaves the row a near-tie, as in the one-pass form.
+template <int N>
+__device__ __forceinline__ void near_tie_cols(float (&d)[N / 2], const float* cn, int j0, int lane, float tau,
+                                              const float (&xb)[2], float (&m)[2], float (&thr)[2], float (&hits)[2]) {
+  float mg[2] = {CUDART_INF_F, CUDART_INF_F};
+  min_cols<N>(d, cn, j0, lane, mg);
+  min_quad_merge(mg);
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const float mn = fminf(m[h], mg[h]);
+    thr[h] = fmaf(tau, xb[h], mn);
+    if (m[h] > thr[h]) hits[h] = 0.f;
+    m[h] = mn;
+  }
+  float hg[2];
+  hit_cols<N>(d, j0, thr, hg);
+#pragma unroll
+  for (int h = 0; h < 2; ++h) hits[h] += hg[h];
 }
 // Adds the lane's column offset, then sums over the quad: every lane ends with its rows' totals.  A lane with one hit
 // holds a value in [1, 1.25) (its index part is < 256 / 1024), so floor() is its hit count; a lane with more hits
