@@ -329,6 +329,7 @@ int launch_stream(const ChunkArgs& a, bool mstep, int sm_count, int* grid_out, c
 int launch_tc2(const ChunkArgs& a, bool mstep, int sm_count, int* grid_out, cudaStream_t s);
 int launch_rowpass_mstep(const ChunkArgs& a, int x_dtype, int sm_count, int* parts_out, cudaStream_t s);
 int launch_rowpass_dist(const ChunkArgs& a, int x_dtype, int sm_count, int* parts_out, cudaStream_t s);
+int rowpass_layout(int k, int d, long long n, int sm_count, int* out9);
 // implemented in bkm_aux.cu
 int launch_reduce_partials(const ChunkArgs& a, int sum_parts, int cnt_parts, int pin_parts, bool mstep, int psum_dtype,
                            double* sums, long long* counts, double* dist_sum, cudaStream_t s);

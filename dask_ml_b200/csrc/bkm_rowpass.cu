@@ -343,6 +343,18 @@ static bool make_rp_cfg(int k, int d, int sm_count, int psum_slots, long long n,
   return o <= 227 * 1024;
 }
 
+// binning: one CTA per 4096-row tile, grid-strided past 4 CTAs per SM
+static int bin_grid(const RpCfg& c, int sm_count) {
+  return (int)(c.ntiles < (long long)sm_count * 4 ? c.ntiles : (long long)sm_count * 4);
+}
+// distances: one warp per row, grid-strided past 8 CTAs per SM (and the partial slots)
+static int dist_grid(long long n, int sm_count, int part_slots) {
+  long long grid = (n + 7) / 8;
+  if (grid > (long long)sm_count * 8) grid = (long long)sm_count * 8;
+  if (grid > part_slots) grid = part_slots;
+  return (int)(grid < 1 ? 1 : grid);
+}
+
 int launch_rowpass_mstep(const ChunkArgs& a, int x_dtype, int sm_count, int* parts_out, cudaStream_t s) {
   if (!a.labels) return BKM_EINVAL;                     // the row pass is driven by the labels
   if (x_dtype != BKM_BF16) return BKM_EDTYPE;
@@ -351,8 +363,7 @@ int launch_rowpass_mstep(const ChunkArgs& a, int x_dtype, int sm_count, int* par
   if (!make_rp_cfg(a.k, a.d, sm_count, a.psum_slots, a.n, &c, &fpl)) return BKM_EUNSUPPORTED;
   unsigned* bins = reinterpret_cast<unsigned*>(a.bin_list);
   int* tile_off = a.bin_off;
-  long long nbk = c.ntiles < (long long)sm_count * 4 ? c.ntiles : (long long)sm_count * 4;
-  rowpass_bin_kernel<<<(int)nbk, RP_THREADS, 0, s>>>(a.labels, a.n, c, bins, tile_off, a.k <= 4096 ? a.bal : nullptr, a.k, a.skip);
+  rowpass_bin_kernel<<<bin_grid(c, sm_count), RP_THREADS, 0, s>>>(a.labels, a.n, c, bins, tile_off, a.k <= 4096 ? a.bal : nullptr, a.k, a.skip);
   note_launch();
   BKM_CUDA_TRY(cudaGetLastError());
 #define RP_GO(F)                                                                                                   \
@@ -376,15 +387,31 @@ int launch_rowpass_mstep(const ChunkArgs& a, int x_dtype, int sm_count, int* par
 
 int launch_rowpass_dist(const ChunkArgs& a, int x_dtype, int sm_count, int* parts_out, cudaStream_t s) {
   if (!a.labels) return BKM_EINVAL;
-  long long grid = (a.n + 7) / 8;
-  if (grid > (long long)sm_count * 8) grid = (long long)sm_count * 8;
-  if (grid > a.part_slots) grid = a.part_slots;
-  if (grid < 1) grid = 1;
+  const int grid = dist_grid(a.n, sm_count, a.part_slots);
   if (x_dtype == BKM_BF16) rowpass_dist_kernel<__nv_bfloat16><<<(int)grid, 256, 0, s>>>(a);
   else rowpass_dist_kernel<float><<<(int)grid, 256, 0, s>>>(a);
   note_launch();
   BKM_CUDA_TRY(cudaGetLastError());
-  *parts_out = (int)grid;
+  *parts_out = grid;
+  return 0;
+}
+
+// bkm_debug_tc2_layout's row-pass half: {DS (= CS), NB, KL, RB, tiles_per_block, bin grid, dist grid, FPL, mstep
+// shared-memory bytes} of an n-row call with the workspace ws_layout sizes for sm_count SMs
+int rowpass_layout(int k, int d, long long n, int sm_count, int* out) {
+  const WsLayout W = ws_layout(n, d, k, BKM_BF16, sm_count);
+  RpCfg c;
+  int fpl = 0;
+  if (!make_rp_cfg(k, d, sm_count, W.psum_slots, n, &c, &fpl)) return BKM_EUNSUPPORTED;
+  out[0] = c.CS;
+  out[1] = c.NB;
+  out[2] = c.KL;
+  out[3] = c.RB;
+  out[4] = (int)c.tiles_per_block;
+  out[5] = bin_grid(c, sm_count);
+  out[6] = dist_grid(n, sm_count, W.part_slots);
+  out[7] = fpl;
+  out[8] = (int)c.total;
   return 0;
 }
 

@@ -315,6 +315,20 @@ static bool make_cfg2(int d, int k, int sm_count, Tc2Cfg* c) {
   return o <= 227u * 1024u;
 }
 
+// no more row-tile groups than tiles: a group without a tile would only load its slice
+static void clamp_groups(Tc2Cfg* c, long long n) {
+  const long long ntiles = (n + T2_BM - 1) / T2_BM;
+  if (ntiles < c->G) c->G = (int)ntiles;
+  if (c->G < 1) c->G = 1;
+}
+// slice combine: one thread per row, grid-strided past 8 CTAs per SM
+static int combine_grid(long long n, int sm_count) {
+  const long long nb = (n + 255) / 256;
+  return (int)(nb > sm_count * 8 ? sm_count * 8 : nb);
+}
+// float64 re-check: R2_ROWS deferred rows per CTA and turn
+static int recheck_grid(int sm_count) { return sm_count * 4; }
+
 template <int N>
 static int launch_assign(const ChunkArgs& a, const Tc2Cfg& cfg, cudaStream_t s) {
   BKM_CUDA_TRY(cudaFuncSetAttribute(tc2_assign_kernel<N>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cfg.total));
@@ -331,9 +345,7 @@ int launch_tc2(const ChunkArgs& a0, bool mstep, int sm_count, int* grid_out, cud
   Tc2Cfg cfg;
   if (!make_cfg2(a.d, a.k, sm_count, &cfg)) return BKM_EUNSUPPORTED;
   const Tc2Geom g = tc2_geom(a.k, a.d);
-  const long long ntiles = (a.n + T2_BM - 1) / T2_BM;
-  if (ntiles < cfg.G) cfg.G = (int)ntiles;
-  if (cfg.G < 1) cfg.G = 1;
+  clamp_groups(&cfg, a.n);
   BKM_CUDA_TRY(cudaMemsetAsync(a.defer_cnt, 0, 2 * sizeof(int), s));          // [0] deferred rows, [1] abort word
   int rc;
   switch (wg::mma_n(cfg.NS)) {
@@ -347,14 +359,12 @@ int launch_tc2(const ChunkArgs& a0, bool mstep, int sm_count, int* grid_out, cud
   note_launch(2);
   BKM_CUDA_TRY(cudaGetLastError());
   if (cfg.S > 1) {
-    long long nb = (a.n + 255) / 256;
-    if (nb > sm_count * 8) nb = sm_count * 8;
-    tc2_combine_kernel<<<(int)nb, 256, 0, s>>>(a, cfg.S);
+    tc2_combine_kernel<<<combine_grid(a.n, sm_count), 256, 0, s>>>(a, cfg.S);
     note_launch();
     BKM_CUDA_TRY(cudaGetLastError());
   }
   if (a.k > 1) {
-    tc2_recheck_kernel<__nv_bfloat16><<<sm_count * 4, 256, 0, s>>>(a, g.kp2);
+    tc2_recheck_kernel<__nv_bfloat16><<<recheck_grid(sm_count), 256, 0, s>>>(a, g.kp2);
     note_launch();
     BKM_CUDA_TRY(cudaGetLastError());
   }
@@ -376,3 +386,24 @@ int launch_tc2(const ChunkArgs& a0, bool mstep, int sm_count, int* grid_out, cud
 }
 
 }  // namespace bkm
+
+// The geometry a family-3 chunk call of n rows would use on sm_count SMs, from the configuration functions its
+// launches use (host only, no device call)
+extern "C" int bkm_debug_tc2_layout(int d, int k, int64_t n, int sm_count, int* out) {
+  using namespace bkm;
+  if (!out || n < 1 || sm_count < 1) return BKM_EINVAL;
+  if (!tc2_shape(d, k, BKM_BF16)) return BKM_EUNSUPPORTED;
+  Tc2Cfg cfg;
+  if (!make_cfg2(d, k, sm_count, &cfg)) return BKM_EUNSUPPORTED;
+  clamp_groups(&cfg, n);
+  out[0] = cfg.S;
+  out[1] = cfg.NS;
+  out[2] = wg::mma_n(cfg.NS);
+  out[3] = cfg.KB;
+  out[4] = cfg.KS;
+  out[5] = cfg.G;
+  out[6] = (int)cfg.total;
+  out[7] = combine_grid(n, sm_count);
+  out[8] = recheck_grid(sm_count);
+  return rowpass_layout(k, d, n, sm_count, out + 9);
+}

@@ -114,8 +114,9 @@ extern "C" {
  * 9 = bkm_sgd_order, bkm_sgd_block, bkm_sgd_csr_block
  * 10 = bkm_class_counts_chunk, bkm_csc_class_counts_chunk, bkm_nb_linear_jll_chunk, bkm_nb_csr_jll_chunk
  * 11 = bkm_debug_tc_layout
- * 12 = BKM_FLAG_FULL_PROBE of bkm_distinct_chunk */
-#define BKM_VERSION_MINOR 12
+ * 12 = BKM_FLAG_FULL_PROBE of bkm_distinct_chunk
+ * 13 = bkm_debug_tc2_layout */
+#define BKM_VERSION_MINOR 13
 
 /* element types of X */
 #define BKM_F32 0
@@ -941,6 +942,13 @@ int bkm_debug_trace(long long* out_host, int n);
  * bytes}.  epi: 0 = arg-min (Lloyd / assign; mstep = 1 for the Lloyd call), 1 = transform, 2 = Nystrom column sums,
  * 3 = Nystrom embedding with kw outputs (1..64).  Host only, no device call; BKM_EUNSUPPORTED where no variant runs. */
 int bkm_debug_tc_layout(int d, int k, int epi, int mstep, int kw, int* out4);
+/* The geometry of a bf16 chunk call (large-shape tensor path: d <= 128, k <= 4096) of n rows on sm_count SMs, from
+ * the configuration its launches use: out[0..17] = {S (centre slices), NS (slice width), N (MMA width), KB (64-feature
+ * blocks), KS (16-feature K-steps), G (row-tile groups: grid G * S), E-step dynamic shared-memory bytes, slice-combine
+ * grid, float64 re-check grid, DS (cluster slices of the M-step row pass), NB (its buckets), KL (clusters per slice),
+ * RB (row blocks), 4096-row tiles per row block, binning grid, distance-pass grid, FPL (features per lane), M-step
+ * dynamic shared-memory bytes}.  Host only, no device call; BKM_EUNSUPPORTED where no variant runs. */
+int bkm_debug_tc2_layout(int d, int k, int64_t n, int sm_count, int* out18);
 
 #ifdef __cplusplus
 }
