@@ -222,6 +222,7 @@ SIGNATURES = {
     "bkm_debug_deferred_rows": (_int, [_c_void_p, _i64, _int, _int, _int, ctypes.POINTER(_int)]),
     "bkm_debug_tc_layout": (_int, [_int, _int, _int, _int, _int, ctypes.POINTER(_int)]),
     "bkm_debug_tc2_layout": (_int, [_int, _int, _i64, _int, ctypes.POINTER(_int)]),
+    "bkm_debug_core_layout": (_int, [_int, _int, _i64, _int, _int, _int, _int, ctypes.POINTER(_int)]),
 }
 
 _lib = None

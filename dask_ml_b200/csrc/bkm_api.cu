@@ -436,4 +436,19 @@ int bkm_debug_deferred_rows(const void* workspace, int64_t n, int d, int k, int 
 }
 int bkm_debug_trace(long long* out_host, int n) { return bkm::tc_trace(out_host, n); }
 
+// The CUDA-core kernel a chunk call would run, with chunk_common's fallbacks, from the configuration functions its
+// launches use (host only, no device call)
+int bkm_debug_core_layout(int d, int k, int64_t ldx, int x_dtype, int flags, int mstep, int aligned16, int* out) {
+  if (!out || d <= 0 || k <= 0 || ldx < d) return BKM_EINVAL;
+  if (x_dtype != BKM_F32 && x_dtype != BKM_F64) return dtype_ok(x_dtype) ? BKM_EUNSUPPORTED : BKM_EDTYPE;
+  int family = bkm_kernel_family(d, k, x_dtype, flags);
+  if (family < 0) return family;
+  // the tensor-core kernel runs unless the rows are not 16-byte aligned (and FORCE_TC does not forbid the fallback)
+  if (family == 1 && ((aligned16 && ldx % 4 == 0) || (flags & BKM_FLAG_FORCE_TC))) return BKM_EUNSUPPORTED;
+  for (int i = 0; i < 13; ++i) out[i] = 0;
+  if (family == 2 && aligned16 && stream_layout(d, k, ldx, out) == 0) return 0;
+  for (int i = 0; i < 13; ++i) out[i] = 0;
+  return simt_layout(d, k, x_dtype, mstep != 0, out);
+}
+
 }  // extern "C"

@@ -315,6 +315,7 @@ __device__ __forceinline__ void loop_commit(LoopState* st, double shift, bool co
 
 // implemented in bkm_simt.cu
 int launch_simt(const ChunkArgs& a, bool mstep, int dtype, int sm_count, int* grid_out, cudaStream_t s);
+int simt_layout(int d, int k, int dtype, bool mstep, int* out13);
 // implemented in bkm_tc.cu
 int launch_tc(const ChunkArgs& a, bool mstep, int sm_count, int* grid_out, cudaStream_t s);
 int launch_tc_recheck(const ChunkArgs& a, bool mstep, int sm_count, cudaStream_t s);
@@ -325,6 +326,7 @@ int tc_trace(long long* out, int n);
 // implemented in bkm_stream.cu
 bool stream_supported(int d, int k, int dtype);
 int launch_stream(const ChunkArgs& a, bool mstep, int sm_count, int* grid_out, cudaStream_t s);
+int stream_layout(int d, int k, long long ldx, int* out13);
 // implemented in bkm_tc2.cu / bkm_rowpass.cu
 int launch_tc2(const ChunkArgs& a, bool mstep, int sm_count, int* grid_out, cudaStream_t s);
 int launch_rowpass_mstep(const ChunkArgs& a, int x_dtype, int sm_count, int* parts_out, cudaStream_t s);

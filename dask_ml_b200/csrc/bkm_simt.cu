@@ -281,7 +281,9 @@ simt_chunk_kernel(ChunkArgs a, SimtSmem S) {
         double fd = wd[0]; int fj = wj[0];
         for (int w = 1; w < NW; ++w)
           if (wd[w] < fd || (wd[w] == fd && wj[w] < fj)) { fd = wd[w]; fj = wj[w]; }
-        lab_s[r] = fj; red2_s[f] = fd;
+        // a row with no finite distance (NaN or +-inf entries) kept no centre: label 0, as the streaming and bf16
+        // kernels give it (the M-step indexes the sums by this label)
+        lab_s[r] = fj == 0x7fffffff ? 0 : fj; red2_s[f] = fd;
       }
       __syncthreads();
     }
@@ -379,9 +381,27 @@ static int pick_rt(int k, int d, int J, bool mstep, bool global_mode) {
   return rt;
 }
 
+// The configuration of one call: centres per register block, SMEM or GLOBAL mode, the lane-owns-cluster M-step, and the
+// shared-memory layout with its row tile.  The launch and bkm_debug_core_layout both take it from here.
+struct SimtPlan {
+  int J;
+  bool global_mode, smallk;
+  SimtSmem S;
+};
+
+template <typename T>
+static SimtPlan simt_plan(int k, int d, bool mstep) {
+  SimtPlan p;
+  const int waste8 = (k + 7) / 8 * 8 - k, waste16 = (k + 15) / 16 * 16 - k;
+  p.J = (waste16 <= waste8 && sizeof(T) == 4) ? 16 : 8;
+  p.global_mode = simt_mode_global<T>(k, d, p.J, mstep);
+  p.smallk = mstep && !p.global_mode && k <= 32 && d <= 16;
+  p.S = simt_smem<T>(k, d, p.J, mstep, p.global_mode, pick_rt<T>(k, d, p.J, mstep, p.global_mode));
+  return p;
+}
+
 template <typename T, int J, bool MSTEP, bool GLOBAL, bool SMALLK = false>
-static int launch_one(const ChunkArgs& a, int sm_count, int* grid_out, cudaStream_t s) {
-  SimtSmem S = simt_smem<T>(a.k, a.d, J, MSTEP, GLOBAL, pick_rt<T>(a.k, a.d, J, MSTEP, GLOBAL));
+static int launch_one(const ChunkArgs& a, const SimtSmem& S, int sm_count, int* grid_out, cudaStream_t s) {
   if (S.total > kSmemBudget) return BKM_EUNSUPPORTED;
   auto kern = simt_chunk_kernel<T, J, MSTEP, GLOBAL, SMALLK>;
   BKM_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)S.total));
@@ -401,50 +421,53 @@ static int launch_one(const ChunkArgs& a, int sm_count, int* grid_out, cudaStrea
   return 0;
 }
 
-template <typename T>
-static int launch_T(const ChunkArgs& a, bool mstep, int sm_count, int* grid_out, cudaStream_t s) {
-  const int k = a.k;
-  int waste8 = (k + 7) / 8 * 8 - k, waste16 = (k + 15) / 16 * 16 - k;
-  bool use16 = waste16 <= waste8 && sizeof(T) == 4;
-  int J = use16 ? 16 : 8;
-  bool global_mode = simt_mode_global<T>(k, a.d, J, mstep);
-#define BKM_DISPATCH(JJ)                                                                   \
-  if (mstep) {                                                                             \
-    if (global_mode) return launch_one<T, JJ, true, true>(a, sm_count, grid_out, s);       \
-    if (k <= 32 && a.d <= 16) return launch_one<T, JJ, true, false, true>(a, sm_count, grid_out, s);   /* lane-owns-cluster M-step */ \
-    return launch_one<T, JJ, true, false>(a, sm_count, grid_out, s);                       \
-  } else {                                                                                 \
-    if (global_mode) return launch_one<T, JJ, false, true>(a, sm_count, grid_out, s);      \
-    return launch_one<T, JJ, false, false>(a, sm_count, grid_out, s);                      \
-  }
-  if (J == 16) { BKM_DISPATCH(16) } else { BKM_DISPATCH(8) }
-#undef BKM_DISPATCH
-}
-
 // In GLOBAL mode the kernel accumulates into psum slot 0 with float64 atomics (fp32 inputs too): the
 // caller zeroes it and reduce_partials reads it as a single float64 partial.  grid_out is returned
 // negative in that case.
-int launch_simt(const ChunkArgs& a, bool mstep, int dtype, int sm_count, int* grid_out, cudaStream_t s) {
-  int rc;
-  bool global_mode;
-  if (dtype == BKM_F32) {
-    int J = ((a.k + 15) / 16 * 16 - a.k) <= ((a.k + 7) / 8 * 8 - a.k) ? 16 : 8;
-    global_mode = simt_mode_global<float>(a.k, a.d, J, mstep);
-    if (global_mode && mstep) {
-      BKM_CUDA_TRY(cudaMemsetAsync(a.psum, 0, (size_t)a.k * a.d * sizeof(double), s));
-      note_launch();
-    }
-    rc = launch_T<float>(a, mstep, sm_count, grid_out, s);
-  } else {
-    global_mode = simt_mode_global<double>(a.k, a.d, 8, mstep);
-    if (global_mode && mstep) {
-      BKM_CUDA_TRY(cudaMemsetAsync(a.psum, 0, (size_t)a.k * a.d * sizeof(double), s));
-      note_launch();
-    }
-    rc = launch_T<double>(a, mstep, sm_count, grid_out, s);
+template <typename T>
+static int launch_T(const ChunkArgs& a, bool mstep, int sm_count, int* grid_out, cudaStream_t s) {
+  const SimtPlan p = simt_plan<T>(a.k, a.d, mstep);
+  const SimtSmem& S = p.S;
+  if (p.global_mode && mstep) {
+    BKM_CUDA_TRY(cudaMemsetAsync(a.psum, 0, (size_t)a.k * a.d * sizeof(double), s));
+    note_launch();
   }
-  if (rc == 0 && global_mode) *grid_out = -*grid_out;
+  int rc;
+#define BKM_DISPATCH(JJ)                                                                           \
+  if (mstep) {                                                                                     \
+    if (p.global_mode) rc = launch_one<T, JJ, true, true>(a, S, sm_count, grid_out, s);            \
+    else if (p.smallk) rc = launch_one<T, JJ, true, false, true>(a, S, sm_count, grid_out, s);     \
+    else rc = launch_one<T, JJ, true, false>(a, S, sm_count, grid_out, s);                         \
+  } else {                                                                                         \
+    if (p.global_mode) rc = launch_one<T, JJ, false, true>(a, S, sm_count, grid_out, s);           \
+    else rc = launch_one<T, JJ, false, false>(a, S, sm_count, grid_out, s);                        \
+  }
+  if (p.J == 16) { BKM_DISPATCH(16) } else { BKM_DISPATCH(8) }
+#undef BKM_DISPATCH
+  if (rc == 0 && p.global_mode) *grid_out = -*grid_out;
   return rc;
+}
+
+int launch_simt(const ChunkArgs& a, bool mstep, int dtype, int sm_count, int* grid_out, cudaStream_t s) {
+  return dtype == BKM_F32 ? launch_T<float>(a, mstep, sm_count, grid_out, s)
+                          : launch_T<double>(a, mstep, sm_count, grid_out, s);
+}
+
+// bkm_debug_core_layout's generic-kernel fields: out[0] = 0, out[1..5] = {J, GLOBAL, SMALLK, rows per tile, staged tile
+// pitch (elements)}, out[12] = dynamic shared-memory bytes
+int simt_layout(int d, int k, int dtype, bool mstep, int* out13) {
+  const bool f32 = dtype == BKM_F32;
+  const SimtPlan p = f32 ? simt_plan<float>(k, d, mstep) : simt_plan<double>(k, d, mstep);
+  if (p.S.total > kSmemBudget) return BKM_EUNSUPPORTED;
+  const int d4 = (d + 3) / 4 * 4;
+  out13[0] = 0;
+  out13[1] = p.J;
+  out13[2] = p.global_mode ? 1 : 0;
+  out13[3] = p.smallk ? 1 : 0;
+  out13[4] = p.S.rt;
+  out13[5] = f32 ? tile_pitch<float>(d4) : tile_pitch<double>(d4);
+  out13[12] = (int)p.S.total;
+  return 0;
 }
 
 }  // namespace bkm

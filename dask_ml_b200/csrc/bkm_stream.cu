@@ -344,6 +344,14 @@ stream_chunk_kernel(ChunkArgs a, StreamSmem S) {
 // ==========================================================================================================
 static const int S2_NSTG = 3;       // ring stages per warp (64 rows each)
 
+// Row stride between the rows the two half-warps add in the same M-step turn: 16 >> (trailing zero bits of the row
+// pitch L), 1 from 16 floats up, so that S * L = 16 (mod 32) and the halves read different banks
+__host__ __device__ inline int stream2_pair_stride(int L) {
+  int tz = 0;
+  while (tz < 4 && !((L >> tz) & 1)) ++tz;
+  return 16 >> tz;
+}
+
 struct Stream2Smem {
   uint32_t off_c, off_cn, off_cnt, off_red, off_bar, off_slot, off_lab, off_wsum, off_ring, stage_bytes, total;
 };
@@ -452,8 +460,7 @@ stream2_chunk_kernel(ChunkArgs a, Stream2Smem S) {
 
   int mcnt = 0;
   // pairing of the two half-warps' rows (see stream2_mstep_tile)
-  const int tzL = __ffs(L) - 1;
-  const int msS = tzL >= 4 ? 1 : (16 >> tzL);
+  const int msS = stream2_pair_stride(L);
   const int mf = lane & 15, mh = lane >> 4;
   int* lab_w = reinterpret_cast<int*>(smem + S.off_lab) + warp * 64;
   float* ws_lane = wsum + (size_t)warp * (KC + 1) * 32 + mh * 16 + mf;
@@ -680,10 +687,44 @@ stream2_chunk_kernel(ChunkArgs a, Stream2Smem S) {
   }
 }
 
+// The configuration of one call: which kernel (two rows per thread for k <= 24 at a pitch of at most 32 floats, else
+// one), its feature pairs DH (d <= 4, 8, 12, 14, 16), centres KC (two-row: k rounded up to 4) or centre pairs KPT
+// (one-row: pairs rounded up to an even count), the M-step pair stride, ring stages and rows per tile, and the shared
+// memory.  The launch and bkm_debug_core_layout both take it from here.
+struct StreamPlan {
+  int two_row, DH, KB, msS, nstg, rows;    // KB: KC (two-row) or KPT (one-row)
+  uint32_t stage_bytes, total;
+};
+
+// 0, or BKM_EALIGN when the pitch is too wide for the ring (over 64 floats) / BKM_EUNSUPPORTED when the ring does not
+// fit shared memory: the caller then runs the generic kernel
+static int stream_plan(int d, int k, long long ldx, StreamPlan* p) {
+  if (ldx > 64) return BKM_EALIGN;
+  p->DH = d <= 4 ? 2 : d <= 8 ? 4 : d <= 12 ? 6 : d <= 14 ? 7 : 8;
+  p->two_row = k <= 24 && ldx <= 32;
+  if (p->two_row) {
+    p->KB = (k + 3) / 4 * 4;
+    p->msS = stream2_pair_stride((int)ldx);
+    p->nstg = S2_NSTG;
+    p->rows = 64;
+    const Stream2Smem S = stream2_smem(k, d, ldx, p->KB, (2 * p->DH + 3) / 4 * 4);
+    p->stage_bytes = S.stage_bytes;
+    p->total = S.total;
+  } else {
+    p->KB = (k + 3) / 4 * 2;
+    p->msS = 0;
+    p->nstg = SNSTG;
+    p->rows = 32;
+    const StreamSmem S = stream_smem(k, d, ldx, p->KB, 2 * p->DH);
+    p->stage_bytes = S.stage_bytes;
+    p->total = S.total;
+  }
+  return p->total > 227 * 1024 ? BKM_EUNSUPPORTED : 0;
+}
+
 template <int DH, int KC>
 static int launch_stream2_dk(const ChunkArgs& a, bool mstep, int sm_count, int* grid_out, cudaStream_t s) {
   Stream2Smem S = stream2_smem(a.k, a.d, a.ldx, KC, (2 * DH + 3) / 4 * 4);
-  if (S.total > 227 * 1024) return BKM_EUNSUPPORTED;
   const long long ntiles = (a.n + 63) / 64;
   int occ = 0;
 #define STREAM2_GO(M)                                                                                       \
@@ -709,13 +750,13 @@ static int launch_stream2_dk(const ChunkArgs& a, bool mstep, int sm_count, int* 
 }
 
 template <int DH>
-static int launch_stream2_d(const ChunkArgs& a, bool mstep, int sm_count, int* grid_out, cudaStream_t s) {
-  switch ((a.k + 3) / 4) {
-    case 1: return launch_stream2_dk<DH, 4>(a, mstep, sm_count, grid_out, s);
-    case 2: return launch_stream2_dk<DH, 8>(a, mstep, sm_count, grid_out, s);
-    case 3: return launch_stream2_dk<DH, 12>(a, mstep, sm_count, grid_out, s);
-    case 4: return launch_stream2_dk<DH, 16>(a, mstep, sm_count, grid_out, s);
-    case 5: return launch_stream2_dk<DH, 20>(a, mstep, sm_count, grid_out, s);
+static int launch_stream2_d(const ChunkArgs& a, int KC, bool mstep, int sm_count, int* grid_out, cudaStream_t s) {
+  switch (KC) {
+    case 4: return launch_stream2_dk<DH, 4>(a, mstep, sm_count, grid_out, s);
+    case 8: return launch_stream2_dk<DH, 8>(a, mstep, sm_count, grid_out, s);
+    case 12: return launch_stream2_dk<DH, 12>(a, mstep, sm_count, grid_out, s);
+    case 16: return launch_stream2_dk<DH, 16>(a, mstep, sm_count, grid_out, s);
+    case 20: return launch_stream2_dk<DH, 20>(a, mstep, sm_count, grid_out, s);
     default: return launch_stream2_dk<DH, 24>(a, mstep, sm_count, grid_out, s);
   }
 }
@@ -727,7 +768,6 @@ bool stream_supported(int d, int k, int dtype) {
 template <int DH, int KPT>
 static int launch_stream_dk(const ChunkArgs& a, bool mstep, int sm_count, int* grid_out, cudaStream_t s) {
   StreamSmem S = stream_smem(a.k, a.d, a.ldx, KPT, 2 * DH);
-  if (S.total > 227 * 1024) return BKM_EUNSUPPORTED;
   const long long ntiles = (a.n + 31) / 32;
   int occ = 0;
 #define STREAM_GO(M)                                                                                        \
@@ -753,36 +793,62 @@ static int launch_stream_dk(const ChunkArgs& a, bool mstep, int sm_count, int* g
 }
 
 template <int DH>
-static int launch_stream_d(const ChunkArgs& a, bool mstep, int sm_count, int* grid_out, cudaStream_t s) {
-  switch ((a.k + 3) / 4) {                 // pairs, rounded up to an even count
-    case 1: return launch_stream_dk<DH, 2>(a, mstep, sm_count, grid_out, s);
-    case 2: return launch_stream_dk<DH, 4>(a, mstep, sm_count, grid_out, s);
-    case 3: return launch_stream_dk<DH, 6>(a, mstep, sm_count, grid_out, s);
-    case 4: return launch_stream_dk<DH, 8>(a, mstep, sm_count, grid_out, s);
-    case 5: return launch_stream_dk<DH, 10>(a, mstep, sm_count, grid_out, s);
-    case 6: return launch_stream_dk<DH, 12>(a, mstep, sm_count, grid_out, s);
-    case 7: return launch_stream_dk<DH, 14>(a, mstep, sm_count, grid_out, s);
+static int launch_stream_d(const ChunkArgs& a, int KPT, bool mstep, int sm_count, int* grid_out, cudaStream_t s) {
+  switch (KPT) {                           // pairs, rounded up to an even count
+    case 2: return launch_stream_dk<DH, 2>(a, mstep, sm_count, grid_out, s);
+    case 4: return launch_stream_dk<DH, 4>(a, mstep, sm_count, grid_out, s);
+    case 6: return launch_stream_dk<DH, 6>(a, mstep, sm_count, grid_out, s);
+    case 8: return launch_stream_dk<DH, 8>(a, mstep, sm_count, grid_out, s);
+    case 10: return launch_stream_dk<DH, 10>(a, mstep, sm_count, grid_out, s);
+    case 12: return launch_stream_dk<DH, 12>(a, mstep, sm_count, grid_out, s);
+    case 14: return launch_stream_dk<DH, 14>(a, mstep, sm_count, grid_out, s);
     default: return launch_stream_dk<DH, 16>(a, mstep, sm_count, grid_out, s);
   }
 }
 
-// BKM_EALIGN when the row block cannot be bulk-copied (the caller then falls back to the generic CUDA-core kernel).
+// BKM_EALIGN when the row block cannot be bulk-copied, BKM_EUNSUPPORTED when its ring does not fit (the caller then
+// falls back to the generic CUDA-core kernel).
 int launch_stream(const ChunkArgs& a, bool mstep, int sm_count, int* grid_out, cudaStream_t s) {
   if (!stream_supported(a.d, a.k, BKM_F32)) return BKM_EUNSUPPORTED;
-  if ((reinterpret_cast<uintptr_t>(a.X) & 15) || a.ldx > 64) return BKM_EALIGN;
-  if (a.k <= 24 && a.ldx <= 32) {        // two rows per thread
-    if (a.d <= 4) return launch_stream2_d<2>(a, mstep, sm_count, grid_out, s);
-    if (a.d <= 8) return launch_stream2_d<4>(a, mstep, sm_count, grid_out, s);
-    if (a.d <= 12) return launch_stream2_d<6>(a, mstep, sm_count, grid_out, s);
-    if (a.d <= 14) return launch_stream2_d<7>(a, mstep, sm_count, grid_out, s);
-    return launch_stream2_d<8>(a, mstep, sm_count, grid_out, s);
+  if (reinterpret_cast<uintptr_t>(a.X) & 15) return BKM_EALIGN;
+  StreamPlan p;
+  const int rc = stream_plan(a.d, a.k, a.ldx, &p);
+  if (rc) return rc;
+  if (p.two_row) {                         // two rows per thread
+    switch (p.DH) {
+      case 2: return launch_stream2_d<2>(a, p.KB, mstep, sm_count, grid_out, s);
+      case 4: return launch_stream2_d<4>(a, p.KB, mstep, sm_count, grid_out, s);
+      case 6: return launch_stream2_d<6>(a, p.KB, mstep, sm_count, grid_out, s);
+      case 7: return launch_stream2_d<7>(a, p.KB, mstep, sm_count, grid_out, s);
+      default: return launch_stream2_d<8>(a, p.KB, mstep, sm_count, grid_out, s);
+    }
   }
-  // feature pairs (compile-time): d <= 4, 8, 12, 14, 16
-  if (a.d <= 4) return launch_stream_d<2>(a, mstep, sm_count, grid_out, s);
-  if (a.d <= 8) return launch_stream_d<4>(a, mstep, sm_count, grid_out, s);
-  if (a.d <= 12) return launch_stream_d<6>(a, mstep, sm_count, grid_out, s);
-  if (a.d <= 14) return launch_stream_d<7>(a, mstep, sm_count, grid_out, s);
-  return launch_stream_d<8>(a, mstep, sm_count, grid_out, s);
+  switch (p.DH) {                          // feature pairs (compile-time)
+    case 2: return launch_stream_d<2>(a, p.KB, mstep, sm_count, grid_out, s);
+    case 4: return launch_stream_d<4>(a, p.KB, mstep, sm_count, grid_out, s);
+    case 6: return launch_stream_d<6>(a, p.KB, mstep, sm_count, grid_out, s);
+    case 7: return launch_stream_d<7>(a, p.KB, mstep, sm_count, grid_out, s);
+    default: return launch_stream_d<8>(a, p.KB, mstep, sm_count, grid_out, s);
+  }
+}
+
+// bkm_debug_core_layout's streaming fields: out[0] = 2 (two rows per thread) or 1 (one), out[6..12] = {DH, KC or KPT,
+// M-step pair stride (0 for the one-row kernel), ring stages, rows per tile, stage bytes, dynamic shared-memory bytes};
+// BKM_EALIGN / BKM_EUNSUPPORTED where the call falls back to the generic kernel
+int stream_layout(int d, int k, long long ldx, int* out13) {
+  if (!stream_supported(d, k, BKM_F32)) return BKM_EUNSUPPORTED;
+  StreamPlan p;
+  const int rc = stream_plan(d, k, ldx, &p);
+  if (rc) return rc;
+  out13[0] = p.two_row ? 2 : 1;
+  out13[6] = p.DH;
+  out13[7] = p.KB;
+  out13[8] = p.msS;
+  out13[9] = p.nstg;
+  out13[10] = p.rows;
+  out13[11] = (int)p.stage_bytes;
+  out13[12] = (int)p.total;
+  return 0;
 }
 
 }  // namespace bkm

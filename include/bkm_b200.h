@@ -115,8 +115,9 @@ extern "C" {
  * 10 = bkm_class_counts_chunk, bkm_csc_class_counts_chunk, bkm_nb_linear_jll_chunk, bkm_nb_csr_jll_chunk
  * 11 = bkm_debug_tc_layout
  * 12 = BKM_FLAG_FULL_PROBE of bkm_distinct_chunk
- * 13 = bkm_debug_tc2_layout */
-#define BKM_VERSION_MINOR 13
+ * 13 = bkm_debug_tc2_layout
+ * 14 = bkm_debug_core_layout */
+#define BKM_VERSION_MINOR 14
 
 /* element types of X */
 #define BKM_F32 0
@@ -949,6 +950,15 @@ int bkm_debug_tc_layout(int d, int k, int epi, int mstep, int kw, int* out4);
  * RB (row blocks), 4096-row tiles per row block, binning grid, distance-pass grid, FPL (features per lane), M-step
  * dynamic shared-memory bytes}.  Host only, no device call; BKM_EUNSUPPORTED where no variant runs. */
 int bkm_debug_tc2_layout(int d, int k, int64_t n, int sm_count, int* out18);
+/* The CUDA-core chunk kernel an fp32 / float64 call (bkm_lloyd_chunk with mstep = 1, bkm_assign_chunk with mstep = 0)
+ * with these flags would run, on rows of pitch ldx whose base address is (aligned16 = 1) or is not 16-byte aligned,
+ * fallbacks included, from the configuration its launch uses: out13[0] = kernel (0 = generic, 1 = streaming with one
+ * row per thread, 2 = streaming with two); the generic kernel's out13[1..5] = {J (centres per register block), GLOBAL
+ * mode, SMALLK (lane-owns-cluster M-step), rows per tile, staged tile pitch in elements}; the streaming kernels'
+ * out13[6..11] = {DH (feature pairs), KC (two-row: centres) or KPT (one-row: centre pairs), M-step pair stride (two-row
+ * only), ring stages per warp, rows per tile, stage bytes}; out13[12] = dynamic shared-memory bytes.  Fields of the
+ * other kernel are 0.  Host only, no device call; BKM_EUNSUPPORTED where the tensor-core path runs or no kernel does. */
+int bkm_debug_core_layout(int d, int k, int64_t ldx, int x_dtype, int flags, int mstep, int aligned16, int* out13);
 
 #ifdef __cplusplus
 }
